@@ -22,7 +22,8 @@
 // Per-sample gradients are fp16 with a power-of-two scale PER LAYER, chosen on the device in the
 // same step (no state carried between steps, deterministic): level 0 (dd) from a bound on its
 // largest element, |d rgb_pre|_max * max_n sum_c |W_rgb[c][n]|; levels 1..8 (dpre_8..dpre_1) from
-// the largest elements a PROBE pass of the chain kernel sees on one tile per SM (no stores), each
+// the largest elements a PROBE pass of the chain kernel sees on one tile per SM, spread evenly over
+// each pass (no stores), each
 // mapped to 64 (10 bits of headroom to the fp16 maximum, 20 bits of normal range below; gradients
 // shrink or grow by orders of magnitude through 8 layers, one global scale costs precision in the
 // deep layers: measured 4e-2 relative error at layer 1 vs 4e-3 with per-layer scales).
@@ -455,11 +456,26 @@ struct ChainParams {
   PassBufs pass[2];
   const uint8_t* net[2];      // packed images (backward region at kOffBwd, w_sigma in the fp32 region)
   int n_pass;
-  long long tiles[2];         // 128-sample tiles per pass (probe mode: the first tiles only)
+  long long tiles[2];         // 128-sample tiles visited per pass (probe mode: a subset)
+  long long head[2];          // the real pass visits tiles j < head of both passes first (the probe's tiles)
+  long long span[2];          // 128-sample tiles of the pass; visit j of a pass is tile j * stride mod span
+  long long stride[2];        // coprime to span (so the real pass visits every tile once), ~ span / probe tiles
   const float* lscale;        // [2][kLevels] per-level scales (bwd_scale_kernel)
   unsigned* lamax;            // probe mode: [2][kLevels] maxima of the un-scaled values per level
   int* status;
 };
+
+// Visit t of a chain launch -> (pass, tile): the first head[0] + head[1] visits are visits j < head of pass 0,
+// then of pass 1, the rest the remaining visits of pass 0, then of pass 1; visit j of a pass is tile
+// j * stride mod span.  In probe mode head == tiles, so only the first part exists.
+__device__ __forceinline__ long long chain_tile(const ChainParams& p, long long t, int& ps) {
+  long long j;
+  if (t < p.head[0]) { ps = 0; j = t; }
+  else if (t < p.head[0] + p.head[1]) { ps = 1; j = t - p.head[0]; }
+  else if (t < p.tiles[0] + p.head[1]) { ps = 0; j = t - p.head[1]; }
+  else { ps = 1; j = t - p.tiles[0]; }
+  return j * p.stride[ps] % p.span[ps];
+}
 
 // One step of the chain for this thread's accumulator (2 rows x 64 columns).
 //   kFirst: add the rank-1 sigma-head term
@@ -532,8 +548,8 @@ __global__ void __launch_bounds__(kThreads, 1) chain_bwd_kernel(const ChainParam
       RingState rs;
       int it = 0;
       for (long long t = blockIdx.x; t < total; t += gridDim.x, ++it) {
-        const int ps = (t >= p.tiles[0]) ? 1 : 0;
-        const long long tile = t - (ps ? p.tiles[0] : 0);
+        int ps;
+        const long long tile = chain_tile(p, t, ps);
         const int b = it & 1;
         // the dd tile: rows 0..63 and 64..127 of column block kb are two 8 KiB blocks of the tiled array
         mbar_wait(smem_u32(&sc->a0_empty[b]), ((it >> 1) & 1) ^ 1, 31);
@@ -571,8 +587,8 @@ __global__ void __launch_bounds__(kThreads, 1) chain_bwd_kernel(const ChainParam
     for (int i = 0; i < 8; ++i) { amx[0][i] = 0.f; amx[1][i] = 0.f; }
     int it = 0;
     for (long long t = blockIdx.x; t < total; t += gridDim.x, ++it) {
-      const int ps = (t >= p.tiles[0]) ? 1 : 0;
-      const long long tile = t - (ps ? p.tiles[0] : 0);
+      int ps;
+      const long long tile = chain_tile(p, t, ps);
       const int b = it & 1;
       const PassBufs& pb = p.pass[ps];
       const long long g[2] = {tile * 128 + c.row[0], tile * 128 + c.row[1]};
@@ -746,9 +762,15 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
     // row, the warp 4 rows (512 B, conflict-free).  8 rows are first summed in fp16 pairs (values are scaled
     // to <= 64, so <= 512; the rounding is far below what the sum over 1e5 samples averages out), then
     // converted and added in fp32 - a sixth of the instructions of a scalar fp32 loop.
+    // These warps read every element of every stored gradient level (dd and dpre_1..8 are the A operands of
+    // jobs with a bias), so they also check the levels' ranges: an element at the fp16 clamp (a tile whose
+    // gradients the probe's scale did not cover, saturated by the chain kernel) or a pre-sum that overflowed
+    // makes the weight gradients wrong; it is reported through the status word (code 102), not silently used.
     const int wr = warp - kWgReduceWarp0;
     const uint32_t rc = lane & 7, rph = lane >> 3;
     uint32_t stage = 0, phase = 0;
+    __half2 vmax = __float2half2_rn(0.f);      // largest |element| this lane has seen
+    bool overflow = false;
     for (int pi = p0; pi < p1; ++pi) {
       const WgradJob job = jobs[pi];
       const bool a_act = job.bias_out != nullptr && !(exp_flags & 2u);   // exp bit 1: no reductions
@@ -769,6 +791,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
                 const uint4 v = *reinterpret_cast<const uint4*>(blk + r * 128 + ((rc ^ (r & 7u)) << 4));
                 hacc[0] = bwd_add_x2(hacc[0], v.x); hacc[1] = bwd_add_x2(hacc[1], v.y);
                 hacc[2] = bwd_add_x2(hacc[2], v.z); hacc[3] = bwd_add_x2(hacc[3], v.w);
+                if (!kBwdBf16) {
+                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.x)));
+                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.y)));
+                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.z)));
+                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.w)));
+                }
               }
 #pragma unroll
               for (int qq = 0; qq < 4; ++qq) {
@@ -787,6 +815,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
           for (int i = 0; i < 8; ++i) {     // the four row phases hold partial sums of the same 8 columns
             sa[i] += __shfl_xor_sync(0xffffffffu, sa[i], 8);
             sa[i] += __shfl_xor_sync(0xffffffffu, sa[i], 16);
+            overflow |= !isfinite(sa[i]);
           }
           if (rph == 0) {
 #pragma unroll
@@ -795,6 +824,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
         }
       }
     }
+    const float2 vm = __half22float2(vmax);
+    overflow |= fmaxf(vm.x, vm.y) >= 65504.f;
+    if (__any_sync(0xffffffffu, overflow) && lane == 0) report_fault(status, 102);
   }
 }
 

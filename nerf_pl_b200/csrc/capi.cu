@@ -104,7 +104,8 @@ int device_info(DeviceInfo** out) {
 }
 
 // A kernel of an EARLIER call on this device reported a device-side fault (misaligned shared
-// memory, code 101) through the internal status word: surface it on this call and clear it.
+// memory, code 101; a training backward whose per-sample gradients overflowed fp16, code 102)
+// through the internal status word: surface it on this call and clear it.
 // (The word lives in mapped pinned host memory, so this is a plain host read, no synchronisation;
 // callers that want the fault of THIS call pass their own `status` word or call
 // nerfb200_check_status() after synchronising.)
@@ -113,7 +114,11 @@ int check_sticky_status(DeviceInfo* d) {
   const int st = *d->status_host;
   if (st == 0) return 0;
   *d->status_host = 0;
-  std::snprintf(g_err, sizeof(g_err), "an earlier nerf_pl_b200 kernel reported device status %d", st);
+  if (st == 102)
+    std::snprintf(g_err, sizeof(g_err), "an earlier training backward reported device status 102: a per-sample "
+                  "gradient exceeded the fp16 range of its layer's scale, its weight gradients are wrong");
+  else
+    std::snprintf(g_err, sizeof(g_err), "an earlier nerf_pl_b200 kernel reported device status %d", st);
   return NERFB200_EDEVICE;
 }
 
@@ -963,7 +968,12 @@ int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
     dir_grad_kernel<<<dim3(kDirSlices, L.n_pass), 128, 0, stream>>>(dp);
     g_launches++;
   }
-  // 3. dgrad chain (wgmma): a probe pass over one tile per SM picks the per-layer scales, then the real pass
+  // 3. dgrad chain (wgmma): a probe pass over one tile per SM picks the per-layer scales, then the real pass.
+  // The probe's tiles are spread evenly over each pass: gradients are not uniform over a batch (rays whose
+  // colour is already right carry almost none), and scales taken from the first tiles alone saturate the rest.
+  // Both launches visit the tiles of a pass in the order j -> j * stride mod span (stride coprime to span, about
+  // span / probe tiles), the real pass the probe's tiles first, so its first wave finds them in L2.  A tile the
+  // probe did not see can still exceed its level's range: the wgrad kernel reports that (status 102).
   {
     ChainParams cp;
     cp.n_pass = L.n_pass;
@@ -974,17 +984,32 @@ int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
     cp.lamax = L.lamax;
     cp.status = d->status;
     const long long t0 = L.pass[0].n_pad / 128, t1 = fine ? L.pass[1].n_pad / 128 : 0;
+    const long long half = (d->sm_count + 1) / 2;
+    const long long pt0 = kBwdBf16 ? 0 : (fine ? (t0 < half ? t0 : half) : (t0 < d->sm_count ? t0 : d->sm_count));
+    const long long pt1 = kBwdBf16 ? 0 : (fine ? (t1 < half ? t1 : half) : 0);
+    const long long span[2] = {t0, t1}, pt[2] = {pt0, pt1};
+    auto gcd = [](long long x, long long y) {
+      while (y != 0) { const long long r = x % y; x = y; y = r; }
+      return x;
+    };
+    for (int ps = 0; ps < 2; ++ps) {
+      long long s = (pt[ps] > 0 && span[ps] > pt[ps]) ? span[ps] / pt[ps] : 1;
+      while (span[ps] > 1 && gcd(s, span[ps]) != 1) ++s;
+      cp.span[ps] = span[ps] > 0 ? span[ps] : 1;
+      cp.stride[ps] = s;
+    }
     if (!kBwdBf16) {
-      const long long half = (d->sm_count + 1) / 2;
-      cp.tiles[0] = fine ? (t0 < half ? t0 : half) : (t0 < d->sm_count ? t0 : d->sm_count);
-      cp.tiles[1] = fine ? (t1 < half ? t1 : half) : 0;
-      const int pc = static_cast<int>(cp.tiles[0] + cp.tiles[1]);
+      cp.tiles[0] = cp.head[0] = pt0;
+      cp.tiles[1] = cp.head[1] = pt1;
+      const int pc = static_cast<int>(pt0 + pt1);
       chain_bwd_kernel<true><<<pc, kThreads, kChSmemTotal, stream>>>(cp);
       g_launches++;
       sp.phase = 1;
       bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
       g_launches++;
     }
+    cp.head[0] = pt0;
+    cp.head[1] = pt1;
     cp.tiles[0] = t0;
     cp.tiles[1] = t1;
     const long long total = t0 + t1;

@@ -1,10 +1,12 @@
-"""Stage-by-stage check of the training step against the numpy oracle (run on an H100):
-forward tape in the workspace (sigma, rgb, activations, sign bits, encoded input), compositing
-backward, rgb head (dd), dgrad chain (dpre_l), final gradients.  Localises a wrong kernel in one call.
+"""Stage-by-stage check of the training step (run on an H100): the forward tape in the workspace (activations,
+sign bits, direction layer, heads), the compositing backward, dd, every step of the dgrad chain and the chain as a
+whole in float64 on the device's own masks ("same masks"), and the 48 final gradients against float64 contractions
+of the device's own operands.  Every comparison takes the device's stored inputs of that stage, so a wrong kernel
+stands out in one call.  The reader and the references are tests/train_tape.py, shared with
+tests/test_gpu_train_stages.py.
 
     python tools/bwd_debug.py [n_rays]
 """
-import ctypes
 import os
 import sys
 
@@ -14,71 +16,9 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import nerf_pl_b200 as nb  # noqa: E402
 from nerf_pl_b200 import _lib  # noqa: E402
-from nerf_pl_b200.training import TrainWorkspace  # noqa: E402
 from oracle import nerf_oracle as orc  # noqa: E402
 from oracle import nerf_oracle_grad as og  # noqa: E402
-
-
-def layout(n, Sc, K):
-    """Mirror of csrc/capi.cu make_train_layout (per-pass buffers only)."""
-    off = 0
-    passes = []
-
-    def take(b):
-        nonlocal off
-        o = off
-        off += (b + 1023) // 1024 * 1024
-        return o
-    for ps in range(2 if K > 0 else 1):
-        S = Sc + K if ps else Sc
-        nn = n * S
-        npad = (nn + 127) // 128 * 128
-        d = dict(S=S, n=nn, n_pad=npad)
-        d["enc"] = take(npad * 128); d["act"] = take(npad * 512 * 8); d["mask"] = take(npad * 32 * 8)
-        d["d"] = take(npad * 256); d["sigma"] = take(npad * 4); d["rgb"] = take(npad * 12); d["z"] = take(nn * 4)
-        d["dsigma"] = take(npad * 4); d["dprergb"] = take(npad * 12); d["dd"] = take(npad * 256)
-        d["dpre"] = take(npad * 512 * 8)
-        passes.append(d)
-    return passes
-
-
-def untile(buf, n_pad, C, dtype=np.float16):
-    """tiled (n_pad, C) 16-bit array (csrc/layout.h) -> row-major numpy."""
-    nfb = C // 64
-    a = np.frombuffer(buf, dtype=np.uint8).reshape(n_pad // 64, nfb, 64, 8, 16)      # chunk, fb, row, phys chunk16, bytes
-    out = np.empty((n_pad // 64, 64, nfb, 8, 16), np.uint8)
-    for rr in range(64):
-        for j in range(8):
-            out[:, rr, :, j, :] = a[:, :, rr, j ^ (rr & 7), :]
-    return out.reshape(n_pad, C * 2).view(dtype).reshape(n_pad, C)
-
-
-def decode_masks(m, n_pad):
-    """[n_pad][4 parts] uint2 -> (n_pad, 256) bool 'negative' flags in column order."""
-    m = m.reshape(n_pad, 4, 2)
-    neg = np.zeros((n_pad, 256), bool)
-    for part in range(4):
-        for kb in range(4):
-            for i in range(8):
-                bit = 31 - (8 * kb + i)
-                n0 = kb * 64 + part * 16
-                neg[:, n0 + 2 * i] = (m[:, part, 0] >> bit) & 1
-                neg[:, n0 + 2 * i + 1] = (m[:, part, 1] >> bit) & 1
-    return neg
-
-
-def stat(name, got, ref, scale=1.0):
-    got = np.asarray(got, np.float64)
-    ref = np.asarray(ref, np.float64)
-    if scale is None:       # per-layer power-of-two scale chosen on the device: recover it from the data
-        big = np.abs(ref) > 0.1 * np.abs(ref).max()
-        scale = 2.0 ** np.round(np.log2(np.median(np.abs(got[big]) / np.abs(ref[big]))))
-        name = f"{name} (scale 2^{int(np.log2(scale))})"
-    got = got / scale
-    err = np.abs(got - ref)
-    den = np.linalg.norm(ref) + 1e-30
-    print(f"{name:28s} rel_l2 {np.linalg.norm(got - ref) / den:.3e}  max_abs {err.max():.3e}  ref_absmax {np.abs(ref).max():.3e}"
-          f"  finite {bool(np.isfinite(got).all())}")
+from tests import train_tape as tt  # noqa: E402
 
 
 def main():
@@ -99,91 +39,44 @@ def main():
     out = nb.render_rays_loss(models, emb, torch.from_numpy(rays).to(dev), torch.from_numpy(target).to(dev), 64, False,
                               1.0, 0.0, 64, 32768, True, randoms=rnd)
     torch.cuda.synchronize()
-    print("forward ok, loss", float(out["loss"]), "psnr", float(out["psnr"]))
-    ws_obj = [w for w in TrainWorkspace._pool[(0, n, 64, 64)] if w.busy][0]
+    print("forward ok, loss", float(out["loss"].detach()), "psnr", float(out["psnr"]))
+    ws_obj = out["rgb_coarse"].grad_fn.keep[-1]
     out["loss"].backward()
     torch.cuda.synchronize()
     print("backward ok; status", _lib.load().nerfb200_check_status())
-    raw = ws_obj.buf.cpu().numpy().tobytes()
-    L = layout(n, 64, 64)
-
-    # ---- oracle
+    raw = ws_obj.buf.cpu().numpy()
     loss, res, ref_grads = og.render_rays_loss_grad(ws, rays, target, 64, False, 1.0, 0.0, 64, True, randoms)
     print("oracle loss", loss)
-    o, d = rays[:, :3], rays[:, 3:6]
-    dir_emb = orc.embed(d, 4)
-    zs = [orc.coarse_depths(rays, 64, False, 1.0, randoms["perturb_rand"]), res["z_vals_fine"]]
-    for ps, (tag, w) in enumerate(zip(("coarse", "fine"), ws)):
-        P = L[ps]
-        S, nn, npad = P["S"], P["n"], P["n_pad"]
-        z = zs[ps]
-        zz = np.frombuffer(raw, np.float32, nn, P["z"]).reshape(n, S)
-        stat(f"[{tag}] z", zz, z)
-        xyz = (o[:, None, :] + d[:, None, :] * zz[:, :, None]).astype(np.float32).reshape(-1, 3)
-        x = np.concatenate([orc.embed(xyz, 10), np.repeat(dir_emb, S, axis=0)], -1)
-        tape = og.nerf_forward_tape(w, x)
-        stat(f"[{tag}] sigma", np.frombuffer(raw, np.float32, nn, P["sigma"]), tape["sigma"])
-        stat(f"[{tag}] rgb", np.frombuffer(raw, np.float32, nn * 3, P["rgb"]).reshape(nn, 3), tape["rgb"])
-        enc = untile(raw[P["enc"]:P["enc"] + npad * 128], npad, 64)[:nn]
-        stat(f"[{tag}] enc", enc[:, :63], tape["enc"])
-        for l in range(8):
-            a = untile(raw[P["act"] + l * npad * 512:P["act"] + (l + 1) * npad * 512], npad, 256)[:nn]
-            stat(f"[{tag}] h{l + 1}", a, tape[f"h{l + 1}"])
-        masks = np.frombuffer(raw, np.uint32, npad * 8 * 8, P["mask"]).reshape(8, npad, 8)
-        for l in (0, 7):
-            neg = decode_masks(masks[l], npad)[:nn]
-            agree = (neg == (tape[f"h{l + 1}"] <= 0)).mean()
-            print(f"[{tag}] mask{l + 1} agreement with (h <= 0): {agree:.5f}")
-        dd_row = untile(raw[P["d"]:P["d"] + npad * 256], npad, 128)[:nn]
-        stat(f"[{tag}] d", dd_row, tape["d"])
-        # compositing backward on the oracle's tape
-        diff = (res[f"rgb_{tag}"] - target).astype(np.float64)
-        g_rgb = (2.0 * diff / diff.size).astype(np.float32)
-        dsig, drgbs = og.volume_render_backward(tape["sigma"].reshape(n, S), tape["rgb"].reshape(n, S, 3), zz, d, None, 0.0,
-                                                True, g_rgb)
-        stat(f"[{tag}] dsigma", np.frombuffer(raw, np.float32, nn, P["dsigma"]), dsig.reshape(-1))
-        dpre_rgb = (drgbs.reshape(-1, 3) * tape["rgb"] * (1 - tape["rgb"])).astype(np.float32)
-        got_dp = np.frombuffer(raw, np.float32, nn * 3, P["dprergb"]).reshape(nn, 3)
-        stat(f"[{tag}] dprergb", got_dp, dpre_rgb)
-        amax = max(np.abs(np.frombuffer(raw, np.float32, nn, P["dsigma"])).max(), np.abs(got_dp).max())
-        print(f"[{tag}] amax of this pass {amax:.4e}")
-    # the scale is global over both passes
-    amax_all = 0.0
-    for P in L:
-        amax_all = max(amax_all, np.abs(np.frombuffer(raw, np.float32, P["n"], P["dsigma"])).max(),
-                       np.abs(np.frombuffer(raw, np.float32, P["n"] * 3, P["dprergb"])).max())
-    for ps, (tag, w) in enumerate(zip(("coarse", "fine"), ws)):
-        P = L[ps]
-        S, nn, npad = P["S"], P["n"], P["n_pad"]
-        zz = np.frombuffer(raw, np.float32, nn, P["z"]).reshape(n, S)
-        xyz = (o[:, None, :] + d[:, None, :] * zz[:, :, None]).astype(np.float32).reshape(-1, 3)
-        x = np.concatenate([orc.embed(xyz, 10), np.repeat(dir_emb, S, axis=0)], -1)
-        tape = og.nerf_forward_tape(w, x)
-        dsig = np.frombuffer(raw, np.float32, nn, P["dsigma"]).astype(np.float64)
-        dpre_rgb = np.frombuffer(raw, np.float32, nn * 3, P["dprergb"]).reshape(nn, 3).astype(np.float64)
-        dd = (dpre_rgb @ w["rgb.0.weight"]) * (tape["d"] > 0)
-        got = untile(raw[P["dd"]:P["dd"] + npad * 256], npad, 128)[:nn]
-        stat(f"[{tag}] dd", got, dd, None)
-        Wp = w["dir_encoding.0.weight"][:, :256].astype(np.float64) @ w["xyz_encoding_final.weight"].astype(np.float64)
-        dh = dd @ Wp + dsig[:, None] * w["sigma.weight"].astype(np.float64)
-        dh_m = dh.copy()          # second chain: float64 arithmetic on the DEVICE's ReLU masks (isolates mask flips)
-        masks = np.frombuffer(raw, np.uint32, npad * 8 * 8, P["mask"]).reshape(8, npad, 8)
-        for l in range(7, -1, -1):
-            dp = dh * (tape[f"h{l + 1}"] > 0)
-            dp_m = dh_m * (~decode_masks(masks[l], npad)[:nn])
-            got = untile(raw[P["dpre"] + l * npad * 512:P["dpre"] + (l + 1) * npad * 512], npad, 256)[:nn]
-            stat(f"[{tag}] dpre{l + 1}", got, dp, None)
-            stat(f"[{tag}] dpre{l + 1} same masks", got, dp_m, None)
-            if l > 0:
-                W = w[f"xyz_encoding_{l + 1}.0.weight"].astype(np.float64)
-                dh = dp @ (W[:, 63:] if l == 4 else W)
-                dh_m = dp_m @ (W[:, 63:] if l == 4 else W)
-    grads = {f"{tag}.{k}": p.grad.detach().cpu().numpy() for tag, m in zip(("coarse", "fine"), models)
-             for k, p in m.named_parameters()}
+    dir_emb = orc.embed(rays[:, 3:6], 4)
+    grads = {}
+    for ps, (tag, P) in enumerate(zip(("coarse", "fine"), tt.layout(n, 64, 64))):
+        net = tt.Net(ws[ps])
+        tape = tt.WorkspaceTape(raw, P)
+        fwd = tt.check_forward(tape, net, dir_emb)
+        print(f"[{tag}] forward on the device's inputs:", " ".join(f"{k} {v:.3g}" for k, v in fwd.items()))
+        masks = tt.check_masks(tape)
+        print(f"[{tag}] sign bits vs h == 0: contradictions {masks['illegal']}, "
+              f"agreement {1 - masks['legal_frac']:.6f} (the rest: positive pre-activations that round to 0)")
+        g_rgb = (2.0 * (out[f"rgb_{tag}"].detach().cpu().numpy().astype(np.float64) - target) / (3 * n)).astype(np.float32)
+        comp = tt.check_composite(tape, rays, g_rgb, None, None, None, 0.0, True)
+        print(f"[{tag}] compositing backward:", " ".join(f"{k} {v:.3g}" for k, v in comp.items()))
+        chain = tt.check_chain(tape, net)
+        print(f"[{tag}] scales log2 {[int(np.log2(s)) for s in chain['scales']]}, saturated {chain['saturated']}")
+        for v in range(9):
+            name = "dd" if v == 0 else f"dpre{9 - v}"
+            line = f"[{tag}] {name:6s} one step {chain[f'step{v}']:.3g} ulp"
+            if v:
+                line += f"  same masks rel_l2 {chain[f'acc{v}']:.3e} max {chain[f'accmax{v}']:.3e}"
+            print(line)
+        gref = tt.reference_grads(tape, net, chain["scales"], dir_emb)
+        dev_g = {k: p.grad.detach().cpu().numpy() for k, p in models[ps].named_parameters()}
+        for k, (r, mx) in tt.check_grads(dev_g, gref).items():
+            print(f"[{tag}] grad {k:32s} vs own operands rel {r:.3e} max {mx:.3e}")
+        grads.update({f"{tag}.{k}": v for k, v in dev_g.items()})
     rows, (rel, cos) = og.grad_compare(grads, ref_grads)
     for k, (r, c) in rows.items():
-        print(f"grad {k:36s} rel {r:.3e} cos {c:.6f}")
-    print(f"GLOBAL rel {rel:.3e} cos {cos:.6f}")
+        print(f"grad {k:36s} vs oracle rel {r:.3e} cos {c:.6f}")
+    print(f"GLOBAL vs oracle rel {rel:.3e} cos {cos:.6f}")
 
 
 if __name__ == "__main__":
