@@ -186,6 +186,32 @@ int nerfb200_render_rays_host(const nerfb200_render_args* host_args, void* strea
 int nerfb200_nerf_forward(const float* x, int64_t n, int64_t x_stride, const void* packed,
                           int32_t sigma_only, float* out, void* stream);
 
+/* ---- training a direct NeRF.forward call -------------------------------------------------
+ * Replaces: loss.backward() through models/nerf.py:83-124 NeRF.forward(x) (sigma_only = False, the
+ * default architecture) when the caller renders with its own code.  No gradient with respect to x.
+ * Workspace: nerfb200_nerf_train_workspace_bytes(n) bytes (0 for n <= 0), 1024-byte aligned,
+ * initialised once per n with nerfb200_nerf_train_workspace_init (zeroes it and uploads the wgrad job
+ * table; synchronous with respect to `stream`; a workspace smaller than the bytes for n is
+ * NERFB200_EINVAL).  The forward and the backward of a call use a workspace initialised for the same
+ * n; one workspace holds one call between its forward and its backward. */
+size_t nerfb200_nerf_train_workspace_bytes(int64_t n);
+int nerfb200_nerf_train_workspace_init(void* ws, size_t bytes, int64_t n, void* stream);
+/* Replaces: models/nerf.py:83-124 NeRF.forward(x) in training.  x as for nerfb200_nerf_forward
+ * (x_stride >= 90); out (n,4) [r,g,b,sigma] equals nerfb200_nerf_forward's bit for bit.  Also stores in
+ * `ws`, per sample, what the backward reads: the fp16 encoded-input and direction rows the tensor core
+ * consumed, the 8 hidden activations and their ReLU sign bits, the direction-layer output, sigma, rgb. */
+int nerfb200_nerf_forward_train(const float* x, int64_t n, int64_t x_stride, const void* packed, void* ws, float* out,
+                                void* stream);
+/* Replaces: the backward of models/nerf.py:83-124 for one nerfb200_nerf_forward_train call.
+ * g_out: (n,4) upstream gradient [rgb, sigma], 16-byte aligned; packed / ws: those of the forward;
+ * params: the live 24 fp32 parameters (state_dict order); writes the 24 gradient tensors `grads`
+ * (overwritten, not accumulated).  All kernels are sm_90a code on `stream`: gradient seed, rgb head,
+ * wgmma dgrad chain, wgmma split-K wgrad (with the direction slice of dir_encoding), reduction,
+ * unfolding.  A per-sample gradient outside its layer's fp16 range is reported like the render
+ * backward's (status 102: nerfb200_check_status / the next call). */
+int nerfb200_nerf_backward(const float* g_out, int64_t n, const void* packed, const float* const params[24], void* ws,
+                           float* const grads[24], void* stream);
+
 /* ---- dense sigma query ("next" row: mesh extraction) -------------------------------------
  * Replaces: extract_color_mesh.py:127-140 (embedding_xyz + embedding_dir + cat + nerf(...)[:, -1]
  * per chunk): raw positions xyz (n, xyz_stride >= 3) -> raw sigma (n); the positional encoding is

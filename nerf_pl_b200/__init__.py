@@ -7,10 +7,11 @@ from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
 from .optim import FusedAdam
 from .rendering import render_rays, render_rays_host, render_rays_loss, sample_pdf, searchsorted, volume_render
+from .training import nerf_forward_train
 
 __all__ = [
     "Embedding", "NeRF", "render_rays", "render_rays_loss", "render_rays_host", "FusedAdam", "invalidate_packed", "sample_pdf", "searchsorted", "volume_render",
-    "nerf_forward_fused", "nerf_forward_torch", "nerf_parameters", "packed_weights",
+    "nerf_forward_fused", "nerf_forward_torch", "nerf_forward_train", "nerf_parameters", "packed_weights",
     "batched_inference", "generate_rays", "render_image", "to_uint8", "query_sigma", "mse_psnr",
 ]
 __version__ = "0.1.0"

@@ -37,6 +37,10 @@ EXPORTS = [
     "nerfb200_render_rays",
     "nerfb200_render_rays_host",
     "nerfb200_nerf_forward",
+    "nerfb200_nerf_train_workspace_bytes",
+    "nerfb200_nerf_train_workspace_init",
+    "nerfb200_nerf_forward_train",
+    "nerfb200_nerf_backward",
     "nerfb200_embed",
     "nerfb200_searchsorted",
     "nerfb200_sample_pdf",
@@ -169,6 +173,15 @@ def _declare(lib: ctypes.CDLL) -> None:
                                        c_void_p, c_void_p]
     lib.nerfb200_query_sigma.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]
     lib.nerfb200_query_sigma.restype = c_int32
+    lib.nerfb200_nerf_train_workspace_bytes.argtypes = [c_int64]
+    lib.nerfb200_nerf_train_workspace_bytes.restype = c_size_t
+    lib.nerfb200_nerf_train_workspace_init.argtypes = [c_void_p, c_size_t, c_int64, c_void_p]
+    lib.nerfb200_nerf_train_workspace_init.restype = c_int32
+    lib.nerfb200_nerf_forward_train.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.nerfb200_nerf_forward_train.restype = c_int32
+    lib.nerfb200_nerf_backward.argtypes = [c_void_p, c_int64, c_void_p, POINTER(c_void_p), c_void_p, POINTER(c_void_p),
+                                           c_void_p]
+    lib.nerfb200_nerf_backward.restype = c_int32
     lib.nerfb200_train_workspace_bytes.argtypes = [c_int64, c_int32, c_int32]
     lib.nerfb200_train_workspace_bytes.restype = c_size_t
     lib.nerfb200_train_workspace_init.argtypes = [c_void_p, c_size_t, c_int64, c_int32, c_int32, c_void_p]

@@ -129,8 +129,16 @@ struct MlpParams {
   int sigma_only;
   float* out;              // (n, 4) rgb,sigma  or (n, 1) sigma
   int* status;
+  // training save mode (kSave; x embedded, not sigma_only): what nerfb200_nerf_backward reads, in the formats of
+  // the render path's training workspace (PassBufs: enc, act, mask, d, sigma, rgb; one pass, one sample per row)
+  PassBufs tr;
+  uint8_t* xdir;           // tiled (n_pad, 64) fp16: the direction rows of the direction layer's extra K slice
 };
 
+// kSave: also stores per sample the encoded input rows, the 8 activations and their ReLU sign bits, the direction-layer
+// output, the direction rows and raw sigma / rgb.  The returned values are those of the plain instantiation, bit for bit
+// (the save mode only adds stores).
+template <bool kSave>
 __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   Scratch* sc = reinterpret_cast<Scratch*>(smem + kSmemScratch);
@@ -160,6 +168,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
     const float* const dbias[2] = {b_dir, b_dir};
     uint8_t* enc = smem + kSmemEnc;
     const int t = c.wi * 32 + c.lane;
+    if (kSave) {
+      c.save_act = p.tr.act;
+      c.save_mask = p.tr.mask;
+      c.save_d = p.tr.d;
+      c.save_n = p.tr.n_pad;
+    }
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       // this warpgroup's 64 rows of the ENC tile: two threads per row (the previous tile's MMAs that read
       // them have completed: every layer ends with wgmma.wait_group 0)
@@ -177,21 +191,38 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
             const float v = (k < kEncXyz) ? __ldg(xr + k) : 0.f;
             *reinterpret_cast<__half*>(enc + sw128_off(row, k)) = __float2half_rn(v);
           }
+          if (kSave) {
+            // the same copy-in-place of this thread's four 16-byte chunks as write_dir_rows (mlp_engine.cuh),
+            // padding rows included
+            uint8_t* dst = p.tr.enc + tile * 16384;
+#pragma unroll
+            for (int cc = 0; cc < 4; ++cc) {
+              const uint32_t off = sw128_off(row, ((t & 1) * 4 + cc) * 8);
+              *reinterpret_cast<uint4*>(dst + off) = *reinterpret_cast<const uint4*>(enc + off);
+            }
+          }
         }
         fence_proxy_async();
         wg_bar(c);
       }
-      const DirSrc ds{p.x, p.x_stride, tile * 128, p.n};
+      const DirSrc ds{p.x, p.x_stride, tile * 128, p.n, kSave ? p.xdir : nullptr};
       float sig[2], rgb[2][3];
-      if (so) wg_tile<true, false, false>(c, kSmemEnc, dbias, nullptr, sig, rgb);
-      else wg_tile<false, true, false>(c, kSmemEnc, dbias, &ds, sig, rgb);
+      if (kSave) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) c.grow[s] = (tile * 128 + c.row[s] < p.n) ? tile * 128 + c.row[s] : -1;
+        wg_tile<false, true, true>(c, kSmemEnc, dbias, &ds, sig, rgb);
+      } else if (so) {
+        wg_tile<true, false, false>(c, kSmemEnc, dbias, nullptr, sig, rgb);
+      } else {
+        wg_tile<false, true, false>(c, kSmemEnc, dbias, &ds, sig, rgb);
+      }
       if (c.q == 0) {
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           const long long gi = tile * 128 + c.row[s];
           if (gi >= p.n) continue;
           const float sg = c.cst[kF32BSigma] + sig[s];
-          if (so) {
+          if (so && !kSave) {
             p.out[gi] = sg;
           } else {
             float4 o;
@@ -200,6 +231,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
             o.z = sigmoid_ref(c.cst[kF32BRgb + 2] + rgb[s][2]);
             o.w = sg;
             *reinterpret_cast<float4*>(p.out + gi * 4) = o;
+            if (kSave) {
+              p.tr.sigma[gi] = sg;
+              p.tr.rgb[gi * 3 + 0] = o.x;
+              p.tr.rgb[gi * 3 + 1] = o.y;
+              p.tr.rgb[gi * 3 + 2] = o.z;
+            }
           }
         }
       }

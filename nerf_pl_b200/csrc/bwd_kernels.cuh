@@ -199,6 +199,48 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompBwdParams 
   }
 }
 
+// ------------------------------------------------------------------------ NeRF.forward seed
+// The backward of a direct NeRF.forward call (models/nerf.py:83-124, output [rgb, sigma]) starts from the
+// upstream gradient g (n, 4) instead of from compositing:  d rgb_pre = g_rgb rgb (1 - rgb) through the sigmoid
+// (models/nerf.py:120), d sigma = g_sigma.  Rows n .. n_pad - 1 (padding of the last tile) are written as zero.
+// Also the amax words bwd_scale_kernel's phase 0 reads.  One thread per row.
+struct MlpSeedParams {
+  long long n, n_pad;
+  const float* g;           // (n, 4) upstream gradient [rgb, sigma]
+  const float* rgb;         // (n_pad, 3) stored sigmoid(rgb)
+  float* dsigma;            // (n_pad)
+  float* dprergb;           // (n_pad, 3)
+  unsigned* amax_bits;      // [2]: max |d sigma|, max |d rgb_pre| as float bits
+};
+__global__ void __launch_bounds__(256) mlp_seed_kernel(const MlpSeedParams p) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  float amax = 0.f, amax_rgb = 0.f;
+  if (i < p.n) {
+    const float4 g = __ldg(reinterpret_cast<const float4*>(p.g) + i);
+    const float gc[3] = {g.x, g.y, g.z};
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      const float c = p.rgb[i * 3 + ch];
+      const float dp = gc[ch] * c * (1.f - c);
+      p.dprergb[i * 3 + ch] = dp;
+      amax_rgb = fmaxf(amax_rgb, fabsf(dp));
+    }
+    p.dsigma[i] = g.w;
+    amax = fabsf(g.w);
+  } else if (i < p.n_pad) {
+    p.dsigma[i] = 0.f;
+    p.dprergb[3 * i] = 0.f; p.dprergb[3 * i + 1] = 0.f; p.dprergb[3 * i + 2] = 0.f;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    amax_rgb = fmaxf(amax_rgb, __shfl_xor_sync(0xffffffffu, amax_rgb, o));
+  }
+  const int lane = threadIdx.x & 31;
+  if (lane == 0 && amax > 0.f && amax < 3e38f) atomicMax(p.amax_bits, __float_as_uint(amax));
+  if (lane == 0 && amax_rgb > 0.f && amax_rgb < 3e38f) atomicMax(p.amax_bits + 1, __float_as_uint(amax_rgb));
+}
+
 // Per-pass, per-level scales (see the header comment).  Level v: 0 = dd, v = 1..8 = dpre_{9-v}.
 //   phase 0 (before head_bwd / the probe): every level gets the level-0 scale
 //            2^floor(log2(64 / max(|d rgb_pre|_max wmax_rgb, |d sigma|_max wmax_sigma)))
@@ -282,8 +324,8 @@ struct HeadBwdParams {
   const float* lscale;      // [2][kLevels]: level 0 of each pass scales dd
   const float* rays;
   long long ray_stride;
-  float* raysum[2];         // (n_rays, 128)
-  float* direnc;            // (n_rays, 28): Embedding(3,4)(rays_d), as the forward computes it
+  float* raysum[2];         // (n_rays, 128), or null (NeRF.forward backward: no per-ray direction)
+  float* direnc;            // (n_rays, 28): Embedding(3,4)(rays_d), as the forward computes it, or null (same)
   float* part[2];           // [gridDim.x][kHeadPartFloats] per pass (blocks of the other pass write zeros)
 };
 
@@ -313,7 +355,7 @@ __global__ void __launch_bounds__(kHeadWarps * 32) head_bwd_kernel(const HeadBwd
     for (int c = 0; c < 3; ++c)
 #pragma unroll
       for (int i = 0; i < 4; ++i) w[c][i] = p.w_rgb[ps][c * 128 + 4 * lane + i];
-    if (ps == 0 && lane < 15) {     // Embedding(3,4)(rays_d) exactly as render_kernel.cuh setup_group
+    if (ps == 0 && lane < 15 && p.direnc != nullptr) {     // Embedding(3,4)(rays_d) exactly as render_kernel.cuh setup_group
       const int cc = lane / 5, kk = lane % 5;
       const float dv = p.rays[ray * p.ray_stride + 3 + cc];
       float* de = p.direnc + ray * 28;
@@ -367,7 +409,8 @@ __global__ void __launch_bounds__(kHeadWarps * 32) head_bwd_kernel(const HeadBwd
       *reinterpret_cast<uint2*>(pb.dd + off) = make_uint2(cvt_bwd_x2(val[0] * scale, val[1] * scale),
                                                           cvt_bwd_x2(val[2] * scale, val[3] * scale));
     }
-    *reinterpret_cast<float4*>(p.raysum[ps] + ray * 128 + 4 * lane) = make_float4(rs[0], rs[1], rs[2], rs[3]);
+    if (p.raysum[ps] != nullptr)
+      *reinterpret_cast<float4*>(p.raysum[ps] + ray * 128 + 4 * lane) = make_float4(rs[0], rs[1], rs[2], rs[3]);
   }
   // per-block partial of gW_rgb / gb_rgb: warps in fixed order
 #pragma unroll

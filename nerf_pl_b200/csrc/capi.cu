@@ -84,8 +84,10 @@ int device_info(DeviceInfo** out) {
                                   static_cast<int>(kSmemTotal)), "smem attr render");
     CUDA_TRY(cudaFuncSetAttribute(render_rays_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kSmemTotal)), "smem attr render(save)");
-    CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kSmemTotal)), "smem attr mlp");
+    CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kSmemTotal)), "smem attr mlp(save)");
     CUDA_TRY(cudaFuncSetAttribute(chain_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kChSmemTotal)), "smem attr chain");
     CUDA_TRY(cudaFuncSetAttribute(chain_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -161,18 +163,22 @@ int check_render_shapes(const nerfb200_render_args* a) {
 // One device buffer per (n_rays, N_samples, N_importance); the layout is a pure function of those
 // numbers and the SM count, recomputed on every call (no state kept in the library).
 struct WgJobPlan { int ps, kind, split, n_split; };
-enum { kJ1 = 0, kJ2, kJ3, kJ4, kJ5a, kJ5b, kJ6, kJ7, kJ8, kJ9, kNumJobKinds };
+// kJDir (NeRF.forward backward only): the direction slice gW_dir[:, 256:283] = dd^T xdir over the direction rows
+// the forward fed the tensor core (the render path sums dd per ray instead: dir_grad_kernel)
+enum { kJ1 = 0, kJ2, kJ3, kJ4, kJ5a, kJ5b, kJ6, kJ7, kJ8, kJ9, kNumJobKinds, kJDir = kNumJobKinds, kNumJobKindsMlp };
 constexpr int kWgSlotFloats = 256 * 256 + 256;           // partial of one piece: out (transposed), bias
 constexpr int kMaxWgJobs = 1024;
 constexpr int kMaxWgCtas = 512;
 struct TrainLayout {
   PassBufs pass[2];
   int n_pass, n_rays;
+  int n_kinds;                    // wgrad GEMMs per pass: kNumJobKinds (render path) or kNumJobKindsMlp
+  uint8_t* xdir;                  // NeRF.forward path: tiled (n_pad, 64) fp16 direction rows (else null)
   WgradJob* jobs_dev;             // pieces, in (pass, layer, chunk) order
   int* cta_first_dev;             // [n_cta + 1]: CTA b works on pieces [cta_first[b], cta_first[b + 1])
   int n_jobs, n_cta;
-  int n_split[2][kNumJobKinds];   // pieces of each (pass, layer)
-  int first_job[2][kNumJobKinds];
+  int n_split[2][kNumJobKindsMlp];   // pieces of each (pass, layer)
+  int first_job[2][kNumJobKindsMlp];
   float* wg_part;                 // [n_jobs][kWgSlotFloats]
   int head_grid;                  // blocks of head_bwd_kernel (both passes in one launch)
   float* head_part[2];            // [head_grid][kHeadPartFloats] per pass
@@ -194,8 +200,25 @@ struct TrainLayout;
 void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first);
 
 void job_shape(int kind, int* a_fb, int* b_fb) {
-  *a_fb = (kind == kJ9) ? 2 : 4;
-  *b_fb = (kind == kJ1 || kind == kJ5a) ? 1 : 4;
+  *a_fb = (kind == kJ9 || kind == kJDir) ? 2 : 4;
+  *b_fb = (kind == kJ1 || kind == kJ5a || kind == kJDir) ? 1 : 4;
+}
+
+// The per-pass buffers of a training workspace, in PassBufs order, each from one call of `take`.
+template <class Take>
+void take_pass_bufs(PassBufs& b, Take&& take) {
+  const size_t np = static_cast<size_t>(b.n_pad);
+  b.enc = take(np * 128);
+  b.act = take(np * 512 * 8);
+  b.mask = reinterpret_cast<uint2*>(take(np * 32 * 8));
+  b.d = take(np * 256);
+  b.sigma = reinterpret_cast<float*>(take(np * 4));
+  b.rgb = reinterpret_cast<float*>(take(np * 12));
+  b.z = reinterpret_cast<float*>(take(static_cast<size_t>(b.n) * 4));
+  b.dsigma = reinterpret_cast<float*>(take(np * 4));
+  b.dprergb = reinterpret_cast<float*>(take(np * 12));
+  b.dd = take(np * 256);
+  b.dpre = take(np * 512 * 8);
 }
 
 void make_train_layout(TrainLayout* L, uint8_t* base, int64_t n_rays, int n_samples, int n_importance, int sm_count) {
@@ -207,24 +230,15 @@ void make_train_layout(TrainLayout* L, uint8_t* base, int64_t n_rays, int n_samp
   };
   L->n_pass = n_importance > 0 ? 2 : 1;
   L->n_rays = static_cast<int>(n_rays);
+  L->n_kinds = kNumJobKinds;
+  L->xdir = nullptr;
   std::memset(L->pass, 0, sizeof(L->pass));
   for (int ps = 0; ps < L->n_pass; ++ps) {
     PassBufs& b = L->pass[ps];
     b.S = ps ? n_samples + n_importance : n_samples;
     b.n = n_rays * b.S;
     b.n_pad = (b.n + 127) / 128 * 128;
-    const size_t np = static_cast<size_t>(b.n_pad);
-    b.enc = take(np * 128);
-    b.act = take(np * 512 * 8);
-    b.mask = reinterpret_cast<uint2*>(take(np * 32 * 8));
-    b.d = take(np * 256);
-    b.sigma = reinterpret_cast<float*>(take(np * 4));
-    b.rgb = reinterpret_cast<float*>(take(np * 12));
-    b.z = reinterpret_cast<float*>(take(static_cast<size_t>(b.n) * 4));
-    b.dsigma = reinterpret_cast<float*>(take(np * 4));
-    b.dprergb = reinterpret_cast<float*>(take(np * 12));
-    b.dd = take(np * 256);
-    b.dpre = take(np * 512 * 8);
+    take_pass_bufs(b, take);
   }
   // wgrad plan: the concatenation of all (pass, layer) GEMMs, measured in 8 KiB blocks streamed, is cut
   // into one equal share per SM; a share boundary inside a GEMM splits it into two pieces
@@ -250,6 +264,44 @@ void make_train_layout(TrainLayout* L, uint8_t* base, int64_t n_rays, int n_samp
   L->bytes = off;
 }
 
+// The workspace of a direct NeRF.forward call over n samples (nerfb200_nerf_forward_train / nerfb200_nerf_backward):
+// one pass with one sample per row, the per-pass buffers of the render path in the same order (so one reader serves
+// both), then the direction rows the forward fed the tensor core, the wgrad plan (with the direction-slice GEMM
+// kJDir) and the head partials.  The head kernel views the batch as n_pad / 64 pseudo-rays of 64 samples; nothing
+// per ray (raysum, direnc, dir_part) exists here.
+constexpr int kMlpPseudoRay = 64;
+void make_mlp_train_layout(TrainLayout* L, uint8_t* base, int64_t n, int sm_count) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) -> uint8_t* {
+    uint8_t* ptr = base ? base + off : nullptr;
+    off += (bytes + 1023) & ~static_cast<size_t>(1023);
+    return ptr;
+  };
+  std::memset(L, 0, sizeof(*L));
+  L->n_pass = 1;
+  L->n_kinds = kNumJobKindsMlp;
+  PassBufs& b = L->pass[0];
+  b.S = 1;
+  b.n = n;
+  b.n_pad = (n + 127) / 128 * 128;
+  take_pass_bufs(b, take);
+  L->xdir = take(static_cast<size_t>(b.n_pad) * 128);
+  L->n_rays = static_cast<int>(b.n_pad / kMlpPseudoRay);
+  plan_wgrad(L, sm_count > 0 ? sm_count : 148, nullptr, nullptr);
+  L->jobs_dev = reinterpret_cast<WgradJob*>(take(sizeof(WgradJob) * kMaxWgJobs));
+  L->cta_first_dev = reinterpret_cast<int*>(take(sizeof(int) * (kMaxWgCtas + 1)));
+  L->wg_part = reinterpret_cast<float*>(take(static_cast<size_t>(L->n_jobs) * kWgSlotFloats * 4));
+  L->head_grid = (L->n_rays + kHeadWarps - 1) / kHeadWarps;
+  L->head_part[0] = reinterpret_cast<float*>(take(static_cast<size_t>(L->head_grid) * kHeadPartFloats * 4));
+  L->gWp[0] = reinterpret_cast<float*>(take(128 * 256 * 4));
+  L->gbp[0] = reinterpret_cast<float*>(take(128 * 4));
+  L->lscale = reinterpret_cast<float*>(take(2 * kLevels * 4));
+  L->linv = reinterpret_cast<float*>(take(2 * kLevels * 4));
+  L->lamax = reinterpret_cast<unsigned*>(take(2 * kLevels * 4));
+  L->amax = reinterpret_cast<unsigned*>(take(16));
+  L->bytes = off;
+}
+
 // The wgrad plan of a layout: piece counts per (pass, layer) (always), and when `jobs` / `cta_first` are
 // given the host image of the piece table and of the per-CTA piece ranges.
 void job_operands(const TrainLayout& L, int ps, int k, const uint8_t** A, const uint8_t** B) {
@@ -260,6 +312,7 @@ void job_operands(const TrainLayout& L, int ps, int k, const uint8_t** A, const 
     case kJ5a: *A = b.dpre + 4 * lay; *B = b.enc; break;
     case kJ5b: *A = b.dpre + 4 * lay; *B = b.act + 3 * lay; break;
     case kJ9: *A = b.dd; *B = b.act + 7 * lay; break;
+    case kJDir: *A = b.dd; *B = L.xdir; break;
     default: {
       const int l = (k <= kJ4) ? k + 1 : k;            // kJ2..kJ4 -> layers 2..4, kJ6..kJ8 -> layers 6..8
       *A = b.dpre + static_cast<size_t>(l - 1) * lay;
@@ -281,29 +334,30 @@ void fill_piece(TrainLayout* L, WgradJob* jobs, int piece, int ps, int k, long l
   j.chunk1 = static_cast<int>(c1);
   j.chunk_step = step;
   j.out = slot;
-  j.bias_out = (k == kJ5b) ? nullptr : slot + 256 * 256;
+  j.bias_out = (k == kJ5b || k == kJDir) ? nullptr : slot + 256 * 256;
 }
 
 void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
   if (n_cta > kMaxWgCtas) n_cta = kMaxWgCtas;
+  const int kinds = L->n_kinds;
   long long total = 0;
-  long long work[2][kNumJobKinds];
+  long long work[2][kNumJobKindsMlp];
   for (int ps = 0; ps < L->n_pass; ++ps)
-    for (int k = 0; k < kNumJobKinds; ++k) {
+    for (int k = 0; k < kinds; ++k) {
       int a_fb, b_fb;
       job_shape(k, &a_fb, &b_fb);
       work[ps][k] = (L->pass[ps].n_pad / 64) * (a_fb + b_fb);
       total += work[ps][k];
     }
-  const int n_kinds = L->n_pass * kNumJobKinds;
+  const int n_kinds = L->n_pass * kinds;
   if (env_switches().wg_plan == 1 && n_cta >= n_kinds) {
     // ---- plan 1: whole CTAs per GEMM (largest-remainder apportionment of the SMs by bytes streamed); the
     // CTAs of one GEMM take its chunks round-robin, so together they read ONE moving window of each operand
-    int n_of[2][kNumJobKinds];
-    double frac[2][kNumJobKinds];
+    int n_of[2][kNumJobKindsMlp];
+    double frac[2][kNumJobKindsMlp];
     int used = 0;
     for (int ps = 0; ps < L->n_pass; ++ps)
-      for (int k = 0; k < kNumJobKinds; ++k) {
+      for (int k = 0; k < kinds; ++k) {
         const double share = static_cast<double>(work[ps][k]) * n_cta / static_cast<double>(total);
         int n = static_cast<int>(share);
         if (n < 1) n = 1;
@@ -315,7 +369,7 @@ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
       int bp = 0, bk = 0;
       double best = -1;
       for (int ps = 0; ps < L->n_pass; ++ps)
-        for (int k = 0; k < kNumJobKinds; ++k) {
+        for (int k = 0; k < kinds; ++k) {
           const double load = static_cast<double>(work[ps][k]) / n_of[ps][k];
           if (load > best) { best = load; bp = ps; bk = k; }
         }
@@ -325,7 +379,7 @@ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
     (void)frac;
     int piece = 0;
     for (int ps = 0; ps < L->n_pass; ++ps)
-      for (int k = 0; k < kNumJobKinds; ++k) {
+      for (int k = 0; k < kinds; ++k) {
         const long long chunks = L->pass[ps].n_pad / 64;
         int g = n_of[ps][k];
         if (g > chunks) g = static_cast<int>(chunks);
@@ -347,7 +401,7 @@ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
   long long done = 0;                                  // units handed out so far
   if (cta_first) cta_first[0] = 0;
   for (int ps = 0; ps < L->n_pass; ++ps)
-    for (int k = 0; k < kNumJobKinds; ++k) {
+    for (int k = 0; k < kinds; ++k) {
       int a_fb, b_fb;
       job_shape(k, &a_fb, &b_fb);
       const long long unit = a_fb + b_fb, chunks = L->pass[ps].n_pad / 64;
@@ -399,6 +453,79 @@ struct Arena {
 Arena g_arena[64];
 std::mutex g_host_call_mu;
 std::mutex g_arena_mu;   // separate from g_mu: the host entry calls nerfb200_render_rays (device_info locks g_mu)
+
+// Step 3 of a training backward: the chain kernel's probe pass over pt0 + pt1 tiles spread evenly over each pass, the
+// phase-1 scales, then the real pass over all t0 + t1 tiles (the probe's first).  cp: everything but the visit order.
+void launch_chain(ChainParams& cp, long long t0, long long t1, long long pt0, long long pt1, ScaleParams& sp, int sm_count,
+                  cudaStream_t stream) {
+  const long long span[2] = {t0, t1}, pt[2] = {pt0, pt1};
+  auto gcd = [](long long x, long long y) {
+    while (y != 0) { const long long r = x % y; x = y; y = r; }
+    return x;
+  };
+  for (int ps = 0; ps < 2; ++ps) {
+    long long s = (pt[ps] > 0 && span[ps] > pt[ps]) ? span[ps] / pt[ps] : 1;
+    while (span[ps] > 1 && gcd(s, span[ps]) != 1) ++s;
+    cp.span[ps] = span[ps] > 0 ? span[ps] : 1;
+    cp.stride[ps] = s;
+  }
+  if (!kBwdBf16) {
+    cp.tiles[0] = cp.head[0] = pt0;
+    cp.tiles[1] = cp.head[1] = pt1;
+    const int pc = static_cast<int>(pt0 + pt1);
+    chain_bwd_kernel<true><<<pc, kThreads, kChSmemTotal, stream>>>(cp);
+    g_launches++;
+    sp.phase = 1;
+    bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
+    g_launches++;
+  }
+  cp.head[0] = pt0;
+  cp.head[1] = pt1;
+  cp.tiles[0] = t0;
+  cp.tiles[1] = t1;
+  const long long total = t0 + t1;
+  const int ctas = static_cast<int>(total < sm_count ? total : sm_count);
+  chain_bwd_kernel<false><<<ctas, kThreads, kChSmemTotal, stream>>>(cp);
+  g_launches++;
+}
+
+// Step 5: the reduction items of pass ps that both training backwards share (wgrad GEMMs of layers 1..8 and of the
+// folded W', the head partials), appended to `tab`.  g: the pass's 24 gradient tensors.
+void add_reduce_items(ReduceTable& tab, const TrainLayout& L, int ps, float* const* g) {
+  auto add = [&](const float* part, long long stride, int n_split, float* out, const float* mul, int rows, int cols,
+                 int part_ld, int out_ld, int out_col0, int transposed = 0) {
+    ReduceItem& it = tab.it[tab.n++];
+    it.part = part; it.split_stride = stride; it.n_split = n_split; it.out = out; it.mul = mul;
+    it.rows = rows; it.cols = cols; it.part_ld = part_ld; it.out_ld = out_ld; it.out_col0 = out_col0;
+    it.transposed = transposed;
+    it.by_warp = (n_split >= 128 && rows * cols <= 4096) ? 1 : 0;
+  };
+  const float* linv = L.linv + ps * kLevels;       // level v: 0 = dd, v = 1..8 = dpre_{9-v}
+  auto slot = [&](int kind) { return L.wg_part + static_cast<size_t>(L.first_job[ps][kind]) * kWgSlotFloats; };
+  auto ns = [&](int kind) { return L.n_split[ps][kind]; };
+  add(slot(kJ1), kWgSlotFloats, ns(kJ1), g[0], linv + 8, 256, 63, 256, 63, 0, 1);
+  add(slot(kJ1) + 65536, kWgSlotFloats, ns(kJ1), g[1], linv + 8, 1, 256, 256, 256, 0);
+  const int hidden[6] = {kJ2, kJ3, kJ4, kJ6, kJ7, kJ8};
+  const int layer[6] = {2, 3, 4, 6, 7, 8};
+  for (int i = 0; i < 6; ++i) {
+    const float* inv = linv + (9 - layer[i]);
+    add(slot(hidden[i]), kWgSlotFloats, ns(hidden[i]), g[2 * (layer[i] - 1)], inv, 256, 256, 256, 256, 0, 1);
+    add(slot(hidden[i]) + 65536, kWgSlotFloats, ns(hidden[i]), g[2 * (layer[i] - 1) + 1], inv, 1, 256, 256, 256, 0);
+  }
+  add(slot(kJ5a), kWgSlotFloats, ns(kJ5a), g[8], linv + 4, 256, 63, 256, 319, 0, 1);
+  add(slot(kJ5b), kWgSlotFloats, ns(kJ5b), g[8], linv + 4, 256, 256, 256, 319, 63, 1);
+  add(slot(kJ5a) + 65536, kWgSlotFloats, ns(kJ5a), g[9], linv + 4, 1, 256, 256, 256, 0);
+  add(slot(kJ9), kWgSlotFloats, ns(kJ9), L.gWp[ps], linv, 128, 256, 128, 256, 0, 1);
+  add(slot(kJ9) + 65536, kWgSlotFloats, ns(kJ9), L.gbp[ps], linv, 1, 128, 128, 128, 0);
+  add(L.head_part[ps] + kHeadPartSigW, kHeadPartFloats, L.head_grid, g[20], nullptr, 1, 256, 256, 256, 0);
+  add(L.head_part[ps] + kHeadPartSigB, kHeadPartFloats, L.head_grid, g[21], nullptr, 1, 1, 1, 1, 0);
+  add(L.head_part[ps] + kHeadPartRgbW, kHeadPartFloats, L.head_grid, g[22], nullptr, 1, 384, 384, 384, 0);
+  add(L.head_part[ps] + kHeadPartRgbB, kHeadPartFloats, L.head_grid, g[23], nullptr, 1, 3, 3, 3, 0);
+  if (L.n_kinds == kNumJobKindsMlp)      // direction slice: gW_dir[:, 256:283] = dd^T xdir / s_0 (columns 0..26 of 64)
+    add(slot(kJDir), kWgSlotFloats, ns(kJDir), g[18], linv, 128, 27, 128, 283, 256, 1);
+  else                                   // per-ray direction sums (dir_grad_kernel)
+    add(L.dir_part[ps], 128 * 27, kDirSlices, g[18], nullptr, 128, 27, 27, 283, 256);
+}
 
 }  // namespace
 
@@ -719,7 +846,7 @@ int nerfb200_nerf_forward(const float* x, int64_t n, int64_t x_stride, const voi
   p.status = d->status;
   const long long tiles = (n + 127) / 128;
   const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
-  mlp_forward_kernel<<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
+  mlp_forward_kernel<false><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
   g_launches++;
   CUDA_TRY(cudaGetLastError(), "nerf_forward launch");
   return 0;
@@ -744,9 +871,152 @@ int nerfb200_query_sigma(const float* xyz, int64_t n, int64_t xyz_stride, const 
   p.status = d->status;
   const long long tiles = (n + 127) / 128;
   const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
-  mlp_forward_kernel<<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
+  mlp_forward_kernel<false><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
   g_launches++;
   CUDA_TRY(cudaGetLastError(), "query_sigma launch");
+  return 0;
+}
+
+// ---- training a direct NeRF.forward call (models/nerf.py:83-124)
+size_t nerfb200_nerf_train_workspace_bytes(int64_t n) {
+  if (n <= 0 || n > 0x7fffffffLL) return 0;
+  TrainLayout L;
+  make_mlp_train_layout(&L, nullptr, n, nerfb200_sm_count());
+  return L.bytes;
+}
+
+int nerfb200_nerf_train_workspace_init(void* ws, size_t bytes, int64_t n, void* stream_v) {
+  if (n < 0 || n > 0x7fffffffLL) return fail(NERFB200_EINVAL, "nerf_train_workspace_init: n out of range%s");
+  if (n == 0) return 0;
+  if (!ws) return fail(NERFB200_EINVAL, "nerf_train_workspace_init: workspace is NULL%s");
+  if (reinterpret_cast<uintptr_t>(ws) & 1023) return fail(NERFB200_EINVAL, "nerf train workspace must be 1024-byte aligned%s");
+  if (bytes < nerfb200_nerf_train_workspace_bytes(n)) return fail(NERFB200_EINVAL, "nerf train workspace too small for n%s");
+  DeviceInfo* d = nullptr;
+  int rc = device_info(&d);
+  if (rc) return rc;
+  TrainLayout L;
+  make_mlp_train_layout(&L, static_cast<uint8_t*>(ws), n, d->sm_count);
+  if (bytes < L.bytes) return fail(NERFB200_EINVAL, "nerf train workspace too small for n%s");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  CUDA_TRY(cudaMemsetAsync(ws, 0, L.bytes, stream), "nerf workspace memset");
+  std::vector<WgradJob> jobs(kMaxWgJobs);
+  std::vector<int> cta_first(kMaxWgCtas + 1, 0);
+  std::memset(jobs.data(), 0, sizeof(WgradJob) * kMaxWgJobs);
+  plan_wgrad(&L, d->sm_count, jobs.data(), cta_first.data());
+  CUDA_TRY(cudaMemcpyAsync(L.jobs_dev, jobs.data(), sizeof(WgradJob) * kMaxWgJobs, cudaMemcpyHostToDevice, stream),
+           "nerf job table upload");
+  CUDA_TRY(cudaMemcpyAsync(L.cta_first_dev, cta_first.data(), sizeof(int) * (kMaxWgCtas + 1), cudaMemcpyHostToDevice, stream),
+           "nerf cta table upload");
+  CUDA_TRY(cudaStreamSynchronize(stream), "nerf workspace init sync");
+  return 0;
+}
+
+int nerfb200_nerf_forward_train(const float* x, int64_t n, int64_t x_stride, const void* packed, void* ws, float* out,
+                                void* stream) {
+  if (n < 0 || n > 0x7fffffffLL) return fail(NERFB200_EINVAL, "nerf_forward_train: n out of range%s");
+  if (n == 0) return 0;
+  if (!x || !packed || !ws || !out) return fail(NERFB200_EINVAL, "nerf_forward_train: NULL argument%s");
+  if (x_stride < kEncXyz + kEncDir) return fail(NERFB200_EINVAL, "nerf_forward_train: x_stride < 90%s");
+  if ((reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(packed) & 15))
+    return fail(NERFB200_EINVAL, "nerf_forward_train: out / packed must be 16-byte aligned%s");
+  if (reinterpret_cast<uintptr_t>(ws) & 1023) return fail(NERFB200_EINVAL, "nerf train workspace must be 1024-byte aligned%s");
+  DeviceInfo* d = nullptr;
+  int rc = device_info(&d);
+  if (rc) return rc;
+  if ((rc = check_sticky_status(d)) != 0) return rc;
+  TrainLayout L;
+  make_mlp_train_layout(&L, static_cast<uint8_t*>(ws), n, d->sm_count);
+  MlpParams p;
+  p.raw_xyz = 0;
+  p.x = x; p.x_stride = x_stride; p.n = n;
+  p.net = static_cast<const uint8_t*>(packed);
+  p.sigma_only = 0;
+  p.out = out;
+  p.status = d->status;
+  p.tr = L.pass[0];
+  p.xdir = L.xdir;
+  const long long tiles = (n + 127) / 128;
+  const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
+  mlp_forward_kernel<true><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "nerf_forward_train launch");
+  return 0;
+}
+
+int nerfb200_nerf_backward(const float* g_out, int64_t n, const void* packed, const float* const params[24], void* ws,
+                           float* const grads[24], void* stream_v) {
+  if (n < 0 || n > 0x7fffffffLL) return fail(NERFB200_EINVAL, "nerf_backward: n out of range%s");
+  if (n == 0) return 0;
+  if (!g_out || !packed || !params || !ws || !grads) return fail(NERFB200_EINVAL, "nerf_backward: NULL argument%s");
+  for (int i = 0; i < kNumParams; ++i)
+    if (!params[i] || !grads[i]) return fail(NERFB200_EINVAL, "nerf_backward: NULL parameter / gradient tensor%s");
+  if (reinterpret_cast<uintptr_t>(g_out) & 15) return fail(NERFB200_EINVAL, "nerf_backward: g_out must be 16-byte aligned%s");
+  if (reinterpret_cast<uintptr_t>(ws) & 1023) return fail(NERFB200_EINVAL, "nerf train workspace must be 1024-byte aligned%s");
+  DeviceInfo* d = nullptr;
+  int rc = device_info(&d);
+  if (rc) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  TrainLayout L;
+  make_mlp_train_layout(&L, static_cast<uint8_t*>(ws), n, d->sm_count);
+  const PassBufs& pb = L.pass[0];
+  // 1. seed: upstream gradient -> per-sample d sigma / d rgb_pre (replaces the compositing backward)
+  MlpSeedParams sd;
+  sd.n = n; sd.n_pad = pb.n_pad;
+  sd.g = g_out; sd.rgb = pb.rgb; sd.dsigma = pb.dsigma; sd.dprergb = pb.dprergb;
+  sd.amax_bits = L.amax;
+  mlp_seed_kernel<<<static_cast<int>((pb.n_pad + 255) / 256), 256, 0, stream>>>(sd);
+  g_launches++;
+  ScaleParams sp;
+  sp.n_pass = 1; sp.phase = 0;
+  sp.amax = L.amax; sp.lamax = L.lamax; sp.lscale = L.lscale; sp.linv = L.linv;
+  sp.w_rgb[0] = sp.w_rgb[1] = params[22];
+  sp.w_sigma[0] = sp.w_sigma[1] = params[20];
+  bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
+  g_launches++;
+  // 2. rgb head + ReLU of the direction layer over pseudo-rays of 64 samples (no per-ray direction work)
+  HeadBwdParams hp;
+  hp.n_rays = L.n_rays; hp.n_pass = 1;
+  hp.pass[0] = pb;
+  hp.pass[0].S = kMlpPseudoRay;
+  hp.pass[1] = hp.pass[0];
+  hp.w_rgb[0] = hp.w_rgb[1] = params[22];
+  hp.lscale = L.lscale;
+  hp.rays = nullptr; hp.ray_stride = 0;
+  hp.raysum[0] = hp.raysum[1] = nullptr;
+  hp.direnc = nullptr;
+  hp.part[0] = L.head_part[0]; hp.part[1] = nullptr;
+  head_bwd_kernel<<<L.head_grid, kHeadWarps * 32, 0, stream>>>(hp);
+  g_launches++;
+  // 3. dgrad chain: probe over one tile per SM spread over the batch, then the real pass
+  ChainParams cp;
+  cp.n_pass = 1;
+  cp.pass[0] = cp.pass[1] = pb;
+  cp.net[0] = cp.net[1] = static_cast<const uint8_t*>(packed);
+  cp.lscale = L.lscale;
+  cp.lamax = L.lamax;
+  cp.status = d->status;
+  const long long t0 = pb.n_pad / 128;
+  launch_chain(cp, t0, 0, kBwdBf16 ? 0 : (t0 < d->sm_count ? t0 : d->sm_count), 0, sp, d->sm_count, stream);
+  // 4. split-K wgrad (wgmma), with the direction-slice GEMM dd^T xdir
+  wgrad_kernel<<<L.n_cta, kWgThreads, kWgSmemTotal, stream>>>(L.jobs_dev, L.cta_first_dev,
+                                                               static_cast<uint32_t>(env_switches().wg_copy),
+                                                               env_switches().wg_exp, d->status);
+  g_launches++;
+  // 5. partial sums -> gradient tensors (fixed order), 6. unfold W'
+  ReduceTable tab;
+  tab.n = 0;
+  add_reduce_items(tab, L, 0, grads);
+  wgrad_reduce_kernel<<<dim3(64, tab.n), 256, 0, stream>>>(tab);
+  g_launches++;
+  UnfoldParams up;
+  for (int ps = 0; ps < 2; ++ps) {
+    up.gWp[ps] = L.gWp[0]; up.gbp[ps] = L.gbp[0];
+    up.Wf[ps] = params[16]; up.bf[ps] = params[17]; up.Wd[ps] = params[18];
+    up.gWd[ps] = grads[18]; up.gbd[ps] = grads[19]; up.gWf[ps] = grads[16]; up.gbf[ps] = grads[17];
+  }
+  unfold_kernel<<<dim3((128 * 256 + (256 * 256 + 256 + 31) / 32 + 7) / 8, 1), 256, 0, stream>>>(up);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "nerf_backward launches");
   return 0;
 }
 
@@ -987,35 +1257,7 @@ int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
     const long long half = (d->sm_count + 1) / 2;
     const long long pt0 = kBwdBf16 ? 0 : (fine ? (t0 < half ? t0 : half) : (t0 < d->sm_count ? t0 : d->sm_count));
     const long long pt1 = kBwdBf16 ? 0 : (fine ? (t1 < half ? t1 : half) : 0);
-    const long long span[2] = {t0, t1}, pt[2] = {pt0, pt1};
-    auto gcd = [](long long x, long long y) {
-      while (y != 0) { const long long r = x % y; x = y; y = r; }
-      return x;
-    };
-    for (int ps = 0; ps < 2; ++ps) {
-      long long s = (pt[ps] > 0 && span[ps] > pt[ps]) ? span[ps] / pt[ps] : 1;
-      while (span[ps] > 1 && gcd(s, span[ps]) != 1) ++s;
-      cp.span[ps] = span[ps] > 0 ? span[ps] : 1;
-      cp.stride[ps] = s;
-    }
-    if (!kBwdBf16) {
-      cp.tiles[0] = cp.head[0] = pt0;
-      cp.tiles[1] = cp.head[1] = pt1;
-      const int pc = static_cast<int>(pt0 + pt1);
-      chain_bwd_kernel<true><<<pc, kThreads, kChSmemTotal, stream>>>(cp);
-      g_launches++;
-      sp.phase = 1;
-      bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
-      g_launches++;
-    }
-    cp.head[0] = pt0;
-    cp.head[1] = pt1;
-    cp.tiles[0] = t0;
-    cp.tiles[1] = t1;
-    const long long total = t0 + t1;
-    const int ctas = static_cast<int>(total < d->sm_count ? total : d->sm_count);
-    chain_bwd_kernel<false><<<ctas, kThreads, kChSmemTotal, stream>>>(cp);
-    g_launches++;
+    launch_chain(cp, t0, t1, pt0, pt1, sp, d->sm_count, stream);
   }
   // 4. split-K wgrad (wgmma)
   wgrad_kernel<<<L.n_cta, kWgThreads, kWgSmemTotal, stream>>>(L.jobs_dev, L.cta_first_dev,
@@ -1025,39 +1267,7 @@ int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
   // 5. partial sums -> gradient tensors (fixed order), 6. unfold W'
   ReduceTable tab;
   tab.n = 0;
-  auto add = [&](const float* part, long long stride, int n_split, float* out, const float* mul, int rows, int cols,
-                 int part_ld, int out_ld, int out_col0, int transposed = 0) {
-    ReduceItem& it = tab.it[tab.n++];
-    it.part = part; it.split_stride = stride; it.n_split = n_split; it.out = out; it.mul = mul;
-    it.rows = rows; it.cols = cols; it.part_ld = part_ld; it.out_ld = out_ld; it.out_col0 = out_col0;
-    it.transposed = transposed;
-    it.by_warp = (n_split >= 128 && rows * cols <= 4096) ? 1 : 0;
-  };
-  for (int ps = 0; ps < L.n_pass; ++ps) {
-    const float* linv = L.linv + ps * kLevels;       // level v: 0 = dd, v = 1..8 = dpre_{9-v}
-    auto slot = [&](int kind) { return L.wg_part + static_cast<size_t>(L.first_job[ps][kind]) * kWgSlotFloats; };
-    auto ns = [&](int kind) { return L.n_split[ps][kind]; };
-    float* const* g = grads[ps];
-    add(slot(kJ1), kWgSlotFloats, ns(kJ1), g[0], linv + 8, 256, 63, 256, 63, 0, 1);
-    add(slot(kJ1) + 65536, kWgSlotFloats, ns(kJ1), g[1], linv + 8, 1, 256, 256, 256, 0);
-    const int hidden[6] = {kJ2, kJ3, kJ4, kJ6, kJ7, kJ8};
-    const int layer[6] = {2, 3, 4, 6, 7, 8};
-    for (int i = 0; i < 6; ++i) {
-      const float* inv = linv + (9 - layer[i]);
-      add(slot(hidden[i]), kWgSlotFloats, ns(hidden[i]), g[2 * (layer[i] - 1)], inv, 256, 256, 256, 256, 0, 1);
-      add(slot(hidden[i]) + 65536, kWgSlotFloats, ns(hidden[i]), g[2 * (layer[i] - 1) + 1], inv, 1, 256, 256, 256, 0);
-    }
-    add(slot(kJ5a), kWgSlotFloats, ns(kJ5a), g[8], linv + 4, 256, 63, 256, 319, 0, 1);
-    add(slot(kJ5b), kWgSlotFloats, ns(kJ5b), g[8], linv + 4, 256, 256, 256, 319, 63, 1);
-    add(slot(kJ5a) + 65536, kWgSlotFloats, ns(kJ5a), g[9], linv + 4, 1, 256, 256, 256, 0);
-    add(slot(kJ9), kWgSlotFloats, ns(kJ9), L.gWp[ps], linv, 128, 256, 128, 256, 0, 1);
-    add(slot(kJ9) + 65536, kWgSlotFloats, ns(kJ9), L.gbp[ps], linv, 1, 128, 128, 128, 0);
-    add(L.head_part[ps] + kHeadPartSigW, kHeadPartFloats, L.head_grid, g[20], nullptr, 1, 256, 256, 256, 0);
-    add(L.head_part[ps] + kHeadPartSigB, kHeadPartFloats, L.head_grid, g[21], nullptr, 1, 1, 1, 1, 0);
-    add(L.head_part[ps] + kHeadPartRgbW, kHeadPartFloats, L.head_grid, g[22], nullptr, 1, 384, 384, 384, 0);
-    add(L.head_part[ps] + kHeadPartRgbB, kHeadPartFloats, L.head_grid, g[23], nullptr, 1, 3, 3, 3, 0);
-    add(L.dir_part[ps], 128 * 27, kDirSlices, g[18], nullptr, 128, 27, 27, 283, 256);
-  }
+  for (int ps = 0; ps < L.n_pass; ++ps) add_reduce_items(tab, L, ps, grads[ps]);
   wgrad_reduce_kernel<<<dim3(64, tab.n), 256, 0, stream>>>(tab);   // latency-bound: 64 blocks per item (16 measured 40 us)
   g_launches++;
   UnfoldParams up;

@@ -286,6 +286,7 @@ struct DirSrc {
   long long stride;
   long long row0;      // global row of tile row 0
   long long n;
+  uint8_t* save;       // training save mode: tiled (n_pad, 64) fp16 copy of the rows written here, or null
 };
 
 // NeRF.forward mode: the ENC tile is dead after layer 5; this warpgroup rewrites its 64 rows with the
@@ -299,6 +300,17 @@ __device__ __forceinline__ void write_dir_rows(WgCtx& c, uint32_t enc_off, const
   for (int k = (t & 1) * 32; k < (t & 1) * 32 + 32; ++k) {
     const float v = (k < kEncDir) ? __ldg(src + k) : 0.f;
     *reinterpret_cast<__half*>(enc + sw128_off(row, k)) = __float2half_rn(v);
+  }
+  if (ds.save != nullptr) {
+    // the tile's 128 rows are chunks 2 tile, 2 tile + 1 of the tiled array, whose 128-byte rows carry the same
+    // swizzle as the shared-memory tile: copy this thread's four 16-byte chunks (its own stores above) in place.
+    // Padding rows (copies of row n - 1) are stored too: the array is padded to whole tiles, and their gradient is 0
+    uint8_t* dst = ds.save + ds.row0 * 128;
+#pragma unroll
+    for (int cc = 0; cc < 4; ++cc) {
+      const uint32_t off = sw128_off(row, ((t & 1) * 4 + cc) * 8);
+      *reinterpret_cast<uint4*>(dst + off) = *reinterpret_cast<const uint4*>(enc + off);
+    }
   }
   fence_proxy_async();
   wg_bar(c);

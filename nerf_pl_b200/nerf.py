@@ -5,7 +5,8 @@ the sm_90a kernels of ``libnerf_pl_b200.so``.
 The modules are ordinary ``nn.Module``s so ``utils.get_optimizer`` / ``load_ckpt``
 (reference utils/__init__.py:10-30, 55-76) and pytorch-lightning keep working.  Inference
 (``torch.no_grad`` / no parameter requires grad) runs the wgmma kernel through the C ABI;
-when autograd needs a graph the layers are evaluated with torch ops so gradients exist.
+when autograd needs a graph the layers are evaluated with torch ops so gradients exist, or, with
+``model.autograd_impl = "fused"``, by the sm_90a training kernels (``training.nerf_forward_train``).
 """
 from __future__ import annotations
 
@@ -197,11 +198,17 @@ class Embedding(nn.Module):
 
 class NeRF(nn.Module):
     """8x256 ReLU MLP with a skip at layer 5, sigma head, 256 linear, 283->128 direction layer and
-    a sigmoid rgb head (reference models/nerf.py:41-124); same submodule names and state_dict keys."""
+    a sigmoid rgb head (reference models/nerf.py:41-124); same submodule names and state_dict keys.
+
+    ``autograd_impl`` (instance attribute, not part of the state_dict) selects how a call that needs a
+    gradient graph is evaluated: ``"torch"`` (default) with torch ops, ``"fused"`` with the sm_90a
+    forward-with-save and backward kernels (``nerf_pl_b200.training.nerf_forward_train``; full
+    ``(B, 90) -> (B, 4)`` output of the default architecture, no gradient with respect to ``x``)."""
 
     def __init__(self, D: int = 8, W: int = 256, in_channels_xyz: int = 63, in_channels_dir: int = 27,
                  skips: Sequence[int] = (4,)):
         super().__init__()
+        self.autograd_impl = "torch"
         self.D, self.W = D, W
         self.in_channels_xyz, self.in_channels_dir = in_channels_xyz, in_channels_dir
         self.skips = list(skips)
@@ -220,8 +227,17 @@ class NeRF(nn.Module):
     def forward(self, x: torch.Tensor, sigma_only: bool = False) -> torch.Tensor:
         if not x.is_cuda:
             raise RuntimeError("nerf_pl_b200.NeRF runs on CUDA tensors only (no CPU fallback)")
+        impl = getattr(self, "autograd_impl", "torch")
+        if impl not in ("torch", "fused"):
+            raise ValueError(f"NeRF.autograd_impl must be 'torch' or 'fused', got {impl!r}")
         needs_graph = torch.is_grad_enabled() and (
             x.requires_grad or any(p.requires_grad for p in self.parameters()))
+        if needs_graph and impl == "fused":
+            if sigma_only:
+                raise ValueError("autograd_impl='fused' trains the full (B, 90) -> (B, 4) output; sigma_only=True "
+                                 "is not supported")
+            from .training import nerf_forward_train
+            return nerf_forward_train(self, x)
         if needs_graph or not self.is_default_arch():
             return nerf_forward_torch(self, x, sigma_only)
         return nerf_forward_fused(self, x, sigma_only)

@@ -13,6 +13,10 @@ backward: ``nerfb200_render_backward`` (include/nerf_pl_b200.h): compositing bac
           wgmma dgrad chain -> wgmma split-K wgrad -> fixed-order reduction -> unfolding of the
           packed final.dir layer; fills the 48 ``.grad`` tensors.
 The sampling of the fine depths carries no gradient (models/rendering.py:225-227 ``.detach()``).
+
+``nerf_forward_train`` (end of this file) trains a direct ``NeRF.forward`` call the same way, for callers that
+render with their own code: one save-mode launch of the MLP kernel, then the same backward kernels seeded from
+the upstream (B, 4) gradient.
 """
 from __future__ import annotations
 
@@ -22,7 +26,8 @@ from typing import Dict, List, Optional
 import torch
 
 from . import _lib
-from .nerf import _stream_ptr, nerf_parameters, packed_weights, packed_weights_pair
+from .nerf import (_EXPECTED_SHAPES, _stream_ptr, nerf_forward_fused, nerf_parameters, packed_weights,
+                   packed_weights_pair)
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -218,3 +223,166 @@ def render_rays_train(models, rays, N_samples, use_disp, perturb, noise_std, N_i
         l4 = outs[k]
         res.update(loss=l4[2], psnr=l4[3].detach(), mse_coarse=l4[0].detach(), mse_fine=l4[1].detach())
     return res
+
+
+# ---------------------------------------------------------------------------------------------
+# Training a direct NeRF.forward call (reference models/nerf.py:83-124) for callers that render with their own code:
+# one save-mode launch of the MLP kernel forward (nerfb200_nerf_forward_train), the sm_90a backward kernels of the
+# render path seeded from the upstream (B, 4) gradient (nerfb200_nerf_backward).
+class NerfTrainWorkspace:
+    """Device workspace of one ``nerf_forward_train`` call over ``n`` samples, from a per-device pool.
+
+    A call holds its workspace from its forward until its backward runs, or until its graph is freed without a
+    backward (outputs used only for metrics under grad mode).  Pool policy: a call takes an idle workspace of
+    exactly its ``n``; if there is none it first releases every idle workspace of another size on that device, then
+    makes one.  So calls whose ``n`` varies (the last chunk of a point loop) do not accumulate workspaces: the pool
+    holds the workspaces of the calls whose backward is pending, plus at most the idle ones of a single size."""
+
+    _pool: Dict[int, List["NerfTrainWorkspace"]] = {}
+
+    def __init__(self, dev: torch.device, n: int) -> None:
+        lib = _lib.load()
+        self.n = n
+        self.bytes = int(lib.nerfb200_nerf_train_workspace_bytes(n))
+        if self.bytes == 0:
+            raise ValueError(f"invalid sample count {n}")
+        raw = torch.empty(self.bytes + 1024, dtype=torch.uint8, device=dev)
+        off = (-raw.data_ptr()) % 1024
+        self.raw = raw
+        self.buf = raw[off:off + self.bytes]
+        self.busy = False
+        with torch.cuda.device(dev):
+            _lib.check(lib.nerfb200_nerf_train_workspace_init(self.buf.data_ptr(), self.bytes, n, _stream_ptr()),
+                       "nerfb200_nerf_train_workspace_init")
+
+    @classmethod
+    def acquire(cls, dev: torch.device, n: int) -> "NerfTrainWorkspace":
+        pool = cls._pool.setdefault(dev.index, [])
+        for ws in pool:
+            if not ws.busy and ws.n == n:
+                ws.busy = True
+                return ws
+        pool[:] = [ws for ws in pool if ws.busy]
+        ws = cls(dev, n)
+        ws.busy = True
+        pool.append(ws)
+        return ws
+
+    @classmethod
+    def pool_size(cls, dev: torch.device) -> int:
+        return len(cls._pool.get(dev.index, []))
+
+    @classmethod
+    def clear(cls) -> None:
+        cls._pool.clear()
+
+
+class _Lease:
+    """A call's hold on its workspace: released by the backward, or when autograd frees the graph (the ctx that
+    owns the lease is destroyed) without one."""
+    __slots__ = ("ws",)
+
+    def __init__(self, ws: NerfTrainWorkspace) -> None:
+        self.ws = ws
+
+    def release(self) -> None:
+        if self.ws is not None:
+            self.ws.busy = False
+            self.ws = None
+
+    def __del__(self) -> None:
+        self.release()
+
+
+class FusedNerfFunction(torch.autograd.Function):
+    """(model, x (B, 90) fp32 contiguous, 24 parameter tensors) -> (B, 4) [rgb, sigma]."""
+
+    @staticmethod
+    def forward(ctx, model, x, *params):
+        n = x.shape[0]
+        dev = x.device
+        out = torch.empty(n, 4, dtype=torch.float32, device=dev)
+        ctx.n = n
+        ctx.lease = None
+        if n > 0:
+            lib = _lib.load()
+            blob = packed_weights(model)
+            lease = _Lease(NerfTrainWorkspace.acquire(dev, n))
+            with torch.cuda.device(dev):
+                _lib.check(lib.nerfb200_nerf_forward_train(x.data_ptr(), n, x.stride(0), blob.data_ptr(),
+                                                           lease.ws.buf.data_ptr(), out.data_ptr(), _stream_ptr()),
+                           "nerfb200_nerf_forward_train")
+            ctx.lease = lease
+            ctx.blob = blob
+        ctx.save_for_backward(*params)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        params = list(ctx.saved_tensors)
+        if ctx.n == 0:
+            return (None, None, *[torch.zeros_like(p) for p in params])
+        lease = ctx.lease
+        if lease is None or lease.ws is None:
+            raise RuntimeError("the fused NeRF backward of this call has already run (its workspace is released "
+                               "after one backward; retain_graph=True is not supported with autograd_impl='fused')")
+        dev = params[0].device
+        g = g.detach().to(torch.float32).contiguous()
+        if g.data_ptr() % 16:
+            g = g.clone()
+        sizes, shapes = _param_sizes(params)
+        flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
+        grads = [t.view(shp) for t, shp in zip(flat.split(sizes), shapes)]
+        base, offs = flat.data_ptr(), _offsets(sizes)
+        pc = (ctypes.c_void_p * 24)(*[p.data_ptr() for p in params])
+        gc = (ctypes.c_void_p * 24)(*[base + 4 * o for o in offs])
+        lib = _lib.load()
+        with torch.cuda.device(dev):
+            _lib.check(lib.nerfb200_nerf_backward(g.data_ptr(), ctx.n, ctx.blob.data_ptr(), pc,
+                                                  lease.ws.buf.data_ptr(), gc, _stream_ptr()),
+                       "nerfb200_nerf_backward")
+        lease.release()
+        ctx.blob = None
+        return (None, None, *grads)
+
+
+def nerf_forward_train(model: torch.nn.Module, x: torch.Tensor) -> torch.Tensor:
+    """``model(x)`` (reference models/nerf.py:83-124, ``sigma_only=False``) for training on the sm_90a kernels:
+    ``x`` (B, 90) embedded xyz + direction -> (B, 4) [rgb, sigma].  Works for this package's ``NeRF`` (its
+    ``forward`` calls this when ``autograd_impl == "fused"``) and, duck-typed through ``nerf_parameters``, for
+    the reference's own ``models.nerf.NeRF`` instances.
+
+    When a graph is needed (grad mode on, a parameter requires grad) the forward is one save-mode launch whose
+    output equals ``nerf_forward_fused`` bit for bit, and ``backward`` fills the gradients of the 24 parameters
+    with the sm_90a kernels.  Several calls before one ``backward()`` (coarse and fine nets, a chunked point loop,
+    one model called twice) each hold their own workspace (``NerfTrainWorkspace``); their gradients are summed
+    by autograd.  Otherwise this is ``nerf_forward_fused``.
+
+    Raises ``ValueError`` for what the kernels do not do: ``x.requires_grad`` (no gradient with respect to the
+    input), a non-default architecture, ``x`` not of shape (B, 90); ``RuntimeError`` for CPU tensors.  A backward
+    whose per-sample gradients exceed their layer's fp16 range is reported (device status 102) by the next library
+    call or ``nerfb200_check_status``."""
+    if not x.is_cuda:
+        raise RuntimeError("nerf_pl_b200.nerf_forward_train runs on CUDA tensors only (no CPU fallback)")
+    if x.requires_grad:
+        raise ValueError("autograd_impl='fused' computes no gradient with respect to x; detach the input or use "
+                         "autograd_impl='torch'")
+    if x.dim() != 2 or x.shape[1] != 90:
+        raise ValueError(f"autograd_impl='fused' expects x of shape (B, 90), got {tuple(x.shape)}")
+    is_default = getattr(model, "is_default_arch", None)
+    if is_default is not None and not is_default():
+        raise ValueError("autograd_impl='fused' supports the reference's default NeRF(D=8, W=256, 63, 27, skips=[4]) only")
+    try:
+        params = nerf_parameters(model)
+    except (KeyError, AttributeError) as e:
+        raise ValueError(f"autograd_impl='fused' supports the reference's default NeRF only (missing {e})") from None
+    for p, shp in zip(params, _EXPECTED_SHAPES):
+        if tuple(p.shape) != shp:
+            raise ValueError(f"autograd_impl='fused' supports the reference's default NeRF only: parameter of shape "
+                             f"{tuple(p.shape)}, expected {shp}")
+        if p.device != x.device:
+            raise ValueError("x and the NeRF parameters must be on the same device")
+    if not (torch.is_grad_enabled() and any(p.requires_grad for p in params)):
+        return nerf_forward_fused(model, x)
+    return FusedNerfFunction.apply(model, x.detach().to(torch.float32).contiguous(), *params)
