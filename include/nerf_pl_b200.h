@@ -241,7 +241,8 @@ int nerfb200_searchsorted(const float* a, const float* v, int64_t* out, int64_t 
 
 /* ---- sample_pdf --------------------------------------------------------------------------
  * Replaces: models/rendering.py:14-55 with the random/deterministic u supplied by the caller.
- * bins (n_rays, n_weights+1), weights (n_rays, n_weights), u (n_rays, n_u) -> out (n_rays, n_u). */
+ * bins (n_rays, n_weights+1), weights (n_rays, n_weights), u (n_rays, n_u) -> out (n_rays, n_u).
+ * 1 <= n_weights <= 4096. */
 int nerfb200_sample_pdf(const float* bins, const float* weights, const float* u, int64_t n_rays,
                         int32_t n_weights, int32_t n_u, float* out, void* stream);
 

@@ -294,6 +294,8 @@ __global__ void searchsorted_kernel(const float* __restrict__ a, const float* __
 
 // ------------------------------------------------ sample_pdf (models/rendering.py:14-55)
 // bins (R, nb = nw+1), weights (R, nw), u (R, K) sorted or not; out (R, K).  One warp per ray.
+constexpr int kPdfWarps = 4;             // warps (rays in flight) per block
+constexpr int kPdfMaxWeights = 4096;     // nw <= 4096: kPdfWarps cdfs of nw + 1 floats, 64 KB of shared memory
 __global__ void sample_pdf_kernel(const float* __restrict__ bins, const float* __restrict__ weights,
                                   const float* __restrict__ u, long long n_rays, int nw, int K,
                                   float* __restrict__ out) {

@@ -94,6 +94,9 @@ int device_info(DeviceInfo** out) {
                                   static_cast<int>(kChSmemTotal)), "smem attr chain (probe)");
     CUDA_TRY(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kWgSmemTotal)), "smem attr wgrad");
+    // one cdf of n_weights + 1 floats per warp: above the 48 KB default from n_weights = 3072
+    CUDA_TRY(cudaFuncSetAttribute(sample_pdf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kPdfWarps * (kPdfMaxWeights + 1) * sizeof(float))), "smem attr sample_pdf");
     int* hs = nullptr;
     CUDA_TRY(cudaHostAlloc(&hs, sizeof(int), cudaHostAllocMapped), "status alloc");
     *hs = 0;
@@ -1069,11 +1072,14 @@ int nerfb200_searchsorted(const float* a, const float* v, int64_t* out, int64_t 
 
 int nerfb200_sample_pdf(const float* bins, const float* weights, const float* u, int64_t n_rays,
                         int32_t n_weights, int32_t n_u, float* out, void* stream) {
-  if (n_rays < 0 || n_weights < 1 || n_u < 0 || n_weights > 4096)
+  if (n_rays < 0 || n_weights < 1 || n_u < 0 || n_weights > kPdfMaxWeights)
     return fail(NERFB200_EINVAL, "sample_pdf: bad sizes%s");
   if (n_rays == 0 || n_u == 0) return 0;
   if (!bins || !weights || !u || !out) return fail(NERFB200_EINVAL, "sample_pdf: NULL argument%s");
-  const int wpb = 4;
+  DeviceInfo* d = nullptr;
+  const int rc = device_info(&d);           // opts sample_pdf_kernel in to its shared memory
+  if (rc) return rc;
+  const int wpb = kPdfWarps;
   const size_t sh = wpb * (n_weights + 1) * sizeof(float);
   long long blocks = (n_rays + wpb - 1) / wpb;
   if (blocks > 148 * 8) blocks = 148 * 8;
