@@ -164,7 +164,8 @@ int nerfb200_render_backward(const nerfb200_backward_args* args, void* stream);
 /* ---- optimiser step ("next" row: the caller of the backward) ---------------------------------
  * Replaces: torch.optim.Adam.step() as the reference configures it (utils/__init__.py:16-18:
  * Adam(lr, eps, weight_decay), betas (0.9, 0.999), no amsgrad; train.py:77-82) for up to 64 fp32
- * tensors in one launch.  `step` is the 1-based count of this update (bias correction). */
+ * tensors in one launch.  `step` is the 1-based count of this update (bias correction).  The pointers of a
+ * tensor with numel 0 may be NULL (torch gives empty tensors no storage). */
 int nerfb200_adam_step(int32_t n_tensors, float* const* params, const float* const* grads, float* const* exp_avg,
                        float* const* exp_avg_sq, const int64_t* numel, float lr, float beta1, float beta2, float eps,
                        float weight_decay, int64_t step, void* stream);

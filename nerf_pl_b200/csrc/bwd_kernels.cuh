@@ -975,9 +975,14 @@ __global__ void __launch_bounds__(256) unfold_kernel(const UnfoldParams p) {
 // torch.optim.Adam's update (the reference's default optimiser, utils/__init__.py:16-18:
 // Adam(lr, eps, weight_decay), betas (0.9, 0.999), no amsgrad) for all parameter tensors of the two
 // networks in ONE launch: torch's fused implementation costs two 80 us multi-tensor kernels for
-// these 48 small tensors, a fifth of the remaining step.  Same arithmetic as torch (fp32):
+// these 48 small tensors, a fifth of the remaining step.  Adam's update in fp32:
 //   g = grad + weight_decay * p;  m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2
-//   p -= lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
+//   p -= step_size * m / (sqrt(v) / bias2_sqrt + eps)
+// step_size = lr / (1 - b1^t) and bias2_sqrt = sqrt(1 - b2^t) are computed on the host in double from the fp32
+// hyper-parameters and rounded once (in fp32, 1 - b2^t cancels: ~50 ulps of the update at t = 2..3).  1 - b1 and
+// 1 - b2 are exact in fp32.  torch.optim.Adam instead takes 1 - b2 of the unrounded double b2 (0.001 for 0.999,
+// where 1 - fp32(0.999) = 0.00099998713), so the two differ by ~1e-5 relative in v; tests/adam_ref.py is the
+// float64 model of this kernel that tests/test_gpu_train_loop.py holds it to.
 constexpr int kAdamMaxTensors = 64;
 struct AdamParams {
   int n_tensors;
@@ -987,7 +992,7 @@ struct AdamParams {
   float* v[kAdamMaxTensors];
   int block0[kAdamMaxTensors + 1];     // first block of each tensor (1024 elements per block)
   int numel[kAdamMaxTensors];
-  float lr, beta1, beta2, eps, weight_decay, bias1, bias2_sqrt;     // bias1 = 1 - b1^t, bias2_sqrt = sqrt(1 - b2^t)
+  float beta1, beta2, eps, weight_decay, step_size, bias2_sqrt;    // step_size = lr / (1 - b1^t), bias2_sqrt = sqrt(1 - b2^t)
 };
 __global__ void __launch_bounds__(256) adam_kernel(const __grid_constant__ AdamParams a) {
   int lo = 0, hi = a.n_tensors;
@@ -997,7 +1002,7 @@ __global__ void __launch_bounds__(256) adam_kernel(const __grid_constant__ AdamP
   }
   const int t = lo;
   const int base = (static_cast<int>(blockIdx.x) - a.block0[t]) * 1024;
-  const float step = a.lr / a.bias1;
+  const float step = a.step_size;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const int i = base + q * 256 + threadIdx.x;

@@ -1301,7 +1301,8 @@ int nerfb200_adam_step(int32_t n_tensors, float* const* params, const float* con
   a.n_tensors = n_tensors;
   int blocks = 0;
   for (int i = 0; i < n_tensors; ++i) {
-    if (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i] || numel[i] < 0 || numel[i] > 0x7fffffff)
+    if (numel[i] < 0 || numel[i] > 0x7fffffff ||
+        (numel[i] > 0 && (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i])))
       return fail(NERFB200_EINVAL, "adam_step: NULL tensor / bad size%s");
     a.p[i] = params[i]; a.g[i] = grads[i]; a.m[i] = exp_avg[i]; a.v[i] = exp_avg_sq[i];
     a.numel[i] = static_cast<int>(numel[i]);
@@ -1309,9 +1310,10 @@ int nerfb200_adam_step(int32_t n_tensors, float* const* params, const float* con
     blocks += static_cast<int>((numel[i] + 1023) / 1024);
   }
   a.block0[n_tensors] = blocks;
-  a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
-  a.bias1 = 1.f - std::pow(beta1, static_cast<float>(step));
-  a.bias2_sqrt = std::sqrt(1.f - std::pow(beta2, static_cast<float>(step)));
+  a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
+  // in double, rounded once: 1 - b2^t in fp32 cancels at small t (~50 ulps of the update at t = 2..3)
+  a.step_size = static_cast<float>(static_cast<double>(lr) / (1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step))));
+  a.bias2_sqrt = static_cast<float>(std::sqrt(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step))));
   if (blocks == 0) return 0;
   adam_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
   g_launches++;

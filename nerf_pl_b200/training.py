@@ -36,8 +36,10 @@ def _ptr(t: Optional[torch.Tensor]):
 
 class TrainWorkspace:
     """Device workspace of one (device, n_rays, N_samples, N_importance) shape, reused across steps.
-    ``busy`` is set between a forward and its backward so that a second forward (gradient
-    accumulation over several batches) gets its own buffer."""
+    A render holds its workspace (``busy``) from its forward until its backward runs, or until its graph is
+    freed without one (a skipped batch, a render under grad mode used only for a metric), so that a second
+    forward (gradient accumulation over several batches) gets its own buffer.  The pool of a shape holds as many
+    workspaces as there were pending backwards at once."""
 
     _pool: Dict[tuple, List["TrainWorkspace"]] = {}
 
@@ -71,6 +73,23 @@ class TrainWorkspace:
     @classmethod
     def clear(cls) -> None:
         cls._pool.clear()
+
+
+class _Lease:
+    """A call's hold on its workspace (``TrainWorkspace`` or ``NerfTrainWorkspace``): released by the backward,
+    or when autograd frees the graph (the ctx that owns the lease is destroyed) without one."""
+    __slots__ = ("ws",)
+
+    def __init__(self, ws) -> None:
+        self.ws = ws
+
+    def release(self) -> None:
+        if self.ws is not None:
+            self.ws.busy = False
+            self.ws = None
+
+    def __del__(self) -> None:
+        self.release()
 
 
 def _render_args(cfg, rays, pr, nc, ur, nf, out, blob_c, blob_f, ws, target, loss_out) -> _lib.RenderArgs:
@@ -108,12 +127,16 @@ class FusedRenderFunction(torch.autograd.Function):
             blob_c, blob_f = packed_weights_pair(models[0], models[1])      # one launch for both images
         else:
             blob_c, blob_f = packed_weights(models[0]), None
-        ws = TrainWorkspace.acquire(dev, n, S_c, K)
+        lease = _Lease(TrainWorkspace.acquire(dev, n, S_c, K))
+        ws = lease.ws
         args = _render_args(cfg, rays, pr, nc, ur, nf, out, blob_c, blob_f, ws, target, loss_out)
         with torch.cuda.device(dev):
             _lib.check(lib.nerfb200_render_rays(ctypes.byref(args), _stream_ptr()), "nerfb200_render_rays")
         ctx.cfg = cfg
-        ctx.keep = (rays, pr, nc, ur, nf, target, out, blob_c, blob_f, ws)
+        ctx.lease = lease
+        # detached aliases of the outputs: the returned tensors themselves on ctx would form a cycle (output ->
+        # grad_fn -> ctx -> output) that keeps a dropped graph, and with it the workspace, alive
+        ctx.keep = (rays, pr, nc, ur, nf, target, [o.detach() for o in out], blob_c, blob_f, ws)
         ctx.n_params = len(params)
         ctx.save_for_backward(*params)
         ctx.set_materialize_grads(False)
@@ -124,6 +147,10 @@ class FusedRenderFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *gouts):
+        lease = ctx.lease
+        if lease.ws is None:
+            raise RuntimeError("the fused backward of this render has already run (its training workspace is released "
+                               "after one backward; retain_graph=True is not supported with autograd_impl='fused')")
         cfg = ctx.cfg
         params = list(ctx.saved_tensors)
         rays, pr, nc, ur, nf, target, out, blob_c, blob_f, ws = ctx.keep
@@ -164,7 +191,7 @@ class FusedRenderFunction(torch.autograd.Function):
             grads_coarse=gc, grads_fine=gf)
         with torch.cuda.device(dev):
             _lib.check(lib.nerfb200_render_backward(ctypes.byref(bargs), _stream_ptr()), "nerfb200_render_backward")
-        ws.busy = False
+        lease.release()
         ctx.keep = None
         if K == 0:
             grads = grads[:24] + [None] * (ctx.n_params - 24)
@@ -275,23 +302,6 @@ class NerfTrainWorkspace:
     @classmethod
     def clear(cls) -> None:
         cls._pool.clear()
-
-
-class _Lease:
-    """A call's hold on its workspace: released by the backward, or when autograd frees the graph (the ctx that
-    owns the lease is destroyed) without one."""
-    __slots__ = ("ws",)
-
-    def __init__(self, ws: NerfTrainWorkspace) -> None:
-        self.ws = ws
-
-    def release(self) -> None:
-        if self.ws is not None:
-            self.ws.busy = False
-            self.ws = None
-
-    def __del__(self) -> None:
-        self.release()
 
 
 class FusedNerfFunction(torch.autograd.Function):
