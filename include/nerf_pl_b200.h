@@ -267,6 +267,66 @@ int nerfb200_generate_rays(int32_t H, int32_t W, float focal, const float c2w_ho
 /* Replaces: eval.py:126-128 (clip(img,0,1)*255).astype(uint8) on the rendered image, on device. */
 int nerfb200_to_uint8(const float* src, int64_t n, uint8_t* dst, void* stream);
 
+/* ---- coloured mesh extraction ------------------------------------------------------------
+ * Replaces: extract_color_mesh.py:113-284 (the dense grid, mcubes.marching_cubes, the index->world
+ * transform, open3d's largest-cluster filter and the default colour-averaging loop).  Sizes that
+ * depend on the data come back from a *_count call (it synchronises `stream`); the caller allocates
+ * and runs the matching *_emit call with the SAME workspace.  Conventions: DESIGN.md. */
+
+/* extract_color_mesh.py:113-140.  ranges_host: 6 HOST doubles {xmin, xmax, ymin, ymax, zmin, zmax}.
+ * Positions of the flattened points [start, start + count) of np.stack(np.meshgrid(x, y, z), -1)
+ * .reshape(-1, 3) with x = np.linspace(xmin, xmax, N) etc., cast to float32: point (i*N + j)*N + k is
+ * (x_j, y_i, z_k). */
+int nerfb200_grid_positions(int64_t N, const double ranges_host[6], int64_t start, int64_t count, float* xyz,
+                            void* stream);
+/* The whole grid, `chunk` points at a time (positions -> nerfb200_query_sigma -> max(sigma, 0)):
+ * sigma (N, N, N), sigma[i, j, k] = max(sigma(x_j, y_i, z_k), 0).  Workspace: the positions of one chunk. */
+size_t nerfb200_sigma_grid_workspace_bytes(int64_t chunk);
+int nerfb200_sigma_grid(const void* packed, int64_t N, const double ranges_host[6], int64_t chunk, void* ws,
+                        size_t bytes, float* sigma, void* stream);
+
+/* extract_color_mesh.py:144 mcubes.marching_cubes(sigma, threshold) on a C-order (n0, n1, n2) fp32 grid.
+ * Inside: sigma > threshold.  counts_host[2] = {vertices, triangles}.  vertices (V, 3) fp64 in index
+ * space, ordered by the lower endpoint's linear index then edge axis; triangles (T, 3) int32 ordered by
+ * cell then case-table order; normals (right-hand rule) point from inside to outside.  Either output of
+ * the emit call may be NULL.  At most 4e8 grid points. */
+size_t nerfb200_mc_workspace_bytes(int64_t n0, int64_t n1, int64_t n2);
+int nerfb200_mc_count(const float* sigma, int64_t n0, int64_t n1, int64_t n2, double threshold, void* ws, size_t bytes,
+                      int64_t counts_host[2], void* stream);
+int nerfb200_mc_emit(const float* sigma, int64_t n0, int64_t n1, int64_t n2, double threshold, void* ws, size_t bytes,
+                     double* vertices, int32_t* triangles, void* stream);
+
+/* extract_color_mesh.py:148-154: out (n, 3) fp32 = the reference's world vertices, with its quirks
+ * (divides by N, not N - 1; column 0 takes y_range, column 1 x_range). */
+int nerfb200_mesh_to_world(const double* vertices, int64_t n, int64_t N, const double ranges_host[6], float* out,
+                           void* stream);
+
+/* extract_color_mesh.py:163-171: keep the edge-connected component with the most triangles (ties: the
+ * one holding the lowest-indexed triangle), drop unreferenced vertices; both lists keep their order.
+ * counts_host[2] = {kept vertices, kept triangles}.  vertices (n_verts, 3) fp32. */
+size_t nerfb200_mesh_cluster_workspace_bytes(int64_t n_vertices, int64_t n_triangles);
+int nerfb200_mesh_cluster_count(const int32_t* triangles, int64_t n_tris, int64_t n_verts, void* ws, size_t bytes,
+                                int64_t counts_host[2], void* stream);
+int nerfb200_mesh_cluster_emit(const float* vertices, const int32_t* triangles, int64_t n_tris, int64_t n_verts, void* ws,
+                               size_t bytes, float* vertices_out, int32_t* triangles_out, void* stream);
+
+/* extract_color_mesh.py:240-243 cv2.remap(image, x, y, INTER_LINEAR) (constant 0 border) of a (H, W, 3)
+ * uint8 image at n points xy (n, 2) fp32 -> out (n, 3) uint8. */
+int nerfb200_remap_bilinear(const uint8_t* image, int32_t H, int32_t W, const float* xy, int64_t n, uint8_t* out,
+                            void* stream);
+/* extract_color_mesh.py:220-262 for one view: w2c_host = np.linalg.inv(c2w4)[:3] (12 HOST doubles),
+ * origin_host = float32(c2w[:, 3]).  Writes the sampled colours (n, 3) uint8, depth (n) fp64 and the
+ * occlusion rays (n, 8) [o, (v - o)/|v - o|, near, float32(depth)] for nerfb200_render_rays. */
+int nerfb200_color_project(const float* vertices, int64_t n, const double w2c_host[12], const float origin_host[3],
+                           float focal, int32_t W, int32_t H, const uint8_t* image, float near, uint8_t* colors,
+                           double* depth, float* rays, void* stream);
+/* extract_color_mesh.py:269-277: sum4 (n, 4) fp64 [colour sums, weight sum] += the view's weighted
+ * colour, w = 0.1/depth + (nan_to_num(opacity) < occ_threshold).  Zero sum4 before the first view. */
+int nerfb200_color_accumulate(const uint8_t* colors, const double* depth, const float* opacity, int64_t n,
+                              float occ_threshold, double* sum4, void* stream);
+/* extract_color_mesh.py:283-284: colors (n, 3) = uint8(sum / wsum), truncated. */
+int nerfb200_color_finalize(const double* sum4, int64_t n, uint8_t* colors, void* stream);
+
 /* ---- diagnostics -------------------------------------------------------------------------
  * Number of kernels this library has launched on the calling process so far (all entry
  * points).  bench.py reports the delta as `gpu_launches`. */

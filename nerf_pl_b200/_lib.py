@@ -19,7 +19,8 @@ LIB_PATH = os.path.join(_HERE, "libnerf_pl_b200.so")
 if os.environ.get("NERFB200_LIB"):          # a library built elsewhere (e.g. with extra -D flags); unset in production
     LIB_PATH = os.path.abspath(os.environ["NERFB200_LIB"])
 SOURCES = ["capi.cu"]
-HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh"]
+HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
+           "mesh_kernels.cuh", "mc_table.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -56,6 +57,20 @@ EXPORTS = [
     "nerfb200_launch_count",
     "nerfb200_check_status",
     "nerfb200_sm_count",
+    "nerfb200_sigma_grid_workspace_bytes",
+    "nerfb200_grid_positions",
+    "nerfb200_sigma_grid",
+    "nerfb200_mc_workspace_bytes",
+    "nerfb200_mc_count",
+    "nerfb200_mc_emit",
+    "nerfb200_mesh_to_world",
+    "nerfb200_mesh_cluster_workspace_bytes",
+    "nerfb200_mesh_cluster_count",
+    "nerfb200_mesh_cluster_emit",
+    "nerfb200_remap_bilinear",
+    "nerfb200_color_project",
+    "nerfb200_color_accumulate",
+    "nerfb200_color_finalize",
 ]
 
 class RenderArgs(ctypes.Structure):
@@ -201,6 +216,35 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.nerfb200_check_status.restype = c_int32
     lib.nerfb200_launch_count.restype = c_int64
     lib.nerfb200_sm_count.restype = c_int32
+    # coloured mesh extraction (nerf_pl_b200.mesh)
+    c_double, c_u8p = ctypes.c_double, ctypes.c_void_p
+    lib.nerfb200_sigma_grid_workspace_bytes.argtypes = [c_int64]
+    lib.nerfb200_sigma_grid_workspace_bytes.restype = c_size_t
+    lib.nerfb200_grid_positions.argtypes = [c_int64, POINTER(c_double), c_int64, c_int64, c_void_p, c_void_p]
+    lib.nerfb200_sigma_grid.argtypes = [c_void_p, c_int64, POINTER(c_double), c_int64, c_void_p, c_size_t, c_void_p,
+                                        c_void_p]
+    lib.nerfb200_mc_workspace_bytes.argtypes = [c_int64, c_int64, c_int64]
+    lib.nerfb200_mc_workspace_bytes.restype = c_size_t
+    lib.nerfb200_mc_count.argtypes = [c_void_p, c_int64, c_int64, c_int64, c_double, c_void_p, c_size_t, POINTER(c_int64),
+                                      c_void_p]
+    lib.nerfb200_mc_emit.argtypes = [c_void_p, c_int64, c_int64, c_int64, c_double, c_void_p, c_size_t, c_void_p, c_void_p,
+                                     c_void_p]
+    lib.nerfb200_mesh_to_world.argtypes = [c_void_p, c_int64, c_int64, POINTER(c_double), c_void_p, c_void_p]
+    lib.nerfb200_mesh_cluster_workspace_bytes.argtypes = [c_int64, c_int64]
+    lib.nerfb200_mesh_cluster_workspace_bytes.restype = c_size_t
+    lib.nerfb200_mesh_cluster_count.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_size_t, POINTER(c_int64), c_void_p]
+    lib.nerfb200_mesh_cluster_emit.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_size_t, c_void_p, c_void_p,
+                                               c_void_p]
+    lib.nerfb200_remap_bilinear.argtypes = [c_u8p, c_int32, c_int32, c_void_p, c_int64, c_u8p, c_void_p]
+    lib.nerfb200_color_project.argtypes = [c_void_p, c_int64, POINTER(c_double), POINTER(c_float), c_float, c_int32,
+                                           c_int32, c_u8p, c_float, c_u8p, c_void_p, c_void_p, c_void_p]
+    lib.nerfb200_color_accumulate.argtypes = [c_u8p, c_void_p, c_void_p, c_int64, c_float, c_void_p, c_void_p]
+    lib.nerfb200_color_finalize.argtypes = [c_void_p, c_int64, c_u8p, c_void_p]
+    for name in ("nerfb200_grid_positions", "nerfb200_sigma_grid", "nerfb200_mc_count", "nerfb200_mc_emit",
+                 "nerfb200_mesh_to_world", "nerfb200_mesh_cluster_count", "nerfb200_mesh_cluster_emit",
+                 "nerfb200_remap_bilinear", "nerfb200_color_project", "nerfb200_color_accumulate",
+                 "nerfb200_color_finalize"):
+        getattr(lib, name).restype = c_int32
     for name in ("nerfb200_pack_weights", "nerfb200_pack_weights_pair", "nerfb200_render_rays", "nerfb200_render_rays_host",
                  "nerfb200_nerf_forward", "nerfb200_embed", "nerfb200_searchsorted",
                  "nerfb200_sample_pdf", "nerfb200_composite"):

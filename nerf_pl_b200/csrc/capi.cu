@@ -10,6 +10,9 @@
 #include "../../include/nerf_pl_b200.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
+#include "mesh_kernels.cuh"
+
+#include <thrust/iterator/transform_iterator.h>
 
 using namespace nerfb200;
 
@@ -1328,5 +1331,368 @@ int nerfb200_check_status(void) {
   return check_sticky_status(d);
 }
 
+
+}  // extern "C"
+
+// ---- coloured mesh extraction (extract_color_mesh.py; kernels: mesh_kernels.cuh) --------------------
+namespace {
+
+size_t align256(size_t x) { return (x + 255) & ~static_cast<size_t>(255); }
+
+struct U8ToInt {
+  __host__ __device__ __forceinline__ int operator()(uint8_t v) const { return v; }
+};
+using U8It = thrust::transform_iterator<U8ToInt, const uint8_t*, int>;
+
+// grid-stride launches: one wave of 8 CTAs per SM, capped by NERFB200_MAX_CTAS (the results do not depend on it)
+int mesh_blocks(long long n) {
+  long long b = (n + 255) / 256;
+  if (b > 148 * 8) b = 148 * 8;
+  const int cap = env_switches().max_ctas;
+  if (cap > 0 && b > cap) b = cap;
+  return static_cast<int>(b < 1 ? 1 : b);
+}
+
+constexpr long long kMcMaxPoints = 400LL * 1000 * 1000;   // keeps 3 P vertices and 5 C triangles in int32
+
+struct McLayout {
+  size_t vcnt, vofs, ccnt, cofs, temp, temp_bytes, bytes;
+};
+McLayout mc_layout(long long P, long long C) {
+  size_t t1 = 0, t2 = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, t1, U8It(nullptr, U8ToInt()), static_cast<int*>(nullptr), static_cast<int>(P + 1));
+  cub::DeviceScan::ExclusiveSum(nullptr, t2, U8It(nullptr, U8ToInt()), static_cast<int*>(nullptr), static_cast<int>(C + 1));
+  McLayout L;
+  size_t o = 0;
+  L.vcnt = o; o += align256(P + 1);
+  L.vofs = o; o += align256((P + 1) * sizeof(int));
+  L.ccnt = o; o += align256(C + 1);
+  L.cofs = o; o += align256((C + 1) * sizeof(int));
+  L.temp = o; L.temp_bytes = t1 > t2 ? t1 : t2; o += align256(L.temp_bytes);
+  L.bytes = o;
+  return L;
+}
+
+int mc_prepare(const float* sigma, int64_t n0, int64_t n1, int64_t n2, double thr, void* ws, size_t bytes, McParams* p,
+               McLayout* L, const char* who) {
+  if (n0 < 2 || n1 < 2 || n2 < 2) return fail(NERFB200_EINVAL, "%s: every grid dimension must be >= 2", who);
+  if (n0 * n1 * n2 > kMcMaxPoints) return fail(NERFB200_EUNSUPPORTED, "%s: grid larger than 4e8 points", who);
+  if (!sigma || !ws) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  const long long P = n0 * n1 * n2, C = (n0 - 1) * (n1 - 1) * (n2 - 1);
+  *L = mc_layout(P, C);
+  if (bytes < L->bytes) return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_mc_workspace_bytes", who);
+  char* w = static_cast<char*>(ws);
+  p->sigma = sigma; p->n0 = n0; p->n1 = n1; p->n2 = n2; p->thr = thr;
+  p->vcnt = reinterpret_cast<uint8_t*>(w + L->vcnt);
+  p->vofs = reinterpret_cast<int*>(w + L->vofs);
+  p->ccnt = reinterpret_cast<uint8_t*>(w + L->ccnt);
+  p->cofs = reinterpret_cast<int*>(w + L->cofs);
+  p->vertices = nullptr; p->triangles = nullptr;
+  return 0;
+}
+
+struct ClusterLayout {
+  size_t keys, keys_alt, vals, vals_alt, parent, count, best, tflag, tofs, vflag, vofs, temp, temp_bytes, bytes;
+};
+int bits_for(long long v) {
+  int b = 1;
+  while ((1LL << b) < v) ++b;
+  return b;
+}
+ClusterLayout cluster_layout(long long V, long long T) {
+  const long long E = 3 * T;
+  size_t t1 = 0, t2 = 0, t3 = 0;
+  cub::DoubleBuffer<unsigned long long> kb(nullptr, nullptr);
+  cub::DoubleBuffer<int> vb(nullptr, nullptr);
+  cub::DeviceRadixSort::SortPairs(nullptr, t1, kb, vb, static_cast<int>(E), 0, 2 * bits_for(V));
+  cub::DeviceScan::ExclusiveSum(nullptr, t2, U8It(nullptr, U8ToInt()), static_cast<int*>(nullptr), static_cast<int>(T + 1));
+  cub::DeviceScan::ExclusiveSum(nullptr, t3, U8It(nullptr, U8ToInt()), static_cast<int*>(nullptr), static_cast<int>(V + 1));
+  ClusterLayout L;
+  size_t o = 0;
+  L.keys = o; o += align256(E * 8);
+  L.keys_alt = o; o += align256(E * 8);
+  L.vals = o; o += align256(E * 4);
+  L.vals_alt = o; o += align256(E * 4);
+  L.parent = o; o += align256(T * 4);
+  L.count = o; o += align256(T * 4);
+  L.best = o; o += 256;
+  L.tflag = o; o += align256(T + 1);
+  L.tofs = o; o += align256((T + 1) * 4);
+  L.vflag = o; o += align256(V + 1);
+  L.vofs = o; o += align256((V + 1) * 4);
+  size_t tb = t1 > t2 ? t1 : t2;
+  tb = tb > t3 ? tb : t3;
+  L.temp = o; L.temp_bytes = tb; o += align256(tb);
+  L.bytes = o;
+  return L;
+}
+
+int cluster_prepare(const int32_t* tris, int64_t n_tris, int64_t n_verts, void* ws, size_t bytes, ClusterParams* p,
+                    ClusterLayout* L, const char* who) {
+  if (n_tris < 0 || n_verts < 0 || n_tris > 0x7fffffffLL / 3 || n_verts > 0x7fffffffLL)
+    return fail(NERFB200_EINVAL, "%s: bad mesh size", who);
+  if (n_tris > 0 && (!tris || !ws)) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  *L = cluster_layout(n_verts, n_tris);
+  if (n_tris > 0 && bytes < L->bytes) return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_mesh_cluster_workspace_bytes", who);
+  char* w = static_cast<char*>(ws);
+  p->tris = tris; p->n_tris = n_tris; p->n_verts = n_verts;
+  p->keys = reinterpret_cast<unsigned long long*>(w + L->keys);
+  p->vals = reinterpret_cast<int*>(w + L->vals);
+  p->parent = reinterpret_cast<int*>(w + L->parent);
+  p->count = reinterpret_cast<int*>(w + L->count);
+  p->best = reinterpret_cast<unsigned long long*>(w + L->best);
+  p->tflag = reinterpret_cast<uint8_t*>(w + L->tflag);
+  p->tofs = reinterpret_cast<int*>(w + L->tofs);
+  p->vflag = reinterpret_cast<uint8_t*>(w + L->vflag);
+  p->vofs = reinterpret_cast<int*>(w + L->vofs);
+  p->vin = nullptr; p->vout = nullptr; p->tout = nullptr;
+  return 0;
+}
+
+__global__ void cluster_pack_keys_kernel(unsigned long long* keys, long long n, int bits) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long k = keys[t];
+    keys[t] = ((k >> 32) << bits) | (k & 0xffffffffull);
+  }
+}
+
+int read_two_counts(const int* a, const int* b, int64_t counts_host[2], cudaStream_t s, const char* who) {
+  int h[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(&h[0], a, sizeof(int), cudaMemcpyDeviceToHost, s), who);
+  CUDA_TRY(cudaMemcpyAsync(&h[1], b, sizeof(int), cudaMemcpyDeviceToHost, s), who);
+  CUDA_TRY(cudaStreamSynchronize(s), who);
+  counts_host[0] = h[0];
+  counts_host[1] = h[1];
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t nerfb200_sigma_grid_workspace_bytes(int64_t chunk) {
+  return chunk > 0 ? align256(static_cast<size_t>(chunk) * 3 * sizeof(float)) : 0;
+}
+
+int nerfb200_grid_positions(int64_t N, const double ranges_host[6], int64_t start, int64_t count, float* xyz,
+                            void* stream) {
+  if (N < 2 || start < 0 || count < 0 || start + count > N * N * N)
+    return fail(NERFB200_EINVAL, "grid_positions: bad N / start / count%s");
+  if (count == 0) return 0;
+  if (!ranges_host || !xyz) return fail(NERFB200_EINVAL, "grid_positions: NULL argument%s");
+  GridParams p;
+  for (int a = 0; a < 3; ++a) { p.lo[a] = ranges_host[2 * a]; p.hi[a] = ranges_host[2 * a + 1]; }
+  p.N = N; p.start = start; p.count = count; p.xyz = xyz;
+  mesh_grid_positions_kernel<<<mesh_blocks(count), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "grid_positions launch");
+  return 0;
+}
+
+int nerfb200_sigma_grid(const void* packed, int64_t N, const double ranges_host[6], int64_t chunk, void* ws,
+                        size_t bytes, float* sigma, void* stream) {
+  if (N < 2 || chunk <= 0) return fail(NERFB200_EINVAL, "sigma_grid: N < 2 or chunk <= 0%s");
+  if (!packed || !ranges_host || !ws || !sigma) return fail(NERFB200_EINVAL, "sigma_grid: NULL argument%s");
+  if (bytes < nerfb200_sigma_grid_workspace_bytes(chunk))
+    return fail(NERFB200_EINVAL, "sigma_grid: workspace smaller than nerfb200_sigma_grid_workspace_bytes(chunk)%s");
+  float* xyz = static_cast<float*>(ws);
+  const long long total = N * N * N;
+  for (long long s = 0; s < total; s += chunk) {
+    const long long n = total - s < chunk ? total - s : chunk;
+    int rc = nerfb200_grid_positions(N, ranges_host, s, n, xyz, stream);
+    if (rc) return rc;
+    if ((rc = nerfb200_query_sigma(xyz, n, 3, packed, sigma + s, stream)) != 0) return rc;
+    mesh_relu_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(sigma + s, n);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError(), "sigma_grid relu launch");
+  }
+  return 0;
+}
+
+size_t nerfb200_mc_workspace_bytes(int64_t n0, int64_t n1, int64_t n2) {
+  if (n0 < 2 || n1 < 2 || n2 < 2 || n0 * n1 * n2 > kMcMaxPoints) return 0;
+  return mc_layout(n0 * n1 * n2, (n0 - 1) * (n1 - 1) * (n2 - 1)).bytes;
+}
+
+int nerfb200_mc_count(const float* sigma, int64_t n0, int64_t n1, int64_t n2, double threshold, void* ws, size_t bytes,
+                      int64_t counts_host[2], void* stream) {
+  McParams p;
+  McLayout L;
+  int rc = mc_prepare(sigma, n0, n1, n2, threshold, ws, bytes, &p, &L, "mc_count");
+  if (rc) return rc;
+  if (!counts_host) return fail(NERFB200_EINVAL, "mc_count: counts_host is NULL%s");
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long P = n0 * n1 * n2, C = (n0 - 1) * (n1 - 1) * (n2 - 1);
+  CUDA_TRY(cudaMemsetAsync(p.vcnt + P, 0, 1, s), "mc_count memset");
+  CUDA_TRY(cudaMemsetAsync(p.ccnt + C, 0, 1, s), "mc_count memset");
+  mc_classify_kernel<<<mesh_blocks(P), 256, 0, s>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "mc_classify launch");
+  void* temp = static_cast<char*>(ws) + L.temp;
+  size_t tb = L.temp_bytes;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(temp, tb, U8It(p.vcnt, U8ToInt()), p.vofs, static_cast<int>(P + 1), s), "mc vertex scan");
+  tb = L.temp_bytes;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(temp, tb, U8It(p.ccnt, U8ToInt()), p.cofs, static_cast<int>(C + 1), s), "mc triangle scan");
+  g_launches += 2;
+  return read_two_counts(p.vofs + P, p.cofs + C, counts_host, s, "mc_count readback");
+}
+
+int nerfb200_mc_emit(const float* sigma, int64_t n0, int64_t n1, int64_t n2, double threshold, void* ws, size_t bytes,
+                     double* vertices, int32_t* triangles, void* stream) {
+  McParams p;
+  McLayout L;
+  int rc = mc_prepare(sigma, n0, n1, n2, threshold, ws, bytes, &p, &L, "mc_emit");
+  if (rc) return rc;
+  p.vertices = vertices;
+  p.triangles = triangles;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long P = n0 * n1 * n2, C = (n0 - 1) * (n1 - 1) * (n2 - 1);
+  if (vertices) {
+    mc_emit_vertices_kernel<<<mesh_blocks(P), 256, 0, s>>>(p);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError(), "mc_emit_vertices launch");
+  }
+  if (triangles) {
+    mc_emit_triangles_kernel<<<mesh_blocks(C), 256, 0, s>>>(p);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError(), "mc_emit_triangles launch");
+  }
+  return 0;
+}
+
+int nerfb200_mesh_to_world(const double* vertices, int64_t n, int64_t N, const double ranges_host[6], float* out,
+                           void* stream) {
+  if (n < 0 || N < 1) return fail(NERFB200_EINVAL, "mesh_to_world: bad n / N%s");
+  if (n == 0) return 0;
+  if (!vertices || !ranges_host || !out) return fail(NERFB200_EINVAL, "mesh_to_world: NULL argument%s");
+  ToWorldParams p;
+  p.v = vertices; p.n = n; p.N = static_cast<double>(N); p.out = out;
+  // column 0 takes y_range, column 1 x_range (extract_color_mesh.py:150-151)
+  const int src[3] = {1, 0, 2};
+  for (int c = 0; c < 3; ++c) {
+    const double lo = ranges_host[2 * src[c]], hi = ranges_host[2 * src[c] + 1];
+    p.scale[c] = static_cast<float>(hi - lo);
+    p.offset[c] = static_cast<float>(lo);
+  }
+  mesh_to_world_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "mesh_to_world launch");
+  return 0;
+}
+
+size_t nerfb200_mesh_cluster_workspace_bytes(int64_t n_vertices, int64_t n_triangles) {
+  if (n_vertices < 0 || n_triangles <= 0 || n_triangles > 0x7fffffffLL / 3 || n_vertices > 0x7fffffffLL) return 0;
+  return cluster_layout(n_vertices, n_triangles).bytes;
+}
+
+int nerfb200_mesh_cluster_count(const int32_t* triangles, int64_t n_tris, int64_t n_verts, void* ws, size_t bytes,
+                                int64_t counts_host[2], void* stream) {
+  ClusterParams p;
+  ClusterLayout L;
+  int rc = cluster_prepare(triangles, n_tris, n_verts, ws, bytes, &p, &L, "mesh_cluster_count");
+  if (rc) return rc;
+  if (!counts_host) return fail(NERFB200_EINVAL, "mesh_cluster_count: counts_host is NULL%s");
+  if (n_tris == 0) { counts_host[0] = counts_host[1] = 0; return 0; }
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  char* w = static_cast<char*>(ws);
+  const long long E = 3 * n_tris;
+  const int bits = bits_for(n_verts);
+  cluster_edges_kernel<<<mesh_blocks(n_tris), 256, 0, s>>>(p);
+  cluster_pack_keys_kernel<<<mesh_blocks(E), 256, 0, s>>>(p.keys, E, bits);
+  g_launches += 2;
+  CUDA_TRY(cudaGetLastError(), "cluster edges launch");
+  cub::DoubleBuffer<unsigned long long> kb(p.keys, reinterpret_cast<unsigned long long*>(w + L.keys_alt));
+  cub::DoubleBuffer<int> vb(p.vals, reinterpret_cast<int*>(w + L.vals_alt));
+  size_t tb = L.temp_bytes;
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(w + L.temp, tb, kb, vb, static_cast<int>(E), 0, 2 * bits, s), "cluster edge sort");
+  g_launches++;
+  p.keys = kb.Current();
+  p.vals = vb.Current();
+  CUDA_TRY(cudaMemsetAsync(p.best, 0, sizeof(unsigned long long), s), "cluster memset");
+  CUDA_TRY(cudaMemsetAsync(p.vflag, 0, n_verts + 1, s), "cluster memset");
+  CUDA_TRY(cudaMemsetAsync(p.tflag + n_tris, 0, 1, s), "cluster memset");
+  cluster_union_kernel<<<mesh_blocks(E), 256, 0, s>>>(p);
+  cluster_label_kernel<<<mesh_blocks(n_tris), 256, 0, s>>>(p);
+  cluster_best_kernel<<<mesh_blocks(n_tris), 256, 0, s>>>(p);
+  cluster_flag_kernel<<<mesh_blocks(n_tris), 256, 0, s>>>(p);
+  g_launches += 4;
+  CUDA_TRY(cudaGetLastError(), "cluster union-find launch");
+  tb = L.temp_bytes;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(w + L.temp, tb, U8It(p.tflag, U8ToInt()), p.tofs, static_cast<int>(n_tris + 1), s),
+           "cluster triangle scan");
+  tb = L.temp_bytes;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(w + L.temp, tb, U8It(p.vflag, U8ToInt()), p.vofs, static_cast<int>(n_verts + 1), s),
+           "cluster vertex scan");
+  g_launches += 2;
+  return read_two_counts(p.vofs + n_verts, p.tofs + n_tris, counts_host, s, "mesh_cluster_count readback");
+}
+
+int nerfb200_mesh_cluster_emit(const float* vertices, const int32_t* triangles, int64_t n_tris, int64_t n_verts, void* ws,
+                               size_t bytes, float* vertices_out, int32_t* triangles_out, void* stream) {
+  ClusterParams p;
+  ClusterLayout L;
+  int rc = cluster_prepare(triangles, n_tris, n_verts, ws, bytes, &p, &L, "mesh_cluster_emit");
+  if (rc) return rc;
+  if (n_tris == 0) return 0;
+  if (!vertices || !vertices_out || !triangles_out) return fail(NERFB200_EINVAL, "mesh_cluster_emit: NULL argument%s");
+  p.vin = vertices; p.vout = vertices_out; p.tout = triangles_out;
+  const long long n = n_tris > n_verts ? n_tris : n_verts;
+  cluster_emit_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "mesh_cluster_emit launch");
+  return 0;
+}
+
+int nerfb200_remap_bilinear(const uint8_t* image, int32_t H, int32_t W, const float* xy, int64_t n, uint8_t* out,
+                            void* stream) {
+  if (H <= 0 || W <= 0 || n < 0) return fail(NERFB200_EINVAL, "remap_bilinear: bad H / W / n%s");
+  if (n == 0) return 0;
+  if (!image || !xy || !out) return fail(NERFB200_EINVAL, "remap_bilinear: NULL argument%s");
+  remap_bilinear_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(image, H, W, xy, n, out);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "remap_bilinear launch");
+  return 0;
+}
+
+int nerfb200_color_project(const float* vertices, int64_t n, const double w2c_host[12], const float origin_host[3],
+                           float focal, int32_t W, int32_t H, const uint8_t* image, float near, uint8_t* colors,
+                           double* depth, float* rays, void* stream) {
+  if (n < 0 || H <= 0 || W <= 0) return fail(NERFB200_EINVAL, "color_project: bad n / H / W%s");
+  if (n == 0) return 0;
+  if (!vertices || !w2c_host || !origin_host || !image || !colors || !depth || !rays)
+    return fail(NERFB200_EINVAL, "color_project: NULL argument%s");
+  ColorProjectParams p;
+  p.vertices = vertices; p.n = n;
+  for (int i = 0; i < 12; ++i) p.w2c[i] = w2c_host[i];
+  for (int i = 0; i < 3; ++i) p.origin[i] = origin_host[i];
+  p.focal = focal; p.W = W; p.H = H; p.image = image; p.near = near;
+  p.colors = colors; p.depth = depth; p.rays = rays;
+  color_project_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "color_project launch");
+  return 0;
+}
+
+int nerfb200_color_accumulate(const uint8_t* colors, const double* depth, const float* opacity, int64_t n,
+                              float occ_threshold, double* sum4, void* stream) {
+  if (n < 0) return fail(NERFB200_EINVAL, "color_accumulate: n < 0%s");
+  if (n == 0) return 0;
+  if (!colors || !depth || !opacity || !sum4) return fail(NERFB200_EINVAL, "color_accumulate: NULL argument%s");
+  color_accumulate_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(colors, depth, opacity, n,
+                                                                                          occ_threshold, sum4);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "color_accumulate launch");
+  return 0;
+}
+
+int nerfb200_color_finalize(const double* sum4, int64_t n, uint8_t* colors, void* stream) {
+  if (n < 0) return fail(NERFB200_EINVAL, "color_finalize: n < 0%s");
+  if (n == 0) return 0;
+  if (!sum4 || !colors) return fail(NERFB200_EINVAL, "color_finalize: NULL argument%s");
+  color_finalize_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(sum4, n, colors);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "color_finalize launch");
+  return 0;
+}
 
 }  // extern "C"

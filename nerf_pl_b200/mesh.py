@@ -1,0 +1,264 @@
+"""Coloured mesh extraction on the device (the reference's ``extract_color_mesh.py``, ``README_mesh.md``).
+
+sigma grid -> marching cubes -> index-to-world transform -> largest cluster -> occlusion-aware vertex
+colours, every stage an sm_90a kernel of ``libnerf_pl_b200.so`` (csrc/mesh_kernels.cuh); the grid query and
+the occlusion renders run the existing fused MLP / render launches.  Replaces PyMCubes
+(``mcubes.marching_cubes``), open3d (``cluster_connected_triangles`` + ``remove_unreferenced_vertices``),
+``cv2.remap`` and the numpy projection loop; ``write_ply`` writes what plyfile wrote.  Conventions and the
+reference's quirks that are kept: DESIGN.md "Coloured mesh extraction".
+"""
+from __future__ import annotations
+
+import ctypes
+from typing import Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from . import _lib
+from .nerf import Embedding, _stream_ptr, packed_weights
+from .rendering import render_rays
+
+
+def _ranges(x_range, y_range, z_range):
+    vals = [float(v) for r in (x_range, y_range, z_range) for v in r]
+    if len(vals) != 6:
+        raise ValueError("x_range, y_range and z_range must each be (min, max)")
+    return (ctypes.c_double * 6)(*vals)
+
+
+def _device_of(model: torch.nn.Module) -> torch.device:
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("nerf_pl_b200.mesh runs on CUDA only (no CPU fallback)")
+    return dev
+
+
+def _cuda(t: torch.Tensor, what: str) -> torch.Tensor:
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise RuntimeError(f"{what} must be a CUDA tensor (nerf_pl_b200 has no CPU fallback)")
+    return t
+
+
+def _workspace(nbytes: int, device) -> torch.Tensor:
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
+@torch.no_grad()
+def grid_positions(N: int, x_range, y_range, z_range, start: int = 0, count: Optional[int] = None,
+                   device=None) -> torch.Tensor:
+    """Points [start, start+count) of ``torch.FloatTensor(np.stack(np.meshgrid(x, y, z), -1).reshape(-1, 3))``
+    with ``x = np.linspace(*x_range, N)`` etc. (extract_color_mesh.py:119-123), built on the device."""
+    device = torch.device("cuda") if device is None else torch.device(device)
+    count = N ** 3 - start if count is None else count
+    out = torch.empty(count, 3, dtype=torch.float32, device=device)
+    lib = _lib.load()
+    with torch.cuda.device(device):
+        _lib.check(lib.nerfb200_grid_positions(N, _ranges(x_range, y_range, z_range), start, count, out.data_ptr(),
+                                               _stream_ptr()), "nerfb200_grid_positions")
+    return out
+
+
+@torch.no_grad()
+def sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk: int = 1 << 21) -> torch.Tensor:
+    """(N, N, N) fp32 ``max(sigma, 0)`` of ``model`` on the reference's grid (extract_color_mesh.py:113-140):
+    ``sigma[i, j, k] = max(sigma(x_j, y_i, z_k), 0)`` (np.meshgrid's 'xy' indexing).  ``chunk`` points are
+    queried per launch; the scratch is their positions only."""
+    dev = _device_of(model)
+    out = torch.empty(N, N, N, dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    blob = packed_weights(model)
+    chunk = int(min(chunk, N ** 3))
+    ws = _workspace(lib.nerfb200_sigma_grid_workspace_bytes(chunk), dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.nerfb200_sigma_grid(blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk, ws.data_ptr(),
+                                           ws.numel(), out.data_ptr(), _stream_ptr()), "nerfb200_sigma_grid")
+    return out
+
+
+@torch.no_grad()
+def marching_cubes(sigma: torch.Tensor, threshold: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Drop-in for ``mcubes.marching_cubes(sigma, threshold)`` on a CUDA (n0, n1, n2) grid: index-space
+    vertices (V, 3) float64 and triangles (T, 3) int32, on the device.  Inside is ``sigma > threshold``;
+    normals point from inside to outside; the order is fixed (DESIGN.md)."""
+    s = _cuda(sigma, "sigma").detach().to(torch.float32).contiguous()
+    if s.dim() != 3:
+        raise ValueError("sigma must be a 3-D grid")
+    n0, n1, n2 = s.shape
+    lib = _lib.load()
+    nbytes = lib.nerfb200_mc_workspace_bytes(n0, n1, n2)
+    if nbytes == 0:
+        raise ValueError(f"marching_cubes: unsupported grid shape {tuple(s.shape)}")
+    ws = _workspace(nbytes, s.device)
+    counts = (ctypes.c_int64 * 2)()
+    with torch.cuda.device(s.device):
+        _lib.check(lib.nerfb200_mc_count(s.data_ptr(), n0, n1, n2, float(threshold), ws.data_ptr(), ws.numel(), counts,
+                                         _stream_ptr()), "nerfb200_mc_count")
+        verts = torch.empty(counts[0], 3, dtype=torch.float64, device=s.device)
+        tris = torch.empty(counts[1], 3, dtype=torch.int32, device=s.device)
+        _lib.check(lib.nerfb200_mc_emit(s.data_ptr(), n0, n1, n2, float(threshold), ws.data_ptr(), ws.numel(),
+                                        verts.data_ptr() if counts[0] else None, tris.data_ptr() if counts[1] else None,
+                                        _stream_ptr()), "nerfb200_mc_emit")
+    return verts, tris
+
+
+@torch.no_grad()
+def to_world(vertices: torch.Tensor, N: int, x_range, y_range, z_range) -> torch.Tensor:
+    """extract_color_mesh.py:148-154 on the device, quirks included: divides by N (not N - 1) and swaps the
+    x / y ranges (x takes y_range)."""
+    v = _cuda(vertices, "vertices").detach().to(torch.float64).contiguous()
+    out = torch.empty(v.shape[0], 3, dtype=torch.float32, device=v.device)
+    lib = _lib.load()
+    with torch.cuda.device(v.device):
+        _lib.check(lib.nerfb200_mesh_to_world(v.data_ptr(), v.shape[0], N, _ranges(x_range, y_range, z_range),
+                                              out.data_ptr(), _stream_ptr()), "nerfb200_mesh_to_world")
+    return out
+
+
+@torch.no_grad()
+def keep_largest_cluster(vertices: torch.Tensor, triangles: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """extract_color_mesh.py:163-171: the edge-connected component with the most triangles (ties: the one
+    holding the lowest-indexed triangle), unreferenced vertices removed, order kept."""
+    v = _cuda(vertices, "vertices").detach().to(torch.float32).contiguous()
+    t = _cuda(triangles, "triangles").detach().to(torch.int32).contiguous()
+    if t.shape[0] == 0:
+        return v[:0], t[:0]
+    lib = _lib.load()
+    ws = _workspace(lib.nerfb200_mesh_cluster_workspace_bytes(v.shape[0], t.shape[0]), v.device)
+    counts = (ctypes.c_int64 * 2)()
+    with torch.cuda.device(v.device):
+        _lib.check(lib.nerfb200_mesh_cluster_count(t.data_ptr(), t.shape[0], v.shape[0], ws.data_ptr(), ws.numel(),
+                                                   counts, _stream_ptr()), "nerfb200_mesh_cluster_count")
+        vo = torch.empty(counts[0], 3, dtype=torch.float32, device=v.device)
+        to = torch.empty(counts[1], 3, dtype=torch.int32, device=v.device)
+        _lib.check(lib.nerfb200_mesh_cluster_emit(v.data_ptr(), t.data_ptr(), t.shape[0], v.shape[0], ws.data_ptr(),
+                                                  ws.numel(), vo.data_ptr(), to.data_ptr(), _stream_ptr()),
+                   "nerfb200_mesh_cluster_emit")
+    return vo, to
+
+
+@torch.no_grad()
+def extract_mesh(model: torch.nn.Module, N_grid: int, x_range, y_range, z_range, sigma_threshold: float,
+                 keep_largest: bool = True) -> Tuple[torch.Tensor, torch.Tensor]:
+    """extract_color_mesh.py:113-171: world vertices (V, 3) fp32 and triangles (T, 3) int32 on the device."""
+    sigma = sigma_grid(model, N_grid, x_range, y_range, z_range)
+    vidx, tris = marching_cubes(sigma, sigma_threshold)
+    del sigma
+    verts = to_world(vidx, N_grid, x_range, y_range, z_range)
+    if keep_largest:
+        verts, tris = keep_largest_cluster(verts, tris)
+    return verts, tris
+
+
+@torch.no_grad()
+def remap_bilinear(image: torch.Tensor, xy: torch.Tensor) -> torch.Tensor:
+    """``cv2.remap(image, xy[:, 0], xy[:, 1], cv2.INTER_LINEAR)`` (constant 0 border) of a CUDA (H, W, 3) uint8
+    image at (n, 2) fp32 points -> (n, 3) uint8."""
+    img = _cuda(image, "image").contiguous()
+    if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
+        raise ValueError("image must be (H, W, 3) uint8")
+    p = _cuda(xy, "xy").detach().to(torch.float32).contiguous()
+    out = torch.empty(p.shape[0], 3, dtype=torch.uint8, device=img.device)
+    lib = _lib.load()
+    with torch.cuda.device(img.device):
+        _lib.check(lib.nerfb200_remap_bilinear(img.data_ptr(), img.shape[0], img.shape[1], p.data_ptr(), p.shape[0],
+                                               out.data_ptr(), _stream_ptr()), "nerfb200_remap_bilinear")
+    return out
+
+
+def w2c_of(pose) -> np.ndarray:
+    """extract_color_mesh.py:220-221: ``np.linalg.inv([[c2w], [0, 0, 0, 1]])[:3]`` in float64."""
+    c2w = np.asarray(pose.detach().cpu().numpy() if isinstance(pose, torch.Tensor) else pose, dtype=np.float64)
+    return np.linalg.inv(np.concatenate([c2w.reshape(3, 4), np.array([[0, 0, 0, 1.0]])], 0))[:3]
+
+
+@torch.no_grad()
+def project_view(vertices: torch.Tensor, image: torch.Tensor, pose, focal: float, near: float):
+    """One view of extract_color_mesh.py:215-262: (colours (V, 3) uint8, depth (V) fp64, occlusion rays (V, 8))."""
+    v = _cuda(vertices, "vertices")
+    H, W = image.shape[0], image.shape[1]
+    c2w = np.asarray(pose.detach().cpu().numpy() if isinstance(pose, torch.Tensor) else pose, dtype=np.float64)
+    w2c = (ctypes.c_double * 12)(*w2c_of(c2w).reshape(-1).tolist())
+    origin = (ctypes.c_float * 3)(*np.asarray(c2w.reshape(3, 4)[:, 3], dtype=np.float32).tolist())
+    n = v.shape[0]
+    colors = torch.empty(n, 3, dtype=torch.uint8, device=v.device)
+    depth = torch.empty(n, dtype=torch.float64, device=v.device)
+    rays = torch.empty(n, 8, dtype=torch.float32, device=v.device)
+    lib = _lib.load()
+    with torch.cuda.device(v.device):
+        _lib.check(lib.nerfb200_color_project(v.data_ptr(), n, w2c, origin, float(focal), W, H, image.data_ptr(),
+                                              float(near), colors.data_ptr(), depth.data_ptr(), rays.data_ptr(),
+                                              _stream_ptr()), "nerfb200_color_project")
+    return colors, depth, rays
+
+
+@torch.no_grad()
+def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: torch.Tensor, poses: Sequence,
+                       focal: float, near: float, N_samples: int = 64, occ_threshold: float = 0.2,
+                       white_back: bool = False, return_opacities: bool = False):
+    """extract_color_mesh.py:206-284 (the default colour-averaging method) on the device.
+
+    vertices (V, 3) fp32 world; images (n_views, H, W, 3) uint8 CUDA; poses: n_views (3, 4) camera-to-world;
+    focal: the dataset focal (K is float32 with principal point (W/2, H/2)); near: ``dataset.bounds.min()``.
+    Per view: project + bilinear sample + occlusion rays, the fused ``render_rays`` with ``model`` as the only
+    network (N_importance = 0, test_time), and a float64 accumulation in view order.  Returns (V, 3) uint8
+    (and the per-view opacities (n_views, V) when ``return_opacities``)."""
+    v = _cuda(vertices, "vertices").detach().to(torch.float32).contiguous()
+    imgs = _cuda(images, "images").contiguous()
+    if imgs.dtype != torch.uint8 or imgs.dim() != 4 or imgs.shape[3] != 3:
+        raise ValueError("images must be (n_views, H, W, 3) uint8")
+    if len(poses) != imgs.shape[0]:
+        raise ValueError("one pose per image")
+    n = v.shape[0]
+    sum4 = torch.zeros(n, 4, dtype=torch.float64, device=v.device)
+    emb = [Embedding(3, 10), Embedding(3, 4)]
+    lib = _lib.load()
+    opac = []
+    for idx in range(imgs.shape[0]):
+        colors, depth, rays = project_view(v, imgs[idx], poses[idx], focal, near)
+        res = render_rays([model], emb, rays, N_samples, False, 0, 0, 0, 1024 * 32, white_back, test_time=True,
+                          match_reference_rng=False)
+        opacity = res["opacity_coarse"].contiguous()
+        if return_opacities:
+            opac.append(opacity)
+        with torch.cuda.device(v.device):
+            _lib.check(lib.nerfb200_color_accumulate(colors.data_ptr(), depth.data_ptr(), opacity.data_ptr(), n,
+                                                     float(np.float32(occ_threshold)), sum4.data_ptr(), _stream_ptr()),
+                       "nerfb200_color_accumulate")
+    out = torch.empty(n, 3, dtype=torch.uint8, device=v.device)
+    with torch.cuda.device(v.device):
+        _lib.check(lib.nerfb200_color_finalize(sum4.data_ptr(), n, out.data_ptr(), _stream_ptr()),
+                   "nerfb200_color_finalize")
+    if return_opacities:
+        return out, (torch.stack(opac) if opac else torch.empty(0, n, device=v.device))
+    return out
+
+
+def write_ply(path: str, vertices, triangles, colors=None) -> None:
+    """The binary little-endian PLY plyfile writes at extract_color_mesh.py:286-297: element ``vertex`` with
+    float ``x y z`` (and uchar ``red green blue``), element ``face`` with ``list uchar int vertex_indices``."""
+    def host(a):
+        return a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+
+    v = host(vertices).astype(np.float32).reshape(-1, 3)
+    t = host(triangles).astype(np.int32).reshape(-1, 3)
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if colors is not None:
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    vert = np.empty(len(v), dtype=fields)
+    vert["x"], vert["y"], vert["z"] = v[:, 0], v[:, 1], v[:, 2]
+    if colors is not None:
+        c = host(colors).astype(np.uint8).reshape(-1, 3)
+        vert["red"], vert["green"], vert["blue"] = c[:, 0], c[:, 1], c[:, 2]
+    face = np.empty(len(t), dtype=[("n", "u1"), ("vertex_indices", "<i4", (3,))])
+    face["n"] = 3
+    face["vertex_indices"] = t
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}"]
+    head += [f"property float {k}" for k in ("x", "y", "z")]
+    if colors is not None:
+        head += [f"property uchar {k}" for k in ("red", "green", "blue")]
+    head += [f"element face {len(t)}", "property list uchar int vertex_indices", "end_header"]
+    with open(path, "wb") as f:
+        f.write(("\n".join(head) + "\n").encode("ascii"))
+        f.write(vert.tobytes())
+        f.write(face.tobytes())
