@@ -285,6 +285,28 @@ size_t nerfb200_sigma_grid_workspace_bytes(int64_t chunk);
 int nerfb200_sigma_grid(const void* packed, int64_t N, const double ranges_host[6], int64_t chunk, void* ws,
                         size_t bytes, float* sigma, void* stream);
 
+/* extract_mesh.ipynb "Search for tight bounds": nerf_fine(cat(embedding_xyz(xyz), embedding_dir(0))) at raw
+ * positions xyz (n rows of xyz_stride >= 3 floats, encoded in-kernel) with the direction (0, 0, 0):
+ * rgbsigma (n, 4) [sigmoid rgb, raw sigma], 16-byte aligned.  Bit for bit NeRF.forward on the same fp16 xyz
+ * encoding followed by the embedded zero direction. */
+int nerfb200_query_rgb_sigma(const float* xyz, int64_t n, int64_t xyz_stride, const void* packed, float* rgbsigma,
+                             void* stream);
+/* The whole grid of nerfb200_grid_positions, `chunk` points at a time: rgbsigma (N, N, N, 4), raw sigma
+ * (no max(sigma, 0)).  Workspace: nerfb200_sigma_grid_workspace_bytes(chunk).  2 <= N <= 1625. */
+int nerfb200_rgb_sigma_grid(const void* packed, int64_t N, const double ranges_host[6], int64_t chunk, void* ws,
+                            size_t bytes, float* rgbsigma, void* stream);
+
+/* extract_mesh.ipynb "Generate .vol file for volume rendering in Unity" on a (N^3, 4) rgbsigma grid (16-byte
+ * aligned, raw sigma, point (i*N + j)*N + k): a = 1 - exp(float32(-(xmax - xmin)/N) * max(sigma, 0)) in float32
+ * (exp correctly rounded); the points with a > 0 in increasing order as (M, 2) uint32 pairs
+ * [i, r << 24 + g << 16 + b << 8 + trunc(a * 255)], r = trunc(rgb * 255).  2 <= N <= 1625 (uint32 indices).
+ * count_host = M; the emit call takes the same workspace. */
+size_t nerfb200_volume_workspace_bytes(int64_t N);
+int nerfb200_volume_count(const float* rgbsigma, int64_t N, double xmin, double xmax, void* ws, size_t bytes,
+                          int64_t* count_host, void* stream);
+int nerfb200_volume_emit(const float* rgbsigma, int64_t N, double xmin, double xmax, void* ws, size_t bytes,
+                         uint32_t* packed_out, void* stream);
+
 /* extract_color_mesh.py:144 mcubes.marching_cubes(sigma, threshold) on a C-order (n0, n1, n2) fp32 grid.
  * Inside: sigma > threshold.  counts_host[2] = {vertices, triangles}.  vertices (V, 3) fp64 in index
  * space, ordered by the lower endpoint's linear index then edge axis; triangles (T, 3) int32 ordered by

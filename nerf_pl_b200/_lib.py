@@ -71,6 +71,11 @@ EXPORTS = [
     "nerfb200_color_project",
     "nerfb200_color_accumulate",
     "nerfb200_color_finalize",
+    "nerfb200_query_rgb_sigma",
+    "nerfb200_rgb_sigma_grid",
+    "nerfb200_volume_workspace_bytes",
+    "nerfb200_volume_count",
+    "nerfb200_volume_emit",
 ]
 
 class RenderArgs(ctypes.Structure):
@@ -240,10 +245,20 @@ def _declare(lib: ctypes.CDLL) -> None:
                                            c_int32, c_u8p, c_float, c_u8p, c_void_p, c_void_p, c_void_p]
     lib.nerfb200_color_accumulate.argtypes = [c_u8p, c_void_p, c_void_p, c_int64, c_float, c_void_p, c_void_p]
     lib.nerfb200_color_finalize.argtypes = [c_void_p, c_int64, c_u8p, c_void_p]
+    # Unity volume (.vol)
+    lib.nerfb200_query_rgb_sigma.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]
+    lib.nerfb200_rgb_sigma_grid.argtypes = [c_void_p, c_int64, POINTER(c_double), c_int64, c_void_p, c_size_t,
+                                            c_void_p, c_void_p]
+    lib.nerfb200_volume_workspace_bytes.argtypes = [c_int64]
+    lib.nerfb200_volume_workspace_bytes.restype = c_size_t
+    lib.nerfb200_volume_count.argtypes = [c_void_p, c_int64, c_double, c_double, c_void_p, c_size_t, POINTER(c_int64),
+                                          c_void_p]
+    lib.nerfb200_volume_emit.argtypes = [c_void_p, c_int64, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p]
     for name in ("nerfb200_grid_positions", "nerfb200_sigma_grid", "nerfb200_mc_count", "nerfb200_mc_emit",
                  "nerfb200_mesh_to_world", "nerfb200_mesh_cluster_count", "nerfb200_mesh_cluster_emit",
                  "nerfb200_remap_bilinear", "nerfb200_color_project", "nerfb200_color_accumulate",
-                 "nerfb200_color_finalize"):
+                 "nerfb200_color_finalize", "nerfb200_query_rgb_sigma", "nerfb200_rgb_sigma_grid",
+                 "nerfb200_volume_count", "nerfb200_volume_emit"):
         getattr(lib, name).restype = c_int32
     for name in ("nerfb200_pack_weights", "nerfb200_pack_weights_pair", "nerfb200_render_rays", "nerfb200_render_rays_host",
                  "nerfb200_nerf_forward", "nerfb200_embed", "nerfb200_searchsorted",

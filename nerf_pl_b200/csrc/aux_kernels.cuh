@@ -120,8 +120,22 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackParams2 pp2) {
 }
 
 // ------------------------------------------------ NeRF.forward (models/nerf.py:83-124)
+// The row DirSrc reads in raw-position mode with stride 0: 63 unused xyz columns, then Embedding(3, 4) of the
+// direction (0, 0, 0) (extract_mesh.ipynb's dir_ = zeros): [0 0 0, sin 0 x3, cos 0 x3, ...], exactly 0 and 1 in fp16.
+struct ZeroDirRow {
+  float v[kEncXyz + kEncDir];
+};
+constexpr ZeroDirRow make_zero_dir_row() {
+  ZeroDirRow r{};
+  for (int k = 0; k < (kEncDir - 3) / 6; ++k)
+    for (int c = 0; c < 3; ++c) r.v[kEncXyz + 3 + 6 * k + 3 + c] = 1.f;
+  return r;
+}
+__device__ const ZeroDirRow kZeroDirRow = make_zero_dir_row();
+
 struct MlpParams {
-  int raw_xyz;             // 1: x is (n, x_stride>=3) raw positions, encoded in-kernel; sigma only
+  int raw_xyz;             // 1: x is (n, x_stride>=3) raw positions, encoded in-kernel; with sigma_only = 0 the
+                           // direction is (0, 0, 0) (kZeroDirRow)
   const float* x;          // (n, x_stride): embedded xyz (63) [+ embedded dir (27)]
   long long x_stride;
   long long n;
@@ -205,7 +219,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
         fence_proxy_async();
         wg_bar(c);
       }
-      const DirSrc ds{p.x, p.x_stride, tile * 128, p.n, kSave ? p.xdir : nullptr};
+      const DirSrc ds = p.raw_xyz ? DirSrc{kZeroDirRow.v, 0, tile * 128, p.n, nullptr}
+                                  : DirSrc{p.x, p.x_stride, tile * 128, p.n, kSave ? p.xdir : nullptr};
       float sig[2], rgb[2][3];
       if (kSave) {
 #pragma unroll

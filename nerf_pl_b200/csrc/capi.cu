@@ -883,6 +883,32 @@ int nerfb200_query_sigma(const float* xyz, int64_t n, int64_t xyz_stride, const 
   return 0;
 }
 
+int nerfb200_query_rgb_sigma(const float* xyz, int64_t n, int64_t xyz_stride, const void* packed, float* rgbsigma,
+                             void* stream) {
+  if (n < 0) return fail(NERFB200_EINVAL, "query_rgb_sigma: n < 0%s");
+  if (n == 0) return 0;
+  if (!xyz || !packed || !rgbsigma) return fail(NERFB200_EINVAL, "query_rgb_sigma: NULL argument%s");
+  if (xyz_stride < 3) return fail(NERFB200_EINVAL, "query_rgb_sigma: xyz_stride < 3%s");
+  if (reinterpret_cast<uintptr_t>(rgbsigma) & 15) return fail(NERFB200_EINVAL, "query_rgb_sigma: out must be 16-byte aligned%s");
+  DeviceInfo* d = nullptr;
+  int rc = device_info(&d);
+  if (rc) return rc;
+  if ((rc = check_sticky_status(d)) != 0) return rc;
+  MlpParams p;
+  p.raw_xyz = 1;
+  p.x = xyz; p.x_stride = xyz_stride; p.n = n;
+  p.net = static_cast<const uint8_t*>(packed);
+  p.sigma_only = 0;
+  p.out = rgbsigma;
+  p.status = d->status;
+  const long long tiles = (n + 127) / 128;
+  const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
+  mlp_forward_kernel<false><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "query_rgb_sigma launch");
+  return 0;
+}
+
 // ---- training a direct NeRF.forward call (models/nerf.py:83-124)
 size_t nerfb200_nerf_train_workspace_bytes(int64_t n) {
   if (n <= 0 || n > 0x7fffffffLL) return 0;
@@ -1466,6 +1492,45 @@ int read_two_counts(const int* a, const int* b, int64_t counts_host[2], cudaStre
   return 0;
 }
 
+// The .vol indices are uint32 (extract_mesh.ipynb casts them): N^3 < 2^32 up to N = 1625.
+constexpr long long kVolMaxN = 1625;
+
+struct VolumeLayout {
+  long long tiles;
+  size_t tcnt, tofs, temp, temp_bytes, bytes;
+};
+VolumeLayout volume_layout(long long N) {
+  VolumeLayout L;
+  L.tiles = (N * N * N + kVolTile - 1) / kVolTile;
+  size_t tb = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tb, static_cast<const unsigned long long*>(nullptr),
+                                static_cast<unsigned long long*>(nullptr), static_cast<int>(L.tiles + 1));
+  size_t o = 0;
+  L.tcnt = o; o += align256((L.tiles + 1) * sizeof(unsigned long long));
+  L.tofs = o; o += align256((L.tiles + 1) * sizeof(unsigned long long));
+  L.temp = o; L.temp_bytes = tb; o += align256(tb);
+  L.bytes = o;
+  return L;
+}
+
+int volume_prepare(const float* rgbsigma, int64_t N, double xmin, double xmax, void* ws, size_t bytes, VolumeParams* p,
+                   VolumeLayout* L, const char* who) {
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625] (uint32 indices)", who);
+  if (!rgbsigma || !ws) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (reinterpret_cast<uintptr_t>(rgbsigma) & 15) return fail(NERFB200_EINVAL, "%s: rgbsigma must be 16-byte aligned", who);
+  *L = volume_layout(N);
+  if (bytes < L->bytes) return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_volume_workspace_bytes", who);
+  char* w = static_cast<char*>(ws);
+  p->rgbsigma = reinterpret_cast<const float4*>(rgbsigma);
+  p->P = N * N * N;
+  // -(xmax - xmin) / N is a Python float; numpy rounds it to float32 before the multiply
+  p->c = static_cast<float>(-(xmax - xmin) / static_cast<double>(N));
+  p->tcnt = reinterpret_cast<unsigned long long*>(w + L->tcnt);
+  p->tofs = reinterpret_cast<unsigned long long*>(w + L->tofs);
+  p->out = nullptr;
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1506,6 +1571,68 @@ int nerfb200_sigma_grid(const void* packed, int64_t N, const double ranges_host[
     g_launches++;
     CUDA_TRY(cudaGetLastError(), "sigma_grid relu launch");
   }
+  return 0;
+}
+
+int nerfb200_rgb_sigma_grid(const void* packed, int64_t N, const double ranges_host[6], int64_t chunk, void* ws,
+                            size_t bytes, float* rgbsigma, void* stream) {
+  if (N < 2 || N > kVolMaxN || chunk <= 0) return fail(NERFB200_EINVAL, "rgb_sigma_grid: N not in [2, 1625] or chunk <= 0%s");
+  if (!packed || !ranges_host || !ws || !rgbsigma) return fail(NERFB200_EINVAL, "rgb_sigma_grid: NULL argument%s");
+  if (reinterpret_cast<uintptr_t>(rgbsigma) & 15) return fail(NERFB200_EINVAL, "rgb_sigma_grid: out must be 16-byte aligned%s");
+  if (bytes < nerfb200_sigma_grid_workspace_bytes(chunk))
+    return fail(NERFB200_EINVAL, "rgb_sigma_grid: workspace smaller than nerfb200_sigma_grid_workspace_bytes(chunk)%s");
+  float* xyz = static_cast<float*>(ws);
+  const long long total = N * N * N;
+  for (long long s = 0; s < total; s += chunk) {
+    const long long n = total - s < chunk ? total - s : chunk;
+    int rc = nerfb200_grid_positions(N, ranges_host, s, n, xyz, stream);
+    if (rc) return rc;
+    if ((rc = nerfb200_query_rgb_sigma(xyz, n, 3, packed, rgbsigma + s * 4, stream)) != 0) return rc;
+  }
+  return 0;
+}
+
+size_t nerfb200_volume_workspace_bytes(int64_t N) {
+  if (N < 2 || N > kVolMaxN) return 0;
+  return volume_layout(N).bytes;
+}
+
+int nerfb200_volume_count(const float* rgbsigma, int64_t N, double xmin, double xmax, void* ws, size_t bytes,
+                          int64_t* count_host, void* stream) {
+  VolumeParams p;
+  VolumeLayout L;
+  int rc = volume_prepare(rgbsigma, N, xmin, xmax, ws, bytes, &p, &L, "volume_count");
+  if (rc) return rc;
+  if (!count_host) return fail(NERFB200_EINVAL, "volume_count: count_host is NULL%s");
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemsetAsync(p.tcnt + L.tiles, 0, sizeof(unsigned long long), s), "volume_count memset");
+  volume_count_kernel<<<mesh_blocks(L.tiles * kVolThreads), kVolThreads, 0, s>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "volume_count launch");
+  size_t tb = L.temp_bytes;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(static_cast<char*>(ws) + L.temp, tb, p.tcnt, p.tofs,
+                                         static_cast<int>(L.tiles + 1), s), "volume scan");
+  g_launches++;
+  unsigned long long h = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h, p.tofs + L.tiles, sizeof(h), cudaMemcpyDeviceToHost, s), "volume_count readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "volume_count readback");
+  *count_host = static_cast<int64_t>(h);
+  return 0;
+}
+
+int nerfb200_volume_emit(const float* rgbsigma, int64_t N, double xmin, double xmax, void* ws, size_t bytes,
+                         uint32_t* packed_out, void* stream) {
+  VolumeParams p;
+  VolumeLayout L;
+  int rc = volume_prepare(rgbsigma, N, xmin, xmax, ws, bytes, &p, &L, "volume_emit");
+  if (rc) return rc;
+  if (!packed_out) return fail(NERFB200_EINVAL, "volume_emit: out is NULL%s");
+  if (reinterpret_cast<uintptr_t>(packed_out) & 7) return fail(NERFB200_EINVAL, "volume_emit: out must be 8-byte aligned%s");
+  p.out = reinterpret_cast<uint2*>(packed_out);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  volume_emit_kernel<<<mesh_blocks(L.tiles * kVolThreads), kVolThreads, 0, s>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "volume_emit launch");
   return 0;
 }
 

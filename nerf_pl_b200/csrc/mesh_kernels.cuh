@@ -401,4 +401,70 @@ __global__ void color_finalize_kernel(const double* sum4, long long n, uint8_t* 
   }
 }
 
+// ---- 6. Unity volume (extract_mesh.ipynb "Generate .vol file for volume rendering in Unity") --------------
+// Per point of the (N^3, 4) [rgb, raw sigma] grid: a = 1 - exp(fl32(c) * max(sigma, 0)) in float32, the product
+// rounded once and exp taken in double then rounded to float32 (correctly rounded; numpy's SIMD float32 exp is
+// not).  Kept where a > 0, as (i, r << 24 + g << 16 + b << 8 + trunc(a * 255)) with r = trunc(rgb * 255).
+// Count / emit work on fixed tiles of kVolTile points, so the output order (increasing i) and the bytes do not
+// depend on the launch shape.
+constexpr int kVolThreads = 256;
+constexpr int kVolTile = 16 * kVolThreads;
+
+struct VolumeParams {
+  const float4* rgbsigma;      // (P, 4)
+  long long P;
+  float c;                     // float32(-(xmax - xmin) / N), rounded on the host
+  unsigned long long* tcnt;    // (tiles + 1) kept points per tile
+  unsigned long long* tofs;    // (tiles + 1) exclusive scan of tcnt
+  uint2* out;                  // (M) [i, s]
+};
+
+__device__ __forceinline__ bool volume_point(const float4 v, float c, uint32_t& s) {
+  const float sg = v.w < 0.f ? 0.f : v.w;                       // np.maximum(sigma, 0): NaN stays NaN
+  const float a = __fsub_rn(1.f, __double2float_rn(exp(static_cast<double>(__fmul_rn(c, sg)))));
+  if (!(a > 0.f)) return false;
+  const uint32_t r = static_cast<uint32_t>(__fmul_rn(v.x, 255.f));
+  const uint32_t g = static_cast<uint32_t>(__fmul_rn(v.y, 255.f));
+  const uint32_t b = static_cast<uint32_t>(__fmul_rn(v.z, 255.f));
+  s = (r << 24) + (g << 16) + (b << 8) + static_cast<uint32_t>(__fmul_rn(a, 255.f));
+  return true;
+}
+
+__global__ void __launch_bounds__(kVolThreads) volume_count_kernel(VolumeParams p) {
+  using Reduce = cub::BlockReduce<int, kVolThreads>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const long long tiles = (p.P + kVolTile - 1) / kVolTile;
+  for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
+    int n = 0;
+#pragma unroll 4
+    for (int r = 0; r < kVolTile / kVolThreads; ++r) {
+      const long long q = t * kVolTile + r * kVolThreads + threadIdx.x;
+      uint32_t s;
+      if (q < p.P && volume_point(__ldg(p.rgbsigma + q), p.c, s)) ++n;
+    }
+    const int total = Reduce(tmp).Sum(n);
+    if (threadIdx.x == 0) p.tcnt[t] = static_cast<unsigned long long>(total);
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(kVolThreads) volume_emit_kernel(VolumeParams p) {
+  using Scan = cub::BlockScan<int, kVolThreads>;
+  __shared__ typename Scan::TempStorage tmp;
+  const long long tiles = (p.P + kVolTile - 1) / kVolTile;
+  for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
+    unsigned long long base = p.tofs[t];
+    for (int r = 0; r < kVolTile / kVolThreads; ++r) {
+      const long long q = t * kVolTile + r * kVolThreads + threadIdx.x;
+      uint32_t s = 0;
+      const int keep = (q < p.P && volume_point(__ldg(p.rgbsigma + q), p.c, s)) ? 1 : 0;
+      int rank, total;
+      Scan(tmp).ExclusiveSum(keep, rank, total);
+      if (keep) p.out[base + rank] = make_uint2(static_cast<uint32_t>(q), s);
+      base += static_cast<unsigned long long>(total);
+      __syncthreads();
+    }
+  }
+}
+
 }  // namespace nerfb200

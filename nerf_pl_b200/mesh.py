@@ -6,6 +6,9 @@ the occlusion renders run the existing fused MLP / render launches.  Replaces Py
 (``mcubes.marching_cubes``), open3d (``cluster_connected_triangles`` + ``remove_unreferenced_vertices``),
 ``cv2.remap`` and the numpy projection loop; ``write_ply`` writes what plyfile wrote.  Conventions and the
 reference's quirks that are kept: DESIGN.md "Coloured mesh extraction".
+
+The Unity volume export of extract_mesh.ipynb is ``rgb_sigma_grid`` -> ``pack_volume`` -> ``write_vol`` (DESIGN.md
+"Unity volume").
 """
 from __future__ import annotations
 
@@ -232,6 +235,77 @@ def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: t
     if return_opacities:
         return out, (torch.stack(opac) if opac else torch.empty(0, n, device=v.device))
     return out
+
+
+@torch.no_grad()
+def query_rgb_sigma(model: torch.nn.Module, xyz: torch.Tensor) -> torch.Tensor:
+    """(n, 4) [sigmoid rgb, raw sigma] of ``model`` at positions xyz (n, 3) with the direction (0, 0, 0), one fused
+    launch (encoding in-kernel): ``nerf(cat(embedding_xyz(xyz), embedding_dir(zeros)))`` of extract_mesh.ipynb."""
+    x = _cuda(xyz, "xyz").detach().to(torch.float32).contiguous()
+    if x.dim() != 2 or x.shape[1] != 3:
+        raise ValueError("xyz must be (n, 3)")
+    out = torch.empty(x.shape[0], 4, dtype=torch.float32, device=x.device)
+    lib = _lib.load()
+    blob = packed_weights(model)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.nerfb200_query_rgb_sigma(x.data_ptr(), x.shape[0], 3, blob.data_ptr(), out.data_ptr(),
+                                                _stream_ptr()), "nerfb200_query_rgb_sigma")
+    return out
+
+
+@torch.no_grad()
+def rgb_sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk: int = 1 << 21) -> torch.Tensor:
+    """(N, N, N, 4) fp32 [sigmoid rgb, raw sigma] of ``model`` on the grid of ``sigma_grid`` with the direction
+    (0, 0, 0): extract_mesh.ipynb's ``rgbsigma`` ("Search for tight bounds"), reshaped.  Raw sigma: no
+    ``max(sigma, 0)``.  ``chunk`` points are queried per launch; the scratch is their positions only."""
+    dev = _device_of(model)
+    out = torch.empty(N, N, N, 4, dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    blob = packed_weights(model)
+    chunk = int(min(chunk, N ** 3))
+    ws = _workspace(lib.nerfb200_sigma_grid_workspace_bytes(chunk), dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.nerfb200_rgb_sigma_grid(blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk,
+                                               ws.data_ptr(), ws.numel(), out.data_ptr(), _stream_ptr()),
+                   "nerfb200_rgb_sigma_grid")
+    return out
+
+
+@torch.no_grad()
+def pack_volume(rgbsigma: torch.Tensor, x_range) -> torch.Tensor:
+    """extract_mesh.ipynb "Generate .vol file for volume rendering in Unity" on a CUDA (N, N, N, 4) rgbsigma grid
+    (raw sigma): (M, 2) uint32 rows [i, r << 24 + g << 16 + b << 8 + a8] of the points with alpha > 0, in
+    increasing flat index i, where a = 1 - exp(float32(-(xmax - xmin) / N) * max(sigma, 0)) (float32, exp
+    correctly rounded), a8 = trunc(255 a) and r = trunc(255 rgb).  Only ``x_range`` enters alpha, as in the
+    notebook.  N <= 1625 (the indices are uint32)."""
+    g = _cuda(rgbsigma, "rgbsigma").detach().to(torch.float32).contiguous()
+    if g.dim() != 4 or g.shape[3] != 4 or not (g.shape[0] == g.shape[1] == g.shape[2]):
+        raise ValueError("rgbsigma must be (N, N, N, 4)")
+    N = g.shape[0]
+    xmin, xmax = (float(v) for v in x_range)
+    lib = _lib.load()
+    nbytes = lib.nerfb200_volume_workspace_bytes(N)
+    if nbytes == 0:
+        raise ValueError(f"pack_volume: N = {N} outside [2, 1625]")
+    ws = _workspace(nbytes, g.device)
+    count = ctypes.c_int64()
+    with torch.cuda.device(g.device):
+        _lib.check(lib.nerfb200_volume_count(g.data_ptr(), N, xmin, xmax, ws.data_ptr(), ws.numel(), ctypes.byref(count),
+                                             _stream_ptr()), "nerfb200_volume_count")
+        # torch has no uint32 arithmetic to speak of; the rows are stored as int32 and viewed as uint32
+        out = torch.empty(count.value, 2, dtype=torch.int32, device=g.device)
+        if count.value:
+            _lib.check(lib.nerfb200_volume_emit(g.data_ptr(), N, xmin, xmax, ws.data_ptr(), ws.numel(), out.data_ptr(),
+                                                _stream_ptr()), "nerfb200_volume_emit")
+    return out.view(torch.uint32)
+
+
+def write_vol(path: str, packed) -> None:
+    """The .vol file of extract_mesh.ipynb: the (M, 2) uint32 rows of ``pack_volume`` as little-endian uint32,
+    row by row (``res.tobytes()``)."""
+    a = packed.detach().cpu().numpy() if isinstance(packed, torch.Tensor) else np.asarray(packed)
+    with open(path, "wb") as f:
+        f.write(np.ascontiguousarray(a.reshape(-1), dtype="<u4").tobytes())
 
 
 def write_ply(path: str, vertices, triangles, colors=None) -> None:

@@ -1,7 +1,8 @@
 """Device time per stage of the coloured-mesh workflow (nerf_pl_b200.mesh) on the trained test weights.
 
 Stages at N_grid 256 and 512 over [-1.5, 1.5]^3, threshold 20: sigma grid, marching cubes (count + emit),
-index -> world, largest cluster; colour fusion over 100 views at 800 x 800.  CUDA events around each stage;
+index -> world, largest cluster; the Unity volume's rgb+sigma grid and its pack (count + emit); colour fusion
+over 100 views at 800 x 800.  CUDA events around each stage;
 prints the card name and power limit with the numbers, and one JSON line.  The bytes columns are the
 minimum traffic of the MC and cluster passes (every array read / written once), as a share of the card's
 HBM bandwidth (3.35 TB/s on an H100 SXM).
@@ -80,9 +81,16 @@ def main():
         r = {"sigma_grid_ms": ms_sig, "marching_cubes_ms": ms_mc, "to_world_ms": ms_w, "cluster_ms": ms_cl,
              "vertices": V, "triangles": T, "kept_triangles": int(kt.shape[0]),
              "mc_hbm_share": mc_bytes / (ms_mc * 1e-3) / HBM, "cluster_hbm_share": cl_bytes / (ms_cl * 1e-3) / HBM}
+        del sigma, vi, tri, vw
+        # Unity volume (extract_mesh.ipynb): rgb+sigma grid, then alpha / pack / compaction (count + emit); the pack
+        # reads the 16-byte rows twice
+        ms_rgb, rgbsigma = timed(lambda: mesh.rgb_sigma_grid(model, N, RANGE, RANGE, RANGE))
+        ms_vol, vol = timed(lambda: mesh.pack_volume(rgbsigma, RANGE))
+        r.update({"rgb_sigma_grid_ms": ms_rgb, "volume_pack_ms": ms_vol, "volume_voxels": int(vol.shape[0]),
+                  "volume_hbm_share": (2 * P * 16 + vol.shape[0] * 8) / (ms_vol * 1e-3) / HBM})
+        del rgbsigma, vol
         res[f"N{N}"] = r
         print(f"N_grid {N}: " + ", ".join(f"{k} {v:.4g}" if isinstance(v, float) else f"{k} {v}" for k, v in r.items()))
-        del sigma, vi, tri, vw
         if N == args.grids[0]:
             verts = kv
     H = W = 800
