@@ -117,8 +117,14 @@ typedef struct nerfb200_render_args {
    * counter-based, so the numbers do not depend on the launch shape and a host replica reproduces them
    * (tests/philox.py).  The reference draws these with torch.rand from the global generator
    * (models/rendering.py:203, :39); the tensor inputs remain the way to replay a seeded torch stream.  The Gaussian
-   * noise inputs (noise_std > 0) are always tensors. */
-  uint64_t rng_seed;
+   * noise inputs (noise_std > 0) are always tensors.
+   * rng_in_kernel == 2: the key is read from DEVICE memory, *rng_seed_dev (same Philox stream for the same value), so
+   * that a captured CUDA graph can advance it between replays; rng_seed_dev shares the storage of rng_seed, which
+   * keeps this struct's layout (ABI version 3) unchanged for existing callers. */
+  union {
+    uint64_t rng_seed;
+    const uint64_t* rng_seed_dev;
+  };
   int32_t rng_in_kernel;
 } nerfb200_render_args;
 
@@ -169,6 +175,16 @@ int nerfb200_render_backward(const nerfb200_backward_args* args, void* stream);
 int nerfb200_adam_step(int32_t n_tensors, float* const* params, const float* const* grads, float* const* exp_avg,
                        float* const* exp_avg_sq, const int64_t* numel, float lr, float beta1, float beta2, float eps,
                        float weight_decay, int64_t step, void* stream);
+/* The same update with no per-step host values, so that a CUDA graph can replay it (torch.optim.Adam(capturable=True)):
+ * `lr_dev` is a device fp32 scalar; `steps` holds one device pointer per tensor to its fp32 step count BEFORE this
+ * update (torch's 0-dim state["step"]; the caller increments it afterwards).  Tensors at different step counts go in
+ * the same launch.  The bias corrections are formed on the device in double, as nerfb200_adam_step forms them on the
+ * host; the device pow is not correctly rounded, so they can differ by one fp32 ulp from the host's (m and v never
+ * differ: they do not depend on the step). */
+int nerfb200_adam_step_dev(int32_t n_tensors, float* const* params, const float* const* grads, float* const* exp_avg,
+                           float* const* exp_avg_sq, const int64_t* numel, const float* lr_dev,
+                           const float* const* steps, float beta1, float beta2, float eps, float weight_decay,
+                           void* stream);
 
 /* Same call with HOST buffers; returns with the requested outputs readable on the host (synchronises `stream`).
  * The packed weight images stay device-resident.  This is the end-to-end entry the reference's eval.py loop

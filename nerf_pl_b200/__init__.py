@@ -4,18 +4,19 @@ signatures, executed by hand-written wgmma (sm_90a) CUDA kernels through a C-ABI
 (``include/nerf_pl_b200.h``).  See DESIGN.md and INTEGRATION.md."""
 from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_forward_torch, nerf_parameters,
                    packed_weights)
+from .data import DeviceRayBatches
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
 from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, pack_volume, query_rgb_sigma, rgb_sigma_grid,
                    sigma_grid, write_ply, write_vol)
 from .optim import FusedAdam
 from .rendering import render_rays, render_rays_host, render_rays_loss, sample_pdf, searchsorted, volume_render
-from .training import nerf_forward_train
+from .training import CapturedTrainStep, nerf_forward_train
 
 __all__ = [
     "Embedding", "NeRF", "render_rays", "render_rays_loss", "render_rays_host", "FusedAdam", "invalidate_packed", "sample_pdf", "searchsorted", "volume_render",
     "nerf_forward_fused", "nerf_forward_torch", "nerf_forward_train", "nerf_parameters", "packed_weights",
     "batched_inference", "generate_rays", "render_image", "to_uint8", "query_sigma", "mse_psnr",
     "sigma_grid", "marching_cubes", "extract_mesh", "fuse_vertex_colors", "write_ply",
-    "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol",
+    "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
 ]
 __version__ = "0.1.0"

@@ -52,6 +52,7 @@ EXPORTS = [
     "nerfb200_train_workspace_init",
     "nerfb200_render_backward",
     "nerfb200_adam_step",
+    "nerfb200_adam_step_dev",
     "nerfb200_generate_rays",
     "nerfb200_to_uint8",
     "nerfb200_launch_count",
@@ -113,7 +114,7 @@ class RenderArgs(ctypes.Structure):
         ("train_workspace", c_void_p),
         ("target", c_void_p),
         ("loss_out", c_void_p),
-        ("rng_seed", ctypes.c_uint64),
+        ("rng_seed", ctypes.c_uint64),          # with rng_in_kernel == 2: the device address of the seed (rng_seed_dev)
         ("rng_in_kernel", c_int32),
     ]
 
@@ -211,6 +212,10 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.nerfb200_adam_step.argtypes = [c_int32, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
                                        POINTER(c_int64), c_float, c_float, c_float, c_float, c_float, c_int64, c_void_p]
     lib.nerfb200_adam_step.restype = c_int32
+    lib.nerfb200_adam_step_dev.argtypes = [c_int32, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
+                                           POINTER(c_void_p), POINTER(c_int64), c_void_p, POINTER(c_void_p), c_float,
+                                           c_float, c_float, c_float, c_void_p]
+    lib.nerfb200_adam_step_dev.restype = c_int32
     lib.nerfb200_mse_psnr.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]
     lib.nerfb200_mse_psnr.restype = c_int32
     lib.nerfb200_generate_rays.argtypes = [c_int32, c_int32, c_float, POINTER(c_float), c_float, c_float, c_int32,

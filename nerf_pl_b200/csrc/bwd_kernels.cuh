@@ -994,15 +994,19 @@ struct AdamParams {
   int numel[kAdamMaxTensors];
   float beta1, beta2, eps, weight_decay, step_size, bias2_sqrt;    // step_size = lr / (1 - b1^t), bias2_sqrt = sqrt(1 - b2^t)
 };
-__global__ void __launch_bounds__(256) adam_kernel(const __grid_constant__ AdamParams a) {
+// The tensor block blockIdx.x belongs to.
+__device__ __forceinline__ int adam_tensor_of_block(const AdamParams& a) {
   int lo = 0, hi = a.n_tensors;
-  while (hi - lo > 1) {        // the tensor this block belongs to
+  while (hi - lo > 1) {
     const int mid = (lo + hi) >> 1;
     if (a.block0[mid] <= static_cast<int>(blockIdx.x)) lo = mid; else hi = mid;
   }
-  const int t = lo;
+  return lo;
+}
+
+// Block blockIdx.x's 1024 elements of tensor t: the update shared by both kernels below.
+__device__ __forceinline__ void adam_update_block(const AdamParams& a, int t, float step, float bias2_sqrt) {
   const int base = (static_cast<int>(blockIdx.x) - a.block0[t]) * 1024;
-  const float step = a.step_size;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const int i = base + q * 256 + threadIdx.x;
@@ -1013,9 +1017,33 @@ __global__ void __launch_bounds__(256) adam_kernel(const __grid_constant__ AdamP
       const float v = a.beta2 * a.v[t][i] + (1.f - a.beta2) * g * g;
       a.m[t][i] = m;
       a.v[t][i] = v;
-      a.p[t][i] = pv - step * m / (sqrtf(v) / a.bias2_sqrt + a.eps);
+      a.p[t][i] = pv - step * m / (sqrtf(v) / bias2_sqrt + a.eps);
     }
   }
+}
+
+__global__ void __launch_bounds__(256) adam_kernel(const __grid_constant__ AdamParams a) {
+  adam_update_block(a, adam_tensor_of_block(a), a.step_size, a.bias2_sqrt);
+}
+
+// The capturable form (nerfb200_adam_step_dev): lr and each tensor's step count are read from device memory, and the
+// bias corrections are formed here in double from the same fp32 values the host path starts from (step_size and
+// bias2_sqrt of AdamParams are unused).  Thread 0 forms them once per block.
+struct AdamDevParams {
+  AdamParams a;
+  const float* lr;                           // device fp32 scalar
+  const float* step[kAdamMaxTensors];        // device fp32 step count of each tensor before this update
+};
+__global__ void __launch_bounds__(256) adam_dev_kernel(const __grid_constant__ AdamDevParams d) {
+  __shared__ float corr[2];
+  const int t = adam_tensor_of_block(d.a);
+  if (threadIdx.x == 0) {
+    const double k = static_cast<double>(*d.step[t]) + 1.0;
+    corr[0] = static_cast<float>(static_cast<double>(*d.lr) / (1.0 - pow(static_cast<double>(d.a.beta1), k)));
+    corr[1] = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(d.a.beta2), k)));
+  }
+  __syncthreads();
+  adam_update_block(d.a, t, corr[0], corr[1]);
 }
 
 }  // namespace nerfb200

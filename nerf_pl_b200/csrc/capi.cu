@@ -150,6 +150,7 @@ int check_render_shapes(const nerfb200_render_args* a) {
     if (!a->rgb_fine || !a->depth_fine || !a->opacity_fine)
       return fail(NERFB200_EINVAL, "fine outputs are NULL with N_importance>0%s");
   }
+  if (a->rng_in_kernel == 2 && !a->rng_seed_dev) return fail(NERFB200_EINVAL, "rng_in_kernel = 2 needs rng_seed_dev%s");
   if (a->perturb > 0.f && !a->rng_in_kernel) {
     if (!a->perturb_rand) return fail(NERFB200_EINVAL, "perturb>0 needs perturb_rand%s");
     if (a->n_importance > 0 && !a->u_rand) return fail(NERFB200_EINVAL, "perturb>0 needs u_rand%s");
@@ -626,7 +627,7 @@ int nerfb200_render_rays(const nerfb200_render_args* a, void* stream) {
   p.weights_fine = a->weights_fine;
   p.status = a->status ? a->status : d->status;
   p.z_coarse = a->z_coarse;
-  p.rng_seed = a->rng_seed;
+  p.rng_seed = a->rng_seed;               // with rng_in_kernel == 2 the bits of rng_seed_dev (the union)
   p.rng_in_kernel = a->rng_in_kernel;
   p.train = 0;
   p.target = nullptr; p.loss_part = nullptr; p.loss_out = nullptr; p.loss_counter = nullptr;
@@ -1347,6 +1348,39 @@ int nerfb200_adam_step(int32_t n_tensors, float* const* params, const float* con
   adam_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
   g_launches++;
   CUDA_TRY(cudaGetLastError(), "adam_step launch");
+  return 0;
+}
+
+int nerfb200_adam_step_dev(int32_t n_tensors, float* const* params, const float* const* grads, float* const* exp_avg,
+                           float* const* exp_avg_sq, const int64_t* numel, const float* lr_dev,
+                           const float* const* steps, float beta1, float beta2, float eps, float weight_decay,
+                           void* stream) {
+  if (n_tensors < 0 || n_tensors > kAdamMaxTensors) return fail(NERFB200_EINVAL, "adam_step_dev: at most 64 tensors per call%s");
+  if (n_tensors == 0) return 0;
+  if (!params || !grads || !exp_avg || !exp_avg_sq || !numel || !lr_dev || !steps)
+    return fail(NERFB200_EINVAL, "adam_step_dev: NULL argument%s");
+  AdamDevParams d;
+  AdamParams& a = d.a;
+  a.n_tensors = n_tensors;
+  int blocks = 0;
+  for (int i = 0; i < n_tensors; ++i) {
+    if (numel[i] < 0 || numel[i] > 0x7fffffff ||
+        (numel[i] > 0 && (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i] || !steps[i])))
+      return fail(NERFB200_EINVAL, "adam_step_dev: NULL tensor / bad size%s");
+    a.p[i] = params[i]; a.g[i] = grads[i]; a.m[i] = exp_avg[i]; a.v[i] = exp_avg_sq[i];
+    d.step[i] = steps[i];
+    a.numel[i] = static_cast<int>(numel[i]);
+    a.block0[i] = blocks;
+    blocks += static_cast<int>((numel[i] + 1023) / 1024);
+  }
+  a.block0[n_tensors] = blocks;
+  a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
+  a.step_size = a.bias2_sqrt = 0.f;
+  d.lr = lr_dev;
+  if (blocks == 0) return 0;
+  adam_dev_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(d);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "adam_step_dev launch");
   return 0;
 }
 

@@ -7,7 +7,18 @@ L2 weight decay added to the gradient; no amsgrad / maximize.  The bias correcti
 (csrc/bwd_kernels.cuh adam_kernel states where the result differs from torch's).
 
 As in torch.optim.Adam, a parameter whose ``grad`` is None is skipped and keeps its own step count; parameters at
-different step counts get their own bias corrections (one launch per distinct step)."""
+different step counts get their own bias corrections (one launch per distinct step).
+
+``capturable=True`` (as in ``torch.optim.Adam(capturable=True)``): the step reads nothing on the host, so a CUDA graph
+can capture and replay it (``nerf_pl_b200.training.CapturedTrainStep``).  ``step`` is then a 0-dim float32 tensor on
+the parameter's device, the learning rate is read from a device scalar per group, and the bias corrections are formed
+on the device (C ABI ``nerfb200_adam_step_dev``; one launch for all tensors whatever their step counts).
+``group["lr"]`` stays a float that schedulers change as usual: each eager ``step()`` and each
+``CapturedTrainStep.step()`` copies it into the device scalar when it has changed (``sync_lr``).  m and v are
+bit-identical to the non-capturable update; p can differ by an ulp where the device ``pow`` rounds a bias correction
+differently from the host's.  ``load_state_dict`` puts the step counts on the device (capturable) or the host (not
+capturable), whichever form the checkpoint has, so checkpoints move between both forms and ``torch.optim.Adam``.
+A captured graph holds the addresses of the state tensors: after ``load_state_dict`` capture a new graph."""
 from __future__ import annotations
 
 import ctypes
@@ -27,22 +38,62 @@ def _check_tensor(t: torch.Tensor, p: torch.Tensor, contiguous: bool = True) -> 
 
 
 class FusedAdam(torch.optim.Optimizer):
-    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0):
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0,
+                 capturable: bool = False):
         if lr < 0 or eps < 0 or not 0 <= betas[0] < 1 or not 0 <= betas[1] < 1 or weight_decay < 0:
             raise ValueError("invalid Adam hyper-parameter")
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
+        if capturable:
+            defaults["capturable"] = True
+        super().__init__(params, defaults)
         self._cache = {}
+        self._lr_dev = {}           # group index -> device fp32 scalar (capturable)
+        self._lr_host = {}          # group index -> the float last copied into it
+
+    @property
+    def capturable(self) -> bool:
+        return bool(self.defaults.get("capturable", False))
 
     def __setstate__(self, state):
         """Runs in ``load_state_dict`` (and unpickling): a number ``step`` (checkpoints of earlier versions) becomes
-        a tensor as torch.optim.Adam stores it, and the launch tables of the replaced state are dropped."""
+        a tensor as torch.optim.Adam stores it, on the parameter's device when capturable and on the host otherwise;
+        the launch tables of the replaced state are dropped.  The mode is this optimiser's, not the checkpoint's."""
         super().__setstate__(state)
+        cap = self.capturable
         for group in self.param_groups:
+            if cap:
+                group["capturable"] = True
+            elif "capturable" in group:
+                group["capturable"] = False
             for p in group["params"]:
                 st = self.state.get(p, {})
-                if len(st) and not torch.is_tensor(st["step"]):
-                    st["step"] = torch.tensor(float(st["step"]), dtype=torch.float32)
+                if len(st):
+                    step = st["step"]
+                    if not torch.is_tensor(step):
+                        step = torch.tensor(float(step), dtype=torch.float32)
+                    st["step"] = step.to(dtype=torch.float32, device=p.device if cap else "cpu")
         self._cache = {}
+        self.__dict__.setdefault("_lr_dev", {})
+        self._lr_host = {}
+
+    def sync_lr(self) -> None:
+        """Copy each group's ``lr`` into its device scalar where it has changed (capturable; a no-op otherwise).
+        Not to be called while a graph is being captured: the copy is a host value."""
+        if not self.capturable:
+            return
+        for gi, group in enumerate(self.param_groups):
+            lr = float(group["lr"])
+            t = self._lr_dev.get(gi)
+            if t is None:
+                dev = next((p.device for p in group["params"]), None)
+                if dev is None:
+                    continue
+                t = torch.empty((), dtype=torch.float32, device=dev)
+                self._lr_dev[gi] = t
+                self._lr_host.pop(gi, None)
+            if self._lr_host.get(gi) != lr:
+                t.fill_(lr)
+                self._lr_host[gi] = lr
 
     @staticmethod
     def _tables(ps, sts):
@@ -64,6 +115,13 @@ class FusedAdam(torch.optim.Optimizer):
             with torch.enable_grad():
                 loss = closure()
         lib = _lib.load()
+        cap = self.capturable
+        if cap:
+            if torch.cuda.is_current_stream_capturing():
+                if len(self._lr_dev) < len(self.param_groups):
+                    raise RuntimeError("FusedAdam(capturable=True): run one eager step before capturing a graph")
+            else:
+                self.sync_lr()
         for gi, group in enumerate(self.param_groups):
             if group.get("amsgrad") or group.get("maximize") or group.get("decoupled_weight_decay"):
                 raise RuntimeError("FusedAdam has no amsgrad / maximize / decoupled weight decay")
@@ -73,12 +131,15 @@ class FusedAdam(torch.optim.Optimizer):
             sts = [self.state[p] for p in ps]
             for p, st in zip(ps, sts):
                 if len(st) == 0:
-                    st["step"] = torch.tensor(0.0, dtype=torch.float32)
+                    st["step"] = torch.zeros((), dtype=torch.float32, device=p.device if cap else "cpu")
                     st["exp_avg"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
                     st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
                 elif not torch.is_tensor(st["step"]):
                     st["step"] = torch.tensor(float(st["step"]), dtype=torch.float32)
             steps = [st["step"] for st in sts]
+            if cap:
+                self._step_dev(lib, gi, group, ps, sts, steps)
+                continue
             ts = [int(s) for s in steps]
             # the tables hold raw pointers: rebuilt whenever a parameter or a state tensor is another allocation
             key = (tuple([p.data_ptr() for p in ps]) + tuple([st["exp_avg"].data_ptr() for st in sts]) +
@@ -109,3 +170,35 @@ class FusedAdam(torch.optim.Optimizer):
                                    "nerfb200_adam_step")
             torch._foreach_add_(steps, 1.0)
         return loss
+
+    def _step_dev(self, lib, gi, group, ps, sts, steps) -> None:
+        """The capturable update of one group: no host value that changes from step to step enters the launch."""
+        for st, p in zip(sts, ps):
+            if not (torch.is_tensor(st["step"]) and st["step"].device == p.device and st["step"].dim() == 0
+                    and st["step"].dtype == torch.float32):
+                raise RuntimeError("FusedAdam(capturable=True) keeps each step count as a 0-dim float32 tensor on the "
+                                   "parameter's device")
+        key = (tuple([p.data_ptr() for p in ps]) + tuple([st["exp_avg"].data_ptr() for st in sts]) +
+               tuple([st["exp_avg_sq"].data_ptr() for st in sts]) + tuple([s.data_ptr() for s in steps]))
+        cache = self._cache.get(gi)
+        if cache is None or cache["key"] != key:
+            for p, st in zip(ps, sts):
+                for t in (p, p.grad, st["exp_avg"], st["exp_avg_sq"]):
+                    _check_tensor(t, p, contiguous=t is not p.grad)
+            chunks = self._tables(ps, sts)
+            for ch, i0 in zip(chunks, range(0, len(ps), 64)):
+                ch["step"] = (ctypes.c_void_p * len(ch["ps"]))(*[s.data_ptr() for s in steps[i0:i0 + 64]])
+            cache = dict(key=key, chunks=chunks, dev=ps[0].device)
+            self._cache[gi] = cache
+        lr = self._lr_dev[gi]
+        b1, b2 = group["betas"]
+        with torch.cuda.device(cache["dev"]):
+            for ch in cache["chunks"]:
+                gs = [p.grad if p.grad.is_contiguous() else p.grad.contiguous() for p in ch["ps"]]
+                garr = (ctypes.c_void_p * len(gs))(*[g.data_ptr() for g in gs])
+                _lib.check(lib.nerfb200_adam_step_dev(len(gs), ch["p"], garr, ch["m"], ch["v"], ch["numel"],
+                                                      lr.data_ptr(), ch["step"], float(b1), float(b2),
+                                                      float(group["eps"]), float(group["weight_decay"]),
+                                                      _stream_ptr()),
+                           "nerfb200_adam_step_dev")
+        torch._foreach_add_(steps, 1.0)

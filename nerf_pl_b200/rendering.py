@@ -163,6 +163,16 @@ def _draw_randoms(n: int, S_c: int, K: int, perturb: float, noise_std: float, de
 _KERNEL_RNG_CALLS = 0
 
 
+def _seed_fields(seed) -> Dict[str, int]:
+    """The RenderArgs fields of a kernel seed: None (tensor inputs), an int, or a device int64 tensor holding it
+    (rng_in_kernel == 2: the kernel reads the key at that address)."""
+    if seed is None:
+        return dict(rng_seed=0, rng_in_kernel=0)
+    if torch.is_tensor(seed):
+        return dict(rng_seed=seed.data_ptr(), rng_in_kernel=2)
+    return dict(rng_seed=seed, rng_in_kernel=1)
+
+
 def _resolve_randoms(randoms, n, S_c, K, perturb, noise_std, dev, match_rng):
     """-> (perturb_rand, noise_coarse, u_rand, noise_fine, kernel_seed | None).
 
@@ -170,18 +180,28 @@ def _resolve_randoms(randoms, n, S_c, K, perturb, noise_std, dev, match_rng):
     ``"kernel"`` or ``{"seed": int}``: the two uniform inputs are then generated inside the render kernel
     (Philox4x32-10 keyed by the seed, include/nerf_pl_b200.h ``rng_in_kernel``) - no generator launch, no (N, S)
     tensors.  ``"kernel"`` derives the seed from ``torch.initial_seed()`` and a per-process call counter
-    (deterministic under ``torch.manual_seed``; a CUDA graph replays the captured seed).  The Gaussian noise
-    inputs (``noise_std > 0``) are tensors in every mode."""
+    (deterministic under ``torch.manual_seed``).  Because that seed is a host value, ``"kernel"`` is refused while
+    a CUDA graph is being captured (a replay would reuse it); there ``{"seed": t}`` with ``t`` a one-element int64
+    CUDA tensor keys the numbers from device memory (its 64 bits are the seed; ``CapturedTrainStep`` advances it
+    inside the graph).  The Gaussian noise inputs (``noise_std > 0``) are tensors in every mode."""
     global _KERNEL_RNG_CALLS
     seed = None
     if isinstance(randoms, str):
         if randoms != "kernel":
             raise ValueError("randoms must be None, a dict of tensors, {'seed': int} or 'kernel'")
+        if torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing():
+            raise ValueError("randoms='kernel' derives its seed on the host, so a captured graph would replay one "
+                             "seed: pass {'seed': <int64 CUDA tensor>} or use nerf_pl_b200.CapturedTrainStep")
         _KERNEL_RNG_CALLS += 1
         seed = (torch.initial_seed() * 0x9E3779B97F4A7C15 + _KERNEL_RNG_CALLS * 0xD1B54A32D192ED03) & 0xFFFFFFFFFFFFFFFF
         randoms = {}
     elif randoms is not None and "seed" in randoms:
-        seed = int(randoms["seed"]) & 0xFFFFFFFFFFFFFFFF
+        seed = randoms["seed"]
+        if torch.is_tensor(seed):
+            if not (seed.is_cuda and seed.dtype == torch.int64 and seed.numel() == 1 and seed.device == dev):
+                raise ValueError("a tensor seed must be a one-element int64 tensor on the rays' device")
+        else:
+            seed = int(seed) & 0xFFFFFFFFFFFFFFFF
     if randoms is None:
         pr, nc, ur, nf = _draw_randoms(n, S_c, K, perturb, noise_std, dev, match_rng)
     else:
@@ -292,7 +312,7 @@ def render_rays(models: List[torch.nn.Module],
         opacity_coarse=_ptr(out["opacity_coarse"]), rgb_fine=_ptr(out["rgb_fine"]),
         depth_fine=_ptr(out["depth_fine"]), opacity_fine=_ptr(out["opacity_fine"]),
         z_fine=_ptr(z_fine), weights_coarse=_ptr(w_c), weights_fine=_ptr(w_f),
-        status=None, max_ctas=0, rng_seed=seed or 0, rng_in_kernel=int(seed is not None))
+        status=None, max_ctas=0, **_seed_fields(seed))
     if torch.cuda.current_device() == dev.index:
         _lib.check(lib.nerfb200_render_rays(ctypes.byref(args), _stream_ptr()), "nerfb200_render_rays")
     else:
@@ -373,7 +393,7 @@ def render_rays_host(models: List[torch.nn.Module],
             rgb_coarse=_ptr(res.get("rgb_coarse")), depth_coarse=_ptr(res.get("depth_coarse")),
             opacity_coarse=_ptr(res.get("opacity_coarse")), rgb_fine=_ptr(res.get("rgb_fine")),
             depth_fine=_ptr(res.get("depth_fine")), opacity_fine=_ptr(res.get("opacity_fine")),
-            rng_seed=seed or 0, rng_in_kernel=int(seed is not None))
+            **_seed_fields(seed))
         _lib.check(lib.nerfb200_render_rays_host(ctypes.byref(args), _stream_ptr()), "nerfb200_render_rays_host")
     return res
 

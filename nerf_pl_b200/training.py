@@ -28,6 +28,8 @@ import torch
 from . import _lib
 from .nerf import (_EXPECTED_SHAPES, _stream_ptr, nerf_forward_fused, nerf_parameters, packed_weights,
                    packed_weights_pair)
+from .data import DeviceRayBatches, next_step_schedule
+from .rendering import _draw_randoms, _seed_fields
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -53,6 +55,7 @@ class TrainWorkspace:
         self.raw = raw
         self.buf = raw[off:off + self.bytes]
         self.busy = False
+        self.key = (dev.index, n, S_c, K)
         with torch.cuda.device(dev):
             _lib.check(lib.nerfb200_train_workspace_init(self.buf.data_ptr(), self.bytes, n, S_c, K, _stream_ptr()),
                        "nerfb200_train_workspace_init")
@@ -105,7 +108,7 @@ def _render_args(cfg, rays, pr, nc, ur, nf, out, blob_c, blob_f, ws, target, los
         opacity_fine=_ptr(out[5]) if K > 0 else None,
         z_fine=None, weights_coarse=None, weights_fine=None, status=None, max_ctas=0, z_coarse=None,
         train_workspace=ws.buf.data_ptr(), target=_ptr(target), loss_out=_ptr(loss_out),
-        rng_seed=cfg.get("rng_seed") or 0, rng_in_kernel=int(cfg.get("rng_seed") is not None))
+        **_seed_fields(cfg.get("rng_seed")))
 
 
 class FusedRenderFunction(torch.autograd.Function):
@@ -127,7 +130,10 @@ class FusedRenderFunction(torch.autograd.Function):
             blob_c, blob_f = packed_weights_pair(models[0], models[1])      # one launch for both images
         else:
             blob_c, blob_f = packed_weights(models[0]), None
-        lease = _Lease(TrainWorkspace.acquire(dev, n, S_c, K))
+        own = cfg.get("workspace")        # a workspace outside the pool (CapturedTrainStep's)
+        if own is not None and own.key != (dev.index, n, S_c, K):
+            raise ValueError("the given training workspace is of another shape")
+        lease = _Lease(own if own is not None else TrainWorkspace.acquire(dev, n, S_c, K))
         ws = lease.ws
         args = _render_args(cfg, rays, pr, nc, ur, nf, out, blob_c, blob_f, ws, target, loss_out)
         with torch.cuda.device(dev):
@@ -227,14 +233,14 @@ def _params_of(models, N_importance) -> List[torch.Tensor]:
 
 def render_rays_train(models, rays, N_samples, use_disp, perturb, noise_std, N_importance, white_back,
                       pr, nc, ur, nf, target: Optional[torch.Tensor] = None,
-                      rng_seed: Optional[int] = None) -> Dict[str, torch.Tensor]:
+                      rng_seed=None, workspace: Optional[TrainWorkspace] = None) -> Dict[str, torch.Tensor]:
     """Differentiable render_rays (test_time=False) through FusedRenderFunction.  With ``target``
     (n,3) the result also carries ``loss`` (losses.py:9-14 MSELoss of the batch), ``psnr``
     (metrics.py:4-13, of the finest pass), ``mse_coarse`` and ``mse_fine`` computed by the same
     launch; ``loss.backward()`` then seeds the backward inside the kernels."""
     cfg = dict(models=list(models), N_samples=int(N_samples), N_importance=int(N_importance),
                use_disp=bool(use_disp), perturb=float(perturb), noise_std=float(noise_std),
-               white_back=bool(white_back), rng_seed=rng_seed)
+               white_back=bool(white_back), rng_seed=rng_seed, workspace=workspace)
     params = _params_of(models, N_importance)
     if target is not None:
         target = target.detach().to(torch.float32).contiguous()
@@ -396,3 +402,161 @@ def nerf_forward_train(model: torch.nn.Module, x: torch.Tensor) -> torch.Tensor:
     if not (torch.is_grad_enabled() and any(p.requires_grad for p in params)):
         return nerf_forward_fused(model, x)
     return FusedNerfFunction.apply(model, x.detach().to(torch.float32).contiguous(), *params)
+
+
+# ---------------------------------------------------------------------------------------------
+# One training step (batch gather, fused render + loss, fused backward, capturable FusedAdam) as ONE CUDA graph.
+_CAPTURED_SEEDS = 0
+
+
+class CapturedTrainStep:
+    """The reference's training step (train.py:103-117 with the optimiser step) captured once as a CUDA graph and
+    replayed by ``step()``: no Python, no host-side kernel launches and no host synchronisation per step.
+
+    ``models`` (coarse[, fine]) are trained on ``batches`` (a ``DeviceRayBatches``) by ``optimizer``, a
+    ``FusedAdam(capturable=True)`` over their parameters; the other arguments are ``render_rays_loss``'s.  Each
+    replay gathers the next batch from a device-resident epoch permutation at a device-side offset, renders it with
+    the loss fused in, runs the backward and the Adam update.  Only full batches are used (``drop_last`` semantics:
+    ``len(batches)`` with ``drop_last=True`` steps per epoch); when the host-side step count completes an epoch,
+    ``step()`` draws the next permutation into the same buffer before the replay.  ``step()`` returns the device
+    scalars ``(loss, psnr)`` of the step; they are overwritten by the next replay, so clone them to keep them.
+
+    Random inputs: ``randoms=None`` draws the uniforms (and the noise when ``noise_std > 0``) with torch's CUDA
+    generator, which advances across replays by itself.  ``randoms="kernel"`` (or ``{"seed": s}``) draws the
+    uniforms inside the render kernel keyed by a device word (``seed_word``) that each replay increments, so replay
+    k uses seed s + k.
+
+    Construction runs ``warmup`` eager steps on a side stream (first-call set-up: library attributes, packed weight
+    images, Adam state, the step's workspace), then restores the parameters, the Adam state and the seed they
+    changed, sets the gradients to None and captures one step; it raises ``RuntimeError`` with torch's reason if
+    the capture fails.  The step's training workspace belongs to this object for its whole life (it is not in
+    ``TrainWorkspace``'s pool), so eager training calls of the same shape between replays never touch it.
+    The gradients of every parameter the optimizer holds are set to None before the warm-up and before the capture,
+    so parameters outside ``models`` (the fine model when ``N_importance == 0``, other groups) are neither warmed up
+    nor updated by the replays.  Between replays the models' ``.grad`` are the graph's own buffers.  ``launches_per_step`` is the number of
+    library kernels one replay runs (counted while capturing)."""
+
+    def __init__(self, models, batches, optimizer, N_samples: int = 64, use_disp: bool = False, perturb: float = 1.0,
+                 noise_std: float = 1.0, N_importance: int = 64, white_back: bool = False, randoms=None,
+                 warmup: int = 3):
+        from .optim import FusedAdam
+        global _CAPTURED_SEEDS
+        if not (isinstance(optimizer, FusedAdam) and optimizer.capturable):
+            raise ValueError("CapturedTrainStep needs FusedAdam(..., capturable=True): a non-capturable step reads "
+                             "its step count on the host and would replay step 1 forever")
+        if not isinstance(batches, DeviceRayBatches):
+            raise TypeError("batches must be a nerf_pl_b200.DeviceRayBatches")
+        S_c, K = int(N_samples), int(N_importance)
+        if K > 0 and len(models) < 2:
+            raise ValueError("N_importance > 0 needs a fine model (models[1])")
+        B = batches.batch_size
+        self.per_epoch = batches.samples_per_rank // B
+        if self.per_epoch == 0:
+            raise ValueError("the dataset has no full batch for this rank")
+        self.models = list(models)[:2 if K > 0 else 1]
+        self.params = _params_of(self.models, K)
+        owned = {id(p) for g in optimizer.param_groups for p in g["params"]}
+        if any(id(p) not in owned for p in self.params):
+            raise ValueError("the optimizer does not hold every parameter of the models")
+        self.batches, self.optimizer = batches, optimizer
+        self.cfg = dict(N_samples=S_c, use_disp=bool(use_disp), perturb=float(perturb), noise_std=float(noise_std),
+                        N_importance=K, white_back=bool(white_back))
+        dev = batches.device
+        self.seed_word = None
+        if isinstance(randoms, str) or (isinstance(randoms, dict) and "seed" in randoms):
+            if isinstance(randoms, str):
+                if randoms != "kernel":
+                    raise ValueError("randoms must be None, 'kernel' or {'seed': int}")
+                _CAPTURED_SEEDS += 1
+                s = (torch.initial_seed() * 0x9E3779B97F4A7C15 + _CAPTURED_SEEDS * 0xBF58476D1CE4E5B9) \
+                    & 0xFFFFFFFFFFFFFFFF
+            else:
+                s = int(randoms["seed"]) & 0xFFFFFFFFFFFFFFFF
+            s = s - (1 << 64) if s >= 1 << 63 else s          # the same 64 bits as an int64
+            self.seed_word = torch.tensor(s, dtype=torch.int64, device=dev)
+        elif randoms is not None:
+            raise ValueError("randoms must be None, 'kernel' or {'seed': int}")
+        self.workspace = TrainWorkspace(dev, B, S_c, K)
+        self._perm = batches.next_permutation().clone()
+        self._offset = torch.zeros((), dtype=torch.int64, device=dev)
+        self._arange = torch.arange(B, device=dev)
+        self.steps = 0                  # replays so far
+        self.epoch = 0                  # epoch of the next replay (0-based)
+        self._warm_and_capture(int(warmup), dev)
+
+    def _body(self):
+        """One step on the static buffers (run eagerly while warming up, then once under capture)."""
+        c = self.cfg
+        B, S_c, K = self._arange.shape[0], c["N_samples"], c["N_importance"]
+        idx = self._perm.index_select(0, self._offset + self._arange)
+        batch = self.batches.gather(idx)
+        if self.seed_word is not None:
+            pr = ur = None
+            nc = torch.randn(B, S_c, device=idx.device) if c["noise_std"] > 0 else None
+            nf = torch.randn(B, S_c + K, device=idx.device) if c["noise_std"] > 0 and K > 0 else None
+        else:
+            pr, nc, ur, nf = _draw_randoms(B, S_c, K, c["perturb"], c["noise_std"], idx.device, False)
+        res = render_rays_train(self.models, batch["rays"], S_c, c["use_disp"], c["perturb"], c["noise_std"], K,
+                                c["white_back"], pr, nc, ur, nf, target=batch["rgbs"], rng_seed=self.seed_word,
+                                workspace=self.workspace)
+        res["loss"].backward()
+        self.optimizer.step()
+        self._offset.add_(B)
+        if self.seed_word is not None:
+            self.seed_word.add_(1)
+        self.batch_indices = idx
+        self.randoms = {k: v for k, v in (("perturb_rand", pr), ("noise_coarse", nc), ("u_rand", ur),
+                                          ("noise_fine", nf)) if v is not None}
+        return res["loss"].detach(), res["psnr"]
+
+    def _warm_and_capture(self, warmup: int, dev) -> None:
+        opt = self.optimizer
+        with torch.no_grad():
+            saved_p = [p.detach().clone() for p in self.params]
+            saved_st = [{k: v.clone() for k, v in opt.state[p].items()} if len(opt.state.get(p, {})) else None
+                        for p in self.params]
+            saved_seed = None if self.seed_word is None else self.seed_word.clone()
+        opt.sync_lr()
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(max(warmup, 1)):
+                opt.zero_grad(set_to_none=True)     # every parameter the optimizer holds: no stale gradient steps
+                self._offset.zero_()        # every warm-up step takes the first batch: never past the permutation
+                self._body()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        with torch.no_grad():               # the warm-up steps leave no trace
+            for p, q in zip(self.params, saved_p):
+                p.copy_(q)
+            for p, snap in zip(self.params, saved_st):
+                st = opt.state[p]
+                for k in ("step", "exp_avg", "exp_avg_sq"):
+                    if snap is None:
+                        st[k].zero_()
+                    else:
+                        st[k].copy_(snap[k])
+            self._offset.zero_()
+            if saved_seed is not None:
+                self.seed_word.copy_(saved_seed)
+        opt.zero_grad(set_to_none=True)     # captured: only the models' parameters get gradients, hence updates
+        lib = _lib.load()
+        self.graph = torch.cuda.CUDAGraph()
+        n0 = lib.nerfb200_launch_count()
+        try:
+            with torch.cuda.graph(self.graph):
+                self._loss, self._psnr = self._body()
+        except Exception as e:
+            raise RuntimeError(f"CapturedTrainStep: capturing the training step failed: {e}") from e
+        self.launches_per_step = int(lib.nerfb200_launch_count() - n0)
+
+    def step(self):
+        """Replay one training step; returns the device scalars (loss, psnr) of this step."""
+        reshuffle, epoch, _ = next_step_schedule(self.steps, self.per_epoch)
+        if reshuffle:                       # the previous epoch is done: reshuffle outside the graph
+            self._perm.copy_(self.batches.next_permutation())
+            self._offset.zero_()
+            self.epoch = epoch
+        self.optimizer.sync_lr()
+        self.graph.replay()
+        self.steps += 1
+        return self._loss, self._psnr
