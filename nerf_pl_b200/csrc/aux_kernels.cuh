@@ -3,8 +3,6 @@
 // fuses all of them; these entries exist so each row has its own parity test and so callers
 // that use the pieces directly (extract_color_mesh.py:127-140) have a drop-in.
 #pragma once
-#include <cuda_bf16.h>
-
 #include "render_kernel.cuh"
 
 namespace nerfb200 {
@@ -13,7 +11,6 @@ namespace nerfb200 {
 struct PackParams {
   const float* p[kNumParams];   // device pointers, order in layout.h
   uint8_t* out;
-  int bwd_bf16;                 // element type of the backward region: 1 = bf16, 0 = fp16
 };
 
 struct PackParams2 {
@@ -88,10 +85,8 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackParams2 pp2) {
       const int ld = (L == 5) ? 319 : 256, n0 = (L == 5) ? 63 : 0;
       v = pp.p[2 * (L - 1)][static_cast<long long>(kb * 64 + k) * ld + n0 + n];
     }
-    uint16_t bits;
-    if (pp.bwd_bf16) bits = __bfloat16_as_ushort(__float2bfloat16_rn(v));
-    else bits = __half_as_ushort(__float2half_rn(v));
-    *reinterpret_cast<uint16_t*>(pp.out + kOffBwd + static_cast<uint32_t>(slice) * kSliceBytes256 + sw128_off(n, k)) = bits;
+    *reinterpret_cast<__half*>(pp.out + kOffBwd + static_cast<uint32_t>(slice) * kSliceBytes256 + sw128_off(n, k)) =
+        __float2half_rn(v);
     return;
   }
   float* o = reinterpret_cast<float*>(pp.out + kHalfRegionBytes);

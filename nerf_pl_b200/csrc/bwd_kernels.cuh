@@ -31,41 +31,22 @@
 // un-scaled per layer by the reduction.
 // fp16 rather than bf16 because the wgrad GEMM contracts the gradients with the forward's fp16
 // activations and wgmma takes its two 16-bit operands in one type (f16 x f16 or bf16 x bf16, PTX ISA
-// "wgmma.mma_async"); -DNERFB200_BWD_BF16 switches only the gradient conversions to bf16 (it would need
-// bf16 activations from the forward and bf16 wgmma, and is not wired up).
+// "wgmma.mma_async").
 #pragma once
-#include <cuda_bf16.h>
-
 #include "render_kernel.cuh"
 
 namespace nerfb200 {
 
-#ifdef NERFB200_BWD_BF16
-constexpr bool kBwdBf16 = true;
-#else
-constexpr bool kBwdBf16 = false;
-#endif
-
 __device__ __forceinline__ uint32_t cvt_bwd_x2(float lo, float hi) {
   uint32_t d;
-  if (kBwdBf16) asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
-  else asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
-__device__ __forceinline__ uint16_t cvt_bwd(float v) {
-  if (kBwdBf16) return __bfloat16_as_ushort(__float2bfloat16_rn(v));
-  return static_cast<uint16_t>(cvt_bwd_x2(v, 0.f) & 0xFFFFu);
-}
-// packed 16-bit add (gradient element type)
+// packed fp16 add
 __device__ __forceinline__ uint32_t bwd_add_x2(uint32_t a, uint32_t b) {
   uint32_t d;
-  if (kBwdBf16) asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  else asm("add.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+  asm("add.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
   return d;
-}
-__device__ __forceinline__ float2 bwd_x2_to_float2(uint32_t p) {
-  if (kBwdBf16) return make_float2(__uint_as_float(p << 16), __uint_as_float(p & 0xFFFF0000u));
-  return __half22float2(*reinterpret_cast<const __half2*>(&p));
 }
 
 // ------------------------------------------------------------------------- compositing backward
@@ -272,18 +253,16 @@ __global__ void __launch_bounds__(128) bwd_scale_kernel(const ScaleParams p) {
       }
       if (t < kLevels) {
         float s = 1.f;
-        if (!kBwdBf16) {
-          const float bound = fmaxf(__uint_as_float(p.amax[2 * ps + 1]) * red[0][0], __uint_as_float(p.amax[2 * ps]) * red[1][0]);
-          if (bound > 0.f) s = exp2f(floorf(log2f(64.f / bound)));
-          s = fminf(fmaxf(s, 1e-30f), 1e30f);
-        }
+        const float bound = fmaxf(__uint_as_float(p.amax[2 * ps + 1]) * red[0][0], __uint_as_float(p.amax[2 * ps]) * red[1][0]);
+        if (bound > 0.f) s = exp2f(floorf(log2f(64.f / bound)));
+        s = fminf(fmaxf(s, 1e-30f), 1e30f);
         p.lscale[ps * kLevels + t] = s;
         p.linv[ps * kLevels + t] = 1.f / s;
         p.lamax[ps * kLevels + t] = 0u;
       }
       __syncthreads();
       if (t < 2) p.amax[2 * ps + t] = 0u;
-    } else if (t == 0 && !kBwdBf16) {
+    } else if (t == 0) {
       const float s0 = p.lscale[ps * kLevels];
       float prev = s0;
       for (int v = 1; v < kLevels; ++v) {
@@ -714,12 +693,12 @@ struct WgScratch {
   uint64_t empty[kWgStages];
 };
 
-// Persistent: CTA b works through pieces [cta_first[b], cta_first[b + 1]) - the host cuts the
-// concatenation of all (pass, layer) GEMMs into one equal-byte share per SM (capi.cu plan_wgrad), so
-// there is exactly one wave and every SM streams the same number of bytes.
+// CTA b works through pieces [cta_first[b], cta_first[b + 1]).  The host (capi.cu plan_wgrad) gives every
+// (pass, layer) GEMM whole CTAs, one piece each, in proportion to the bytes it streams (at least one per
+// GEMM); the CTAs of one GEMM take its chunks round-robin.  CTAs do not synchronise with each other, so the
+// grid may run in more than one wave.
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __restrict__ jobs,
-                                                               const int* __restrict__ cta_first, uint32_t copy_bytes,
-                                                               uint32_t exp_flags, int* status) {
+                                                               const int* __restrict__ cta_first, int* status) {
   extern __shared__ __align__(1024) uint8_t smem[];
   WgScratch* sc = reinterpret_cast<WgScratch*>(smem + kWgScratch);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -751,8 +730,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
             mbar_arrive_expect_tx(full, kWgABytes + b_bytes);
             const uint8_t* sa = job.a + static_cast<unsigned long long>(c) * a_bytes + hh * kWgABytes;
             const uint8_t* sb = job.b + static_cast<unsigned long long>(c) * b_bytes;
-            for (uint32_t o = 0; o < kWgABytes; o += copy_bytes) bulk_g2s(dst + o, sa + o, min(copy_bytes, kWgABytes - o), full);
-            for (uint32_t o = 0; o < b_bytes; o += copy_bytes) bulk_g2s(dst + kWgABytes + o, sb + o, min(copy_bytes, b_bytes - o), full);
+            bulk_g2s(dst, sa, kWgABytes, full);
+            bulk_g2s(dst + kWgABytes, sb, b_bytes, full);
             if (++stage == kWgStages) { stage = 0; phase ^= 1; }
           }
         }
@@ -773,19 +752,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
         for (int c = job.chunk0; c < job.chunk1; c += job.chunk_step) {
           mbar_wait(smem_u32(&sc->full[stage]), phase, 52);
           const uint32_t base = smem_u32(smem + stage * kWgStageBytes);
-          if (!(exp_flags & 1u)) {      // exp bit 0: no MMAs (timing experiment)
-            wgmma_fence();
+          wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {        // 16 samples = two 8-row groups = 2048 B per K step
-              const uint64_t ad = make_desc_mn_sw128(base + w * 8192 + j * 2048, 8192, 1024);
-              const uint64_t bd = make_desc_mn_sw128(base + kWgABytes + j * 2048, 8192, 1024);
-              if (N == 256) wgmma_n256_ss_mn(acc, ad, bd, 1u);
-              else wgmma_n64_ss_mn(reinterpret_cast<float(&)[32]>(acc), ad, bd, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            reg_fence(acc);
+          for (int j = 0; j < 4; ++j) {        // 16 samples = two 8-row groups = 2048 B per K step
+            const uint64_t ad = make_desc_mn_sw128(base + w * 8192 + j * 2048, 8192, 1024);
+            const uint64_t bd = make_desc_mn_sw128(base + kWgABytes + j * 2048, 8192, 1024);
+            if (N == 256) wgmma_n256_ss_mn(acc, ad, bd, 1u);
+            else wgmma_n64_ss_mn(reinterpret_cast<float(&)[32]>(acc), ad, bd, 1u);
           }
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(acc);
           __syncwarp();
           if (lane == 0) mbar_arrive(smem_u32(&sc->empty[stage]));
           if (++stage == kWgStages) { stage = 0; phase ^= 1; }
@@ -816,7 +793,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
     bool overflow = false;
     for (int pi = p0; pi < p1; ++pi) {
       const WgradJob job = jobs[pi];
-      const bool a_act = job.bias_out != nullptr && !(exp_flags & 2u);   // exp bit 1: no reductions
+      const bool a_act = job.bias_out != nullptr;
       for (int hh = 0; hh < (job.a_fb >> 1); ++hh) {
         float sa[8];
 #pragma unroll
@@ -834,16 +811,14 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
                 const uint4 v = *reinterpret_cast<const uint4*>(blk + r * 128 + ((rc ^ (r & 7u)) << 4));
                 hacc[0] = bwd_add_x2(hacc[0], v.x); hacc[1] = bwd_add_x2(hacc[1], v.y);
                 hacc[2] = bwd_add_x2(hacc[2], v.z); hacc[3] = bwd_add_x2(hacc[3], v.w);
-                if (!kBwdBf16) {
-                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.x)));
-                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.y)));
-                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.z)));
-                  vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.w)));
-                }
+                vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.x)));
+                vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.y)));
+                vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.z)));
+                vmax = __hmax2(vmax, __habs2(*reinterpret_cast<const __half2*>(&v.w)));
               }
 #pragma unroll
               for (int qq = 0; qq < 4; ++qq) {
-                const float2 f = bwd_x2_to_float2(hacc[qq]);
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hacc[qq]));
                 sa[2 * qq] += f.x;
                 sa[2 * qq + 1] += f.y;
               }

@@ -41,24 +41,13 @@ struct DeviceInfo {
   bool attrs_set = false;
   int* status = nullptr;        // device view of the mapped status word below
   volatile int* status_host = nullptr;   // pinned, mapped: the kernels write it, the host polls it without a sync
-  long long* timeline = nullptr;
 };
 
-// Experiment switches are read ONCE per process (NERFB200_FLAGS: bit 1 = device timeline in
-// -DNERFB200_TIMELINE builds; NERFB200_MAX_CTAS: cap on the persistent grid).  Unset in production.
+// Read ONCE per process.  NERFB200_MAX_CTAS caps the persistent grids (render and mesh kernels), so tests can
+// show that results do not depend on the grid; unset in production.
 struct EnvSwitches {
-  unsigned flags = 0;
   int max_ctas = 0;
-  int wg_plan = 1;        // wgrad plan: 0 = contiguous equal-byte shares, 1 = whole CTAs per GEMM, chunks interleaved
-  int wg_copy = 32768;    // bytes per bulk copy of a wgrad operand chunk
-  unsigned wg_exp = 0;    // wgrad timing experiments: bit 0 = no MMAs, bit 1 = no CUDA-core reductions
-  int no_zero_copy = 0;   // host entry: always stage through device memory (A/B of the mapped-memory fast path)
   EnvSwitches() {
-    if (const char* v = std::getenv("NERFB200_NO_ZERO_COPY")) no_zero_copy = std::atoi(v);
-    if (const char* v = std::getenv("NERFB200_WG_EXP")) wg_exp = static_cast<unsigned>(std::atoi(v));
-    if (const char* v = std::getenv("NERFB200_WG_PLAN")) wg_plan = std::atoi(v);
-    if (const char* v = std::getenv("NERFB200_WG_COPY")) wg_copy = std::atoi(v);
-    if (const char* f = std::getenv("NERFB200_FLAGS")) flags = static_cast<unsigned>(std::strtoul(f, nullptr, 0));
     if (const char* mc = std::getenv("NERFB200_MAX_CTAS")) max_ctas = std::atoi(mc);
   }
 };
@@ -203,7 +192,6 @@ struct TrainLayout {
   size_t bytes;
 };
 
-struct TrainLayout;
 void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first);
 
 void job_shape(int kind, int* a_fb, int* b_fb) {
@@ -228,56 +216,16 @@ void take_pass_bufs(PassBufs& b, Take&& take) {
   b.dpre = take(np * 512 * 8);
 }
 
-void make_train_layout(TrainLayout* L, uint8_t* base, int64_t n_rays, int n_samples, int n_importance, int sm_count) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) -> uint8_t* {
-    uint8_t* ptr = base ? base + off : nullptr;
-    off += (bytes + 1023) & ~static_cast<size_t>(1023);
-    return ptr;
-  };
-  L->n_pass = n_importance > 0 ? 2 : 1;
-  L->n_rays = static_cast<int>(n_rays);
-  L->n_kinds = kNumJobKinds;
-  L->xdir = nullptr;
-  std::memset(L->pass, 0, sizeof(L->pass));
-  for (int ps = 0; ps < L->n_pass; ++ps) {
-    PassBufs& b = L->pass[ps];
-    b.S = ps ? n_samples + n_importance : n_samples;
-    b.n = n_rays * b.S;
-    b.n_pad = (b.n + 127) / 128 * 128;
-    take_pass_bufs(b, take);
-  }
-  // wgrad plan: the concatenation of all (pass, layer) GEMMs, measured in 8 KiB blocks streamed, is cut
-  // into one equal share per SM; a share boundary inside a GEMM splits it into two pieces
-  plan_wgrad(L, sm_count > 0 ? sm_count : 148, nullptr, nullptr);
-  L->jobs_dev = reinterpret_cast<WgradJob*>(take(sizeof(WgradJob) * kMaxWgJobs));
-  L->cta_first_dev = reinterpret_cast<int*>(take(sizeof(int) * (kMaxWgCtas + 1)));
-  L->wg_part = reinterpret_cast<float*>(take(static_cast<size_t>(L->n_jobs) * kWgSlotFloats * 4));
-  L->head_grid = static_cast<int>((L->n_pass * n_rays + kHeadWarps - 1) / kHeadWarps);
-  L->direnc = reinterpret_cast<float*>(take(static_cast<size_t>(n_rays) * 28 * 4));
-  for (int ps = 0; ps < 2; ++ps) {
-    L->head_part[ps] = reinterpret_cast<float*>(take(static_cast<size_t>(L->head_grid) * kHeadPartFloats * 4));
-    L->raysum[ps] = reinterpret_cast<float*>(take(static_cast<size_t>(n_rays) * 128 * 4));
-    L->dir_part[ps] = reinterpret_cast<float*>(take(static_cast<size_t>(kDirSlices) * 128 * 27 * 4));
-    L->gWp[ps] = reinterpret_cast<float*>(take(128 * 256 * 4));
-    L->gbp[ps] = reinterpret_cast<float*>(take(128 * 4));
-  }
-  L->lscale = reinterpret_cast<float*>(take(2 * kLevels * 4));
-  L->linv = reinterpret_cast<float*>(take(2 * kLevels * 4));
-  L->lamax = reinterpret_cast<unsigned*>(take(2 * kLevels * 4));
-  L->amax = reinterpret_cast<unsigned*>(take(16));
-  L->loss_part = reinterpret_cast<float*>(take(1024 * 2 * 4));
-  L->loss_counter = reinterpret_cast<unsigned*>(take(16));
-  L->bytes = off;
-}
-
-// The workspace of a direct NeRF.forward call over n samples (nerfb200_nerf_forward_train / nerfb200_nerf_backward):
-// one pass with one sample per row, the per-pass buffers of the render path in the same order (so one reader serves
-// both), then the direction rows the forward fed the tensor core, the wgrad plan (with the direction-slice GEMM
-// kJDir) and the head partials.  The head kernel views the batch as n_pad / 64 pseudo-rays of 64 samples; nothing
-// per ray (raysum, direnc, dir_part) exists here.
+// Both training workspaces.  The render path (nerfb200_render_rays in training mode, nerfb200_render_backward):
+// n rays, a coarse pass of n_samples per ray and, when n_importance > 0, a fine pass of n_samples + n_importance.
+// A direct NeRF.forward call over n samples (`mlp`: nerfb200_nerf_forward_train, nerfb200_nerf_backward): one pass
+// with one sample per row, the per-pass buffers of the render path in the same order (so one reader serves both),
+// then the direction rows the forward fed the tensor core, the wgrad plan (with the direction-slice GEMM kJDir) and
+// the head partials.  Its head kernel views the batch as n_pad / 64 pseudo-rays of 64 samples; nothing per ray
+// (direnc, raysum, dir_part) and no fused loss exists there.
 constexpr int kMlpPseudoRay = 64;
-void make_mlp_train_layout(TrainLayout* L, uint8_t* base, int64_t n, int sm_count) {
+void make_train_layout(TrainLayout* L, uint8_t* base, bool mlp, int64_t n, int n_samples, int n_importance,
+                       int sm_count) {
   size_t off = 0;
   auto take = [&](size_t bytes) -> uint8_t* {
     uint8_t* ptr = base ? base + off : nullptr;
@@ -285,27 +233,41 @@ void make_mlp_train_layout(TrainLayout* L, uint8_t* base, int64_t n, int sm_coun
     return ptr;
   };
   std::memset(L, 0, sizeof(*L));
-  L->n_pass = 1;
-  L->n_kinds = kNumJobKindsMlp;
-  PassBufs& b = L->pass[0];
-  b.S = 1;
-  b.n = n;
-  b.n_pad = (n + 127) / 128 * 128;
-  take_pass_bufs(b, take);
-  L->xdir = take(static_cast<size_t>(b.n_pad) * 128);
-  L->n_rays = static_cast<int>(b.n_pad / kMlpPseudoRay);
+  L->n_pass = n_importance > 0 ? 2 : 1;
+  L->n_kinds = mlp ? kNumJobKindsMlp : kNumJobKinds;
+  for (int ps = 0; ps < L->n_pass; ++ps) {
+    PassBufs& b = L->pass[ps];
+    b.S = ps ? n_samples + n_importance : n_samples;
+    b.n = n * b.S;
+    b.n_pad = (b.n + 127) / 128 * 128;
+    take_pass_bufs(b, take);
+  }
+  if (mlp) L->xdir = take(static_cast<size_t>(L->pass[0].n_pad) * 128);
+  const int64_t head_rays = mlp ? L->pass[0].n_pad / kMlpPseudoRay : n;
+  L->n_rays = static_cast<int>(head_rays);
   plan_wgrad(L, sm_count > 0 ? sm_count : 148, nullptr, nullptr);
   L->jobs_dev = reinterpret_cast<WgradJob*>(take(sizeof(WgradJob) * kMaxWgJobs));
   L->cta_first_dev = reinterpret_cast<int*>(take(sizeof(int) * (kMaxWgCtas + 1)));
   L->wg_part = reinterpret_cast<float*>(take(static_cast<size_t>(L->n_jobs) * kWgSlotFloats * 4));
-  L->head_grid = (L->n_rays + kHeadWarps - 1) / kHeadWarps;
-  L->head_part[0] = reinterpret_cast<float*>(take(static_cast<size_t>(L->head_grid) * kHeadPartFloats * 4));
-  L->gWp[0] = reinterpret_cast<float*>(take(128 * 256 * 4));
-  L->gbp[0] = reinterpret_cast<float*>(take(128 * 4));
+  L->head_grid = static_cast<int>((L->n_pass * head_rays + kHeadWarps - 1) / kHeadWarps);
+  if (!mlp) L->direnc = reinterpret_cast<float*>(take(static_cast<size_t>(n) * 28 * 4));
+  for (int ps = 0; ps < (mlp ? 1 : 2); ++ps) {
+    L->head_part[ps] = reinterpret_cast<float*>(take(static_cast<size_t>(L->head_grid) * kHeadPartFloats * 4));
+    if (!mlp) {
+      L->raysum[ps] = reinterpret_cast<float*>(take(static_cast<size_t>(n) * 128 * 4));
+      L->dir_part[ps] = reinterpret_cast<float*>(take(static_cast<size_t>(kDirSlices) * 128 * 27 * 4));
+    }
+    L->gWp[ps] = reinterpret_cast<float*>(take(128 * 256 * 4));
+    L->gbp[ps] = reinterpret_cast<float*>(take(128 * 4));
+  }
   L->lscale = reinterpret_cast<float*>(take(2 * kLevels * 4));
   L->linv = reinterpret_cast<float*>(take(2 * kLevels * 4));
   L->lamax = reinterpret_cast<unsigned*>(take(2 * kLevels * 4));
   L->amax = reinterpret_cast<unsigned*>(take(16));
+  if (!mlp) {
+    L->loss_part = reinterpret_cast<float*>(take(1024 * 2 * 4));
+    L->loss_counter = reinterpret_cast<unsigned*>(take(16));
+  }
   L->bytes = off;
 }
 
@@ -356,85 +318,47 @@ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
       work[ps][k] = (L->pass[ps].n_pad / 64) * (a_fb + b_fb);
       total += work[ps][k];
     }
-  const int n_kinds = L->n_pass * kinds;
-  if (env_switches().wg_plan == 1 && n_cta >= n_kinds) {
-    // ---- plan 1: whole CTAs per GEMM (largest-remainder apportionment of the SMs by bytes streamed); the
-    // CTAs of one GEMM take its chunks round-robin, so together they read ONE moving window of each operand
-    int n_of[2][kNumJobKindsMlp];
-    double frac[2][kNumJobKindsMlp];
-    int used = 0;
-    for (int ps = 0; ps < L->n_pass; ++ps)
-      for (int k = 0; k < kinds; ++k) {
-        const double share = static_cast<double>(work[ps][k]) * n_cta / static_cast<double>(total);
-        int n = static_cast<int>(share);
-        if (n < 1) n = 1;
-        n_of[ps][k] = n;
-        frac[ps][k] = share - n;
-        used += n;
-      }
-    while (used < n_cta) {          // hand the remaining SMs to the GEMMs with the most work per CTA
-      int bp = 0, bk = 0;
-      double best = -1;
-      for (int ps = 0; ps < L->n_pass; ++ps)
-        for (int k = 0; k < kinds; ++k) {
-          const double load = static_cast<double>(work[ps][k]) / n_of[ps][k];
-          if (load > best) { best = load; bp = ps; bk = k; }
-        }
-      ++n_of[bp][bk];
-      ++used;
-    }
-    (void)frac;
-    int piece = 0;
-    for (int ps = 0; ps < L->n_pass; ++ps)
-      for (int k = 0; k < kinds; ++k) {
-        const long long chunks = L->pass[ps].n_pad / 64;
-        int g = n_of[ps][k];
-        if (g > chunks) g = static_cast<int>(chunks);
-        L->first_job[ps][k] = piece;
-        for (int j = 0; j < g; ++j) {
-          fill_piece(L, jobs, piece, ps, k, j, chunks, g);
-          if (cta_first) cta_first[piece] = piece;
-          ++piece;
-        }
-        L->n_split[ps][k] = g;
-      }
-    if (cta_first) cta_first[piece] = piece;
-    L->n_jobs = piece;
-    L->n_cta = piece;
-    return;
-  }
-  // ---- plan 0: the concatenation of all GEMMs cut into one equal-byte share per SM
-  int cta = 0, piece = 0;
-  long long done = 0;                                  // units handed out so far
-  if (cta_first) cta_first[0] = 0;
+  // whole CTAs per GEMM: a share of the SMs by bytes streamed, at least one (with fewer SMs than GEMMs the grid runs
+  // in more than one wave); the CTAs of one GEMM take its chunks round-robin, so together they read ONE moving window
+  // of each operand
+  int n_of[2][kNumJobKindsMlp];
+  int used = 0;
   for (int ps = 0; ps < L->n_pass; ++ps)
     for (int k = 0; k < kinds; ++k) {
-      int a_fb, b_fb;
-      job_shape(k, &a_fb, &b_fb);
-      const long long unit = a_fb + b_fb, chunks = L->pass[ps].n_pad / 64;
-      L->first_job[ps][k] = piece;
-      long long c = 0;
-      while (c < chunks) {
-        const long long end = total * (cta + 1) / n_cta;
-        long long take_chunks = (end - done + unit - 1) / unit;       // chunks until this CTA's share is full
-        if (take_chunks < 1) take_chunks = 1;
-        if (take_chunks > chunks - c) take_chunks = chunks - c;
-        fill_piece(L, jobs, piece, ps, k, c, c + take_chunks, 1);
-        ++piece;
-        c += take_chunks;
-        done += take_chunks * unit;
-        while (cta < n_cta - 1 && done >= total * (cta + 1) / n_cta) {
-          ++cta;
-          if (cta_first) cta_first[cta] = piece;
-        }
-      }
-      L->n_split[ps][k] = piece - L->first_job[ps][k];
+      const double share = static_cast<double>(work[ps][k]) * n_cta / static_cast<double>(total);
+      int n = static_cast<int>(share);
+      if (n < 1) n = 1;
+      n_of[ps][k] = n;
+      used += n;
     }
-  if (cta_first) {
-    for (int i = cta + 1; i <= n_cta; ++i) cta_first[i] = piece;
+  while (used < n_cta) {          // hand the remaining SMs to the GEMMs with the most work per CTA
+    int bp = 0, bk = 0;
+    double best = -1;
+    for (int ps = 0; ps < L->n_pass; ++ps)
+      for (int k = 0; k < kinds; ++k) {
+        const double load = static_cast<double>(work[ps][k]) / n_of[ps][k];
+        if (load > best) { best = load; bp = ps; bk = k; }
+      }
+    ++n_of[bp][bk];
+    ++used;
   }
+  int piece = 0;
+  for (int ps = 0; ps < L->n_pass; ++ps)
+    for (int k = 0; k < kinds; ++k) {
+      const long long chunks = L->pass[ps].n_pad / 64;
+      int g = n_of[ps][k];
+      if (g > chunks) g = static_cast<int>(chunks);
+      L->first_job[ps][k] = piece;
+      for (int j = 0; j < g; ++j) {
+        fill_piece(L, jobs, piece, ps, k, j, chunks, g);
+        if (cta_first) cta_first[piece] = piece;
+        ++piece;
+      }
+      L->n_split[ps][k] = g;
+    }
+  if (cta_first) cta_first[piece] = piece;
   L->n_jobs = piece;
-  L->n_cta = n_cta;
+  L->n_cta = piece;
 }
 
 // grow-only device arena for the *_host entry
@@ -476,16 +400,14 @@ void launch_chain(ChainParams& cp, long long t0, long long t1, long long pt0, lo
     cp.span[ps] = span[ps] > 0 ? span[ps] : 1;
     cp.stride[ps] = s;
   }
-  if (!kBwdBf16) {
-    cp.tiles[0] = cp.head[0] = pt0;
-    cp.tiles[1] = cp.head[1] = pt1;
-    const int pc = static_cast<int>(pt0 + pt1);
-    chain_bwd_kernel<true><<<pc, kThreads, kChSmemTotal, stream>>>(cp);
-    g_launches++;
-    sp.phase = 1;
-    bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
-    g_launches++;
-  }
+  cp.tiles[0] = cp.head[0] = pt0;
+  cp.tiles[1] = cp.head[1] = pt1;
+  const int pc = static_cast<int>(pt0 + pt1);
+  chain_bwd_kernel<true><<<pc, kThreads, kChSmemTotal, stream>>>(cp);
+  g_launches++;
+  sp.phase = 1;
+  bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
+  g_launches++;
   cp.head[0] = pt0;
   cp.head[1] = pt1;
   cp.tiles[0] = t0;
@@ -534,6 +456,147 @@ void add_reduce_items(ReduceTable& tab, const TrainLayout& L, int ps, float* con
     add(L.dir_part[ps], 128 * 27, kDirSlices, g[18], nullptr, 128, 27, 27, 283, 256);
 }
 
+// Both *_workspace_init entries, after their own checks: zero the workspace (padding rows of the operand arrays are
+// never written afterwards, counters start at zero), upload the wgrad plan, and return once both are on the device.
+int init_train_workspace(TrainLayout& L, void* ws, int sm_count, cudaStream_t stream) {
+  CUDA_TRY(cudaMemsetAsync(ws, 0, L.bytes, stream), "workspace memset");
+  std::vector<WgradJob> jobs(kMaxWgJobs);
+  std::vector<int> cta_first(kMaxWgCtas + 1, 0);
+  std::memset(jobs.data(), 0, sizeof(WgradJob) * kMaxWgJobs);
+  plan_wgrad(&L, sm_count, jobs.data(), cta_first.data());
+  CUDA_TRY(cudaMemcpyAsync(L.jobs_dev, jobs.data(), sizeof(WgradJob) * kMaxWgJobs, cudaMemcpyHostToDevice, stream),
+           "job table upload");
+  CUDA_TRY(cudaMemcpyAsync(L.cta_first_dev, cta_first.data(), sizeof(int) * (kMaxWgCtas + 1), cudaMemcpyHostToDevice, stream),
+           "cta table upload");
+  CUDA_TRY(cudaStreamSynchronize(stream), "workspace init sync");
+  return 0;
+}
+
+// Steps 2-6 of both training backwards, once step 1 has left each pass's per-sample d sigma / d rgb_pre and their
+// maxima in the workspace.  params / grads / net: per pass.  rays: the render path's rays, whose directions the head
+// kernel embeds for the per-ray direction part of gW_dir; null for a direct NeRF.forward call, whose head kernel walks
+// pseudo-rays of 64 samples and whose direction part is the wgrad GEMM kJDir.
+int backward_tail(const TrainLayout& L, const float* const* const params[2], float* const* const grads[2],
+                  const uint8_t* const net[2], const float* rays, long long ray_stride, const DeviceInfo* d,
+                  cudaStream_t stream, const char* what) {
+  const int q1 = L.n_pass > 1 ? 1 : 0;        // table entry of the second pass: a single pass fills both slots
+  ScaleParams sp;
+  sp.n_pass = L.n_pass; sp.phase = 0;
+  sp.amax = L.amax; sp.lamax = L.lamax; sp.lscale = L.lscale; sp.linv = L.linv;
+  sp.w_rgb[0] = params[0][22]; sp.w_rgb[1] = params[q1][22];
+  sp.w_sigma[0] = params[0][20]; sp.w_sigma[1] = params[q1][20];
+  bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
+  g_launches++;
+  // 2. rgb head, ReLU of the direction layer (both passes in one launch), direction part of gW_dir
+  HeadBwdParams hp;
+  hp.n_rays = L.n_rays; hp.n_pass = L.n_pass;
+  hp.pass[0] = L.pass[0]; hp.pass[1] = L.pass[1];
+  if (!rays) {
+    hp.pass[0].S = kMlpPseudoRay;
+    hp.pass[1] = hp.pass[0];
+  }
+  hp.w_rgb[0] = params[0][22]; hp.w_rgb[1] = params[q1][22];
+  hp.lscale = L.lscale;
+  hp.rays = rays; hp.ray_stride = ray_stride;
+  hp.raysum[0] = L.raysum[0]; hp.raysum[1] = L.raysum[1];
+  hp.direnc = L.direnc;
+  hp.part[0] = L.head_part[0]; hp.part[1] = L.head_part[1];
+  head_bwd_kernel<<<L.head_grid, kHeadWarps * 32, 0, stream>>>(hp);
+  g_launches++;
+  if (rays) {
+    DirGradParams dp;
+    dp.n_rays = L.n_rays;
+    dp.raysum[0] = L.raysum[0]; dp.raysum[1] = L.raysum[1];
+    dp.direnc = L.direnc;
+    dp.part[0] = L.dir_part[0]; dp.part[1] = L.dir_part[1];
+    dir_grad_kernel<<<dim3(kDirSlices, L.n_pass), 128, 0, stream>>>(dp);
+    g_launches++;
+  }
+  // 3. dgrad chain (wgmma): a probe pass over one tile per SM picks the per-layer scales, then the real pass.
+  // The probe's tiles are spread evenly over each pass: gradients are not uniform over a batch (rays whose
+  // colour is already right carry almost none), and scales taken from the first tiles alone saturate the rest.
+  // Both launches visit the tiles of a pass in the order j -> j * stride mod span (stride coprime to span, about
+  // span / probe tiles), the real pass the probe's tiles first, so its first wave finds them in L2.  A tile the
+  // probe did not see can still exceed its level's range: the wgrad kernel reports that (status 102).
+  ChainParams cp;
+  cp.n_pass = L.n_pass;
+  cp.pass[0] = L.pass[0]; cp.pass[1] = L.pass[1];
+  cp.net[0] = net[0]; cp.net[1] = net[1];
+  cp.lscale = L.lscale;
+  cp.lamax = L.lamax;
+  cp.status = d->status;
+  const long long t0 = L.pass[0].n_pad / 128, t1 = q1 ? L.pass[1].n_pad / 128 : 0;
+  const long long probe = q1 ? (d->sm_count + 1) / 2 : d->sm_count;      // probe tiles per pass, at most
+  launch_chain(cp, t0, t1, t0 < probe ? t0 : probe, t1 < probe ? t1 : probe, sp, d->sm_count, stream);
+  // 4. split-K wgrad (wgmma)
+  wgrad_kernel<<<L.n_cta, kWgThreads, kWgSmemTotal, stream>>>(L.jobs_dev, L.cta_first_dev, d->status);
+  g_launches++;
+  // 5. partial sums -> gradient tensors (fixed order), 6. unfold W'
+  ReduceTable tab;
+  tab.n = 0;
+  for (int ps = 0; ps < L.n_pass; ++ps) add_reduce_items(tab, L, ps, grads[ps]);
+  wgrad_reduce_kernel<<<dim3(64, tab.n), 256, 0, stream>>>(tab);   // latency-bound: 64 blocks per item (16 measured 40 us)
+  g_launches++;
+  UnfoldParams up;
+  for (int ps = 0; ps < 2; ++ps) {
+    const int q = ps ? q1 : 0;
+    up.gWp[ps] = L.gWp[q]; up.gbp[ps] = L.gbp[q];
+    up.Wf[ps] = params[q][16]; up.bf[ps] = params[q][17]; up.Wd[ps] = params[q][18];
+    up.gWd[ps] = grads[q][18]; up.gbd[ps] = grads[q][19]; up.gWf[ps] = grads[q][16]; up.gbf[ps] = grads[q][17];
+  }
+  // warps: one per gWd output (128 x 256), then one thread per gWf / gbf output
+  unfold_kernel<<<dim3((128 * 256 + (256 * 256 + 256 + 31) / 32 + 7) / 8, L.n_pass), 256, 0, stream>>>(up);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), what);
+  return 0;
+}
+
+// The four entries of mlp_forward_kernel, after their own checks: one CTA per 128-row tile, at most one per SM.  With
+// a NeRF.forward training workspace `ws` the save-mode instantiation also stores what nerfb200_nerf_backward reads.
+int launch_mlp(MlpParams p, void* ws, void* stream, const char* what) {
+  DeviceInfo* d = nullptr;
+  int rc = device_info(&d);
+  if (rc) return rc;
+  if ((rc = check_sticky_status(d)) != 0) return rc;
+  p.status = d->status;
+  const long long tiles = (p.n + 127) / 128;
+  const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
+  if (ws) {
+    TrainLayout L;
+    make_train_layout(&L, static_cast<uint8_t*>(ws), true, p.n, 1, 0, d->sm_count);
+    p.tr = L.pass[0];
+    p.xdir = L.xdir;
+    mlp_forward_kernel<true><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
+  } else {
+    mlp_forward_kernel<false><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
+  }
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), what);
+  return 0;
+}
+
+// The tensor table of both Adam entries: each tensor checked (steps: the device step counts, or null) and given its
+// run of 1024-element blocks.  *blocks: the total.
+int fill_adam_table(AdamParams& a, int32_t n_tensors, float* const* params, const float* const* grads,
+                    float* const* exp_avg, float* const* exp_avg_sq, const int64_t* numel, const float* const* steps,
+                    float beta1, float beta2, float eps, float weight_decay, const char* who, int* blocks) {
+  a.n_tensors = n_tensors;
+  int b = 0;
+  for (int i = 0; i < n_tensors; ++i) {
+    if (numel[i] < 0 || numel[i] > 0x7fffffff ||
+        (numel[i] > 0 && (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i] || (steps && !steps[i]))))
+      return fail(NERFB200_EINVAL, "%s: NULL tensor / bad size", who);
+    a.p[i] = params[i]; a.g[i] = grads[i]; a.m[i] = exp_avg[i]; a.v[i] = exp_avg_sq[i];
+    a.numel[i] = static_cast<int>(numel[i]);
+    a.block0[i] = b;
+    b += static_cast<int>((numel[i] + 1023) / 1024);
+  }
+  a.block0[n_tensors] = b;
+  a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
+  *blocks = b;
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -558,7 +621,6 @@ static int fill_pack_params(PackParams* pp, const float* const params[24], void*
     pp->p[i] = params[i];
   }
   pp->out = static_cast<uint8_t*>(packed);
-  pp->bwd_bf16 = kBwdBf16 ? 1 : 0;
   return 0;
 }
 
@@ -638,7 +700,8 @@ int nerfb200_render_rays(const nerfb200_render_args* a, void* stream) {
   if (a->target && !save) return fail(NERFB200_EINVAL, "the fused loss epilogue needs train_workspace%s");
   if (save) {
     TrainLayout L;
-    make_train_layout(&L, static_cast<uint8_t*>(a->train_workspace), a->n_rays, a->n_samples, a->n_importance, d->sm_count);
+    make_train_layout(&L, static_cast<uint8_t*>(a->train_workspace), false, a->n_rays, a->n_samples, a->n_importance,
+                      d->sm_count);
     p.train = 1;
     p.tr[0] = L.pass[0];
     p.tr[1] = L.pass[1];
@@ -655,17 +718,6 @@ int nerfb200_render_rays(const nerfb200_render_args* a, void* stream) {
       p.loss_counter = L.loss_counter;
     }
   }
-  p.flags = env_switches().flags;
-  p.timeline = nullptr;
-#ifdef NERFB200_TIMELINE
-  if (p.flags & 2u) {
-    if (!d->timeline) {
-      CUDA_TRY(cudaMalloc(&d->timeline, 3 * kTlMax * 2 * sizeof(long long)), "timeline alloc");
-    }
-    CUDA_TRY(cudaMemsetAsync(d->timeline, 0, 3 * kTlMax * 2 * sizeof(long long), static_cast<cudaStream_t>(stream)), "timeline memset");
-    p.timeline = d->timeline;
-  }
-#endif
   const int n_groups = (p.n_rays + 1) / 2;     // two rays share the coarse tile
   int ctas = d->sm_count;
   if (a->max_ctas > 0 && a->max_ctas < ctas) ctas = a->max_ctas;
@@ -726,7 +778,7 @@ int nerfb200_render_rays_host(const nerfb200_render_args* h, void* stream_v) {
     NERFB200_MAP(weights_coarse, float*)
     NERFB200_MAP(weights_fine, float*)
 #undef NERFB200_MAP
-    if (all_mapped && !env_switches().no_zero_copy) {
+    if (all_mapped) {
       int dev0 = 0;
       CUDA_TRY(cudaGetDevice(&dev0), "cudaGetDevice");
       static int* host_status[64] = {nullptr};
@@ -840,23 +892,12 @@ int nerfb200_nerf_forward(const float* x, int64_t n, int64_t x_stride, const voi
     return fail(NERFB200_EINVAL, "nerf_forward: x_stride too small for the input width%s");
   if (!sigma_only && (reinterpret_cast<uintptr_t>(out) & 15))
     return fail(NERFB200_EINVAL, "nerf_forward: out must be 16-byte aligned%s");
-  DeviceInfo* d = nullptr;
-  int rc = device_info(&d);
-  if (rc) return rc;
-  if ((rc = check_sticky_status(d)) != 0) return rc;
-  MlpParams p;
-  p.raw_xyz = 0;
+  MlpParams p{};
   p.x = x; p.x_stride = x_stride; p.n = n;
   p.net = static_cast<const uint8_t*>(packed);
   p.sigma_only = sigma_only;
   p.out = out;
-  p.status = d->status;
-  const long long tiles = (n + 127) / 128;
-  const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
-  mlp_forward_kernel<false><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
-  g_launches++;
-  CUDA_TRY(cudaGetLastError(), "nerf_forward launch");
-  return 0;
+  return launch_mlp(p, nullptr, stream, "nerf_forward launch");
 }
 
 int nerfb200_query_sigma(const float* xyz, int64_t n, int64_t xyz_stride, const void* packed, float* sigma,
@@ -865,23 +906,13 @@ int nerfb200_query_sigma(const float* xyz, int64_t n, int64_t xyz_stride, const 
   if (n == 0) return 0;
   if (!xyz || !packed || !sigma) return fail(NERFB200_EINVAL, "query_sigma: NULL argument%s");
   if (xyz_stride < 3) return fail(NERFB200_EINVAL, "query_sigma: xyz_stride < 3%s");
-  DeviceInfo* d = nullptr;
-  int rc = device_info(&d);
-  if (rc) return rc;
-  if ((rc = check_sticky_status(d)) != 0) return rc;
-  MlpParams p;
+  MlpParams p{};
   p.raw_xyz = 1;
   p.x = xyz; p.x_stride = xyz_stride; p.n = n;
   p.net = static_cast<const uint8_t*>(packed);
   p.sigma_only = 1;
   p.out = sigma;
-  p.status = d->status;
-  const long long tiles = (n + 127) / 128;
-  const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
-  mlp_forward_kernel<false><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
-  g_launches++;
-  CUDA_TRY(cudaGetLastError(), "query_sigma launch");
-  return 0;
+  return launch_mlp(p, nullptr, stream, "query_sigma launch");
 }
 
 int nerfb200_query_rgb_sigma(const float* xyz, int64_t n, int64_t xyz_stride, const void* packed, float* rgbsigma,
@@ -891,30 +922,19 @@ int nerfb200_query_rgb_sigma(const float* xyz, int64_t n, int64_t xyz_stride, co
   if (!xyz || !packed || !rgbsigma) return fail(NERFB200_EINVAL, "query_rgb_sigma: NULL argument%s");
   if (xyz_stride < 3) return fail(NERFB200_EINVAL, "query_rgb_sigma: xyz_stride < 3%s");
   if (reinterpret_cast<uintptr_t>(rgbsigma) & 15) return fail(NERFB200_EINVAL, "query_rgb_sigma: out must be 16-byte aligned%s");
-  DeviceInfo* d = nullptr;
-  int rc = device_info(&d);
-  if (rc) return rc;
-  if ((rc = check_sticky_status(d)) != 0) return rc;
-  MlpParams p;
+  MlpParams p{};
   p.raw_xyz = 1;
   p.x = xyz; p.x_stride = xyz_stride; p.n = n;
   p.net = static_cast<const uint8_t*>(packed);
-  p.sigma_only = 0;
   p.out = rgbsigma;
-  p.status = d->status;
-  const long long tiles = (n + 127) / 128;
-  const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
-  mlp_forward_kernel<false><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
-  g_launches++;
-  CUDA_TRY(cudaGetLastError(), "query_rgb_sigma launch");
-  return 0;
+  return launch_mlp(p, nullptr, stream, "query_rgb_sigma launch");
 }
 
 // ---- training a direct NeRF.forward call (models/nerf.py:83-124)
 size_t nerfb200_nerf_train_workspace_bytes(int64_t n) {
   if (n <= 0 || n > 0x7fffffffLL) return 0;
   TrainLayout L;
-  make_mlp_train_layout(&L, nullptr, n, nerfb200_sm_count());
+  make_train_layout(&L, nullptr, true, n, 1, 0, nerfb200_sm_count());
   return L.bytes;
 }
 
@@ -928,20 +948,9 @@ int nerfb200_nerf_train_workspace_init(void* ws, size_t bytes, int64_t n, void* 
   int rc = device_info(&d);
   if (rc) return rc;
   TrainLayout L;
-  make_mlp_train_layout(&L, static_cast<uint8_t*>(ws), n, d->sm_count);
+  make_train_layout(&L, static_cast<uint8_t*>(ws), true, n, 1, 0, d->sm_count);
   if (bytes < L.bytes) return fail(NERFB200_EINVAL, "nerf train workspace too small for n%s");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  CUDA_TRY(cudaMemsetAsync(ws, 0, L.bytes, stream), "nerf workspace memset");
-  std::vector<WgradJob> jobs(kMaxWgJobs);
-  std::vector<int> cta_first(kMaxWgCtas + 1, 0);
-  std::memset(jobs.data(), 0, sizeof(WgradJob) * kMaxWgJobs);
-  plan_wgrad(&L, d->sm_count, jobs.data(), cta_first.data());
-  CUDA_TRY(cudaMemcpyAsync(L.jobs_dev, jobs.data(), sizeof(WgradJob) * kMaxWgJobs, cudaMemcpyHostToDevice, stream),
-           "nerf job table upload");
-  CUDA_TRY(cudaMemcpyAsync(L.cta_first_dev, cta_first.data(), sizeof(int) * (kMaxWgCtas + 1), cudaMemcpyHostToDevice, stream),
-           "nerf cta table upload");
-  CUDA_TRY(cudaStreamSynchronize(stream), "nerf workspace init sync");
-  return 0;
+  return init_train_workspace(L, ws, d->sm_count, static_cast<cudaStream_t>(stream_v));
 }
 
 int nerfb200_nerf_forward_train(const float* x, int64_t n, int64_t x_stride, const void* packed, void* ws, float* out,
@@ -953,27 +962,11 @@ int nerfb200_nerf_forward_train(const float* x, int64_t n, int64_t x_stride, con
   if ((reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(packed) & 15))
     return fail(NERFB200_EINVAL, "nerf_forward_train: out / packed must be 16-byte aligned%s");
   if (reinterpret_cast<uintptr_t>(ws) & 1023) return fail(NERFB200_EINVAL, "nerf train workspace must be 1024-byte aligned%s");
-  DeviceInfo* d = nullptr;
-  int rc = device_info(&d);
-  if (rc) return rc;
-  if ((rc = check_sticky_status(d)) != 0) return rc;
-  TrainLayout L;
-  make_mlp_train_layout(&L, static_cast<uint8_t*>(ws), n, d->sm_count);
-  MlpParams p;
-  p.raw_xyz = 0;
+  MlpParams p{};
   p.x = x; p.x_stride = x_stride; p.n = n;
   p.net = static_cast<const uint8_t*>(packed);
-  p.sigma_only = 0;
   p.out = out;
-  p.status = d->status;
-  p.tr = L.pass[0];
-  p.xdir = L.xdir;
-  const long long tiles = (n + 127) / 128;
-  const int ctas = static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count);
-  mlp_forward_kernel<true><<<ctas, kThreads, kSmemTotal, static_cast<cudaStream_t>(stream)>>>(p);
-  g_launches++;
-  CUDA_TRY(cudaGetLastError(), "nerf_forward_train launch");
-  return 0;
+  return launch_mlp(p, ws, stream, "nerf_forward_train launch");
 }
 
 int nerfb200_nerf_backward(const float* g_out, int64_t n, const void* packed, const float* const params[24], void* ws,
@@ -990,7 +983,7 @@ int nerfb200_nerf_backward(const float* g_out, int64_t n, const void* packed, co
   if (rc) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   TrainLayout L;
-  make_mlp_train_layout(&L, static_cast<uint8_t*>(ws), n, d->sm_count);
+  make_train_layout(&L, static_cast<uint8_t*>(ws), true, n, 1, 0, d->sm_count);
   const PassBufs& pb = L.pass[0];
   // 1. seed: upstream gradient -> per-sample d sigma / d rgb_pre (replaces the compositing backward)
   MlpSeedParams sd;
@@ -999,58 +992,10 @@ int nerfb200_nerf_backward(const float* g_out, int64_t n, const void* packed, co
   sd.amax_bits = L.amax;
   mlp_seed_kernel<<<static_cast<int>((pb.n_pad + 255) / 256), 256, 0, stream>>>(sd);
   g_launches++;
-  ScaleParams sp;
-  sp.n_pass = 1; sp.phase = 0;
-  sp.amax = L.amax; sp.lamax = L.lamax; sp.lscale = L.lscale; sp.linv = L.linv;
-  sp.w_rgb[0] = sp.w_rgb[1] = params[22];
-  sp.w_sigma[0] = sp.w_sigma[1] = params[20];
-  bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
-  g_launches++;
-  // 2. rgb head + ReLU of the direction layer over pseudo-rays of 64 samples (no per-ray direction work)
-  HeadBwdParams hp;
-  hp.n_rays = L.n_rays; hp.n_pass = 1;
-  hp.pass[0] = pb;
-  hp.pass[0].S = kMlpPseudoRay;
-  hp.pass[1] = hp.pass[0];
-  hp.w_rgb[0] = hp.w_rgb[1] = params[22];
-  hp.lscale = L.lscale;
-  hp.rays = nullptr; hp.ray_stride = 0;
-  hp.raysum[0] = hp.raysum[1] = nullptr;
-  hp.direnc = nullptr;
-  hp.part[0] = L.head_part[0]; hp.part[1] = nullptr;
-  head_bwd_kernel<<<L.head_grid, kHeadWarps * 32, 0, stream>>>(hp);
-  g_launches++;
-  // 3. dgrad chain: probe over one tile per SM spread over the batch, then the real pass
-  ChainParams cp;
-  cp.n_pass = 1;
-  cp.pass[0] = cp.pass[1] = pb;
-  cp.net[0] = cp.net[1] = static_cast<const uint8_t*>(packed);
-  cp.lscale = L.lscale;
-  cp.lamax = L.lamax;
-  cp.status = d->status;
-  const long long t0 = pb.n_pad / 128;
-  launch_chain(cp, t0, 0, kBwdBf16 ? 0 : (t0 < d->sm_count ? t0 : d->sm_count), 0, sp, d->sm_count, stream);
-  // 4. split-K wgrad (wgmma), with the direction-slice GEMM dd^T xdir
-  wgrad_kernel<<<L.n_cta, kWgThreads, kWgSmemTotal, stream>>>(L.jobs_dev, L.cta_first_dev,
-                                                               static_cast<uint32_t>(env_switches().wg_copy),
-                                                               env_switches().wg_exp, d->status);
-  g_launches++;
-  // 5. partial sums -> gradient tensors (fixed order), 6. unfold W'
-  ReduceTable tab;
-  tab.n = 0;
-  add_reduce_items(tab, L, 0, grads);
-  wgrad_reduce_kernel<<<dim3(64, tab.n), 256, 0, stream>>>(tab);
-  g_launches++;
-  UnfoldParams up;
-  for (int ps = 0; ps < 2; ++ps) {
-    up.gWp[ps] = L.gWp[0]; up.gbp[ps] = L.gbp[0];
-    up.Wf[ps] = params[16]; up.bf[ps] = params[17]; up.Wd[ps] = params[18];
-    up.gWd[ps] = grads[18]; up.gbd[ps] = grads[19]; up.gWf[ps] = grads[16]; up.gbf[ps] = grads[17];
-  }
-  unfold_kernel<<<dim3((128 * 256 + (256 * 256 + 256 + 31) / 32 + 7) / 8, 1), 256, 0, stream>>>(up);
-  g_launches++;
-  CUDA_TRY(cudaGetLastError(), "nerf_backward launches");
-  return 0;
+  const float* const* const p2[2] = {params, params};
+  float* const* const g2[2] = {grads, grads};
+  const uint8_t* const net[2] = {static_cast<const uint8_t*>(packed), static_cast<const uint8_t*>(packed)};
+  return backward_tail(L, p2, g2, net, nullptr, 0, d, stream, "nerf_backward launches");
 }
 
 int nerfb200_mse_psnr(const float* rgb_coarse, const float* rgb_fine, const float* target, int64_t n_rays,
@@ -1172,7 +1117,7 @@ int nerfb200_to_uint8(const float* src, int64_t n, uint8_t* dst, void* stream) {
 size_t nerfb200_train_workspace_bytes(int64_t n_rays, int32_t n_samples, int32_t n_importance) {
   if (n_rays <= 0 || n_samples <= 0 || n_importance < 0) return 0;
   TrainLayout L;
-  make_train_layout(&L, nullptr, n_rays, n_samples, n_importance, nerfb200_sm_count());
+  make_train_layout(&L, nullptr, false, n_rays, n_samples, n_importance, nerfb200_sm_count());
   return L.bytes;
 }
 
@@ -1184,21 +1129,9 @@ int nerfb200_train_workspace_init(void* workspace, size_t bytes, int64_t n_rays,
   int rc = device_info(&d);
   if (rc) return rc;
   TrainLayout L;
-  make_train_layout(&L, static_cast<uint8_t*>(workspace), n_rays, n_samples, n_importance, d->sm_count);
+  make_train_layout(&L, static_cast<uint8_t*>(workspace), false, n_rays, n_samples, n_importance, d->sm_count);
   if (bytes < L.bytes) return fail(NERFB200_EINVAL, "train workspace too small%s");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  // padding rows of the operand arrays must be zero (never written afterwards), counters zero
-  CUDA_TRY(cudaMemsetAsync(workspace, 0, L.bytes, stream), "workspace memset");
-  std::vector<WgradJob> jobs(kMaxWgJobs);
-  std::vector<int> cta_first(kMaxWgCtas + 1, 0);
-  std::memset(jobs.data(), 0, sizeof(WgradJob) * kMaxWgJobs);
-  plan_wgrad(&L, d->sm_count, jobs.data(), cta_first.data());
-  CUDA_TRY(cudaMemcpyAsync(L.jobs_dev, jobs.data(), sizeof(WgradJob) * kMaxWgJobs, cudaMemcpyHostToDevice, stream),
-           "job table upload");
-  CUDA_TRY(cudaMemcpyAsync(L.cta_first_dev, cta_first.data(), sizeof(int) * (kMaxWgCtas + 1), cudaMemcpyHostToDevice, stream),
-           "cta table upload");
-  CUDA_TRY(cudaStreamSynchronize(stream), "workspace init sync");
-  return 0;
+  return init_train_workspace(L, workspace, d->sm_count, static_cast<cudaStream_t>(stream_v));
 }
 
 int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
@@ -1219,9 +1152,11 @@ int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
   if (rc) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   TrainLayout L;
-  make_train_layout(&L, static_cast<uint8_t*>(a->train_workspace), a->n_rays, a->n_samples, a->n_importance, d->sm_count);
-  const float* const* params[2] = {b->params_coarse, b->params_fine};
-  float* const* grads[2] = {b->grads_coarse, b->grads_fine};
+  make_train_layout(&L, static_cast<uint8_t*>(a->train_workspace), false, a->n_rays, a->n_samples, a->n_importance,
+                    d->sm_count);
+  const float* const* const params[2] = {b->params_coarse, b->params_fine};
+  float* const* const grads[2] = {b->grads_coarse, b->grads_fine};
+  const uint8_t* const net[2] = {static_cast<const uint8_t*>(a->packed_coarse), static_cast<const uint8_t*>(a->packed_fine)};
   const float* g_rgb[2] = {b->g_rgb_coarse, b->g_rgb_fine};
   const float* g_depth[2] = {b->g_depth_coarse, b->g_depth_fine};
   const float* g_opac[2] = {b->g_opacity_coarse, b->g_opacity_fine};
@@ -1243,81 +1178,7 @@ int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
     composite_bwd_kernel<<<(L.n_rays + 3) / 4, 128, 0, stream>>>(cp);
     g_launches++;
   }
-  ScaleParams sp;
-  sp.n_pass = L.n_pass; sp.phase = 0;
-  sp.amax = L.amax; sp.lamax = L.lamax; sp.lscale = L.lscale; sp.linv = L.linv;
-  for (int ps = 0; ps < 2; ++ps) {
-    const int q = ps < L.n_pass ? ps : 0;
-    sp.w_rgb[ps] = params[q][22];
-    sp.w_sigma[ps] = params[q][20];
-  }
-  bwd_scale_kernel<<<1, 128, 0, stream>>>(sp);
-  g_launches++;
-  // 2. rgb head, ReLU of the direction layer (both passes in one launch), direction part of gW_dir
-  {
-    HeadBwdParams hp;
-    hp.n_rays = L.n_rays; hp.n_pass = L.n_pass;
-    hp.pass[0] = L.pass[0]; hp.pass[1] = L.pass[1];
-    hp.w_rgb[0] = params[0][22]; hp.w_rgb[1] = fine ? params[1][22] : params[0][22];
-    hp.lscale = L.lscale;
-    hp.rays = a->rays; hp.ray_stride = a->ray_stride;
-    hp.raysum[0] = L.raysum[0]; hp.raysum[1] = L.raysum[1];
-    hp.direnc = L.direnc;
-    hp.part[0] = L.head_part[0]; hp.part[1] = L.head_part[1];
-    head_bwd_kernel<<<L.head_grid, kHeadWarps * 32, 0, stream>>>(hp);
-    g_launches++;
-    DirGradParams dp;
-    dp.n_rays = L.n_rays;
-    dp.raysum[0] = L.raysum[0]; dp.raysum[1] = L.raysum[1];
-    dp.direnc = L.direnc;
-    dp.part[0] = L.dir_part[0]; dp.part[1] = L.dir_part[1];
-    dir_grad_kernel<<<dim3(kDirSlices, L.n_pass), 128, 0, stream>>>(dp);
-    g_launches++;
-  }
-  // 3. dgrad chain (wgmma): a probe pass over one tile per SM picks the per-layer scales, then the real pass.
-  // The probe's tiles are spread evenly over each pass: gradients are not uniform over a batch (rays whose
-  // colour is already right carry almost none), and scales taken from the first tiles alone saturate the rest.
-  // Both launches visit the tiles of a pass in the order j -> j * stride mod span (stride coprime to span, about
-  // span / probe tiles), the real pass the probe's tiles first, so its first wave finds them in L2.  A tile the
-  // probe did not see can still exceed its level's range: the wgrad kernel reports that (status 102).
-  {
-    ChainParams cp;
-    cp.n_pass = L.n_pass;
-    cp.pass[0] = L.pass[0]; cp.pass[1] = L.pass[1];
-    cp.net[0] = static_cast<const uint8_t*>(a->packed_coarse);
-    cp.net[1] = static_cast<const uint8_t*>(a->packed_fine);
-    cp.lscale = L.lscale;
-    cp.lamax = L.lamax;
-    cp.status = d->status;
-    const long long t0 = L.pass[0].n_pad / 128, t1 = fine ? L.pass[1].n_pad / 128 : 0;
-    const long long half = (d->sm_count + 1) / 2;
-    const long long pt0 = kBwdBf16 ? 0 : (fine ? (t0 < half ? t0 : half) : (t0 < d->sm_count ? t0 : d->sm_count));
-    const long long pt1 = kBwdBf16 ? 0 : (fine ? (t1 < half ? t1 : half) : 0);
-    launch_chain(cp, t0, t1, pt0, pt1, sp, d->sm_count, stream);
-  }
-  // 4. split-K wgrad (wgmma)
-  wgrad_kernel<<<L.n_cta, kWgThreads, kWgSmemTotal, stream>>>(L.jobs_dev, L.cta_first_dev,
-                                                               static_cast<uint32_t>(env_switches().wg_copy),
-                                                               env_switches().wg_exp, d->status);
-  g_launches++;
-  // 5. partial sums -> gradient tensors (fixed order), 6. unfold W'
-  ReduceTable tab;
-  tab.n = 0;
-  for (int ps = 0; ps < L.n_pass; ++ps) add_reduce_items(tab, L, ps, grads[ps]);
-  wgrad_reduce_kernel<<<dim3(64, tab.n), 256, 0, stream>>>(tab);   // latency-bound: 64 blocks per item (16 measured 40 us)
-  g_launches++;
-  UnfoldParams up;
-  for (int ps = 0; ps < 2; ++ps) {
-    const int q = ps < L.n_pass ? ps : 0;
-    up.gWp[ps] = L.gWp[q]; up.gbp[ps] = L.gbp[q];
-    up.Wf[ps] = params[q][16]; up.bf[ps] = params[q][17]; up.Wd[ps] = params[q][18];
-    up.gWd[ps] = grads[q][18]; up.gbd[ps] = grads[q][19]; up.gWf[ps] = grads[q][16]; up.gbf[ps] = grads[q][17];
-  }
-  // warps: one per gWd output (128 x 256), then one thread per gWf / gbf output
-  unfold_kernel<<<dim3((128 * 256 + (256 * 256 + 256 + 31) / 32 + 7) / 8, L.n_pass), 256, 0, stream>>>(up);
-  g_launches++;
-  CUDA_TRY(cudaGetLastError(), "render_backward launches");
-  return 0;
+  return backward_tail(L, params, grads, net, a->rays, a->ray_stride, d, stream, "render_backward launches");
 }
 
 int nerfb200_adam_step(int32_t n_tensors, float* const* params, const float* const* grads, float* const* exp_avg,
@@ -1328,19 +1189,10 @@ int nerfb200_adam_step(int32_t n_tensors, float* const* params, const float* con
   if (!params || !grads || !exp_avg || !exp_avg_sq || !numel || step < 1)
     return fail(NERFB200_EINVAL, "adam_step: NULL argument / step < 1%s");
   AdamParams a;
-  a.n_tensors = n_tensors;
   int blocks = 0;
-  for (int i = 0; i < n_tensors; ++i) {
-    if (numel[i] < 0 || numel[i] > 0x7fffffff ||
-        (numel[i] > 0 && (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i])))
-      return fail(NERFB200_EINVAL, "adam_step: NULL tensor / bad size%s");
-    a.p[i] = params[i]; a.g[i] = grads[i]; a.m[i] = exp_avg[i]; a.v[i] = exp_avg_sq[i];
-    a.numel[i] = static_cast<int>(numel[i]);
-    a.block0[i] = blocks;
-    blocks += static_cast<int>((numel[i] + 1023) / 1024);
-  }
-  a.block0[n_tensors] = blocks;
-  a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
+  const int rc = fill_adam_table(a, n_tensors, params, grads, exp_avg, exp_avg_sq, numel, nullptr, beta1, beta2, eps,
+                                 weight_decay, "adam_step", &blocks);
+  if (rc) return rc;
   // in double, rounded once: 1 - b2^t in fp32 cancels at small t (~50 ulps of the update at t = 2..3)
   a.step_size = static_cast<float>(static_cast<double>(lr) / (1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step))));
   a.bias2_sqrt = static_cast<float>(std::sqrt(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step))));
@@ -1361,20 +1213,11 @@ int nerfb200_adam_step_dev(int32_t n_tensors, float* const* params, const float*
     return fail(NERFB200_EINVAL, "adam_step_dev: NULL argument%s");
   AdamDevParams d;
   AdamParams& a = d.a;
-  a.n_tensors = n_tensors;
   int blocks = 0;
-  for (int i = 0; i < n_tensors; ++i) {
-    if (numel[i] < 0 || numel[i] > 0x7fffffff ||
-        (numel[i] > 0 && (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i] || !steps[i])))
-      return fail(NERFB200_EINVAL, "adam_step_dev: NULL tensor / bad size%s");
-    a.p[i] = params[i]; a.g[i] = grads[i]; a.m[i] = exp_avg[i]; a.v[i] = exp_avg_sq[i];
-    d.step[i] = steps[i];
-    a.numel[i] = static_cast<int>(numel[i]);
-    a.block0[i] = blocks;
-    blocks += static_cast<int>((numel[i] + 1023) / 1024);
-  }
-  a.block0[n_tensors] = blocks;
-  a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
+  const int rc = fill_adam_table(a, n_tensors, params, grads, exp_avg, exp_avg_sq, numel, steps, beta1, beta2, eps,
+                                 weight_decay, "adam_step_dev", &blocks);
+  if (rc) return rc;
+  for (int i = 0; i < n_tensors; ++i) d.step[i] = steps[i];
   a.step_size = a.bias2_sqrt = 0.f;
   d.lr = lr_dev;
   if (blocks == 0) return 0;

@@ -48,8 +48,8 @@ constexpr int kF32WDirPart = kF32BRgb + 4;       // [28][128] transposed: [j][n]
 constexpr int kF32Count = kF32WDirPart + 28 * 128;
 constexpr uint32_t kFwdBytes = kHalfRegionBytes + kF32Count * 4;
 
-// [backward region]  the transposed ("dgrad") slices the backward chain kernel streams, 16-bit
-// (fp16; bf16 only in a -DNERFB200_BWD_BF16 build, csrc/bwd_kernels.cuh), in consumption order.  A slice is a [256 x 64] K-major
+// [backward region]  the transposed ("dgrad") slices the backward chain kernel streams, fp16, in
+// consumption order.  A slice is a [256 x 64] K-major
 // SWIZZLE_128B block with B[n][k] = W[k0 + k][n0 + n]: n = INPUT feature of the layer (the output
 // column of the dgrad GEMM), k = OUTPUT feature (its contraction index).
 //       slice 0..1     W'        (128 x 256, the folded final.dir matrix above)  k blocks 0..1

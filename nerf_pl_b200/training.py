@@ -36,7 +36,22 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else t.data_ptr()
 
 
-class TrainWorkspace:
+class _Workspace:
+    """A 1024-byte aligned device buffer (``buf``, ``bytes`` long; ``raw`` owns it) prepared by the library entry
+    ``init`` as ``init(buf, bytes, *args, stream)``.  ``busy``: held by a call whose backward is pending."""
+
+    def __init__(self, dev: torch.device, nbytes: int, init: str, *args) -> None:
+        raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
+        off = (-raw.data_ptr()) % 1024
+        self.raw = raw
+        self.buf = raw[off:off + nbytes]
+        self.bytes = nbytes
+        self.busy = False
+        with torch.cuda.device(dev):
+            _lib.check(getattr(_lib.load(), init)(self.buf.data_ptr(), nbytes, *args, _stream_ptr()), init)
+
+
+class TrainWorkspace(_Workspace):
     """Device workspace of one (device, n_rays, N_samples, N_importance) shape, reused across steps.
     A render holds its workspace (``busy``) from its forward until its backward runs, or until its graph is
     freed without one (a skipped batch, a render under grad mode used only for a metric), so that a second
@@ -46,19 +61,11 @@ class TrainWorkspace:
     _pool: Dict[tuple, List["TrainWorkspace"]] = {}
 
     def __init__(self, dev: torch.device, n: int, S_c: int, K: int) -> None:
-        lib = _lib.load()
-        self.bytes = int(lib.nerfb200_train_workspace_bytes(n, S_c, K))
-        if self.bytes == 0:
+        nbytes = int(_lib.load().nerfb200_train_workspace_bytes(n, S_c, K))
+        if nbytes == 0:
             raise ValueError("invalid training shape")
-        raw = torch.empty(self.bytes + 1024, dtype=torch.uint8, device=dev)
-        off = (-raw.data_ptr()) % 1024
-        self.raw = raw
-        self.buf = raw[off:off + self.bytes]
-        self.busy = False
         self.key = (dev.index, n, S_c, K)
-        with torch.cuda.device(dev):
-            _lib.check(lib.nerfb200_train_workspace_init(self.buf.data_ptr(), self.bytes, n, S_c, K, _stream_ptr()),
-                       "nerfb200_train_workspace_init")
+        super().__init__(dev, nbytes, "nerfb200_train_workspace_init", n, S_c, K)
 
     @classmethod
     def acquire(cls, dev: torch.device, n: int, S_c: int, K: int) -> "TrainWorkspace":
@@ -262,7 +269,7 @@ def render_rays_train(models, rays, N_samples, use_disp, perturb, noise_std, N_i
 # Training a direct NeRF.forward call (reference models/nerf.py:83-124) for callers that render with their own code:
 # one save-mode launch of the MLP kernel forward (nerfb200_nerf_forward_train), the sm_90a backward kernels of the
 # render path seeded from the upstream (B, 4) gradient (nerfb200_nerf_backward).
-class NerfTrainWorkspace:
+class NerfTrainWorkspace(_Workspace):
     """Device workspace of one ``nerf_forward_train`` call over ``n`` samples, from a per-device pool.
 
     A call holds its workspace from its forward until its backward runs, or until its graph is freed without a
@@ -274,19 +281,11 @@ class NerfTrainWorkspace:
     _pool: Dict[int, List["NerfTrainWorkspace"]] = {}
 
     def __init__(self, dev: torch.device, n: int) -> None:
-        lib = _lib.load()
-        self.n = n
-        self.bytes = int(lib.nerfb200_nerf_train_workspace_bytes(n))
-        if self.bytes == 0:
+        nbytes = int(_lib.load().nerfb200_nerf_train_workspace_bytes(n))
+        if nbytes == 0:
             raise ValueError(f"invalid sample count {n}")
-        raw = torch.empty(self.bytes + 1024, dtype=torch.uint8, device=dev)
-        off = (-raw.data_ptr()) % 1024
-        self.raw = raw
-        self.buf = raw[off:off + self.bytes]
-        self.busy = False
-        with torch.cuda.device(dev):
-            _lib.check(lib.nerfb200_nerf_train_workspace_init(self.buf.data_ptr(), self.bytes, n, _stream_ptr()),
-                       "nerfb200_nerf_train_workspace_init")
+        self.n = n
+        super().__init__(dev, nbytes, "nerfb200_nerf_train_workspace_init", n)
 
     @classmethod
     def acquire(cls, dev: torch.device, n: int) -> "NerfTrainWorkspace":
