@@ -11,7 +11,9 @@ import ctypes
 import os
 import subprocess
 import threading
-from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int32, c_int64, c_size_t, c_void_p
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
@@ -28,56 +30,8 @@ NVCC_FLAGS = [
     "-diag-suppress", "550",
 ]
 
-# Every symbol include/nerf_pl_b200.h declares (tests check the library exports all of them).
-EXPORTS = [
-    "nerfb200_abi_version",
-    "nerfb200_last_error",
-    "nerfb200_packed_bytes",
-    "nerfb200_pack_weights",
-    "nerfb200_pack_weights_pair",
-    "nerfb200_render_rays",
-    "nerfb200_render_rays_host",
-    "nerfb200_nerf_forward",
-    "nerfb200_nerf_train_workspace_bytes",
-    "nerfb200_nerf_train_workspace_init",
-    "nerfb200_nerf_forward_train",
-    "nerfb200_nerf_backward",
-    "nerfb200_embed",
-    "nerfb200_searchsorted",
-    "nerfb200_sample_pdf",
-    "nerfb200_composite",
-    "nerfb200_query_sigma",
-    "nerfb200_mse_psnr",
-    "nerfb200_train_workspace_bytes",
-    "nerfb200_train_workspace_init",
-    "nerfb200_render_backward",
-    "nerfb200_adam_step",
-    "nerfb200_adam_step_dev",
-    "nerfb200_generate_rays",
-    "nerfb200_to_uint8",
-    "nerfb200_launch_count",
-    "nerfb200_check_status",
-    "nerfb200_sm_count",
-    "nerfb200_sigma_grid_workspace_bytes",
-    "nerfb200_grid_positions",
-    "nerfb200_sigma_grid",
-    "nerfb200_mc_workspace_bytes",
-    "nerfb200_mc_count",
-    "nerfb200_mc_emit",
-    "nerfb200_mesh_to_world",
-    "nerfb200_mesh_cluster_workspace_bytes",
-    "nerfb200_mesh_cluster_count",
-    "nerfb200_mesh_cluster_emit",
-    "nerfb200_remap_bilinear",
-    "nerfb200_color_project",
-    "nerfb200_color_accumulate",
-    "nerfb200_color_finalize",
-    "nerfb200_query_rgb_sigma",
-    "nerfb200_rgb_sigma_grid",
-    "nerfb200_volume_workspace_bytes",
-    "nerfb200_volume_count",
-    "nerfb200_volume_emit",
-]
+ABI_VERSION = 3
+
 
 class RenderArgs(ctypes.Structure):
     """Mirror of ``nerfb200_render_args`` (include/nerf_pl_b200.h)."""
@@ -139,6 +93,65 @@ class BackwardArgs(ctypes.Structure):
     ]
 
 
+_vp, _i32, _i64, _f32, _f64, _sz = c_void_p, c_int32, c_int64, c_float, c_double, c_size_t
+_P, _RA, _BA = POINTER(c_void_p), POINTER(RenderArgs), POINTER(BackwardArgs)
+
+# Every entry include/nerf_pl_b200.h declares, in header order: name -> (restype, argtypes); tests check it against
+# the header's prototypes.  Pointers and arrays are c_void_p or POINTER(...).  The entries that take a stream take it
+# last; ``call`` appends it.
+SIGNATURES = {
+    "nerfb200_abi_version": (_i32, []),
+    "nerfb200_last_error": (c_char_p, []),
+    "nerfb200_packed_bytes": (_sz, []),
+    "nerfb200_pack_weights": (_i32, [_P, _vp, _vp]),
+    "nerfb200_pack_weights_pair": (_i32, [_P, _vp, _P, _vp, _vp]),
+    "nerfb200_render_rays": (_i32, [_RA, _vp]),
+    "nerfb200_train_workspace_bytes": (_sz, [_i64, _i32, _i32]),
+    "nerfb200_train_workspace_init": (_i32, [_vp, _sz, _i64, _i32, _i32, _vp]),
+    "nerfb200_render_backward": (_i32, [_BA, _vp]),
+    "nerfb200_adam_step": (_i32, [_i32, _P, _P, _P, _P, POINTER(_i64), _f32, _f32, _f32, _f32, _f32, _i64, _vp]),
+    "nerfb200_adam_step_dev": (_i32, [_i32, _P, _P, _P, _P, POINTER(_i64), _vp, _P, _f32, _f32, _f32, _f32, _vp]),
+    "nerfb200_render_rays_host": (_i32, [_RA, _vp]),
+    "nerfb200_nerf_forward": (_i32, [_vp, _i64, _i64, _vp, _i32, _vp, _vp]),
+    "nerfb200_nerf_train_workspace_bytes": (_sz, [_i64]),
+    "nerfb200_nerf_train_workspace_init": (_i32, [_vp, _sz, _i64, _vp]),
+    "nerfb200_nerf_forward_train": (_i32, [_vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "nerfb200_nerf_backward": (_i32, [_vp, _i64, _vp, _P, _vp, _P, _vp]),
+    "nerfb200_query_sigma": (_i32, [_vp, _i64, _i64, _vp, _vp, _vp]),
+    "nerfb200_mse_psnr": (_i32, [_vp, _vp, _vp, _i64, _vp, _vp]),
+    "nerfb200_embed": (_i32, [_vp, _i64, _i32, _vp, _vp]),
+    "nerfb200_searchsorted": (_i32, [_vp, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _vp]),
+    "nerfb200_sample_pdf": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
+    "nerfb200_composite": (_i32, [_vp, _vp, _vp, _vp, _vp, _f32, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "nerfb200_generate_rays": (_i32, [_i32, _i32, _f32, POINTER(_f32), _f32, _f32, _i32, _vp, _vp]),
+    "nerfb200_to_uint8": (_i32, [_vp, _i64, _vp, _vp]),
+    "nerfb200_grid_positions": (_i32, [_i64, POINTER(_f64), _i64, _i64, _vp, _vp]),
+    "nerfb200_sigma_grid_workspace_bytes": (_sz, [_i64]),
+    "nerfb200_sigma_grid": (_i32, [_vp, _i64, POINTER(_f64), _i64, _vp, _sz, _vp, _vp]),
+    "nerfb200_query_rgb_sigma": (_i32, [_vp, _i64, _i64, _vp, _vp, _vp]),
+    "nerfb200_rgb_sigma_grid": (_i32, [_vp, _i64, POINTER(_f64), _i64, _vp, _sz, _vp, _vp]),
+    "nerfb200_volume_workspace_bytes": (_sz, [_i64]),
+    "nerfb200_volume_count": (_i32, [_vp, _i64, _f64, _f64, _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_volume_emit": (_i32, [_vp, _i64, _f64, _f64, _vp, _sz, _vp, _vp]),
+    "nerfb200_mc_workspace_bytes": (_sz, [_i64, _i64, _i64]),
+    "nerfb200_mc_count": (_i32, [_vp, _i64, _i64, _i64, _f64, _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_mc_emit": (_i32, [_vp, _i64, _i64, _i64, _f64, _vp, _sz, _vp, _vp, _vp]),
+    "nerfb200_mesh_to_world": (_i32, [_vp, _i64, _i64, POINTER(_f64), _vp, _vp]),
+    "nerfb200_mesh_cluster_workspace_bytes": (_sz, [_i64, _i64]),
+    "nerfb200_mesh_cluster_count": (_i32, [_vp, _i64, _i64, _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_mesh_cluster_emit": (_i32, [_vp, _vp, _i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "nerfb200_remap_bilinear": (_i32, [_vp, _i32, _i32, _vp, _i64, _vp, _vp]),
+    "nerfb200_color_project": (_i32, [_vp, _i64, POINTER(_f64), POINTER(_f32), _f32, _i32, _i32, _vp, _f32, _vp, _vp,
+                                      _vp, _vp]),
+    "nerfb200_color_accumulate": (_i32, [_vp, _vp, _vp, _i64, _f32, _vp, _vp]),
+    "nerfb200_color_finalize": (_i32, [_vp, _i64, _vp, _vp]),
+    "nerfb200_launch_count": (_i64, []),
+    "nerfb200_check_status": (_i32, []),
+    "nerfb200_sm_count": (_i32, []),
+}
+EXPORTS = tuple(SIGNATURES)     # tests check the library exports all of them
+
+
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
         if cand and (os.path.isabs(cand) and os.path.exists(cand) or not os.path.isabs(cand)):
@@ -175,102 +188,6 @@ _lib = None
 _lock = threading.Lock()
 
 
-def _declare(lib: ctypes.CDLL) -> None:
-    lib.nerfb200_abi_version.restype = c_int32
-    lib.nerfb200_last_error.restype = c_char_p
-    lib.nerfb200_packed_bytes.restype = c_size_t
-    lib.nerfb200_pack_weights.argtypes = [POINTER(c_void_p), c_void_p, c_void_p]
-    lib.nerfb200_pack_weights_pair.argtypes = [POINTER(c_void_p), c_void_p, POINTER(c_void_p), c_void_p, c_void_p]
-    lib.nerfb200_render_rays.argtypes = [POINTER(RenderArgs), c_void_p]
-    lib.nerfb200_render_rays_host.argtypes = [POINTER(RenderArgs), c_void_p]
-    lib.nerfb200_nerf_forward.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_int32, c_void_p, c_void_p]
-    lib.nerfb200_embed.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_void_p]
-    lib.nerfb200_searchsorted.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int32,
-                                          c_int32, c_int32, c_void_p]
-    lib.nerfb200_sample_pdf.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32,
-                                        c_void_p, c_void_p]
-    lib.nerfb200_composite.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float,
-                                       c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p,
-                                       c_void_p, c_void_p]
-    lib.nerfb200_query_sigma.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]
-    lib.nerfb200_query_sigma.restype = c_int32
-    lib.nerfb200_nerf_train_workspace_bytes.argtypes = [c_int64]
-    lib.nerfb200_nerf_train_workspace_bytes.restype = c_size_t
-    lib.nerfb200_nerf_train_workspace_init.argtypes = [c_void_p, c_size_t, c_int64, c_void_p]
-    lib.nerfb200_nerf_train_workspace_init.restype = c_int32
-    lib.nerfb200_nerf_forward_train.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.nerfb200_nerf_forward_train.restype = c_int32
-    lib.nerfb200_nerf_backward.argtypes = [c_void_p, c_int64, c_void_p, POINTER(c_void_p), c_void_p, POINTER(c_void_p),
-                                           c_void_p]
-    lib.nerfb200_nerf_backward.restype = c_int32
-    lib.nerfb200_train_workspace_bytes.argtypes = [c_int64, c_int32, c_int32]
-    lib.nerfb200_train_workspace_bytes.restype = c_size_t
-    lib.nerfb200_train_workspace_init.argtypes = [c_void_p, c_size_t, c_int64, c_int32, c_int32, c_void_p]
-    lib.nerfb200_train_workspace_init.restype = c_int32
-    lib.nerfb200_render_backward.argtypes = [POINTER(BackwardArgs), c_void_p]
-    lib.nerfb200_render_backward.restype = c_int32
-    lib.nerfb200_adam_step.argtypes = [c_int32, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
-                                       POINTER(c_int64), c_float, c_float, c_float, c_float, c_float, c_int64, c_void_p]
-    lib.nerfb200_adam_step.restype = c_int32
-    lib.nerfb200_adam_step_dev.argtypes = [c_int32, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
-                                           POINTER(c_void_p), POINTER(c_int64), c_void_p, POINTER(c_void_p), c_float,
-                                           c_float, c_float, c_float, c_void_p]
-    lib.nerfb200_adam_step_dev.restype = c_int32
-    lib.nerfb200_mse_psnr.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]
-    lib.nerfb200_mse_psnr.restype = c_int32
-    lib.nerfb200_generate_rays.argtypes = [c_int32, c_int32, c_float, POINTER(c_float), c_float, c_float, c_int32,
-                                           c_void_p, c_void_p]
-    lib.nerfb200_generate_rays.restype = c_int32
-    lib.nerfb200_to_uint8.argtypes = [c_void_p, c_int64, c_void_p, c_void_p]
-    lib.nerfb200_to_uint8.restype = c_int32
-    lib.nerfb200_check_status.restype = c_int32
-    lib.nerfb200_launch_count.restype = c_int64
-    lib.nerfb200_sm_count.restype = c_int32
-    # coloured mesh extraction (nerf_pl_b200.mesh)
-    c_double, c_u8p = ctypes.c_double, ctypes.c_void_p
-    lib.nerfb200_sigma_grid_workspace_bytes.argtypes = [c_int64]
-    lib.nerfb200_sigma_grid_workspace_bytes.restype = c_size_t
-    lib.nerfb200_grid_positions.argtypes = [c_int64, POINTER(c_double), c_int64, c_int64, c_void_p, c_void_p]
-    lib.nerfb200_sigma_grid.argtypes = [c_void_p, c_int64, POINTER(c_double), c_int64, c_void_p, c_size_t, c_void_p,
-                                        c_void_p]
-    lib.nerfb200_mc_workspace_bytes.argtypes = [c_int64, c_int64, c_int64]
-    lib.nerfb200_mc_workspace_bytes.restype = c_size_t
-    lib.nerfb200_mc_count.argtypes = [c_void_p, c_int64, c_int64, c_int64, c_double, c_void_p, c_size_t, POINTER(c_int64),
-                                      c_void_p]
-    lib.nerfb200_mc_emit.argtypes = [c_void_p, c_int64, c_int64, c_int64, c_double, c_void_p, c_size_t, c_void_p, c_void_p,
-                                     c_void_p]
-    lib.nerfb200_mesh_to_world.argtypes = [c_void_p, c_int64, c_int64, POINTER(c_double), c_void_p, c_void_p]
-    lib.nerfb200_mesh_cluster_workspace_bytes.argtypes = [c_int64, c_int64]
-    lib.nerfb200_mesh_cluster_workspace_bytes.restype = c_size_t
-    lib.nerfb200_mesh_cluster_count.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_size_t, POINTER(c_int64), c_void_p]
-    lib.nerfb200_mesh_cluster_emit.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_size_t, c_void_p, c_void_p,
-                                               c_void_p]
-    lib.nerfb200_remap_bilinear.argtypes = [c_u8p, c_int32, c_int32, c_void_p, c_int64, c_u8p, c_void_p]
-    lib.nerfb200_color_project.argtypes = [c_void_p, c_int64, POINTER(c_double), POINTER(c_float), c_float, c_int32,
-                                           c_int32, c_u8p, c_float, c_u8p, c_void_p, c_void_p, c_void_p]
-    lib.nerfb200_color_accumulate.argtypes = [c_u8p, c_void_p, c_void_p, c_int64, c_float, c_void_p, c_void_p]
-    lib.nerfb200_color_finalize.argtypes = [c_void_p, c_int64, c_u8p, c_void_p]
-    # Unity volume (.vol)
-    lib.nerfb200_query_rgb_sigma.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]
-    lib.nerfb200_rgb_sigma_grid.argtypes = [c_void_p, c_int64, POINTER(c_double), c_int64, c_void_p, c_size_t,
-                                            c_void_p, c_void_p]
-    lib.nerfb200_volume_workspace_bytes.argtypes = [c_int64]
-    lib.nerfb200_volume_workspace_bytes.restype = c_size_t
-    lib.nerfb200_volume_count.argtypes = [c_void_p, c_int64, c_double, c_double, c_void_p, c_size_t, POINTER(c_int64),
-                                          c_void_p]
-    lib.nerfb200_volume_emit.argtypes = [c_void_p, c_int64, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p]
-    for name in ("nerfb200_grid_positions", "nerfb200_sigma_grid", "nerfb200_mc_count", "nerfb200_mc_emit",
-                 "nerfb200_mesh_to_world", "nerfb200_mesh_cluster_count", "nerfb200_mesh_cluster_emit",
-                 "nerfb200_remap_bilinear", "nerfb200_color_project", "nerfb200_color_accumulate",
-                 "nerfb200_color_finalize", "nerfb200_query_rgb_sigma", "nerfb200_rgb_sigma_grid",
-                 "nerfb200_volume_count", "nerfb200_volume_emit"):
-        getattr(lib, name).restype = c_int32
-    for name in ("nerfb200_pack_weights", "nerfb200_pack_weights_pair", "nerfb200_render_rays", "nerfb200_render_rays_host",
-                 "nerfb200_nerf_forward", "nerfb200_embed", "nerfb200_searchsorted",
-                 "nerfb200_sample_pdf", "nerfb200_composite"):
-        getattr(lib, name).restype = c_int32
-
-
 def load() -> ctypes.CDLL:
     """Load the library (never builds implicitly: build() is the explicit step)."""
     global _lib
@@ -281,8 +198,10 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            _declare(lib)
-            if lib.nerfb200_abi_version() != 3:
+            for name, (restype, argtypes) in SIGNATURES.items():
+                fn = getattr(lib, name)
+                fn.restype, fn.argtypes = restype, argtypes
+            if lib.nerfb200_abi_version() != ABI_VERSION:
                 raise RuntimeError("libnerf_pl_b200.so ABI version mismatch")
             _lib = lib
     return _lib
@@ -301,3 +220,20 @@ def check(rc: int, what: str) -> None:
     if rc in (-1, -2):
         raise ValueError(f"{what}: {msg}")
     raise NerfB200Error(f"{what}: {msg} (code {rc})")
+
+
+def _stream_ptr() -> ctypes.c_void_p:
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def call(name: str, device, *args) -> None:
+    """Call the stream-taking entry ``name`` with ``args`` and the current stream of ``device`` appended, and raise
+    what ``check`` raises for its return code.  ``device`` is made current for the call unless it already is; None,
+    or a device without an index, means the current device."""
+    fn = getattr(load(), name)
+    if device is None or device.index is None or device.index == torch.cuda.current_device():
+        rc = fn(*args, _stream_ptr())
+    else:
+        with torch.cuda.device(device):
+            rc = fn(*args, _stream_ptr())
+    check(rc, name)

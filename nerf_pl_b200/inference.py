@@ -12,7 +12,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
-from .nerf import _stream_ptr, packed_weights
+from .nerf import packed_weights
 from .rendering import render_rays
 from .sharded import render_rays_sharded
 
@@ -30,10 +30,8 @@ def generate_rays(H: int, W: int, focal: float, c2w, near: float, far: float, nd
         raise ValueError("c2w must be (3, 4)")
     arr = (ctypes.c_float * 12)(*c2w_t.tolist())
     rays = torch.empty(H * W, 8, dtype=torch.float32, device=device)
-    lib = _lib.load()
-    with torch.cuda.device(device):
-        _lib.check(lib.nerfb200_generate_rays(H, W, float(focal), arr, float(near), float(far), int(bool(ndc)),
-                                              rays.data_ptr(), _stream_ptr()), "nerfb200_generate_rays")
+    _lib.call("nerfb200_generate_rays", device, H, W, float(focal), arr, float(near), float(far), int(bool(ndc)),
+              rays.data_ptr())
     return rays
 
 
@@ -43,10 +41,7 @@ def to_uint8(img: torch.Tensor) -> torch.Tensor:
         raise RuntimeError("nerf_pl_b200.to_uint8 runs on CUDA tensors only (no CPU fallback)")
     src = img.detach().to(torch.float32).contiguous()
     dst = torch.empty(src.shape, dtype=torch.uint8, device=src.device)
-    lib = _lib.load()
-    with torch.cuda.device(src.device):
-        _lib.check(lib.nerfb200_to_uint8(src.data_ptr(), src.numel(), dst.data_ptr(), _stream_ptr()),
-                   "nerfb200_to_uint8")
+    _lib.call("nerfb200_to_uint8", src.device, src.data_ptr(), src.numel(), dst.data_ptr())
     return dst
 
 
@@ -96,11 +91,8 @@ def query_sigma(model: torch.nn.Module, xyz: torch.Tensor) -> torch.Tensor:
         raise ValueError("xyz must be a (N, 3) CUDA tensor")
     x = xyz.detach().to(torch.float32).contiguous()
     out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
-    lib = _lib.load()
     blob = packed_weights(model)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.nerfb200_query_sigma(x.data_ptr(), x.shape[0], 3, blob.data_ptr(), out.data_ptr(),
-                                            _stream_ptr()), "nerfb200_query_sigma")
+    _lib.call("nerfb200_query_sigma", x.device, x.data_ptr(), x.shape[0], 3, blob.data_ptr(), out.data_ptr())
     return out
 
 
@@ -114,11 +106,7 @@ def mse_psnr(results: Dict[str, torch.Tensor], targets: torch.Tensor) -> Dict[st
         raise ValueError("results must hold CUDA rgb_coarse and/or rgb_fine")
     t = targets.detach().to(torch.float32).contiguous()
     out = torch.empty(4, dtype=torch.float32, device=ref.device)
-    lib = _lib.load()
     keep = [None if v is None else v.detach().float().contiguous() for v in (rc, rf)]
-    with torch.cuda.device(ref.device):
-        _lib.check(lib.nerfb200_mse_psnr(None if keep[0] is None else keep[0].data_ptr(),
-                                         None if keep[1] is None else keep[1].data_ptr(),
-                                         t.data_ptr(), t.shape[0], out.data_ptr(), _stream_ptr()),
-                   "nerfb200_mse_psnr")
+    _lib.call("nerfb200_mse_psnr", ref.device, None if keep[0] is None else keep[0].data_ptr(),
+              None if keep[1] is None else keep[1].data_ptr(), t.data_ptr(), t.shape[0], out.data_ptr())
     return {"loss": out[2] if rc is not None else out[1], "psnr": out[3], "mse_coarse": out[0], "mse_fine": out[1]}

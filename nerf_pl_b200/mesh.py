@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .nerf import Embedding, _stream_ptr, packed_weights
+from .nerf import Embedding, packed_weights
 from .rendering import render_rays
 
 
@@ -55,10 +55,7 @@ def grid_positions(N: int, x_range, y_range, z_range, start: int = 0, count: Opt
     device = torch.device("cuda") if device is None else torch.device(device)
     count = N ** 3 - start if count is None else count
     out = torch.empty(count, 3, dtype=torch.float32, device=device)
-    lib = _lib.load()
-    with torch.cuda.device(device):
-        _lib.check(lib.nerfb200_grid_positions(N, _ranges(x_range, y_range, z_range), start, count, out.data_ptr(),
-                                               _stream_ptr()), "nerfb200_grid_positions")
+    _lib.call("nerfb200_grid_positions", device, N, _ranges(x_range, y_range, z_range), start, count, out.data_ptr())
     return out
 
 
@@ -69,13 +66,11 @@ def sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk:
     queried per launch; the scratch is their positions only."""
     dev = _device_of(model)
     out = torch.empty(N, N, N, dtype=torch.float32, device=dev)
-    lib = _lib.load()
     blob = packed_weights(model)
     chunk = int(min(chunk, N ** 3))
-    ws = _workspace(lib.nerfb200_sigma_grid_workspace_bytes(chunk), dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.nerfb200_sigma_grid(blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk, ws.data_ptr(),
-                                           ws.numel(), out.data_ptr(), _stream_ptr()), "nerfb200_sigma_grid")
+    ws = _workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
+    _lib.call("nerfb200_sigma_grid", dev, blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk, ws.data_ptr(),
+              ws.numel(), out.data_ptr())
     return out
 
 
@@ -88,20 +83,17 @@ def marching_cubes(sigma: torch.Tensor, threshold: float) -> Tuple[torch.Tensor,
     if s.dim() != 3:
         raise ValueError("sigma must be a 3-D grid")
     n0, n1, n2 = s.shape
-    lib = _lib.load()
-    nbytes = lib.nerfb200_mc_workspace_bytes(n0, n1, n2)
+    nbytes = _lib.load().nerfb200_mc_workspace_bytes(n0, n1, n2)
     if nbytes == 0:
         raise ValueError(f"marching_cubes: unsupported grid shape {tuple(s.shape)}")
     ws = _workspace(nbytes, s.device)
     counts = (ctypes.c_int64 * 2)()
-    with torch.cuda.device(s.device):
-        _lib.check(lib.nerfb200_mc_count(s.data_ptr(), n0, n1, n2, float(threshold), ws.data_ptr(), ws.numel(), counts,
-                                         _stream_ptr()), "nerfb200_mc_count")
-        verts = torch.empty(counts[0], 3, dtype=torch.float64, device=s.device)
-        tris = torch.empty(counts[1], 3, dtype=torch.int32, device=s.device)
-        _lib.check(lib.nerfb200_mc_emit(s.data_ptr(), n0, n1, n2, float(threshold), ws.data_ptr(), ws.numel(),
-                                        verts.data_ptr() if counts[0] else None, tris.data_ptr() if counts[1] else None,
-                                        _stream_ptr()), "nerfb200_mc_emit")
+    _lib.call("nerfb200_mc_count", s.device, s.data_ptr(), n0, n1, n2, float(threshold), ws.data_ptr(), ws.numel(),
+              counts)
+    verts = torch.empty(counts[0], 3, dtype=torch.float64, device=s.device)
+    tris = torch.empty(counts[1], 3, dtype=torch.int32, device=s.device)
+    _lib.call("nerfb200_mc_emit", s.device, s.data_ptr(), n0, n1, n2, float(threshold), ws.data_ptr(), ws.numel(),
+              verts.data_ptr() if counts[0] else None, tris.data_ptr() if counts[1] else None)
     return verts, tris
 
 
@@ -111,10 +103,8 @@ def to_world(vertices: torch.Tensor, N: int, x_range, y_range, z_range) -> torch
     x / y ranges (x takes y_range)."""
     v = _cuda(vertices, "vertices").detach().to(torch.float64).contiguous()
     out = torch.empty(v.shape[0], 3, dtype=torch.float32, device=v.device)
-    lib = _lib.load()
-    with torch.cuda.device(v.device):
-        _lib.check(lib.nerfb200_mesh_to_world(v.data_ptr(), v.shape[0], N, _ranges(x_range, y_range, z_range),
-                                              out.data_ptr(), _stream_ptr()), "nerfb200_mesh_to_world")
+    _lib.call("nerfb200_mesh_to_world", v.device, v.data_ptr(), v.shape[0], N, _ranges(x_range, y_range, z_range),
+              out.data_ptr())
     return out
 
 
@@ -126,17 +116,14 @@ def keep_largest_cluster(vertices: torch.Tensor, triangles: torch.Tensor) -> Tup
     t = _cuda(triangles, "triangles").detach().to(torch.int32).contiguous()
     if t.shape[0] == 0:
         return v[:0], t[:0]
-    lib = _lib.load()
-    ws = _workspace(lib.nerfb200_mesh_cluster_workspace_bytes(v.shape[0], t.shape[0]), v.device)
+    ws = _workspace(_lib.load().nerfb200_mesh_cluster_workspace_bytes(v.shape[0], t.shape[0]), v.device)
     counts = (ctypes.c_int64 * 2)()
-    with torch.cuda.device(v.device):
-        _lib.check(lib.nerfb200_mesh_cluster_count(t.data_ptr(), t.shape[0], v.shape[0], ws.data_ptr(), ws.numel(),
-                                                   counts, _stream_ptr()), "nerfb200_mesh_cluster_count")
-        vo = torch.empty(counts[0], 3, dtype=torch.float32, device=v.device)
-        to = torch.empty(counts[1], 3, dtype=torch.int32, device=v.device)
-        _lib.check(lib.nerfb200_mesh_cluster_emit(v.data_ptr(), t.data_ptr(), t.shape[0], v.shape[0], ws.data_ptr(),
-                                                  ws.numel(), vo.data_ptr(), to.data_ptr(), _stream_ptr()),
-                   "nerfb200_mesh_cluster_emit")
+    _lib.call("nerfb200_mesh_cluster_count", v.device, t.data_ptr(), t.shape[0], v.shape[0], ws.data_ptr(), ws.numel(),
+              counts)
+    vo = torch.empty(counts[0], 3, dtype=torch.float32, device=v.device)
+    to = torch.empty(counts[1], 3, dtype=torch.int32, device=v.device)
+    _lib.call("nerfb200_mesh_cluster_emit", v.device, v.data_ptr(), t.data_ptr(), t.shape[0], v.shape[0], ws.data_ptr(),
+              ws.numel(), vo.data_ptr(), to.data_ptr())
     return vo, to
 
 
@@ -162,10 +149,8 @@ def remap_bilinear(image: torch.Tensor, xy: torch.Tensor) -> torch.Tensor:
         raise ValueError("image must be (H, W, 3) uint8")
     p = _cuda(xy, "xy").detach().to(torch.float32).contiguous()
     out = torch.empty(p.shape[0], 3, dtype=torch.uint8, device=img.device)
-    lib = _lib.load()
-    with torch.cuda.device(img.device):
-        _lib.check(lib.nerfb200_remap_bilinear(img.data_ptr(), img.shape[0], img.shape[1], p.data_ptr(), p.shape[0],
-                                               out.data_ptr(), _stream_ptr()), "nerfb200_remap_bilinear")
+    _lib.call("nerfb200_remap_bilinear", img.device, img.data_ptr(), img.shape[0], img.shape[1], p.data_ptr(),
+              p.shape[0], out.data_ptr())
     return out
 
 
@@ -187,11 +172,8 @@ def project_view(vertices: torch.Tensor, image: torch.Tensor, pose, focal: float
     colors = torch.empty(n, 3, dtype=torch.uint8, device=v.device)
     depth = torch.empty(n, dtype=torch.float64, device=v.device)
     rays = torch.empty(n, 8, dtype=torch.float32, device=v.device)
-    lib = _lib.load()
-    with torch.cuda.device(v.device):
-        _lib.check(lib.nerfb200_color_project(v.data_ptr(), n, w2c, origin, float(focal), W, H, image.data_ptr(),
-                                              float(near), colors.data_ptr(), depth.data_ptr(), rays.data_ptr(),
-                                              _stream_ptr()), "nerfb200_color_project")
+    _lib.call("nerfb200_color_project", v.device, v.data_ptr(), n, w2c, origin, float(focal), W, H, image.data_ptr(),
+              float(near), colors.data_ptr(), depth.data_ptr(), rays.data_ptr())
     return colors, depth, rays
 
 
@@ -215,7 +197,6 @@ def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: t
     n = v.shape[0]
     sum4 = torch.zeros(n, 4, dtype=torch.float64, device=v.device)
     emb = [Embedding(3, 10), Embedding(3, 4)]
-    lib = _lib.load()
     opac = []
     for idx in range(imgs.shape[0]):
         colors, depth, rays = project_view(v, imgs[idx], poses[idx], focal, near)
@@ -224,14 +205,10 @@ def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: t
         opacity = res["opacity_coarse"].contiguous()
         if return_opacities:
             opac.append(opacity)
-        with torch.cuda.device(v.device):
-            _lib.check(lib.nerfb200_color_accumulate(colors.data_ptr(), depth.data_ptr(), opacity.data_ptr(), n,
-                                                     float(np.float32(occ_threshold)), sum4.data_ptr(), _stream_ptr()),
-                       "nerfb200_color_accumulate")
+        _lib.call("nerfb200_color_accumulate", v.device, colors.data_ptr(), depth.data_ptr(), opacity.data_ptr(), n,
+                  float(np.float32(occ_threshold)), sum4.data_ptr())
     out = torch.empty(n, 3, dtype=torch.uint8, device=v.device)
-    with torch.cuda.device(v.device):
-        _lib.check(lib.nerfb200_color_finalize(sum4.data_ptr(), n, out.data_ptr(), _stream_ptr()),
-                   "nerfb200_color_finalize")
+    _lib.call("nerfb200_color_finalize", v.device, sum4.data_ptr(), n, out.data_ptr())
     if return_opacities:
         return out, (torch.stack(opac) if opac else torch.empty(0, n, device=v.device))
     return out
@@ -245,11 +222,8 @@ def query_rgb_sigma(model: torch.nn.Module, xyz: torch.Tensor) -> torch.Tensor:
     if x.dim() != 2 or x.shape[1] != 3:
         raise ValueError("xyz must be (n, 3)")
     out = torch.empty(x.shape[0], 4, dtype=torch.float32, device=x.device)
-    lib = _lib.load()
     blob = packed_weights(model)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.nerfb200_query_rgb_sigma(x.data_ptr(), x.shape[0], 3, blob.data_ptr(), out.data_ptr(),
-                                                _stream_ptr()), "nerfb200_query_rgb_sigma")
+    _lib.call("nerfb200_query_rgb_sigma", x.device, x.data_ptr(), x.shape[0], 3, blob.data_ptr(), out.data_ptr())
     return out
 
 
@@ -260,14 +234,11 @@ def rgb_sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, ch
     ``max(sigma, 0)``.  ``chunk`` points are queried per launch; the scratch is their positions only."""
     dev = _device_of(model)
     out = torch.empty(N, N, N, 4, dtype=torch.float32, device=dev)
-    lib = _lib.load()
     blob = packed_weights(model)
     chunk = int(min(chunk, N ** 3))
-    ws = _workspace(lib.nerfb200_sigma_grid_workspace_bytes(chunk), dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.nerfb200_rgb_sigma_grid(blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk,
-                                               ws.data_ptr(), ws.numel(), out.data_ptr(), _stream_ptr()),
-                   "nerfb200_rgb_sigma_grid")
+    ws = _workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
+    _lib.call("nerfb200_rgb_sigma_grid", dev, blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk,
+              ws.data_ptr(), ws.numel(), out.data_ptr())
     return out
 
 
@@ -283,20 +254,18 @@ def pack_volume(rgbsigma: torch.Tensor, x_range) -> torch.Tensor:
         raise ValueError("rgbsigma must be (N, N, N, 4)")
     N = g.shape[0]
     xmin, xmax = (float(v) for v in x_range)
-    lib = _lib.load()
-    nbytes = lib.nerfb200_volume_workspace_bytes(N)
+    nbytes = _lib.load().nerfb200_volume_workspace_bytes(N)
     if nbytes == 0:
         raise ValueError(f"pack_volume: N = {N} outside [2, 1625]")
     ws = _workspace(nbytes, g.device)
     count = ctypes.c_int64()
-    with torch.cuda.device(g.device):
-        _lib.check(lib.nerfb200_volume_count(g.data_ptr(), N, xmin, xmax, ws.data_ptr(), ws.numel(), ctypes.byref(count),
-                                             _stream_ptr()), "nerfb200_volume_count")
-        # torch has no uint32 arithmetic to speak of; the rows are stored as int32 and viewed as uint32
-        out = torch.empty(count.value, 2, dtype=torch.int32, device=g.device)
-        if count.value:
-            _lib.check(lib.nerfb200_volume_emit(g.data_ptr(), N, xmin, xmax, ws.data_ptr(), ws.numel(), out.data_ptr(),
-                                                _stream_ptr()), "nerfb200_volume_emit")
+    _lib.call("nerfb200_volume_count", g.device, g.data_ptr(), N, xmin, xmax, ws.data_ptr(), ws.numel(),
+              ctypes.byref(count))
+    # torch has no uint32 arithmetic to speak of; the rows are stored as int32 and viewed as uint32
+    out = torch.empty(count.value, 2, dtype=torch.int32, device=g.device)
+    if count.value:
+        _lib.call("nerfb200_volume_emit", g.device, g.data_ptr(), N, xmin, xmax, ws.data_ptr(), ws.numel(),
+                  out.data_ptr())
     return out.view(torch.uint32)
 
 

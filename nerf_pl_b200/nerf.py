@@ -17,6 +17,7 @@ import torch
 from torch import nn
 
 from . import _lib
+from ._lib import _stream_ptr  # noqa: F401  (defined in _lib; code that imported it from this module keeps working)
 
 _PARAM_ORDER = (
     [(f"xyz_encoding_{i}", 0) for i in range(1, 9)]
@@ -46,8 +47,12 @@ _EXPECTED_SHAPES = (
 )
 
 
-def _stream_ptr() -> ctypes.c_void_p:
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+def _aligned_buffer(nbytes: int, dev) -> torch.Tensor:
+    """``nbytes`` of device memory at a 1024-byte boundary: the library wants that alignment, torch's caching
+    allocator guarantees 512.  The view keeps the larger allocation it is cut from alive."""
+    raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
+    off = (-raw.data_ptr()) % 1024
+    return raw[off:off + nbytes]
 
 
 class PackedWeights:
@@ -80,7 +85,6 @@ class PackedWeights:
             key = (ptrs, tuple([p._version for p in params]))
             if self.blob is not None and key == self.key:
                 return False
-        lib = _lib.load()
         if ptrs != self.ptrs:            # first use / storage changed: validate, (re)allocate, rebuild the pointer table
             for p, shp in zip(params, _EXPECTED_SHAPES):
                 if tuple(p.shape) != shp:
@@ -91,11 +95,7 @@ class PackedWeights:
                     raise ValueError("NeRF parameters must be contiguous float32 CUDA tensors")
             dev = params[0].device
             if self.blob is None or self.blob.device != dev:
-                # the library wants 1024-byte alignment; torch's caching allocator guarantees 512
-                raw = torch.empty(lib.nerfb200_packed_bytes() + 1024, dtype=torch.uint8, device=dev)
-                off = (-raw.data_ptr()) % 1024
-                self.raw = raw
-                self.blob = raw[off:off + lib.nerfb200_packed_bytes()]
+                self.blob = _aligned_buffer(_lib.load().nerfb200_packed_bytes(), dev)
             self.arr = (ctypes.c_void_p * 24)(*[ctypes.c_void_p(a) for a in ptrs])
             self.blob_ptr = ctypes.c_void_p(self.blob.data_ptr())
             self.ptrs = ptrs
@@ -105,12 +105,7 @@ class PackedWeights:
 
     def get(self, model: nn.Module) -> torch.Tensor:
         if self.prepare(model):
-            lib = _lib.load()
-            if torch.cuda.current_device() == self.dev.index:
-                _lib.check(lib.nerfb200_pack_weights(self.arr, self.blob_ptr, _stream_ptr()), "nerfb200_pack_weights")
-            else:
-                with torch.cuda.device(self.dev):
-                    _lib.check(lib.nerfb200_pack_weights(self.arr, self.blob_ptr, _stream_ptr()), "nerfb200_pack_weights")
+            _lib.call("nerfb200_pack_weights", self.dev, self.arr, self.blob_ptr)
         return self.blob
 
 
@@ -123,20 +118,16 @@ def invalidate_packed(model: nn.Module) -> None:
             cache.key = ()
 
 
-def packed_weights(model: nn.Module) -> torch.Tensor:
-    cache = model.__dict__.get("_nerfb200_packed")
-    if cache is None:
-        cache = PackedWeights()
-        model.__dict__["_nerfb200_packed"] = cache
-    return cache.get(model)
-
-
 def _cache_of(model: nn.Module) -> PackedWeights:
     cache = model.__dict__.get("_nerfb200_packed")
     if cache is None:
         cache = PackedWeights()
         model.__dict__["_nerfb200_packed"] = cache
     return cache
+
+
+def packed_weights(model: nn.Module) -> torch.Tensor:
+    return _cache_of(model).get(model)
 
 
 def packed_weights_pair(coarse: nn.Module, fine: nn.Module):
@@ -147,17 +138,12 @@ def packed_weights_pair(coarse: nn.Module, fine: nn.Module):
         blob = ca.get(coarse)
         return blob, blob
     na, nb_ = ca.prepare(coarse), cb.prepare(fine)
-    if na or nb_:
-        lib = _lib.load()
-        with torch.cuda.device(ca.dev):
-            if na and nb_ and ca.dev == cb.dev:
-                _lib.check(lib.nerfb200_pack_weights_pair(ca.arr, ca.blob_ptr, cb.arr, cb.blob_ptr, _stream_ptr()),
-                           "nerfb200_pack_weights_pair")
-            else:
-                for need, c in ((na, ca), (nb_, cb)):
-                    if need:
-                        with torch.cuda.device(c.dev):
-                            _lib.check(lib.nerfb200_pack_weights(c.arr, c.blob_ptr, _stream_ptr()), "nerfb200_pack_weights")
+    if na and nb_ and ca.dev == cb.dev:
+        _lib.call("nerfb200_pack_weights_pair", ca.dev, ca.arr, ca.blob_ptr, cb.arr, cb.blob_ptr)
+    else:
+        for need, c in ((na, ca), (nb_, cb)):
+            if need:
+                _lib.call("nerfb200_pack_weights", c.dev, c.arr, c.blob_ptr)
     return ca.blob, cb.blob
 
 
@@ -180,12 +166,9 @@ class Embedding(nn.Module):
         fused = (x.is_cuda and self.logscale and self.in_channels == 3 and x.dtype == torch.float32
                  and x.dim() == 2 and not (torch.is_grad_enabled() and x.requires_grad))
         if fused:
-            lib = _lib.load()
             xc = x.contiguous()
             out = torch.empty(xc.shape[0], self.out_channels, dtype=torch.float32, device=x.device)
-            with torch.cuda.device(x.device):
-                _lib.check(lib.nerfb200_embed(xc.data_ptr(), xc.shape[0], self.N_freqs, out.data_ptr(),
-                                              _stream_ptr()), "nerfb200_embed")
+            _lib.call("nerfb200_embed", x.device, xc.data_ptr(), xc.shape[0], self.N_freqs, out.data_ptr())
             return out
         if not x.is_cuda:
             raise RuntimeError("nerf_pl_b200.Embedding runs on CUDA tensors only (no CPU fallback)")
@@ -245,17 +228,14 @@ class NeRF(nn.Module):
 
 def nerf_forward_fused(model: nn.Module, x: torch.Tensor, sigma_only: bool = False) -> torch.Tensor:
     """NeRF.forward through the wgmma tile engine (C ABI ``nerfb200_nerf_forward``)."""
-    lib = _lib.load()
     width = 63 if sigma_only else 90
     if x.dim() != 2 or x.shape[1] != width:
         raise ValueError(f"expected x of shape (B, {width}), got {tuple(x.shape)}")
     xc = x.detach().to(torch.float32).contiguous()
     blob = packed_weights(model)
     out = torch.empty(xc.shape[0], 1 if sigma_only else 4, dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.nerfb200_nerf_forward(xc.data_ptr(), xc.shape[0], xc.stride(0), blob.data_ptr(),
-                                             int(sigma_only), out.data_ptr(), _stream_ptr()),
-                   "nerfb200_nerf_forward")
+    _lib.call("nerfb200_nerf_forward", x.device, xc.data_ptr(), xc.shape[0], xc.stride(0), blob.data_ptr(),
+              int(sigma_only), out.data_ptr())
     return out
 
 

@@ -26,7 +26,6 @@ import ctypes
 import torch
 
 from . import _lib
-from .nerf import _stream_ptr
 
 
 def _check_tensor(t: torch.Tensor, p: torch.Tensor, contiguous: bool = True) -> None:
@@ -108,13 +107,40 @@ class FusedAdam(torch.optim.Optimizer):
                                numel=(ctypes.c_int64 * n)(*[p.numel() for p in ch])))
         return chunks
 
+    def _cached_tables(self, gi, ps, sts, steps=None):
+        """The launch tables of group ``gi`` (``_tables``; with the capturable step counts ``steps``, each chunk also
+        gets their ``step`` table).  They hold raw pointers: rebuilt, after checking the tensors, whenever a parameter
+        or a state tensor is another allocation."""
+        key = (tuple([p.data_ptr() for p in ps]) + tuple([st["exp_avg"].data_ptr() for st in sts]) +
+               tuple([st["exp_avg_sq"].data_ptr() for st in sts]))
+        if steps is not None:
+            key += tuple([s.data_ptr() for s in steps])
+        cache = self._cache.get(gi)
+        if cache is None or cache["key"] != key:
+            for p, st in zip(ps, sts):
+                for t in (p, p.grad, st["exp_avg"], st["exp_avg_sq"]):
+                    _check_tensor(t, p, contiguous=t is not p.grad)
+            chunks = self._tables(ps, sts)
+            if steps is not None:
+                for ch, i0 in zip(chunks, range(0, len(ps), 64)):
+                    ch["step"] = (ctypes.c_void_p * len(ch["ps"]))(*[s.data_ptr() for s in steps[i0:i0 + 64]])
+            cache = dict(key=key, chunks=chunks)
+            self._cache[gi] = cache
+        return cache["chunks"]
+
+    @staticmethod
+    def _grads(ch):
+        """The chunk's gradients, made contiguous where they are not (the caller keeps them alive through the launch),
+        and their pointer array."""
+        gs = [p.grad if p.grad.is_contiguous() else p.grad.contiguous() for p in ch["ps"]]
+        return gs, (ctypes.c_void_p * len(gs))(*[g.data_ptr() for g in gs])
+
     @torch.no_grad()
     def step(self, closure=None):
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        lib = _lib.load()
         cap = self.capturable
         if cap:
             if torch.cuda.is_current_stream_capturing():
@@ -138,67 +164,39 @@ class FusedAdam(torch.optim.Optimizer):
                     st["step"] = torch.tensor(float(st["step"]), dtype=torch.float32)
             steps = [st["step"] for st in sts]
             if cap:
-                self._step_dev(lib, gi, group, ps, sts, steps)
+                self._step_dev(gi, group, ps, sts, steps)
                 continue
             ts = [int(s) for s in steps]
-            # the tables hold raw pointers: rebuilt whenever a parameter or a state tensor is another allocation
-            key = (tuple([p.data_ptr() for p in ps]) + tuple([st["exp_avg"].data_ptr() for st in sts]) +
-                   tuple([st["exp_avg_sq"].data_ptr() for st in sts]))
-            cache = self._cache.get(gi)
-            if cache is None or cache["key"] != key:
-                for p, st in zip(ps, sts):
-                    for t in (p, p.grad, st["exp_avg"], st["exp_avg_sq"]):
-                        _check_tensor(t, p, contiguous=t is not p.grad)
-                cache = dict(key=key, chunks=self._tables(ps, sts), dev=ps[0].device)
-                self._cache[gi] = cache
+            chunks = self._cached_tables(gi, ps, sts)
             if all(t == ts[0] for t in ts):
-                launches = [(ts[0], cache["chunks"])]
+                launches = [(ts[0], chunks)]
             else:                                 # parameters at different step counts (some skipped a step)
                 by_t = {}
                 for i, t in enumerate(ts):
                     by_t.setdefault(t, []).append(i)
                 launches = [(t, self._tables([ps[i] for i in ix], [sts[i] for i in ix])) for t, ix in by_t.items()]
             b1, b2 = group["betas"]
-            with torch.cuda.device(cache["dev"]):
-                for t, chunks in launches:
-                    for ch in chunks:
-                        gs = [p.grad if p.grad.is_contiguous() else p.grad.contiguous() for p in ch["ps"]]
-                        garr = (ctypes.c_void_p * len(gs))(*[g.data_ptr() for g in gs])
-                        _lib.check(lib.nerfb200_adam_step(len(gs), ch["p"], garr, ch["m"], ch["v"], ch["numel"],
-                                                          float(group["lr"]), float(b1), float(b2), float(group["eps"]),
-                                                          float(group["weight_decay"]), t + 1, _stream_ptr()),
-                                   "nerfb200_adam_step")
+            for t, chunks in launches:
+                for ch in chunks:
+                    gs, garr = self._grads(ch)
+                    _lib.call("nerfb200_adam_step", ps[0].device, len(gs), ch["p"], garr, ch["m"], ch["v"], ch["numel"],
+                              float(group["lr"]), float(b1), float(b2), float(group["eps"]),
+                              float(group["weight_decay"]), t + 1)
             torch._foreach_add_(steps, 1.0)
         return loss
 
-    def _step_dev(self, lib, gi, group, ps, sts, steps) -> None:
+    def _step_dev(self, gi, group, ps, sts, steps) -> None:
         """The capturable update of one group: no host value that changes from step to step enters the launch."""
         for st, p in zip(sts, ps):
             if not (torch.is_tensor(st["step"]) and st["step"].device == p.device and st["step"].dim() == 0
                     and st["step"].dtype == torch.float32):
                 raise RuntimeError("FusedAdam(capturable=True) keeps each step count as a 0-dim float32 tensor on the "
                                    "parameter's device")
-        key = (tuple([p.data_ptr() for p in ps]) + tuple([st["exp_avg"].data_ptr() for st in sts]) +
-               tuple([st["exp_avg_sq"].data_ptr() for st in sts]) + tuple([s.data_ptr() for s in steps]))
-        cache = self._cache.get(gi)
-        if cache is None or cache["key"] != key:
-            for p, st in zip(ps, sts):
-                for t in (p, p.grad, st["exp_avg"], st["exp_avg_sq"]):
-                    _check_tensor(t, p, contiguous=t is not p.grad)
-            chunks = self._tables(ps, sts)
-            for ch, i0 in zip(chunks, range(0, len(ps), 64)):
-                ch["step"] = (ctypes.c_void_p * len(ch["ps"]))(*[s.data_ptr() for s in steps[i0:i0 + 64]])
-            cache = dict(key=key, chunks=chunks, dev=ps[0].device)
-            self._cache[gi] = cache
         lr = self._lr_dev[gi]
         b1, b2 = group["betas"]
-        with torch.cuda.device(cache["dev"]):
-            for ch in cache["chunks"]:
-                gs = [p.grad if p.grad.is_contiguous() else p.grad.contiguous() for p in ch["ps"]]
-                garr = (ctypes.c_void_p * len(gs))(*[g.data_ptr() for g in gs])
-                _lib.check(lib.nerfb200_adam_step_dev(len(gs), ch["p"], garr, ch["m"], ch["v"], ch["numel"],
-                                                      lr.data_ptr(), ch["step"], float(b1), float(b2),
-                                                      float(group["eps"]), float(group["weight_decay"]),
-                                                      _stream_ptr()),
-                           "nerfb200_adam_step_dev")
+        for ch in self._cached_tables(gi, ps, sts, steps):
+            gs, garr = self._grads(ch)
+            _lib.call("nerfb200_adam_step_dev", ps[0].device, len(gs), ch["p"], garr, ch["m"], ch["v"], ch["numel"],
+                      lr.data_ptr(), ch["step"], float(b1), float(b2), float(group["eps"]),
+                      float(group["weight_decay"]))
         torch._foreach_add_(steps, 1.0)

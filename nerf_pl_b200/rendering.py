@@ -13,7 +13,7 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from . import _lib
-from .nerf import _stream_ptr, nerf_forward_torch, packed_weights
+from .nerf import nerf_forward_torch, packed_weights
 
 __all__ = ["render_rays", "render_rays_host", "render_rays_loss", "sample_pdf", "searchsorted", "volume_render"]
 
@@ -50,6 +50,19 @@ def _check_embeddings(embeddings: Sequence) -> None:
         _EMB_OK.add((id(ex), id(ed)))
 
 
+def _check_render_inputs(name: str, models, embeddings, N_importance: int, rays: Optional[torch.Tensor]) -> None:
+    """The argument checks of render_rays, render_rays_loss and render_rays_host (``name``, the public function the
+    messages name).  ``rays`` are device rays; None for render_rays_host, which checks its host rays itself."""
+    if rays is not None:
+        if rays.dim() != 2 or rays.shape[1] != 8:
+            raise ValueError("rays must be (N_rays, 8)")
+        if not rays.is_cuda:
+            raise RuntimeError(f"nerf_pl_b200.{name} runs on CUDA tensors only (no CPU fallback)")
+    _check_embeddings(embeddings)
+    if N_importance > 0 and len(models) < 2:
+        raise ValueError("N_importance > 0 needs a fine model (models[1])")
+
+
 def searchsorted(a: torch.Tensor, v: torch.Tensor, out: Optional[torch.Tensor] = None,
                  side: str = "left") -> torch.Tensor:
     """Row-wise batched binary search; same contract as torchsearchsorted.searchsorted
@@ -65,7 +78,6 @@ def searchsorted(a: torch.Tensor, v: torch.Tensor, out: Optional[torch.Tensor] =
     if not a.is_cuda:
         raise RuntimeError("nerf_pl_b200.searchsorted runs on CUDA tensors only (no CPU fallback)")
     _require_fp32("searchsorted", a, v)
-    lib = _lib.load()
     nrow = max(a.shape[0], v.shape[0])
     if out is None:
         out = torch.empty(nrow, v.shape[1], dtype=torch.long, device=v.device)
@@ -73,11 +85,8 @@ def searchsorted(a: torch.Tensor, v: torch.Tensor, out: Optional[torch.Tensor] =
         assert out.shape == (nrow, v.shape[1]) and out.dtype == torch.long and out.is_contiguous()
     ac = a.to(torch.float32).contiguous()
     vc = v.to(torch.float32).contiguous()
-    with torch.cuda.device(a.device):
-        _lib.check(lib.nerfb200_searchsorted(ac.data_ptr(), vc.data_ptr(), out.data_ptr(), ac.shape[0],
-                                             vc.shape[0], ac.shape[1], vc.shape[1],
-                                             1 if side == "right" else 0, _stream_ptr()),
-                   "nerfb200_searchsorted")
+    _lib.call("nerfb200_searchsorted", a.device, ac.data_ptr(), vc.data_ptr(), out.data_ptr(), ac.shape[0],
+              vc.shape[0], ac.shape[1], vc.shape[1], 1 if side == "right" else 0)
     return out
 
 
@@ -99,13 +108,10 @@ def sample_pdf(bins: torch.Tensor, weights: torch.Tensor, N_importance: int, det
         else:
             u = torch.rand(n_rays, N_importance, device=bins.device)
     u = u.to(torch.float32).contiguous()
-    lib = _lib.load()
     out = torch.empty(n_rays, N_importance, dtype=torch.float32, device=bins.device)
     bc, wc = bins.to(torch.float32).contiguous(), weights.detach().to(torch.float32).contiguous()
-    with torch.cuda.device(bins.device):
-        _lib.check(lib.nerfb200_sample_pdf(bc.data_ptr(), wc.data_ptr(), u.data_ptr(), n_rays, n_w,
-                                           N_importance, out.data_ptr(), _stream_ptr()),
-                   "nerfb200_sample_pdf")
+    _lib.call("nerfb200_sample_pdf", bins.device, bc.data_ptr(), wc.data_ptr(), u.data_ptr(), n_rays, n_w,
+              N_importance, out.data_ptr())
     return out
 
 
@@ -118,7 +124,6 @@ def volume_render(sigmas: torch.Tensor, rgbs: Optional[torch.Tensor], z_vals: to
         raise RuntimeError("nerf_pl_b200.volume_render runs on CUDA tensors only (no CPU fallback)")
     _require_fp32("volume_render", sigmas, rgbs, z_vals, dirs, noise)
     n, S = sigmas.shape
-    lib = _lib.load()
     dev = sigmas.device
     f32 = dict(dtype=torch.float32, device=dev)
     weights = torch.empty(n, S, **f32)
@@ -128,11 +133,8 @@ def volume_render(sigmas: torch.Tensor, rgbs: Optional[torch.Tensor], z_vals: to
     keep = [sigmas.float().contiguous(), None if rgbs is None else rgbs.float().contiguous(),
             z_vals.float().contiguous(), dirs.float().contiguous(),
             None if noise is None else noise.float().contiguous()]
-    with torch.cuda.device(dev):
-        _lib.check(lib.nerfb200_composite(_ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]),
-                                          _ptr(keep[4]), float(noise_std), int(bool(white_back)), n, S,
-                                          weights.data_ptr(), _ptr(rgb), _ptr(depth), opac.data_ptr(),
-                                          _stream_ptr()), "nerfb200_composite")
+    _lib.call("nerfb200_composite", dev, _ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]), _ptr(keep[4]),
+              float(noise_std), int(bool(white_back)), n, S, weights.data_ptr(), _ptr(rgb), _ptr(depth), opac.data_ptr())
     return weights, rgb, depth, opac
 
 
@@ -171,6 +173,23 @@ def _seed_fields(seed) -> Dict[str, int]:
     if torch.is_tensor(seed):
         return dict(rng_seed=seed.data_ptr(), rng_in_kernel=2)
     return dict(rng_seed=seed, rng_in_kernel=1)
+
+
+def _render_args(rays, S_c: int, K: int, use_disp, perturb: float, noise_std: float, white_back, test_time,
+                 packed, randoms, outs: Dict[str, Optional[torch.Tensor]], seed, workspace=None, target=None,
+                 loss_out=None) -> _lib.RenderArgs:
+    """The ``nerfb200_render_args`` of one render.  ``packed``: the (coarse, fine | None) weight images; ``randoms``:
+    (perturb_rand, noise_coarse, u_rand, noise_fine), each None when not drawn; ``outs``: output tensors keyed by field
+    name; ``workspace``: a training workspace.  Every field not given is zero / NULL."""
+    pr, nc, ur, nf = randoms
+    return _lib.RenderArgs(
+        rays=rays.data_ptr(), n_rays=rays.shape[0], ray_stride=rays.stride(0),
+        packed_coarse=packed[0].data_ptr(), packed_fine=_ptr(packed[1]),
+        n_samples=S_c, n_importance=K, use_disp=int(bool(use_disp)), perturb=perturb, noise_std=noise_std,
+        white_back=int(bool(white_back)), test_time=int(bool(test_time)),
+        perturb_rand=_ptr(pr), noise_coarse=_ptr(nc), u_rand=_ptr(ur), noise_fine=_ptr(nf),
+        train_workspace=None if workspace is None else workspace.buf.data_ptr(), target=_ptr(target),
+        loss_out=_ptr(loss_out), **{k: _ptr(t) for k, t in outs.items()}, **_seed_fields(seed))
 
 
 def _resolve_randoms(randoms, n, S_c, K, perturb, noise_std, dev, match_rng):
@@ -254,13 +273,7 @@ def render_rays(models: List[torch.nn.Module],
     del chunk
     if autograd_impl not in ("fused", "torch"):
         raise ValueError("autograd_impl must be 'fused' or 'torch'")
-    if rays.dim() != 2 or rays.shape[1] != 8:
-        raise ValueError("rays must be (N_rays, 8)")
-    if not rays.is_cuda:
-        raise RuntimeError("nerf_pl_b200.render_rays runs on CUDA tensors only (no CPU fallback)")
-    _check_embeddings(embeddings)
-    if N_importance > 0 and len(models) < 2:
-        raise ValueError("N_importance > 0 needs a fine model (models[1])")
+    _check_render_inputs("render_rays", models, embeddings, N_importance, rays)
     needs_graph = torch.is_grad_enabled() and any(
         p.requires_grad for m in models[:2] for p in m.parameters())
 
@@ -299,25 +312,10 @@ def render_rays(models: List[torch.nn.Module],
     w_c = torch.empty(n, S_c, **f32) if extras else None
     w_f = torch.empty(n, S_f, **f32) if (extras and K > 0) else None
 
-    lib = _lib.load()
-    blob_c = packed_weights(models[0])
-    blob_f = packed_weights(models[1]) if K > 0 else None
-    args = _lib.RenderArgs(
-        rays=rays_c.data_ptr(), n_rays=n, ray_stride=rays_c.stride(0),
-        packed_coarse=blob_c.data_ptr(), packed_fine=_ptr(blob_f),
-        n_samples=S_c, n_importance=K, use_disp=int(bool(use_disp)), perturb=perturb,
-        noise_std=noise_std, white_back=int(bool(white_back)), test_time=int(bool(test_time)),
-        perturb_rand=_ptr(pr), noise_coarse=_ptr(nc), u_rand=_ptr(ur), noise_fine=_ptr(nf),
-        rgb_coarse=_ptr(out["rgb_coarse"]), depth_coarse=_ptr(out["depth_coarse"]),
-        opacity_coarse=_ptr(out["opacity_coarse"]), rgb_fine=_ptr(out["rgb_fine"]),
-        depth_fine=_ptr(out["depth_fine"]), opacity_fine=_ptr(out["opacity_fine"]),
-        z_fine=_ptr(z_fine), weights_coarse=_ptr(w_c), weights_fine=_ptr(w_f),
-        status=None, max_ctas=0, **_seed_fields(seed))
-    if torch.cuda.current_device() == dev.index:
-        _lib.check(lib.nerfb200_render_rays(ctypes.byref(args), _stream_ptr()), "nerfb200_render_rays")
-    else:
-        with torch.cuda.device(dev):
-            _lib.check(lib.nerfb200_render_rays(ctypes.byref(args), _stream_ptr()), "nerfb200_render_rays")
+    packed = (packed_weights(models[0]), packed_weights(models[1]) if K > 0 else None)
+    args = _render_args(rays_c, S_c, K, use_disp, perturb, noise_std, white_back, test_time, packed, (pr, nc, ur, nf),
+                        dict(out, z_fine=z_fine, weights_coarse=w_c, weights_fine=w_f), seed)
+    _lib.call("nerfb200_render_rays", dev, ctypes.byref(args))
 
     if needs_graph:
         return _render_with_graph(models, embeddings, rays_c, S_c, K, bool(use_disp), perturb, noise_std,
@@ -358,9 +356,7 @@ def render_rays_host(models: List[torch.nn.Module],
     del chunk
     if rays.is_cuda or rays.dim() != 2 or rays.shape[1] != 8 or rays.dtype != torch.float32:
         raise ValueError("rays must be a (N_rays, 8) float32 CPU tensor")
-    _check_embeddings(embeddings)
-    if N_importance > 0 and len(models) < 2:
-        raise ValueError("N_importance > 0 needs a fine model (models[1])")
+    _check_render_inputs("render_rays_host", models, embeddings, N_importance, None)
     dev = next(models[0].parameters()).device
     if dev.type != "cuda":
         raise RuntimeError("the models must live on a CUDA device (no CPU fallback)")
@@ -368,33 +364,22 @@ def render_rays_host(models: List[torch.nn.Module],
     if rays.stride(1) != 1 or rays.stride(0) < 8:
         rays = rays.contiguous()          # a row stride (column slice of a wider tensor) is passed through
     pinned = rays.is_pinned()       # results then come back in pinned memory too: the C entry's zero-copy path
-    with torch.cuda.device(dev):
-        pr, nc, ur, nf, seed = _resolve_randoms(randoms, n, S_c, K, float(perturb), float(noise_std), dev,
-                                                match_reference_rng)
-        keys = ["opacity_coarse"] if test_time else ["rgb_coarse", "depth_coarse", "opacity_coarse"]
-        if K > 0:
-            keys += ["rgb_fine", "depth_fine", "opacity_fine"]
-        res = {}
-        for k in keys:
-            shape = (n, 3) if k.startswith("rgb") else (n,)
-            t = out[k] if out is not None and k in out else torch.empty(shape, dtype=torch.float32, pin_memory=pinned)
-            if t.is_cuda or t.shape != shape or t.dtype != torch.float32 or not t.is_contiguous():
-                raise ValueError(f"out[{k!r}] must be a contiguous float32 CPU tensor of shape {shape}")
-            res[k] = t
-        lib = _lib.load()
-        blob_c = packed_weights(models[0])
-        blob_f = packed_weights(models[1]) if K > 0 else None
-        args = _lib.RenderArgs(
-            rays=rays.data_ptr(), n_rays=n, ray_stride=rays.stride(0),
-            packed_coarse=blob_c.data_ptr(), packed_fine=_ptr(blob_f),
-            n_samples=S_c, n_importance=K, use_disp=int(bool(use_disp)), perturb=float(perturb),
-            noise_std=float(noise_std), white_back=int(bool(white_back)), test_time=int(bool(test_time)),
-            perturb_rand=_ptr(pr), noise_coarse=_ptr(nc), u_rand=_ptr(ur), noise_fine=_ptr(nf),
-            rgb_coarse=_ptr(res.get("rgb_coarse")), depth_coarse=_ptr(res.get("depth_coarse")),
-            opacity_coarse=_ptr(res.get("opacity_coarse")), rgb_fine=_ptr(res.get("rgb_fine")),
-            depth_fine=_ptr(res.get("depth_fine")), opacity_fine=_ptr(res.get("opacity_fine")),
-            **_seed_fields(seed))
-        _lib.check(lib.nerfb200_render_rays_host(ctypes.byref(args), _stream_ptr()), "nerfb200_render_rays_host")
+    perturb, noise_std = float(perturb), float(noise_std)
+    pr, nc, ur, nf, seed = _resolve_randoms(randoms, n, S_c, K, perturb, noise_std, dev, match_reference_rng)
+    keys = ["opacity_coarse"] if test_time else ["rgb_coarse", "depth_coarse", "opacity_coarse"]
+    if K > 0:
+        keys += ["rgb_fine", "depth_fine", "opacity_fine"]
+    res = {}
+    for k in keys:
+        shape = (n, 3) if k.startswith("rgb") else (n,)
+        t = out[k] if out is not None and k in out else torch.empty(shape, dtype=torch.float32, pin_memory=pinned)
+        if t.is_cuda or t.shape != shape or t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError(f"out[{k!r}] must be a contiguous float32 CPU tensor of shape {shape}")
+        res[k] = t
+    packed = (packed_weights(models[0]), packed_weights(models[1]) if K > 0 else None)
+    args = _render_args(rays, S_c, K, use_disp, perturb, noise_std, white_back, test_time, packed, (pr, nc, ur, nf),
+                        res, seed)
+    _lib.call("nerfb200_render_rays_host", dev, ctypes.byref(args))
     return res
 
 
@@ -419,13 +404,7 @@ def render_rays_loss(models: List[torch.nn.Module],
     ``psnr``, ``mse_coarse``, ``mse_fine``; ``loss.backward()`` runs the fused sm_90a backward with
     the gradient seed 2 (rgb - rgbs) / (3 N) formed inside the compositing-backward kernel."""
     del chunk
-    if rays.dim() != 2 or rays.shape[1] != 8:
-        raise ValueError("rays must be (N_rays, 8)")
-    if not rays.is_cuda:
-        raise RuntimeError("nerf_pl_b200.render_rays_loss runs on CUDA tensors only (no CPU fallback)")
-    _check_embeddings(embeddings)
-    if N_importance > 0 and len(models) < 2:
-        raise ValueError("N_importance > 0 needs a fine model (models[1])")
+    _check_render_inputs("render_rays_loss", models, embeddings, N_importance, rays)
     n, S_c, K = rays.shape[0], int(N_samples), int(N_importance)
     if n == 0:
         raise ValueError("empty ray batch")

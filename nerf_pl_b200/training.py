@@ -26,29 +26,21 @@ from typing import Dict, List, Optional
 import torch
 
 from . import _lib
-from .nerf import (_EXPECTED_SHAPES, _stream_ptr, nerf_forward_fused, nerf_parameters, packed_weights,
+from .nerf import (_EXPECTED_SHAPES, _aligned_buffer, nerf_forward_fused, nerf_parameters, packed_weights,
                    packed_weights_pair)
 from .data import DeviceRayBatches, next_step_schedule
-from .rendering import _draw_randoms, _seed_fields
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else t.data_ptr()
+from .rendering import _draw_randoms, _ptr, _render_args
 
 
 class _Workspace:
-    """A 1024-byte aligned device buffer (``buf``, ``bytes`` long; ``raw`` owns it) prepared by the library entry
-    ``init`` as ``init(buf, bytes, *args, stream)``.  ``busy``: held by a call whose backward is pending."""
+    """A 1024-byte aligned device buffer (``buf``, ``bytes`` long) prepared by the library entry ``init`` as
+    ``init(buf, bytes, *args, stream)``.  ``busy``: held by a call whose backward is pending."""
 
     def __init__(self, dev: torch.device, nbytes: int, init: str, *args) -> None:
-        raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-        off = (-raw.data_ptr()) % 1024
-        self.raw = raw
-        self.buf = raw[off:off + nbytes]
+        self.buf = _aligned_buffer(nbytes, dev)
         self.bytes = nbytes
         self.busy = False
-        with torch.cuda.device(dev):
-            _lib.check(getattr(_lib.load(), init)(self.buf.data_ptr(), nbytes, *args, _stream_ptr()), init)
+        _lib.call(init, dev, self.buf.data_ptr(), nbytes, *args)
 
 
 class TrainWorkspace(_Workspace):
@@ -102,20 +94,7 @@ class _Lease:
         self.release()
 
 
-def _render_args(cfg, rays, pr, nc, ur, nf, out, blob_c, blob_f, ws, target, loss_out) -> _lib.RenderArgs:
-    K = cfg["N_importance"]
-    return _lib.RenderArgs(
-        rays=rays.data_ptr(), n_rays=rays.shape[0], ray_stride=rays.stride(0),
-        packed_coarse=blob_c.data_ptr(), packed_fine=_ptr(blob_f),
-        n_samples=cfg["N_samples"], n_importance=K, use_disp=int(cfg["use_disp"]), perturb=cfg["perturb"],
-        noise_std=cfg["noise_std"], white_back=int(cfg["white_back"]), test_time=0,
-        perturb_rand=_ptr(pr), noise_coarse=_ptr(nc), u_rand=_ptr(ur), noise_fine=_ptr(nf),
-        rgb_coarse=out[0].data_ptr(), depth_coarse=out[1].data_ptr(), opacity_coarse=out[2].data_ptr(),
-        rgb_fine=_ptr(out[3]) if K > 0 else None, depth_fine=_ptr(out[4]) if K > 0 else None,
-        opacity_fine=_ptr(out[5]) if K > 0 else None,
-        z_fine=None, weights_coarse=None, weights_fine=None, status=None, max_ctas=0, z_coarse=None,
-        train_workspace=ws.buf.data_ptr(), target=_ptr(target), loss_out=_ptr(loss_out),
-        **_seed_fields(cfg.get("rng_seed")))
+_OUTPUTS = ("rgb_coarse", "depth_coarse", "opacity_coarse", "rgb_fine", "depth_fine", "opacity_fine")
 
 
 class FusedRenderFunction(torch.autograd.Function):
@@ -132,7 +111,6 @@ class FusedRenderFunction(torch.autograd.Function):
         if K > 0:
             out += [torch.empty(n, 3, **f32), torch.empty(n, **f32), torch.empty(n, **f32)]
         loss_out = torch.empty(4, **f32) if target is not None else None
-        lib = _lib.load()
         if K > 0:
             blob_c, blob_f = packed_weights_pair(models[0], models[1])      # one launch for both images
         else:
@@ -141,15 +119,18 @@ class FusedRenderFunction(torch.autograd.Function):
         if own is not None and own.key != (dev.index, n, S_c, K):
             raise ValueError("the given training workspace is of another shape")
         lease = _Lease(own if own is not None else TrainWorkspace.acquire(dev, n, S_c, K))
-        ws = lease.ws
-        args = _render_args(cfg, rays, pr, nc, ur, nf, out, blob_c, blob_f, ws, target, loss_out)
-        with torch.cuda.device(dev):
-            _lib.check(lib.nerfb200_render_rays(ctypes.byref(args), _stream_ptr()), "nerfb200_render_rays")
+        args = _render_args(rays, S_c, K, cfg["use_disp"], cfg["perturb"], cfg["noise_std"], cfg["white_back"], False,
+                            (blob_c, blob_f), (pr, nc, ur, nf), dict(zip(_OUTPUTS, out)), cfg.get("rng_seed"),
+                            lease.ws, target, loss_out)
+        _lib.call("nerfb200_render_rays", dev, ctypes.byref(args))
         ctx.cfg = cfg
         ctx.lease = lease
-        # detached aliases of the outputs: the returned tensors themselves on ctx would form a cycle (output ->
-        # grad_fn -> ctx -> output) that keeps a dropped graph, and with it the workspace, alive
-        ctx.keep = (rays, pr, nc, ur, nf, target, [o.detach() for o in out], blob_c, blob_f, ws)
+        # the backward takes the same render args without the loss epilogue (its seed comes in the backward args)
+        args.target = args.loss_out = None
+        ctx.args = args
+        # what the args point to.  Detached aliases of the outputs: the returned tensors themselves on ctx would form
+        # a cycle (output -> grad_fn -> ctx -> output) that keeps a dropped graph, and with it the workspace, alive
+        ctx.keep = (rays, pr, nc, ur, nf, target, [o.detach() for o in out], blob_c, blob_f, lease.ws)
         ctx.n_params = len(params)
         ctx.save_for_backward(*params)
         ctx.set_materialize_grads(False)
@@ -164,12 +145,9 @@ class FusedRenderFunction(torch.autograd.Function):
         if lease.ws is None:
             raise RuntimeError("the fused backward of this render has already run (its training workspace is released "
                                "after one backward; retain_graph=True is not supported with autograd_impl='fused')")
-        cfg = ctx.cfg
         params = list(ctx.saved_tensors)
-        rays, pr, nc, ur, nf, target, out, blob_c, blob_f, ws = ctx.keep
-        K = cfg["N_importance"]
-        dev = rays.device
-        lib = _lib.load()
+        rays, target = ctx.keep[0], ctx.keep[5]
+        K = ctx.cfg["N_importance"]
         g = [None if t is None else t.detach().to(torch.float32).contiguous() for t in gouts]
         g6 = g[:6] + [None] * (6 - min(len(g), 6))
         if K == 0:
@@ -184,28 +162,17 @@ class FusedRenderFunction(torch.autograd.Function):
                 # seed restricted to one pass is not provided); take the gradient of the total loss
                 loss_grad = g4          # the kernel reads element 2 (address passed below)
                 use_target = target
-        # one allocation for all gradients (the kernels write every element), views per parameter
-        sizes, shapes = _param_sizes(params)
-        flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
-        grads = [t.view(shp) for t, shp in zip(flat.split(sizes), shapes)]
-        base, offs = flat.data_ptr(), _offsets(sizes)
-        pc = (ctypes.c_void_p * 24)(*[p.data_ptr() for p in params[:24]])
-        gc = (ctypes.c_void_p * 24)(*[base + 4 * o for o in offs[:24]])
-        pf = gf = None
-        if K > 0:
-            pf = (ctypes.c_void_p * 24)(*[p.data_ptr() for p in params[24:48]])
-            gf = (ctypes.c_void_p * 24)(*[base + 4 * o for o in offs[24:48]])
-        rargs = _render_args(cfg, rays, pr, nc, ur, nf, out, blob_c, blob_f, ws, None, None)
+        grads, tables = _grad_buffers(params, rays.device)
+        (pc, gc), (pf, gf) = tables[0], (tables[1] if K > 0 else (None, None))
         bargs = _lib.BackwardArgs(
-            render=ctypes.pointer(rargs), params_coarse=pc, params_fine=pf,
+            render=ctypes.pointer(ctx.args), params_coarse=pc, params_fine=pf,
             g_rgb_coarse=_ptr(g6[0]), g_depth_coarse=_ptr(g6[1]), g_opacity_coarse=_ptr(g6[2]),
             g_rgb_fine=_ptr(g6[3]), g_depth_fine=_ptr(g6[4]), g_opacity_fine=_ptr(g6[5]),
             target=_ptr(use_target), loss_grad=None if loss_grad is None else loss_grad.data_ptr() + 8,
             grads_coarse=gc, grads_fine=gf)
-        with torch.cuda.device(dev):
-            _lib.check(lib.nerfb200_render_backward(ctypes.byref(bargs), _stream_ptr()), "nerfb200_render_backward")
+        _lib.call("nerfb200_render_backward", rays.device, ctypes.byref(bargs))
         lease.release()
-        ctx.keep = None
+        ctx.keep = ctx.args = None
         if K == 0:
             grads = grads[:24] + [None] * (ctx.n_params - 24)
         return (None, None, None, None, None, None, None, *grads)
@@ -223,12 +190,15 @@ def _param_sizes(params):
     return hit
 
 
-def _offsets(sizes):
-    out, o = [], 0
-    for n in sizes:
-        out.append(o)
-        o += n
-    return out
+def _grad_buffers(params, dev):
+    """The gradients of ``params`` as views of one allocation (the kernels write every element), and per network
+    (24 parameters each) the ctypes pointer arrays (parameters, gradients) the backward entries take."""
+    sizes, shapes = _param_sizes(params)
+    flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
+    grads = [t.view(shp) for t, shp in zip(flat.split(sizes), shapes)]
+    tables = [((ctypes.c_void_p * 24)(*[p.data_ptr() for p in params[i:i + 24]]),
+               (ctypes.c_void_p * 24)(*[t.data_ptr() for t in grads[i:i + 24]])) for i in range(0, len(params), 24)]
+    return grads, tables
 
 
 def _params_of(models, N_importance) -> List[torch.Tensor]:
@@ -320,13 +290,10 @@ class FusedNerfFunction(torch.autograd.Function):
         ctx.n = n
         ctx.lease = None
         if n > 0:
-            lib = _lib.load()
             blob = packed_weights(model)
             lease = _Lease(NerfTrainWorkspace.acquire(dev, n))
-            with torch.cuda.device(dev):
-                _lib.check(lib.nerfb200_nerf_forward_train(x.data_ptr(), n, x.stride(0), blob.data_ptr(),
-                                                           lease.ws.buf.data_ptr(), out.data_ptr(), _stream_ptr()),
-                           "nerfb200_nerf_forward_train")
+            _lib.call("nerfb200_nerf_forward_train", dev, x.data_ptr(), n, x.stride(0), blob.data_ptr(),
+                      lease.ws.buf.data_ptr(), out.data_ptr())
             ctx.lease = lease
             ctx.blob = blob
         ctx.save_for_backward(*params)
@@ -346,17 +313,8 @@ class FusedNerfFunction(torch.autograd.Function):
         g = g.detach().to(torch.float32).contiguous()
         if g.data_ptr() % 16:
             g = g.clone()
-        sizes, shapes = _param_sizes(params)
-        flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
-        grads = [t.view(shp) for t, shp in zip(flat.split(sizes), shapes)]
-        base, offs = flat.data_ptr(), _offsets(sizes)
-        pc = (ctypes.c_void_p * 24)(*[p.data_ptr() for p in params])
-        gc = (ctypes.c_void_p * 24)(*[base + 4 * o for o in offs])
-        lib = _lib.load()
-        with torch.cuda.device(dev):
-            _lib.check(lib.nerfb200_nerf_backward(g.data_ptr(), ctx.n, ctx.blob.data_ptr(), pc,
-                                                  lease.ws.buf.data_ptr(), gc, _stream_ptr()),
-                       "nerfb200_nerf_backward")
+        grads, [(pc, gc)] = _grad_buffers(params, dev)
+        _lib.call("nerfb200_nerf_backward", dev, g.data_ptr(), ctx.n, ctx.blob.data_ptr(), pc, lease.ws.buf.data_ptr(), gc)
         lease.release()
         ctx.blob = None
         return (None, None, *grads)

@@ -31,6 +31,85 @@ def test_header_symbols_exported(lib):
         assert hasattr(lib, name), name
 
 
+def _header_prototypes():
+    """{name: (return type, [argument declarations])} of every function include/nerf_pl_b200.h declares."""
+    hdr = open(os.path.join(ROOT, "include", "nerf_pl_b200.h")).read()
+    hdr = re.sub(r"/\*.*?\*/", " ", hdr, flags=re.S)
+    hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
+    protos = {}
+    for decl in hdr.split(";"):
+        m = re.search(r"(.*?)\b(nerfb200_\w+)\s*\((.*)\)\s*$", decl.strip(), re.S)
+        if m:
+            ret = " ".join(re.split(r"[{}]", m.group(1))[-1].split())
+            args = [] if m.group(3).strip() == "void" else [" ".join(a.split()) for a in m.group(3).split(",")]
+            protos[m.group(2)] = (ret, args)
+    return protos
+
+
+def test_signature_table_matches_the_header():
+    """Every prototype of include/nerf_pl_b200.h against _lib.SIGNATURES: the same names, argument counts, argument
+    kinds and return types (a wrong width would silently corrupt the argument)."""
+    protos = _header_prototypes()
+    assert len(protos) == 47
+    assert set(protos) == set(_lib.SIGNATURES), set(protos) ^ set(_lib.SIGNATURES)
+    assert list(protos) == list(_lib.EXPORTS)           # header order
+    scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "size_t": ctypes.c_size_t,
+               "float": ctypes.c_float, "double": ctypes.c_double}
+    returns = {"int": ctypes.c_int32, "size_t": ctypes.c_size_t, "int64_t": ctypes.c_int64,
+               "const char*": ctypes.c_char_p}
+    for name, (ret, args) in protos.items():
+        restype, argtypes = _lib.SIGNATURES[name]
+        assert restype is returns[ret], (name, ret, restype)
+        assert len(argtypes) == len(args), (name, args, argtypes)
+        for decl, t in zip(args, argtypes):
+            if "*" in decl or "[" in decl:
+                assert t is ctypes.c_void_p or issubclass(t, ctypes._Pointer), (name, decl, t)
+            else:
+                base = decl.replace("const ", "").rsplit(" ", 1)[0]
+                assert t is scalars[base], (name, decl, t)
+
+
+def test_call_appends_the_stream_and_maps_return_codes(monkeypatch):
+    """_lib.call against a fake library: the stream goes last, 0 returns, -1 / -2 raise ValueError and a positive
+    code NerfB200Error, both with the entry's name and the library's message."""
+    class Fake:
+        rc = 0
+        calls = []
+
+        def nerfb200_embed(self, *args):
+            self.calls.append(args)
+            return self.rc
+
+        def nerfb200_last_error(self):
+            return b"what went wrong"
+
+    fake, stream = Fake(), object()
+    monkeypatch.setattr(_lib, "load", lambda: fake)
+    monkeypatch.setattr(_lib, "_stream_ptr", lambda: stream)
+    assert _lib.call("nerfb200_embed", None, 1, 2.5) is None
+    assert _lib.call("nerfb200_embed", torch.device("cuda"), 3) is None      # no index: the current device
+    assert fake.calls == [(1, 2.5, stream), (3, stream)]
+    for rc in (-1, -2):
+        fake.rc = rc
+        with pytest.raises(ValueError) as e:
+            _lib.call("nerfb200_embed", None, 4)
+        assert str(e.value) == "nerfb200_embed: what went wrong"
+    fake.rc = 700
+    with pytest.raises(_lib.NerfB200Error) as e:
+        _lib.call("nerfb200_embed", None, 5)
+    assert str(e.value) == "nerfb200_embed: what went wrong (code 700)"
+    assert fake.calls[-1] == (5, stream)
+
+
+def test_entries_are_called_through_lib_call():
+    """Only _lib.py picks the stream and maps return codes; every other module goes through _lib.call."""
+    pkg = os.path.join(ROOT, "nerf_pl_b200")
+    for fn in os.listdir(pkg):
+        if fn.endswith(".py") and fn != "_lib.py":
+            src = open(os.path.join(pkg, fn)).read()
+            assert "_lib.check(" not in src and ".cuda_stream" not in src, fn
+
+
 def test_abi_basics(lib):
     assert lib.nerfb200_abi_version() == 3
     # layout.h: 30 x 32 KiB + 5 x 16 KiB fp16 slices + fp32 tail, rounded to 1 KiB, + 30 backward slices
