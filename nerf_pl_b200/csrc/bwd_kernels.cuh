@@ -14,8 +14,8 @@
 //                         forward, 30 transposed weight slices per tile; writes dpre_l (tiled)
 //   wgrad_kernel          split-K wgmma GEMMs gW_l = dpre_l^T h_{l-1}: one CTA per (layer, sample
 //                         range), both operands MN-major straight from the tiled arrays, fp32
-//                         accumulators in registers for the CTA's whole range; bias gradients as column
-//                         sums on the CUDA cores of the same tiles
+//                         accumulators in registers per piece of the CTA's range, the pieces added in
+//                         fp32; bias gradients as column sums on the CUDA cores of the same tiles
 //   wgrad_reduce_kernel   fixed-order sum of the per-CTA partials into the .grad tensors
 //   unfold_kernel         chain rule through the pack-time folding W' = W_dir[:, :256] W_final
 //
@@ -664,8 +664,9 @@ __global__ void __launch_bounds__(kThreads, 1) chain_bwd_kernel(const ChainParam
 // tensor core contracts over the samples.  The output rows are taken 128 at a time ("halves" of
 // M = 256): per half and chunk, consumer warpgroup w accumulates
 //   D_w[64 x N] += A[:, 64 (2 half + w) ..]^T[64 x 64] . B[64 x N]      4 x wgmma (K = 16 samples)
-// in registers for the CTA's whole range and writes it out once, as a partial that
-// wgrad_reduce_kernel sums in a fixed order.  The kernel is HBM-bound by construction: the point of
+// in registers over one piece (a range of chunks) and writes it out, or adds it in fp32 to what the CTA's earlier
+// pieces wrote, as the CTA's partial, which wgrad_reduce_kernel sums with the other CTAs' partials in a fixed
+// order.  The kernel is HBM-bound by construction: the point of
 // the layout is that it reads the operands with no transposition pass and no staging through
 // registers.  Two more warps reduce the same shared-memory tiles on the CUDA cores: column sums of A
 // (the bias gradients).
@@ -684,6 +685,7 @@ struct WgradJob {          // one piece: a (pass, layer) GEMM over a contiguous 
   int b_fb;                // column blocks of B: N = 64 b_fb
   int chunk0, chunk1;      // 64-sample chunks chunk0, chunk0 + chunk_step, ... < chunk1
   int chunk_step;          // > 1: the CTAs of one GEMM interleave their chunks (they read one moving window of HBM)
+  int add;                 // 1: add into the partial, which the CTA's previous piece wrote; 0: write it
   float* out;              // partial, TRANSPOSED: element (m, n) at out[n * 64 a_fb + m]
   float* bias_out;         // partial column sums of A (64 a_fb) or null
 };
@@ -694,9 +696,9 @@ struct WgScratch {
 };
 
 // CTA b works through pieces [cta_first[b], cta_first[b + 1]).  The host (capi.cu plan_wgrad) gives every
-// (pass, layer) GEMM whole CTAs, one piece each, in proportion to the bytes it streams (at least one per
-// GEMM); the CTAs of one GEMM take its chunks round-robin.  CTAs do not synchronise with each other, so the
-// grid may run in more than one wave.
+// (pass, layer) GEMM whole CTAs in proportion to the bytes it streams (at least one per GEMM); the CTAs of one
+// GEMM take its chunks round-robin, each its share as consecutive pieces of a bounded length into one partial.
+// CTAs do not synchronise with each other, so the grid may run in more than one wave.
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __restrict__ jobs,
                                                                const int* __restrict__ cta_first, int* status) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -767,12 +769,21 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
           if (lane == 0) mbar_arrive(smem_u32(&sc->empty[stage]));
           if (++stage == kWgStages) { stage = 0; phase ^= 1; }
         }
-        // ---- drain: element (m, n) at out[n * M + m]
+        // ---- drain: element (m, n) at out[n * M + m].  The element belongs to this thread in every piece of the
+        // CTA, so its reductions (no value returned) add in program order: the sum is deterministic
         const int m0 = 64 * (2 * hh + w) + 16 * wi + (lane >> 2);
+        if (job.add) {
 #pragma unroll
-        for (int i = 0; i < 128; ++i) {
-          const int n = 8 * (i >> 2) + 2 * q + (i & 1);
-          if (n < N) job.out[static_cast<long long>(n) * M + m0 + 8 * ((i >> 1) & 1)] = acc[i];
+          for (int i = 0; i < 128; ++i) {
+            const int n = 8 * (i >> 2) + 2 * q + (i & 1);
+            if (n < N) atomicAdd(job.out + static_cast<long long>(n) * M + m0 + 8 * ((i >> 1) & 1), acc[i]);
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 128; ++i) {
+            const int n = 8 * (i >> 2) + 2 * q + (i & 1);
+            if (n < N) job.out[static_cast<long long>(n) * M + m0 + 8 * ((i >> 1) & 1)] = acc[i];
+          }
         }
       }
     }
@@ -837,7 +848,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradJob* __
           }
           if (rph == 0) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) job.bias_out[(2 * hh + wr) * 64 + rc * 8 + i] = sa[i];
+            for (int i = 0; i < 8; ++i) {
+              float* o = job.bias_out + (2 * hh + wr) * 64 + rc * 8 + i;
+              if (job.add) atomicAdd(o, sa[i]);
+              else *o = sa[i];
+            }
           }
         }
       }

@@ -108,9 +108,12 @@ def _lists_inverted(z):
 
 
 def run_case(name, dev, emb):
-    c = dict(DEFAULTS, **CASES[name])
+    return run_render(dict(DEFAULTS, **CASES[name]), 200 + list(CASES).index(name), dev, emb)
+
+
+def run_render(c, seed, dev, emb):
+    """The three renders of configuration `c` (DEFAULTS' keys) on rays and random numbers drawn from `seed`."""
     n, S, K = c["n"], c["S"], c["K"]
-    seed = 200 + list(CASES).index(name)
     rays = _rays(c, seed)
     rs = np.random.RandomState(seed)
     target = rs.uniform(0, 1, (n, 3)).astype(F32)
@@ -245,12 +248,11 @@ def enc_report(run):
     return worst, xmax
 
 
-@pytest.mark.parametrize("name", list(CASES))
-def test_forward_stages(name, dev, emb):
-    run = run_case(name, dev, emb)
+def forward_report(run, sm_count):
+    """Stages 1-4 of one run_render result against their bars: (printable lines, violations)."""
     c, n, S, K = run["c"], run["n"], run["S"], run["K"]
     bad = mode_findings(run)
-    lines = [f"[{name}] n {n} S {S} K {K}"]
+    lines = []
     # coarse depths: the existing bitwise pin
     zc = tt.WorkspaceTape(run["raw"], tt.layout(n, S, K)[0]).z()
     zref = orc.coarse_depths(run["rays"], S, c["use_disp"], c["perturb"], run["rnd"].get("perturb_rand"))
@@ -274,9 +276,8 @@ def test_forward_stages(name, dev, emb):
         bar = rt.BARS["weights_last" if k.endswith("last") else "weights" if k.endswith("weights") else "sums"]
         if not v <= bar:
             bad.append(f"compositing {k}: {v:.3g} > {bar}")
-    sm = torch.cuda.get_device_properties(dev).multi_processor_count
     tr = run["train"]
-    lr = loss_report(n, S, K, tr["rgb_coarse"], tr.get("rgb_fine"), run["target"], tr, sm)
+    lr = loss_report(n, S, K, tr["rgb_coarse"], tr.get("rgb_fine"), run["target"], tr, sm_count)
     lines.append("loss: " + " ".join(f"{k} {v:.3g}" for k, v in lr.items()))
     for k, v in lr.items():
         if not v <= rt.BARS["psnr" if k == "psnr" else "loss"]:
@@ -285,7 +286,14 @@ def test_forward_stages(name, dev, emb):
     lines.append(f"enc: {enc:.3g} (max |x| {xmax:.3g})")
     if not enc <= tt.BARS["enc"]:
         bad.append(f"enc: {enc:.3g} > {tt.BARS['enc']} at max |x| {xmax:.3g}")
-    print("\n" + "\n".join(lines))
+    return lines, bad
+
+
+@pytest.mark.parametrize("name", list(CASES))
+def test_forward_stages(name, dev, emb):
+    run = run_case(name, dev, emb)
+    lines, bad = forward_report(run, torch.cuda.get_device_properties(dev).multi_processor_count)
+    print(f"\n[{name}] n {run['n']} S {run['S']} K {run['K']}\n" + "\n".join(lines))
     assert not bad, "\n".join(bad)
 
 
@@ -368,7 +376,7 @@ def _vr_inputs(S, seed):
     return sig, rgb, z, d, noise
 
 
-@pytest.mark.parametrize("S", [32, 96, 192])
+@pytest.mark.parametrize("S", [32, 64, 96, 128, 160, 192])
 @pytest.mark.parametrize("noise_std,wb", [(0.0, False), (1.0, True)])
 def test_volume_render_vs_float64(S, noise_std, wb, dev):
     sig, rgb, z, d, noise = _vr_inputs(S, S)

@@ -77,11 +77,13 @@ def _tiles(n_pad, seed):
 
 
 def run_step(name, dev, emb):
-    """One training step of case `name`.  Returns the inputs, the workspace bytes, the gradients and the upstream
-    gradient seeds of each pass."""
-    c = dict(DEFAULTS, **CASES[name])
+    return run_train(dict(DEFAULTS, **CASES[name]), 70 + list(CASES).index(name), dev, emb)
+
+
+def run_train(c, seed, dev, emb):
+    """One training step of configuration `c` (DEFAULTS' keys) on rays and random numbers drawn from `seed`.
+    Returns the inputs, the workspace bytes, the gradients and the upstream gradient seeds of each pass."""
     n, S, K = c["n"], c["S"], c["K"]
-    seed = 70 + list(CASES).index(name)
     ws_np = cases.trained_weights() if c["weights"] == "trained" else cases.weights()
     if c["golden"]:
         rays, target, randoms, *_ = cases.load_grad_case(c["golden"])
@@ -96,9 +98,10 @@ def run_step(name, dev, emb):
             randoms["noise_coarse"] = rs.randn(n, S).astype(np.float32)
             if K:
                 randoms["noise_fine"] = rs.randn(n, S + K).astype(np.float32)
-    if c["rng"] == "seed":
-        rnd = {"seed": 1000 + seed}
-        randoms = philox.randoms(1000 + seed, n, S, K)
+    if c["rng"] == "seed":             # the uniforms from the kernel's Philox stream, the noise still from tensors
+        noise = {k: v for k, v in randoms.items() if k.startswith("noise")}
+        rnd = dict(_to_dev(noise, dev), seed=1000 + seed)
+        randoms = dict(philox.randoms(1000 + seed, n, S, K), **noise)
     else:
         rnd = _to_dev(randoms, dev)
     models = _models(ws_np, dev)
@@ -148,8 +151,9 @@ def run_step(name, dev, emb):
                 ws=ws_np, z_fine=z_fine, seed=seed)
 
 
-def stage_report(run):
-    """All stage comparisons of one step: (printable lines, violations of the bars)."""
+def stage_report(run, device="cpu"):
+    """All stage comparisons of one step: (printable lines, violations of the bars).  `device`: the torch device of
+    the float64 gradient contractions (tt.reference_grads)."""
     c, n, S, K, rays = run["c"], run["n"], run["S"], run["K"], run["rays"]
     dir_emb = orc.embed(rays[:, 3:6], 4)
     lines, bad = [], []
@@ -178,7 +182,7 @@ def stage_report(run):
         masks = tt.check_masks(sub)
         comp = tt.check_composite(full, rays, *run["seeds"][ps], run["noise"][ps], c["noise_std"], c["white_back"])
         chain = tt.check_chain(sub, net)
-        ref = tt.reference_grads(full, net, chain["scales"], dir_emb)
+        ref = tt.reference_grads(full, net, chain["scales"], dir_emb, device)
         gr = tt.check_grads(run["grads"][ps], ref)
         bad += [f"{tag} {b}" for b in tt.failures(fwd, masks, chain, comp, gr, noise=c["noise_std"] > 0)]
         lines.append(f"{tag}: enc {enc_err:.3g} ulp; " + " ".join(f"{k} {v:.3g}" for k, v in fwd.items()))

@@ -18,6 +18,18 @@ RENDER = {
     (4096, 128, 64): 12015335424, (4096, 64, 128): 9623533568,
     (65536, 32, 0): 19334854656, (65536, 64, 0): 38469269504, (65536, 64, 64): 115091863552,
     (65536, 128, 64): 191629522944, (65536, 64, 128): 153360693248,
+    # fine passes of 64, 96, 128, 160 samples from K = 32, 96, 160; the 128-sample coarse pass alone
+    (1, 32, 32): 14984192, (1, 64, 32): 14984192, (1, 128, 32): 21412864, (1, 32, 96): 14984192,
+    (1, 64, 96): 21412864, (1, 32, 160): 21412864, (1, 128, 0): 8550400,
+    (127, 32, 32): 153649152, (127, 64, 32): 228392960, (127, 128, 32): 375549952, (127, 32, 96): 227227648,
+    (127, 64, 96): 301971456, (127, 32, 160): 301971456, (127, 128, 0): 189689856,
+    (1024, 32, 32): 941799424, (1024, 64, 32): 1539749888, (1024, 128, 32): 2735650816, (1024, 32, 96): 1539749888,
+    (1024, 64, 96): 2137700352, (1024, 32, 160): 2137700352, (1024, 128, 0): 1239447552,
+    (4096, 32, 32): 3644028928, (4096, 64, 32): 6035830784, (4096, 128, 32): 10819434496,
+    (4096, 32, 96): 6035830784, (4096, 64, 96): 8427632640, (4096, 32, 160): 8427632640, (4096, 128, 0): 4834621440,
+    (65536, 32, 32): 57688619008, (65536, 64, 32): 95957448704, (65536, 128, 32): 172495108096,
+    (65536, 32, 96): 95957448704, (65536, 64, 96): 134226278400, (65536, 32, 160): 134226278400,
+    (65536, 128, 0): 76738099200,
 }
 NERF = {1: 7176192, 128: 7176192, 129: 14147584, 196608: 1860153344, 10 ** 6: 9301867520}
 

@@ -204,6 +204,18 @@ def test_workspace_reader_round_trip(syn):
     assert tt.failures(chain=tt.check_chain(full, syn["net"])) == []
 
 
+def test_reference_grads_do_not_depend_on_the_parts():
+    """reference_grads of a workspace summed one tile at a time equals the sum over the whole array tape to float64
+    rounding: 96-sample rays straddle the parts, and the last tile, a part of its own, is half padding."""
+    syn = synthetic(5, 96)
+    raw, P = workspace_bytes(syn)
+    whole = tt.reference_grads(tt.ArrayTape(syn["S"], syn["arrays"]), syn["net"], syn["scales"], syn["dir_emb"])
+    tape = tt.WorkspaceTape(raw, P)
+    assert len(tape.parts(1)) == P["n_pad"] // 128 > 2
+    for k, v in tt.reference_grads(tape, syn["net"], syn["scales"], syn["dir_emb"], tiles_per_part=1).items():
+        np.testing.assert_allclose(v, whole[k], rtol=1e-12, atol=1e-12 * np.abs(whole[k]).max(), err_msg=k)
+
+
 def test_correct_device_passes(syn):
     assert all_failures(syn, device_grads(syn)) == []
     chain = tt.check_chain(tt.ArrayTape(syn["S"], syn["arrays"]), syn["net"])

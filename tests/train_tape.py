@@ -122,6 +122,10 @@ class Tape:
     def ray_of_rows(self):
         return self.rows // self.S
 
+    def parts(self, tiles: int) -> list:
+        """The tape as consecutive parts of at most `tiles` 128-sample tiles each (one part where it has no tiles)."""
+        return [self]
+
 
 class WorkspaceTape(Tape):
     """A pass of a real training workspace (`raw`: its bytes as a uint8 array), decoded on demand."""
@@ -131,11 +135,15 @@ class WorkspaceTape(Tape):
         self.S, self.n, self.n_pad = P["S"], P["n"], P["n_pad"]
         n_tiles = self.n_pad // 128
         tiles = np.arange(n_tiles) if tiles is None else np.unique(np.asarray(tiles) % n_tiles)
+        self.tiles = tiles
         self.chunks = np.stack([2 * tiles, 2 * tiles + 1], 1).reshape(-1)
         rows = (self.chunks[:, None] * 64 + np.arange(64)[None, :]).reshape(-1)
         self.valid = rows < self.n
         self.rows = rows[self.valid]
         self.all_rows = tiles is None or len(tiles) == n_tiles
+
+    def parts(self, tiles: int) -> list:
+        return [WorkspaceTape(self.raw, self.P, self.tiles[i:i + tiles]) for i in range(0, len(self.tiles), tiles)]
 
     def _f32(self, key, width=1):
         a = np.frombuffer(self.raw, np.float32, self.n_pad * width if key != "z" else self.n, self.P[key])
@@ -427,55 +435,72 @@ def check_composite(tape: Tape, rays, g_rgb, g_depth, g_opac, noise, noise_std, 
             "dprergb": float((np.abs(dp_dev - dp_ref) / den_p).max())}
 
 
-def column_sums(a16: np.ndarray) -> np.ndarray:
+def column_sums(a16: np.ndarray, device="cpu") -> np.ndarray:
     """Column sums of a stored 16-bit gradient array the way the wgrad kernel's reduction warps form them: in each
     64-row chunk, rows h 32 + 4 i + p (i = 0..7) are added in fp16, one correctly rounded addition at a time (as
     add.rn.f16x2 does), for each (h, p); those 8-row sums are then exact inputs of a float64 sum.  What is left
-    against the device is fp32 summation error only."""
-    a = np.asarray(a16, np.float16)
+    against the device is fp32 summation error only.  Computed in torch on `device`: the float64 sum of two fp16
+    values is exact, and its rounding to fp16 through fp32 rounds once (24 >= 2 * 11 + 2 bits)."""
+    import torch
+    a = torch.from_numpy(np.ascontiguousarray(a16, np.float16)).to(device)
     n, C = a.shape
-    pad = np.zeros(((n + 63) // 64 * 64, C), np.float16)
+    pad = torch.zeros(((n + 63) // 64 * 64, C), dtype=torch.float16, device=device)
     pad[:n] = a
-    x = pad.reshape(-1, 2, 8, 4, C)            # [chunk, h, i, p, column] = row h 32 + 4 i + p
+    x = pad.view(-1, 2, 8, 4, C)               # [chunk, h, i, p, column] = row h 32 + 4 i + p
     acc = x[:, :, 0]
     for i in range(1, 8):
-        with np.errstate(over="ignore"):
-            acc = (acc.astype(F64) + x[:, :, i].astype(F64)).astype(np.float16)
-    return acc.astype(F64).sum((0, 1, 2))
+        acc = (acc.double() + x[:, :, i].double()).half()
+    return acc.double().sum((0, 1, 2)).cpu().numpy()
 
 
-def reference_grads(tape: Tape, net: Net, scales, dir_emb: np.ndarray) -> Dict[str, np.ndarray]:
+def reference_grads(tape: Tape, net: Net, scales, dir_emb: np.ndarray, device="cpu",
+                    tiles_per_part: int = 2048) -> Dict[str, np.ndarray]:
     """The 24 gradient tensors as float64 contractions of the device's own operands (all samples): the wgrad
     GEMMs sum_s dpre_l^T h_{l-1} / s_l and bias sums (with the kernel's fp16 8-row pre-sums, `column_sums`),
     layer 5 as its 63 encoding and 256 hidden columns, the heads, W' from dd, the direction part from the per-ray
-    sums of the un-scaled dd, and the unfolding of W' (csrc/bwd_kernels.cuh unfold_kernel)."""
+    sums of the un-scaled dd, and the unfolding of W' (csrc/bwd_kernels.cuh unfold_kernel).  The sums over samples
+    run over `tape.parts(tiles_per_part)` in torch float64 on `device`, so a pass of millions of samples is never
+    decoded whole; the parts start on tile boundaries, which keeps every 64-row pre-sum of `column_sums` whole."""
+    import torch
     assert tape.all_rows
     w = net.w
-    g = {}
-    enc = tape.enc().astype(F64)[:, :63]
-    for l in range(1, 9):
-        a16 = tape.dpre(l)
-        A = a16.astype(F64) / scales[9 - l]
-        if l == 1:
-            B = enc
-        elif l == 5:
-            B = np.concatenate([enc, tape.h(4).astype(F64)], 1)
-        else:
-            B = tape.h(l - 1).astype(F64)
-        g[f"xyz_encoding_{l}.0.weight"] = A.T @ B
-        g[f"xyz_encoding_{l}.0.bias"] = column_sums(a16) / scales[9 - l]
-    h8 = tape.h(8).astype(F64)
-    dsig = tape.dsigma().astype(F64)
-    g["sigma.weight"] = (dsig @ h8)[None, :]
-    g["sigma.bias"] = np.array([dsig.sum()])
-    dp = tape.dprergb().astype(F64)
-    g["rgb.0.weight"] = dp.T @ tape.d().astype(F64)
-    g["rgb.0.bias"] = dp.sum(0)
-    dd16 = tape.dd()
-    gWp, gbp = (dd16.astype(F64) / scales[0]).T @ h8, column_sums(dd16) / scales[0]
-    ref0, _ = dd_reference(tape, net)
+    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device).double()     # stored 16-bit values go as they are
+    acc = {}
+
+    def add(k, v):
+        acc[k] = v if k not in acc else acc[k] + v
     n_rays = tape.n // tape.S
-    raysum = ref0.reshape(n_rays, tape.S, 128).sum(1)
+    raysum = torch.zeros(n_rays, 128, dtype=torch.float64, device=device)
+    for part in tape.parts(tiles_per_part):
+        enc = T(part.enc()[:, :63])
+        for l in range(1, 9):
+            a16 = part.dpre(l)
+            if l == 1:
+                B = enc
+            elif l == 5:
+                B = torch.cat([enc, T(part.h(4))], 1)
+            else:
+                B = T(part.h(l - 1))
+            add(f"xyz_encoding_{l}.0.weight", T(a16).T @ B)
+            add(f"xyz_encoding_{l}.0.bias", T(column_sums(a16, device)))
+        h8 = T(part.h(8))
+        dsig = T(part.dsigma())
+        add("sigma.weight", (dsig @ h8)[None, :])
+        add("sigma.bias", dsig.sum()[None])
+        dp = T(part.dprergb())
+        add("rgb.0.weight", dp.T @ T(part.d()))
+        add("rgb.0.bias", dp.sum(0))
+        dd16 = part.dd()
+        add("gWp", T(dd16).T @ h8)
+        add("gbp", T(column_sums(dd16, device)))
+        ref0, _ = dd_reference(part, net)
+        raysum.index_add_(0, torch.from_numpy(part.ray_of_rows()).to(device), T(ref0))
+    g = {k: v.cpu().numpy() for k, v in acc.items()}
+    for l in range(1, 9):
+        g[f"xyz_encoding_{l}.0.weight"] /= scales[9 - l]
+        g[f"xyz_encoding_{l}.0.bias"] /= scales[9 - l]
+    gWp, gbp = g.pop("gWp") / scales[0], g.pop("gbp") / scales[0]
+    raysum = raysum.cpu().numpy()
     Wd = w["dir_encoding.0.weight"][:, :256].astype(F64)
     Wf = w["xyz_encoding_final.weight"].astype(F64)
     bf = w["xyz_encoding_final.bias"].astype(F64)
