@@ -364,6 +364,8 @@ int nerfb200_color_accumulate(const uint8_t* colors, const double* depth, const 
                               float occ_threshold, double* sum4, void* stream);
 /* extract_color_mesh.py:283-284: colors (n, 3) = uint8(sum / wsum), truncated. */
 int nerfb200_color_finalize(const double* sum4, int64_t n, uint8_t* colors, void* stream);
+/* The vertex-normal colouring method (--use_vertex_normal, extract_color_mesh.py:187-203) has its own
+ * header, nerf_pl_b200_mesh_normals.h, included at the end of this one. */
 
 /* ---- diagnostics -------------------------------------------------------------------------
  * Number of kernels this library has launched on the calling process so far (all entry
@@ -379,4 +381,5 @@ int nerfb200_sm_count(void);
 #ifdef __cplusplus
 }
 #endif
+#include "nerf_pl_b200_mesh_normals.h"
 #endif /* NERF_PL_B200_H_ */

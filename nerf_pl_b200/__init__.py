@@ -6,8 +6,8 @@ from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_
                    packed_weights)
 from .data import DeviceRayBatches
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
-from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, pack_volume, query_rgb_sigma, rgb_sigma_grid,
-                   sigma_grid, write_ply, write_vol)
+from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, normal_rays, normal_vertex_colors, pack_volume,
+                   query_rgb_sigma, rgb_sigma_grid, sigma_grid, vertex_normals, write_ply, write_vol)
 from .optim import FusedAdam
 from .rendering import render_rays, render_rays_host, render_rays_loss, sample_pdf, searchsorted, volume_render
 from .training import CapturedTrainStep, nerf_forward_train
@@ -18,5 +18,6 @@ __all__ = [
     "batched_inference", "generate_rays", "render_image", "to_uint8", "query_sigma", "mse_psnr",
     "sigma_grid", "marching_cubes", "extract_mesh", "fuse_vertex_colors", "write_ply",
     "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
+    "vertex_normals", "normal_rays", "normal_vertex_colors",
 ]
 __version__ = "0.1.0"

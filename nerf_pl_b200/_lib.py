@@ -151,6 +151,15 @@ SIGNATURES = {
 }
 EXPORTS = tuple(SIGNATURES)     # tests check the library exports all of them
 
+# The same for the companion header include/nerf_pl_b200_mesh_normals.h (the vertex-normal colouring method), which
+# nerf_pl_b200.h includes at its end.
+MESH_NORMALS_SIGNATURES = {
+    "nerfb200_vertex_normals_workspace_bytes": (_sz, [_i64, _i64]),
+    "nerfb200_vertex_normals": (_i32, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
+    "nerfb200_normal_rays": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _vp, _vp]),
+}
+HEADER_SIGNATURES = {"nerf_pl_b200.h": SIGNATURES, "nerf_pl_b200_mesh_normals.h": MESH_NORMALS_SIGNATURES}
+
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
@@ -164,7 +173,7 @@ def needs_build() -> bool:
         return True
     t = os.path.getmtime(LIB_PATH)
     deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS]
-    deps.append(os.path.join(_HERE, "..", "include", "nerf_pl_b200.h"))
+    deps += [os.path.join(_HERE, "..", "include", h) for h in HEADER_SIGNATURES]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
@@ -198,9 +207,10 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (restype, argtypes) in SIGNATURES.items():
-                fn = getattr(lib, name)
-                fn.restype, fn.argtypes = restype, argtypes
+            for table in HEADER_SIGNATURES.values():
+                for name, (restype, argtypes) in table.items():
+                    fn = getattr(lib, name)
+                    fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:
                 raise RuntimeError("libnerf_pl_b200.so ABI version mismatch")
             _lib = lib

@@ -1424,6 +1424,33 @@ int volume_prepare(const float* rgbsigma, int64_t N, double xmin, double xmax, v
   return 0;
 }
 
+// Vertex normals: corner keys / triangle ids (and their sort buffers), triangle normals, the index flag.
+struct NormalsLayout {
+  size_t keys, keys_alt, vals, vals_alt, tri_n, bad, temp, temp_bytes, bytes;
+};
+NormalsLayout normals_layout(long long V, long long T) {
+  const long long E = 3 * T;
+  size_t tb = 0;
+  cub::DoubleBuffer<int> kb(nullptr, nullptr), vb(nullptr, nullptr);
+  cub::DeviceRadixSort::SortPairs(nullptr, tb, kb, vb, static_cast<int>(E), 0, bits_for(V + 1));
+  NormalsLayout L;
+  size_t o = 0;
+  L.keys = o; o += align256(E * 4);
+  L.keys_alt = o; o += align256(E * 4);
+  L.vals = o; o += align256(E * 4);
+  L.vals_alt = o; o += align256(E * 4);
+  L.tri_n = o; o += align256(T * 3 * sizeof(double));
+  L.bad = o; o += 256;
+  L.temp = o; L.temp_bytes = tb; o += align256(tb);
+  L.bytes = o;
+  return L;
+}
+
+// V + 1 (the key of an out-of-range corner) and 3T stay in int32
+bool normals_size_ok(long long V, long long T) {
+  return V >= 0 && T >= 0 && V < 0x7fffffffLL && T <= 0x7fffffffLL / 3;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1712,6 +1739,69 @@ int nerfb200_color_finalize(const double* sum4, int64_t n, uint8_t* colors, void
   color_finalize_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(sum4, n, colors);
   g_launches++;
   CUDA_TRY(cudaGetLastError(), "color_finalize launch");
+  return 0;
+}
+
+size_t nerfb200_vertex_normals_workspace_bytes(int64_t n_verts, int64_t n_tris) {
+  if (!normals_size_ok(n_verts, n_tris)) return 0;
+  return normals_layout(n_verts, n_tris).bytes;
+}
+
+int nerfb200_vertex_normals(const float* vertices, int64_t n_verts, const int32_t* triangles, int64_t n_tris, void* ws,
+                            size_t bytes, double* normals, void* stream) {
+  if (!normals_size_ok(n_verts, n_tris)) return fail(NERFB200_EINVAL, "vertex_normals: bad mesh size%s");
+  if (n_verts == 0) {
+    if (n_tris == 0) return 0;
+    return fail(NERFB200_EINVAL, "vertex_normals: a triangle index is outside [0, n_verts) (n_verts = 0)%s");
+  }
+  if ((n_verts > 0 && (!vertices || !normals)) || (n_tris > 0 && !triangles) || !ws)
+    return fail(NERFB200_EINVAL, "vertex_normals: NULL argument%s");
+  const NormalsLayout L = normals_layout(n_verts, n_tris);
+  if (bytes < L.bytes) return fail(NERFB200_EINVAL, "vertex_normals: workspace smaller than nerfb200_vertex_normals_workspace_bytes%s");
+  char* w = static_cast<char*>(ws);
+  NormalsParams p;
+  p.vertices = vertices; p.tris = triangles; p.n_verts = n_verts; p.n_tris = n_tris;
+  p.keys = reinterpret_cast<int*>(w + L.keys);
+  p.vals = reinterpret_cast<int*>(w + L.vals);
+  p.tri_n = reinterpret_cast<double*>(w + L.tri_n);
+  p.bad = reinterpret_cast<int*>(w + L.bad);
+  p.normals = normals;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemsetAsync(p.bad, 0, sizeof(int), s), "vertex_normals memset");
+  if (n_tris > 0) {
+    normals_triangle_kernel<<<mesh_blocks(n_tris), 256, 0, s>>>(p);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError(), "vertex_normals triangle launch");
+    cub::DoubleBuffer<int> kb(p.keys, reinterpret_cast<int*>(w + L.keys_alt));
+    cub::DoubleBuffer<int> vb(p.vals, reinterpret_cast<int*>(w + L.vals_alt));
+    size_t tb = L.temp_bytes;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(w + L.temp, tb, kb, vb, static_cast<int>(3 * n_tris), 0,
+                                             bits_for(n_verts + 1), s), "vertex_normals corner sort");
+    g_launches++;
+    p.keys = kb.Current();
+    p.vals = vb.Current();
+  }
+  if (n_verts > 0) {
+    normals_vertex_kernel<<<mesh_blocks(n_verts), 256, 0, s>>>(p);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError(), "vertex_normals vertex launch");
+  }
+  int bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(&bad, p.bad, sizeof(int), cudaMemcpyDeviceToHost, s), "vertex_normals readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "vertex_normals readback");
+  if (bad) return fail(NERFB200_EINVAL, "vertex_normals: a triangle index is outside [0, n_verts)%s");
+  return 0;
+}
+
+int nerfb200_normal_rays(const float* vertices, const double* normals, int64_t n, float near, float far, float near_t,
+                         float* rays, void* stream) {
+  if (n < 0) return fail(NERFB200_EINVAL, "normal_rays: n < 0%s");
+  if (n == 0) return 0;
+  if (!vertices || !normals || !rays) return fail(NERFB200_EINVAL, "normal_rays: NULL argument%s");
+  normal_rays_kernel<<<mesh_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(vertices, normals, n, near, far,
+                                                                                     near_t, rays);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "normal_rays launch");
   return 0;
 }
 

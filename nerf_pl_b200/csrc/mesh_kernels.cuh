@@ -467,4 +467,109 @@ __global__ void __launch_bounds__(kVolThreads) volume_emit_kernel(VolumeParams p
   }
 }
 
+// ---- 7. vertex-normal colours (extract_color_mesh.py:187-203, --use_vertex_normal) -----------------
+// Open3D TriangleMesh::ComputeVertexNormals() on a mesh without normals, in float64:
+//   n_t = (v1 - v0) x (v2 - v0), Eigen's component formula, no contraction;
+//   each vertex sums the n_t of its corners in increasing triangle index (corner order within a triangle);
+//   normalize(): s = (x^2 + y^2) + z^2, divide by sqrt(s) when s > 0; then a NaN x becomes (0, 0, 1).
+// The order comes from a stable radix sort of the 3T corners keyed by vertex (the values are triangle ids, so
+// each vertex's segment lists its triangles in increasing order); no floating-point atomics anywhere.
+struct NormalsParams {
+  const float* vertices;   // (V, 3)
+  const int* tris;         // (T, 3)
+  long long n_verts, n_tris;
+  int* keys;               // (3T) corner -> vertex, V for an index outside [0, V)
+  int* vals;               // (3T) corner -> triangle
+  double* tri_n;           // (T, 3) unnormalised triangle normals
+  int* bad;                // set to 1 when an index is outside [0, V)
+  double* normals;         // (V, 3)
+};
+
+// Reads the indices first and checks them before any vertex is addressed; a triangle with an index outside
+// [0, V) flags `bad` and gets a zero normal, and its corners sort after every valid one.
+__global__ void normals_triangle_kernel(NormalsParams p) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < p.n_tris; t += (long long)gridDim.x * blockDim.x) {
+    int a[3];
+    bool ok = true;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      a[c] = p.tris[t * 3 + c];
+      const bool in = a[c] >= 0 && a[c] < p.n_verts;
+      ok = ok && in;
+      p.keys[t * 3 + c] = in ? a[c] : static_cast<int>(p.n_verts);
+      p.vals[t * 3 + c] = static_cast<int>(t);
+    }
+    double n[3] = {0.0, 0.0, 0.0};
+    if (ok) {
+      double e1[3], e2[3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const double v0 = static_cast<double>(p.vertices[static_cast<long long>(a[0]) * 3 + c]);
+        e1[c] = __dsub_rn(static_cast<double>(p.vertices[static_cast<long long>(a[1]) * 3 + c]), v0);
+        e2[c] = __dsub_rn(static_cast<double>(p.vertices[static_cast<long long>(a[2]) * 3 + c]), v0);
+      }
+      n[0] = __dsub_rn(__dmul_rn(e1[1], e2[2]), __dmul_rn(e1[2], e2[1]));
+      n[1] = __dsub_rn(__dmul_rn(e1[2], e2[0]), __dmul_rn(e1[0], e2[2]));
+      n[2] = __dsub_rn(__dmul_rn(e1[0], e2[1]), __dmul_rn(e1[1], e2[0]));
+    } else {
+      *p.bad = 1;
+    }
+    p.tri_n[t * 3 + 0] = n[0];
+    p.tri_n[t * 3 + 1] = n[1];
+    p.tri_n[t * 3 + 2] = n[2];
+  }
+}
+
+__device__ __forceinline__ long long lower_bound_i32(const int* a, long long n, int v) {
+  long long lo = 0, hi = n;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (a[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// One thread per vertex: its segment of the sorted corners, summed in order, then Eigen's normalize().
+__global__ void normals_vertex_kernel(NormalsParams p) {
+  const long long E = p.n_tris * 3;
+  for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < p.n_verts; v += (long long)gridDim.x * blockDim.x) {
+    const long long lo = lower_bound_i32(p.keys, E, static_cast<int>(v));
+    double x = 0.0, y = 0.0, z = 0.0;
+    for (long long s = lo; s < E && p.keys[s] == v; ++s) {
+      const long long t = p.vals[s];
+      x = __dadd_rn(x, p.tri_n[t * 3 + 0]);
+      y = __dadd_rn(y, p.tri_n[t * 3 + 1]);
+      z = __dadd_rn(z, p.tri_n[t * 3 + 2]);
+    }
+    const double sq = __dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z));
+    if (sq > 0.0) {
+      const double r = __dsqrt_rn(sq);
+      x = __ddiv_rn(x, r);
+      y = __ddiv_rn(y, r);
+      z = __ddiv_rn(z, r);
+    }
+    if (isnan(x)) { x = 0.0; y = 0.0; z = 1.0; }
+    p.normals[v * 3 + 0] = x;
+    p.normals[v * 3 + 1] = y;
+    p.normals[v * 3 + 2] = z;
+  }
+}
+
+// :190-193 rays [v - (d * near) * near_t, d, near, far] with d = fl32(normal), every operation fp32 as torch does
+// it on the CPU (the scalars are fp32, rounded on the host).
+__global__ void normal_rays_kernel(const float* vertices, const double* normals, long long n, float near, float far,
+                                   float near_t, float* rays) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x) {
+    float* ray = rays + t * 8;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float d = __double2float_rn(normals[t * 3 + c]);
+      ray[c] = __fsub_rn(vertices[t * 3 + c], __fmul_rn(__fmul_rn(d, near), near_t));
+      ray[3 + c] = d;
+    }
+    ray[6] = near;
+    ray[7] = far;
+  }
+}
+
 }  // namespace nerfb200

@@ -5,7 +5,8 @@ colours, every stage an sm_90a kernel of ``libnerf_pl_b200.so`` (csrc/mesh_kerne
 the occlusion renders run the existing fused MLP / render launches.  Replaces PyMCubes
 (``mcubes.marching_cubes``), open3d (``cluster_connected_triangles`` + ``remove_unreferenced_vertices``),
 ``cv2.remap`` and the numpy projection loop; ``write_ply`` writes what plyfile wrote.  Conventions and the
-reference's quirks that are kept: DESIGN.md "Coloured mesh extraction".
+reference's quirks that are kept: DESIGN.md "Coloured mesh extraction".  The ``--use_vertex_normal`` method is
+``vertex_normals`` -> ``normal_rays`` -> the fused render of both networks, in one call: ``normal_vertex_colors``.
 
 The Unity volume export of extract_mesh.ipynb is ``rgb_sigma_grid`` -> ``pack_volume`` -> ``write_vol`` (DESIGN.md
 "Unity volume").
@@ -19,6 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .inference import to_uint8
 from .nerf import Embedding, packed_weights
 from .rendering import render_rays
 
@@ -212,6 +214,77 @@ def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: t
     if return_opacities:
         return out, (torch.stack(opac) if opac else torch.empty(0, n, device=v.device))
     return out
+
+
+def _mesh_vertices(vertices: torch.Tensor) -> torch.Tensor:
+    v = _cuda(vertices, "vertices")
+    if v.dim() != 2 or v.shape[1] != 3 or not v.is_floating_point():
+        raise ValueError("vertices must be (V, 3) floating point")
+    return v.detach().to(torch.float32).contiguous()
+
+
+@torch.no_grad()
+def vertex_normals(vertices: torch.Tensor, triangles: torch.Tensor) -> torch.Tensor:
+    """Drop-in for ``np.asarray(mesh.compute_vertex_normals().vertex_normals)`` (extract_color_mesh.py:189-190) on a
+    mesh without normals: (V, 3) float64 on the device, open3d's definition bit for bit (DESIGN.md "Vertex-normal
+    colours").  vertices (V, 3) are taken in float32, the precision the reference's PLY round trip leaves them in;
+    triangles (T, 3) integer.  An index outside [0, V) raises ValueError."""
+    v = _mesh_vertices(vertices)
+    t = _cuda(triangles, "triangles")
+    if t.dim() != 2 or t.shape[1] != 3 or t.is_floating_point() or t.is_complex() or t.dtype == torch.bool:
+        raise ValueError("triangles must be (T, 3) integer")
+    if t.device != v.device:
+        raise ValueError("vertices and triangles must be on the same device")
+    n_v, n_t = v.shape[0], t.shape[0]
+    if t.dtype != torch.int32:
+        # an index beyond int32 stays out of range through the cast
+        t = t.to(torch.int64).clamp(-1, n_v)
+    t = t.detach().to(torch.int32).contiguous()
+    nbytes = _lib.load().nerfb200_vertex_normals_workspace_bytes(n_v, n_t)
+    if nbytes == 0:
+        raise ValueError(f"vertex_normals: unsupported mesh size (V = {n_v}, T = {n_t})")
+    out = torch.empty(n_v, 3, dtype=torch.float64, device=v.device)
+    ws = _workspace(nbytes, v.device)
+    _lib.call("nerfb200_vertex_normals", v.device, v.data_ptr(), n_v, t.data_ptr(), n_t, ws.data_ptr(), ws.numel(),
+              out.data_ptr())
+    return out
+
+
+@torch.no_grad()
+def normal_rays(vertices: torch.Tensor, normals: torch.Tensor, near: float, far: float,
+                near_t: float = 1.0) -> torch.Tensor:
+    """extract_color_mesh.py:190-193 on the device: (V, 8) float32 rays ``[v - d * near * near_t, d, near, far]`` with
+    ``d = float32(normals)``, bit for bit the reference's CPU torch expression (``near``, ``far`` and ``near_t``
+    rounded to float32 as torch rounds them)."""
+    v = _mesh_vertices(vertices)
+    n = _cuda(normals, "normals")
+    if n.shape != v.shape or not n.is_floating_point():
+        raise ValueError("normals must be floating point and shaped like vertices (V, 3)")
+    n = n.detach().to(torch.float64).contiguous()
+    rays = torch.empty(v.shape[0], 8, dtype=torch.float32, device=v.device)
+    _lib.call("nerfb200_normal_rays", v.device, v.data_ptr(), n.data_ptr(), v.shape[0], float(np.float32(near)),
+              float(np.float32(far)), float(np.float32(near_t)), rays.data_ptr())
+    return rays
+
+
+@torch.no_grad()
+def normal_vertex_colors(nerf_coarse: torch.nn.Module, nerf_fine: torch.nn.Module, vertices: torch.Tensor,
+                         triangles: torch.Tensor, near: float, far: float, N_samples: int = 64,
+                         N_importance: int = 64, near_t: float = 1.0, white_back: bool = False) -> torch.Tensor:
+    """extract_color_mesh.py:187-203 and 280-281 (``--use_vertex_normal``) on the device: (V, 3) uint8 vertex colours
+    ``(rgb_fine * 255).astype(uint8)`` of rays that start at ``v - n * near * near_t`` and run along the open3d
+    vertex normal n.  One ``vertex_normals``, one ``normal_rays``, one fused ``render_rays`` of all V rays with both
+    networks (test_time, perturb 0, noise 0), and ``to_uint8``.  near / far: ``dataset.bounds.min()`` / ``.max()``;
+    white_back: ``dataset.white_back``."""
+    _device_of(nerf_coarse)
+    _device_of(nerf_fine)
+    if int(N_importance) <= 0:
+        raise ValueError("normal_vertex_colors needs N_importance > 0 (the colours are rgb_fine)")
+    normals = vertex_normals(vertices, triangles)
+    rays = normal_rays(vertices, normals, near, far, near_t)
+    res = render_rays([nerf_coarse, nerf_fine], [Embedding(3, 10), Embedding(3, 4)], rays, int(N_samples), False, 0, 0,
+                      int(N_importance), 1024 * 32, bool(white_back), test_time=True, match_reference_rng=False)
+    return to_uint8(res["rgb_fine"])
 
 
 @torch.no_grad()

@@ -1,8 +1,9 @@
 """Device time per stage of the coloured-mesh workflow (nerf_pl_b200.mesh) on the trained test weights.
 
 Stages at N_grid 256 and 512 over [-1.5, 1.5]^3, threshold 20: sigma grid, marching cubes (count + emit),
-index -> world, largest cluster; the Unity volume's rgb+sigma grid and its pack (count + emit); colour fusion
-over 100 views at 800 x 800.  CUDA events around each stage;
+index -> world, largest cluster; the Unity volume's rgb+sigma grid and its pack (count + emit); the vertex-normal
+colours of the kept mesh (normals, rays, the render of one ray per vertex at 64 + 64 samples, and the whole
+``normal_vertex_colors`` call); colour fusion over 100 views at 800 x 800.  CUDA events around each stage;
 prints the card name and power limit with the numbers, and one JSON line.  The bytes columns are the
 minimum traffic of the MC and cluster passes (every array read / written once), as a share of the card's
 HBM bandwidth (3.35 TB/s on an H100 SXM).
@@ -67,6 +68,10 @@ def main():
     model = nb.NeRF()
     model.load_state_dict({k: torch.from_numpy(v) for k, v in cases.trained_weights()[1].items()})
     model = model.cuda().eval()
+    coarse = nb.NeRF()
+    coarse.load_state_dict({k: torch.from_numpy(v) for k, v in cases.trained_weights()[0].items()})
+    coarse = coarse.cuda().eval()
+    emb = [nb.Embedding(3, 10), nb.Embedding(3, 4)]
     res = {"card": card()}
     print("card, power limit:", res["card"])
     for N in args.grids:
@@ -89,6 +94,17 @@ def main():
         r.update({"rgb_sigma_grid_ms": ms_rgb, "volume_pack_ms": ms_vol, "volume_voxels": int(vol.shape[0]),
                   "volume_hbm_share": (2 * P * 16 + vol.shape[0] * 8) / (ms_vol * 1e-3) / HBM})
         del rgbsigma, vol
+        # vertex-normal colours (--use_vertex_normal) on the kept mesh: normals, rays, one render of V rays at 64 + 64
+        ms_nrm, nrm = timed(lambda: nb.vertex_normals(kv, kt))
+        ms_rays, rays = timed(lambda: nb.normal_rays(kv, nrm, 2.0, 6.0))
+        with torch.no_grad():
+            ms_rend, _ = timed(lambda: nb.render_rays([coarse, model], emb, rays, 64, False, 0, 0, 64, 32768, True,
+                                                      test_time=True, match_reference_rng=False))
+        ms_vn, _ = timed(lambda: nb.normal_vertex_colors(coarse, model, kv, kt, 2.0, 6.0, white_back=True))
+        r.update({"normals_ms": ms_nrm, "normal_rays_ms": ms_rays, "normal_render_ms": ms_rend,
+                  "normal_colors_total_ms": ms_vn, "normal_rays": int(kv.shape[0]),
+                  "normal_render_Msamples_per_s": kv.shape[0] * 128 / (ms_rend * 1e-3) / 1e6})
+        del nrm, rays
         res[f"N{N}"] = r
         print(f"N_grid {N}: " + ", ".join(f"{k} {v:.4g}" if isinstance(v, float) else f"{k} {v}" for k, v in r.items()))
         if N == args.grids[0]:
