@@ -382,4 +382,5 @@ int nerfb200_sm_count(void);
 }
 #endif
 #include "nerf_pl_b200_mesh_normals.h"
+#include "nerf_pl_b200_occupancy.h"
 #endif /* NERF_PL_B200_H_ */

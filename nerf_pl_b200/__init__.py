@@ -4,6 +4,7 @@ signatures, executed by hand-written wgmma (sm_90a) CUDA kernels through a C-ABI
 (``include/nerf_pl_b200.h``).  See DESIGN.md and INTEGRATION.md."""
 from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_forward_torch, nerf_parameters,
                    packed_weights)
+from .culling import OccupancyGrid, cull_rays, occupancy_grid, pack_occupancy, render_rays_culled, scatter_results
 from .data import DeviceRayBatches
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
 from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, normal_rays, normal_vertex_colors, pack_volume,
@@ -19,5 +20,6 @@ __all__ = [
     "sigma_grid", "marching_cubes", "extract_mesh", "fuse_vertex_colors", "write_ply",
     "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
     "vertex_normals", "normal_rays", "normal_vertex_colors",
+    "OccupancyGrid", "occupancy_grid", "pack_occupancy", "cull_rays", "scatter_results", "render_rays_culled",
 ]
 __version__ = "0.1.0"

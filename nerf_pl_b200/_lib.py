@@ -22,7 +22,7 @@ if os.environ.get("NERFB200_LIB"):          # a library built elsewhere (e.g. wi
     LIB_PATH = os.path.abspath(os.environ["NERFB200_LIB"])
 SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
-           "mesh_kernels.cuh", "mc_table.h"]
+           "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -158,7 +158,18 @@ MESH_NORMALS_SIGNATURES = {
     "nerfb200_vertex_normals": (_i32, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
     "nerfb200_normal_rays": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _vp, _vp]),
 }
-HEADER_SIGNATURES = {"nerf_pl_b200.h": SIGNATURES, "nerf_pl_b200_mesh_normals.h": MESH_NORMALS_SIGNATURES}
+# And for include/nerf_pl_b200_occupancy.h (empty-space skipping at render time), included after it.
+OCCUPANCY_SIGNATURES = {
+    "nerfb200_occupancy_workspace_bytes": (_sz, [_i64]),
+    "nerfb200_occupancy_pack": (_i32, [_vp, _i64, _f64, _i32, _vp, _sz, _vp, _vp]),
+    "nerfb200_occupancy_popcount": (_i32, [_vp, _i64, _vp, _vp]),
+    "nerfb200_cull_workspace_bytes": (_sz, [_i64]),
+    "nerfb200_cull_count": (_i32, [_vp, _i64, _vp, _i64, POINTER(_f64), _vp, _sz, _vp, POINTER(_i64), _vp]),
+    "nerfb200_cull_emit": (_i32, [_vp, _i64, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "nerfb200_scatter_results": (_i32, [_P, _P, _vp, _i64, _i64, _i32, _vp]),
+}
+HEADER_SIGNATURES = {"nerf_pl_b200.h": SIGNATURES, "nerf_pl_b200_mesh_normals.h": MESH_NORMALS_SIGNATURES,
+                     "nerf_pl_b200_occupancy.h": OCCUPANCY_SIGNATURES}
 
 
 def _nvcc() -> str:

@@ -11,6 +11,7 @@
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
+#include "occupancy_kernels.cuh"
 
 #include <thrust/iterator/transform_iterator.h>
 
@@ -1802,6 +1803,180 @@ int nerfb200_normal_rays(const float* vertices, const double* normals, int64_t n
                                                                                      near_t, rays);
   g_launches++;
   CUDA_TRY(cudaGetLastError(), "normal_rays launch");
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- empty-space skipping (include/nerf_pl_b200_occupancy.h; kernels: occupancy_kernels.cuh) ------------------
+namespace {
+
+struct CullLayout {
+  long long tiles;
+  size_t tcnt, tofs, bytes;
+};
+CullLayout cull_layout(long long n) {
+  CullLayout L;
+  L.tiles = (n + kCullTile - 1) / kCullTile;
+  size_t o = 0;
+  L.tcnt = o; o += align256((L.tiles + 1) * sizeof(int));
+  L.tofs = o; o += align256((L.tiles + 1) * sizeof(long long));
+  L.bytes = o;
+  return L;
+}
+
+// one CTA per tile of rays, capped like the other grid-stride launches
+int cull_blocks(long long tiles) {
+  long long b = tiles < 148 * 8 ? tiles : 148 * 8;
+  const int cap = env_switches().max_ctas;
+  if (cap > 0 && b > cap) b = cap;
+  return static_cast<int>(b < 1 ? 1 : b);
+}
+
+int cull_prepare(const float* rays, int64_t n, void* ws, size_t bytes, CullParams* p, CullLayout* L, const char* who) {
+  if (n < 0) return fail(NERFB200_EINVAL, "%s: n_rays < 0", who);
+  *L = cull_layout(n);
+  if (n == 0) return 0;
+  if (!rays || !ws) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (reinterpret_cast<uintptr_t>(rays) & 15) return fail(NERFB200_EINVAL, "%s: rays must be 16-byte aligned", who);
+  if (bytes < L->bytes) return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_cull_workspace_bytes", who);
+  char* w = static_cast<char*>(ws);
+  p->rays = rays; p->n = n;
+  p->tcnt = reinterpret_cast<int*>(w + L->tcnt);
+  p->tofs = reinterpret_cast<long long*>(w + L->tofs);
+  p->bits = nullptr; p->flag = nullptr; p->live_idx = nullptr; p->live_rays = nullptr;
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t nerfb200_occupancy_workspace_bytes(int64_t N) {
+  if (N < 2 || N > kVolMaxN) return 0;
+  return 2 * align256(static_cast<size_t>((N - 1) * (N - 1) * (N - 1)));
+}
+
+int nerfb200_occupancy_pack(const float* sigma, int64_t N, double sigma_threshold, int32_t dilate, void* ws,
+                            size_t bytes, uint32_t* bits, void* stream) {
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "occupancy_pack: N must be in [2, 1625]%s");
+  if (dilate < 0) return fail(NERFB200_EINVAL, "occupancy_pack: dilate < 0%s");
+  if (sigma_threshold != sigma_threshold) return fail(NERFB200_EINVAL, "occupancy_pack: sigma_threshold is NaN%s");
+  if (!sigma || !ws || !bits) return fail(NERFB200_EINVAL, "occupancy_pack: NULL argument%s");
+  if (bytes < nerfb200_occupancy_workspace_bytes(N))
+    return fail(NERFB200_EINVAL, "occupancy_pack: workspace smaller than nerfb200_occupancy_workspace_bytes%s");
+  const long long M = N - 1, C = M * M * M;
+  uint8_t* a = static_cast<uint8_t*>(ws);
+  uint8_t* b = a + align256(static_cast<size_t>(C));
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  occ_cells_kernel<<<mesh_blocks(C), 256, 0, s>>>(sigma, N, sigma_threshold, a);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "occupancy cells launch");
+  // a radius of M - 1 cells already reaches across the grid
+  const int radius = static_cast<int>(dilate < M - 1 ? dilate : M - 1);
+  if (radius > 0) {
+    const long long stride[3] = {1, M, M * M};
+    for (int ax = 0; ax < 3; ++ax) {
+      occ_dilate_axis_kernel<<<mesh_blocks(C), 256, 0, s>>>(a, b, M, stride[ax], radius);
+      g_launches++;
+      CUDA_TRY(cudaGetLastError(), "occupancy dilate launch");
+      uint8_t* t = a; a = b; b = t;
+    }
+  }
+  occ_pack_kernel<<<mesh_blocks(C), 256, 0, s>>>(a, C, bits);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "occupancy pack launch");
+  return 0;
+}
+
+int nerfb200_occupancy_popcount(const uint32_t* bits, int64_t N, int64_t* count, void* stream) {
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "occupancy_popcount: N must be in [2, 1625]%s");
+  if (!bits || !count) return fail(NERFB200_EINVAL, "occupancy_popcount: NULL argument%s");
+  const long long C = (N - 1) * (N - 1) * (N - 1), words = (C + 31) / 32;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemsetAsync(count, 0, sizeof(*count), s), "occupancy_popcount memset");
+  occ_popcount_kernel<<<mesh_blocks(words), 256, 0, s>>>(bits, words, reinterpret_cast<unsigned long long*>(count));
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "occupancy_popcount launch");
+  return 0;
+}
+
+size_t nerfb200_cull_workspace_bytes(int64_t n_rays) {
+  return n_rays < 0 ? 0 : cull_layout(n_rays).bytes;
+}
+
+int nerfb200_cull_count(const float* rays, int64_t n_rays, const uint32_t* bits, int64_t N,
+                        const double ranges_host[6], void* ws, size_t bytes, uint8_t* flag, int64_t* n_live_host,
+                        void* stream) {
+  CullParams p;
+  CullLayout L;
+  int rc = cull_prepare(rays, n_rays, ws, bytes, &p, &L, "cull_count");
+  if (rc) return rc;
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "cull_count: N must be in [2, 1625]%s");
+  if (!n_live_host || !ranges_host) return fail(NERFB200_EINVAL, "cull_count: NULL argument%s");
+  for (int a = 0; a < 3; ++a) {
+    const double lo = ranges_host[2 * a], hi = ranges_host[2 * a + 1];
+    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
+      return fail(NERFB200_EINVAL, "cull_count: every range must be finite with min != max%s");
+    p.lo[a] = lo;
+    p.scale[a] = static_cast<double>(N - 1) / (hi - lo);
+  }
+  *n_live_host = 0;
+  if (n_rays == 0) return 0;
+  if (!bits || !flag) return fail(NERFB200_EINVAL, "cull_count: NULL argument%s");
+  p.bits = bits; p.M = N - 1; p.flag = flag;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  cull_classify_kernel<<<cull_blocks(L.tiles), kCullTile, 0, s>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "cull classify launch");
+  cull_scan_kernel<<<1, 1024, 0, s>>>(p.tcnt, p.tofs, L.tiles);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "cull scan launch");
+  long long h = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h, p.tofs + L.tiles, sizeof(h), cudaMemcpyDeviceToHost, s), "cull_count readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "cull_count readback");
+  *n_live_host = h;
+  return 0;
+}
+
+int nerfb200_cull_emit(const float* rays, int64_t n_rays, const uint8_t* flag, void* ws, size_t bytes,
+                       int64_t* live_idx, float* live_rays, void* stream) {
+  CullParams p;
+  CullLayout L;
+  int rc = cull_prepare(rays, n_rays, ws, bytes, &p, &L, "cull_emit");
+  if (rc) return rc;
+  if (n_rays == 0) return 0;
+  if (!flag || !live_idx || !live_rays) return fail(NERFB200_EINVAL, "cull_emit: NULL argument%s");
+  if (reinterpret_cast<uintptr_t>(live_rays) & 15) return fail(NERFB200_EINVAL, "cull_emit: live_rays must be 16-byte aligned%s");
+  p.flag = const_cast<uint8_t*>(flag);
+  p.live_idx = reinterpret_cast<long long*>(live_idx);
+  p.live_rays = live_rays;
+  cull_emit_kernel<<<cull_blocks(L.tiles), kCullTile, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "cull emit launch");
+  return 0;
+}
+
+int nerfb200_scatter_results(const float* const src_host[6], float* const dst_host[6], const int64_t* live_idx,
+                             int64_t n_live, int64_t n_rays, int32_t white_back, void* stream) {
+  if (n_rays < 0 || n_live < 0 || n_live > n_rays) return fail(NERFB200_EINVAL, "scatter_results: bad n_live / n_rays%s");
+  if (!src_host || !dst_host) return fail(NERFB200_EINVAL, "scatter_results: NULL argument%s");
+  if (n_rays == 0) return 0;
+  if (n_live > 0 && !live_idx) return fail(NERFB200_EINVAL, "scatter_results: live_idx is NULL%s");
+  ScatterParams p;
+  bool any = false;
+  for (int k = 0; k < 6; ++k) {
+    if (n_live > 0 && (src_host[k] == nullptr) != (dst_host[k] == nullptr))
+      return fail(NERFB200_EINVAL, "scatter_results: a result is NULL on one side only%s");
+    p.src[k] = src_host[k]; p.dst[k] = dst_host[k];
+    any |= dst_host[k] != nullptr;
+  }
+  if (!any) return fail(NERFB200_EINVAL, "scatter_results: no result to write%s");
+  p.live_idx = reinterpret_cast<const long long*>(live_idx);
+  p.n_live = n_live; p.n = n_rays; p.bg = white_back ? 1.f : 0.f;
+  scatter_results_kernel<<<mesh_blocks(n_rays), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError(), "scatter_results launch");
   return 0;
 }
 

@@ -1,0 +1,247 @@
+// Empty-space skipping at render time: an occupancy bit field built from a dense sigma grid, rays classified
+// against it by an exact cell walk, the live rays compacted in order, and the rendered results scattered back
+// over a vacuum background.  The render kernel is not involved: these kernels run in front of and behind it.
+// Conventions and the conservativeness argument: DESIGN.md "Empty-space skipping".
+//
+// AXIS ORDER.  The sigma grid is the one of nerfb200_sigma_grid: sigma[i, j, k] = sigma(x_j, y_i, z_k), flat
+// (i * N + j) * N + k (np.meshgrid's 'xy' indexing: the FIRST index is y).  The occupancy grid undoes it: cell
+// (cx, cy, cz) spans [x_cx, x_cx+1] x [y_cy, y_cy+1] x [z_cz, z_cz+1] with x_j = linspace(x_range, N)[j] etc.,
+// its corners are sigma[cy + dy, cx + dx, cz + dz], its flat index is c = (cz * M + cy) * M + cx with M = N - 1
+// (x fastest), and it is bit c % 32 of word c / 32.  The bits past the last cell are 0.
+#pragma once
+#include <cstdint>
+#include <cuda_runtime.h>
+
+namespace nerfb200 {
+
+// ---- 1. sigma grid -> cells -> dilation -> bits ---------------------------------------------------------
+// A cell is occupied iff a corner has sigma > thr, which is "the largest of its 8 corners > thr" with a NaN
+// corner counting as not above.  The comparison is made in double, as marching cubes makes it.
+__global__ void occ_cells_kernel(const float* __restrict__ sigma, long long N, double thr, uint8_t* __restrict__ occ) {
+  const long long M = N - 1, C = M * M * M;
+  for (long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    const long long cx = c % M, cy = (c / M) % M, cz = c / (M * M);
+    bool any = false;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const long long j = cx + (q & 1), i = cy + ((q >> 1) & 1), k = cz + ((q >> 2) & 1);
+      any |= static_cast<double>(sigma[(i * N + j) * N + k]) > thr;
+    }
+    occ[c] = any;
+  }
+}
+
+// One axis of the Chebyshev dilation (a box dilation is separable): out = OR of in over [-r, r] along the axis
+// of stride `stride` cells, clipped to the grid.
+__global__ void occ_dilate_axis_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, long long M,
+                                       long long stride, int r) {
+  const long long C = M * M * M;
+  for (long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    const long long a = (c / stride) % M;
+    const long long lo = a - r < 0 ? 0 : a - r, hi = a + r > M - 1 ? M - 1 : a + r;
+    uint8_t v = 0;
+    for (long long b = lo; b <= hi && !v; ++b) v = in[c + (b - a) * stride];
+    out[c] = v;
+  }
+}
+
+// 32 cells per word by warp ballot.  The launch has a multiple of 32 threads and every lane of a warp runs the
+// same number of rounds (the bound is rounded up to a whole word).
+__global__ void occ_pack_kernel(const uint8_t* __restrict__ occ, long long C, uint32_t* __restrict__ bits) {
+  const long long C_pad = (C + 31) / 32 * 32;
+  for (long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x; c < C_pad; c += (long long)gridDim.x * blockDim.x) {
+    const unsigned w = __ballot_sync(0xffffffffu, c < C && occ[c] != 0);
+    if ((threadIdx.x & 31) == 0) bits[c >> 5] = w;
+  }
+}
+
+__global__ void occ_popcount_kernel(const uint32_t* __restrict__ bits, long long n_words, unsigned long long* total) {
+  unsigned long long s = 0;
+  for (long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x; w < n_words; w += (long long)gridDim.x * blockDim.x)
+    s += __popc(bits[w]);
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0 && s) atomicAdd(total, s);
+}
+
+// ---- 2. ray classification -------------------------------------------------------------------------------
+struct CullParams {
+  const float* rays;      // (n, 8) [o, d, near, far]
+  long long n;
+  const uint32_t* bits;
+  long long M;            // cells per axis
+  double lo[3], scale[3]; // grid coordinate g = (p - lo) * scale, scale = M / (hi - lo): the box is [0, M]^3
+  uint8_t* flag;          // (n)
+  int* tcnt;              // live rays of each tile
+  long long* tofs;        // exclusive scan of tcnt, n_tiles + 1
+  long long* live_idx;
+  float* live_rays;
+};
+
+constexpr int kCullTile = 256;   // rays per tile = threads per block
+
+// Live iff the segment o + t d, t in [near, far], crosses an occupied cell.  Amanatides-Woo in grid coordinates,
+// in double; each boundary time is recomputed from the cell index, so no error accumulates along the walk.
+// Space outside the box is empty.  A ray the walk cannot judge (a non-finite value, far <= near) is live: the
+// renderer then sees it unchanged.
+__device__ __forceinline__ bool cull_ray_live(const CullParams& p, const float* r) {
+  float v[8];
+#pragma unroll
+  for (int a = 0; a < 8; ++a) v[a] = r[a];
+  bool finite = true;
+#pragma unroll
+  for (int a = 0; a < 8; ++a) finite &= isfinite(v[a]);
+  if (!finite || !(v[7] > v[6])) return true;
+  const double M = static_cast<double>(p.M);
+  double o[3], d[3], inv[3];
+  double t0 = v[6], t1 = v[7];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    o[a] = (static_cast<double>(v[a]) - p.lo[a]) * p.scale[a];
+    d[a] = static_cast<double>(v[3 + a]) * p.scale[a];
+    if (d[a] == 0.0) {
+      inv[a] = 0.0;
+      if (o[a] < 0.0 || o[a] > M) return false;
+    } else {
+      inv[a] = 1.0 / d[a];
+      const double ta = (0.0 - o[a]) * inv[a], tb = (M - o[a]) * inv[a];
+      t0 = fmax(t0, fmin(ta, tb));
+      t1 = fmin(t1, fmax(ta, tb));
+    }
+  }
+  if (!(t0 <= t1)) return false;
+  long long cell[3];
+  double tnext[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double g = floor(o[a] + t0 * d[a]);
+    cell[a] = static_cast<long long>(fmin(fmax(g, 0.0), M - 1.0));
+  }
+  const double inf = __longlong_as_double(0x7ff0000000000000LL);
+  const long long steps = 3 * p.M + 3;
+  for (long long s = 0; s < steps; ++s) {
+    const long long c = (cell[2] * p.M + cell[1]) * p.M + cell[0];
+    if ((p.bits[c >> 5] >> (c & 31)) & 1u) return true;
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+      tnext[a] = d[a] == 0.0 ? inf : (static_cast<double>(cell[a] + (d[a] > 0.0 ? 1 : 0)) - o[a]) * inv[a];
+    const int ax = tnext[0] <= tnext[1] ? (tnext[0] <= tnext[2] ? 0 : 2) : (tnext[1] <= tnext[2] ? 1 : 2);
+    // unrolled over the axis so that the per-axis arrays stay in registers
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      if (a != ax) continue;
+      if (!(tnext[a] <= t1)) return false;
+      cell[a] += d[a] > 0.0 ? 1 : -1;
+      if (cell[a] < 0 || cell[a] >= p.M) return false;
+    }
+  }
+  return false;
+}
+
+// One tile of kCullTile rays per round: the flags and the tile's live count.
+__global__ void cull_classify_kernel(CullParams p) {
+  const long long n_tiles = (p.n + kCullTile - 1) / kCullTile;
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const long long i = tile * kCullTile + threadIdx.x;
+    const bool live = i < p.n && cull_ray_live(p, p.rays + i * 8);
+    if (i < p.n) p.flag[i] = live;
+    const int cnt = __syncthreads_count(live);
+    if (threadIdx.x == 0) p.tcnt[tile] = cnt;
+  }
+}
+
+// Exclusive scan of the tile counts by one block of 1024 threads, 1024 tiles per round with a running carry;
+// tofs[n_tiles] is the total.
+__global__ void cull_scan_kernel(const int* __restrict__ tcnt, long long* __restrict__ tofs, long long n_tiles) {
+  __shared__ long long warp_sum[32];
+  __shared__ long long carry;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (long long base = 0; base < n_tiles; base += 1024) {
+    const long long i = base + threadIdx.x;
+    const long long own = i < n_tiles ? tcnt[i] : 0;
+    long long incl = own;
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long up = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += up;
+    }
+    if (lane == 31) warp_sum[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+      long long w = warp_sum[lane];
+      for (int o = 1; o < 32; o <<= 1) {
+        const long long up = __shfl_up_sync(0xffffffffu, w, o);
+        if (lane >= o) w += up;
+      }
+      warp_sum[lane] = w;   // inclusive over the warps
+    }
+    __syncthreads();
+    const long long before = carry + (warp ? warp_sum[warp - 1] : 0) + incl - own;
+    if (i < n_tiles) tofs[i] = before;
+    __syncthreads();
+    if (threadIdx.x == 1023) carry = before + own;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) tofs[n_tiles] = carry;
+}
+
+// The stable compaction: live ray i goes to row tofs[tile] + (live rays before it in the tile), so live_idx is
+// increasing.  The index and the 32-byte ray are written in the same pass.
+__global__ void cull_emit_kernel(CullParams p) {
+  __shared__ int warp_cnt[kCullTile / 32];
+  const long long n_tiles = (p.n + kCullTile - 1) / kCullTile;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const long long i = tile * kCullTile + threadIdx.x;
+    const bool live = i < p.n && p.flag[i] != 0;
+    const unsigned m = __ballot_sync(0xffffffffu, live);
+    if (lane == 0) warp_cnt[warp] = __popc(m);
+    __syncthreads();
+    if (live) {
+      long long row = p.tofs[tile] + __popc(m & ((1u << lane) - 1u));
+      for (int w = 0; w < warp; ++w) row += warp_cnt[w];
+      p.live_idx[row] = i;
+      const float4* src = reinterpret_cast<const float4*>(p.rays + i * 8);
+      float4* dst = reinterpret_cast<float4*>(p.live_rays + row * 8);
+      dst[0] = src[0];
+      dst[1] = src[1];
+    }
+    __syncthreads();
+  }
+}
+
+// ---- 3. scatter with background fill ------------------------------------------------------------------
+// The six result tensors of a render in the order rgb_coarse, depth_coarse, opacity_coarse, rgb_fine, depth_fine,
+// opacity_fine; a NULL pair is skipped.
+struct ScatterParams {
+  const float* src[6];    // compacted (n_live, 3) / (n_live)
+  float* dst[6];          // full size
+  const long long* live_idx;
+  long long n_live, n;
+  float bg;               // rgb of a ray through vacuum: 1 with white_back, else 0 (depth and opacity: 0)
+};
+
+// One thread per output ray: its row among the live rays by binary search of the increasing live_idx, then every
+// key is written once, from the render or from the vacuum value.
+__global__ void scatter_results_kernel(ScatterParams p) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < p.n; i += (long long)gridDim.x * blockDim.x) {
+    long long lo = 0, hi = p.n_live;
+    while (lo < hi) {
+      const long long mid = (lo + hi) >> 1;
+      if (p.live_idx[mid] < i) lo = mid + 1; else hi = mid;
+    }
+    const bool live = lo < p.n_live && p.live_idx[lo] == i;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      if (!p.dst[k]) continue;
+      if (k % 3 == 0) {
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) p.dst[k][i * 3 + ch] = live ? p.src[k][lo * 3 + ch] : p.bg;
+      } else {
+        p.dst[k][i] = live ? p.src[k][lo] : 0.f;
+      }
+    }
+  }
+}
+
+}  // namespace nerfb200

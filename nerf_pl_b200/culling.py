@@ -1,0 +1,227 @@
+"""Empty-space skipping at render time (DESIGN.md "Empty-space skipping").
+
+``occupancy_grid`` turns a trained network into a bit field of occupied cells; ``cull_rays`` classifies rays
+against it and compacts the live ones; ``render_rays_culled`` renders only those with the ordinary fused kernel and
+scatters the results back over the value a ray through vacuum renders.  Every stage is an sm_90a kernel of
+``libnerf_pl_b200.so`` (csrc/occupancy_kernels.cuh, include/nerf_pl_b200_occupancy.h); the render kernel is not
+touched.  The reference has no counterpart: it evaluates every sample of every ray.
+
+What it guarantees.  A live ray is rendered by the same kernel on an ordinary ``(n_live, 8)`` tensor, and with
+``perturb = noise_std = 0`` a ray's result does not depend on its row: live pixels are bit-identical to the
+unculled render.  A culled pixel is *approximated* by the vacuum value.  The cell walk is exact and the dilation
+adds a margin, but sigma is only sampled at the grid points and the trained sigma of empty space is small, not
+zero: the error of a culled pixel is an empirical bound governed by ``N``, ``sigma_threshold`` and ``dilate``, not
+a proof.  Space outside the grid's box counts as empty.  Culling is for inference only: training must see the
+background rays to learn that they are empty.
+"""
+from __future__ import annotations
+
+import ctypes
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
+
+import torch
+
+from . import _lib
+from .rendering import render_rays
+
+RESULT_KEYS = ("rgb_coarse", "depth_coarse", "opacity_coarse", "rgb_fine", "depth_fine", "opacity_fine")
+
+
+def _ranges(x_range, y_range, z_range) -> Tuple[float, ...]:
+    vals = tuple(float(v) for r in (x_range, y_range, z_range) for v in r)
+    if len(vals) != 6:
+        raise ValueError("x_range, y_range and z_range must each be (min, max)")
+    return vals
+
+
+class OccupancyGrid:
+    """The occupied cells of a ``N``-point grid over ``x_range x y_range x z_range``: ``bits`` is a CUDA tensor of
+    ``ceil((N-1)^3 / 32)`` uint32 words (stored as int32), one bit per cell, x fastest.  Cell ``(cx, cy, cz)`` spans
+    ``[x_cx, x_cx+1] x [y_cy, y_cy+1] x [z_cz, z_cz+1]`` of ``np.linspace(*range, N)``; note that ``nb.sigma_grid``
+    indexes ``[y, x, z]``, and this object does not."""
+
+    def __init__(self, bits: torch.Tensor, N: int, x_range, y_range, z_range, dilate: int = 0):
+        N = int(N)
+        if not 2 <= N <= 1625:
+            raise ValueError(f"OccupancyGrid: N = {N} outside [2, 1625]")
+        words = ((N - 1) ** 3 + 31) // 32
+        if not isinstance(bits, torch.Tensor) or not bits.is_cuda:
+            raise RuntimeError("OccupancyGrid: bits must be a CUDA tensor (nerf_pl_b200 has no CPU fallback)")
+        if bits.dtype not in (torch.int32, torch.uint32) or bits.numel() != words:
+            raise ValueError(f"OccupancyGrid: bits must hold {words} 32-bit words")
+        self.bits = bits.contiguous().view(torch.int32).reshape(-1)
+        self.N = N
+        self.ranges = _ranges(x_range, y_range, z_range)
+        if any(self.ranges[2 * a] == self.ranges[2 * a + 1] for a in range(3)):
+            raise ValueError("OccupancyGrid: every range needs min != max")
+        self.dilate = int(dilate)
+
+    @property
+    def device(self) -> torch.device:
+        return self.bits.device
+
+    def n_cells(self) -> int:
+        return (self.N - 1) ** 3
+
+    def occupied_fraction(self) -> float:
+        """Occupied cells over all cells (a popcount reduction on the device)."""
+        count = torch.empty(1, dtype=torch.int64, device=self.device)
+        _lib.call("nerfb200_occupancy_popcount", self.device, self.bits.data_ptr(), self.N, count.data_ptr())
+        return int(count.item()) / self.n_cells()
+
+    def to_dense(self) -> torch.Tensor:
+        """(N-1, N-1, N-1) bool, indexed ``[cx, cy, cz]`` (for tests and inspection)."""
+        M = self.N - 1
+        shifts = torch.arange(32, dtype=torch.int32, device=self.device)
+        flat = ((self.bits[:, None] >> shifts) & 1).reshape(-1)[:M ** 3].bool()
+        return flat.view(M, M, M).permute(2, 1, 0).contiguous()
+
+    def state_dict(self) -> Dict[str, object]:
+        return {"bits": self.bits.detach().cpu(), "N": self.N, "ranges": tuple(self.ranges), "dilate": self.dilate}
+
+    def load_state_dict(self, state: Dict[str, object]) -> "OccupancyGrid":
+        self.__dict__.update(OccupancyGrid.from_state_dict(state, self.device).__dict__)
+        return self
+
+    @classmethod
+    def from_state_dict(cls, state: Dict[str, object], device="cuda") -> "OccupancyGrid":
+        """The grid of a ``state_dict()`` saved beside a checkpoint, on ``device``."""
+        r = tuple(state["ranges"])
+        return cls(torch.as_tensor(state["bits"]).to(device), state["N"], r[0:2], r[2:4], r[4:6], state["dilate"])
+
+
+def _workspace(nbytes: int, device) -> torch.Tensor:
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
+@torch.no_grad()
+def pack_occupancy(sigma: torch.Tensor, x_range, y_range, z_range, sigma_threshold: float,
+                   dilate: int = 1) -> OccupancyGrid:
+    """The occupancy grid of a CUDA (N, N, N) sigma grid in ``nb.sigma_grid``'s order (``sigma[i, j, k] =
+    sigma(x_j, y_i, z_k)``): a cell is occupied iff the largest sigma of its 8 corners is ``> sigma_threshold``; the
+    set is dilated by ``dilate`` cells in Chebyshev distance and packed."""
+    if not isinstance(sigma, torch.Tensor) or not sigma.is_cuda:
+        raise RuntimeError("pack_occupancy: sigma must be a CUDA tensor (nerf_pl_b200 has no CPU fallback)")
+    if sigma.dim() != 3 or not (sigma.shape[0] == sigma.shape[1] == sigma.shape[2]):
+        raise ValueError("sigma must be (N, N, N)")
+    s = sigma.detach().to(torch.float32).contiguous()
+    N = s.shape[0]
+    nbytes = _lib.load().nerfb200_occupancy_workspace_bytes(N)
+    if nbytes == 0:
+        raise ValueError(f"pack_occupancy: N = {N} outside [2, 1625]")
+    ws = _workspace(nbytes, s.device)
+    bits = torch.empty(((N - 1) ** 3 + 31) // 32, dtype=torch.int32, device=s.device)
+    _lib.call("nerfb200_occupancy_pack", s.device, s.data_ptr(), N, float(sigma_threshold), int(dilate), ws.data_ptr(),
+              ws.numel(), bits.data_ptr())
+    return OccupancyGrid(bits, N, x_range, y_range, z_range, dilate)
+
+
+@torch.no_grad()
+def occupancy_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, sigma_threshold: float, dilate: int = 1,
+                   chunk: int = 1 << 21) -> OccupancyGrid:
+    """The occupancy grid of ``model`` (the network that decides the picture: the fine one): ``nb.sigma_grid`` on N^3
+    points, with ``N`` and the ranges as for mesh extraction, then ``pack_occupancy``.  The float sigma grid is
+    transient.  A ray that only crosses unoccupied cells will be given the vacuum value, so choose
+    ``sigma_threshold`` well below the density of anything visible (see the module docstring for what is and is
+    not guaranteed)."""
+    from .mesh import sigma_grid     # mesh imports inference, which imports this module
+    sigma = sigma_grid(model, int(N), x_range, y_range, z_range, chunk)
+    grid = pack_occupancy(sigma, x_range, y_range, z_range, sigma_threshold, dilate)
+    del sigma
+    return grid
+
+
+def _check_rays(rays: torch.Tensor, occupancy: OccupancyGrid) -> torch.Tensor:
+    if not isinstance(occupancy, OccupancyGrid):
+        raise ValueError("occupancy must be a nerf_pl_b200.OccupancyGrid")
+    if not isinstance(rays, torch.Tensor) or not rays.is_cuda:
+        raise RuntimeError("rays must be a CUDA tensor (nerf_pl_b200 has no CPU fallback)")
+    if rays.dim() != 2 or rays.shape[1] != 8:
+        raise ValueError("rays must be (n, 8) [o, d, near, far]")
+    if rays.device != occupancy.device:
+        raise ValueError("rays and the occupancy grid must be on the same device")
+    return rays.detach().to(torch.float32).contiguous()
+
+
+@torch.no_grad()
+def cull_rays(rays: torch.Tensor, occupancy: OccupancyGrid, return_flag: bool = False):
+    """(live_idx (n_live) int64, increasing; live_rays (n_live, 8) = rays[live_idx]) of the rays whose segment
+    ``o + t d, t in [near, far]`` crosses an occupied cell.  The rays are taken as given: for NDC rays use a grid
+    built over NDC coordinates.  A ray with a non-finite value or ``far <= near`` is live.  ``return_flag`` adds
+    the per-ray uint8 flag.  Synchronises (the number of live rays sizes the outputs)."""
+    r = _check_rays(rays, occupancy)
+    dev, n = r.device, r.shape[0]
+    ws = _workspace(_lib.load().nerfb200_cull_workspace_bytes(n), dev)
+    flag = torch.empty(n, dtype=torch.uint8, device=dev)
+    n_live = ctypes.c_int64()
+    _lib.call("nerfb200_cull_count", dev, r.data_ptr(), n, occupancy.bits.data_ptr(), occupancy.N,
+              (ctypes.c_double * 6)(*occupancy.ranges), ws.data_ptr(), ws.numel(), flag.data_ptr(), ctypes.byref(n_live))
+    live_idx = torch.empty(n_live.value, dtype=torch.int64, device=dev)
+    live_rays = torch.empty(n_live.value, 8, dtype=torch.float32, device=dev)
+    if n_live.value:
+        _lib.call("nerfb200_cull_emit", dev, r.data_ptr(), n, flag.data_ptr(), ws.data_ptr(), ws.numel(),
+                  live_idx.data_ptr(), live_rays.data_ptr())
+    return (live_idx, live_rays, flag) if return_flag else (live_idx, live_rays)
+
+
+def result_keys(N_importance: int, test_time: bool) -> List[str]:
+    keys = ["opacity_coarse"] if test_time else ["rgb_coarse", "depth_coarse", "opacity_coarse"]
+    return keys + (["rgb_fine", "depth_fine", "opacity_fine"] if N_importance > 0 else [])
+
+
+@torch.no_grad()
+def scatter_results(compact: Optional[Dict[str, torch.Tensor]], live_idx: torch.Tensor, n_rays: int, white_back: bool,
+                    keys: Optional[Sequence[str]] = None) -> Dict[str, torch.Tensor]:
+    """Full-size results of a render of compacted rays, in one launch: row ``live_idx[r]`` of every key is row r of
+    ``compact``; every other ray gets the vacuum value (opacity 0, depth 0, rgb 1 if ``white_back`` else 0).
+    ``keys`` names the results when there is no live ray (``compact`` may then be None)."""
+    dev = live_idx.device
+    n_live = live_idx.shape[0]
+    keys = list(compact) if keys is None else list(keys)
+    if not keys or any(k not in RESULT_KEYS for k in keys):
+        raise ValueError(f"scatter_results: keys must be among {RESULT_KEYS}")
+    src = {k: compact[k].detach().to(torch.float32).contiguous() for k in keys} if n_live else {}
+    out = {k: torch.empty((n_rays, 3) if k.startswith("rgb") else (n_rays,), dtype=torch.float32, device=dev)
+           for k in keys}
+    for k in src:
+        if src[k].shape != (n_live,) + tuple(out[k].shape[1:]) or src[k].device != dev:
+            raise ValueError(f"scatter_results: {k} must be {(n_live,) + tuple(out[k].shape[1:])} on {dev}")
+    ptrs = lambda d: (ctypes.c_void_p * 6)(*[d[k].data_ptr() if k in d else None for k in RESULT_KEYS])  # noqa: E731
+    idx = live_idx.to(torch.int64).contiguous()
+    _lib.call("nerfb200_scatter_results", dev, ptrs(src), ptrs(out), idx.data_ptr() if n_live else None, n_live,
+              int(n_rays), int(bool(white_back)))
+    return out
+
+
+def render_culled(render_fn: Callable[[torch.Tensor], Dict[str, torch.Tensor]], rays: torch.Tensor,
+                  occupancy: OccupancyGrid, keys: Sequence[str], white_back: bool) -> Dict[str, torch.Tensor]:
+    """cull -> ``render_fn(live_rays)`` -> scatter.  With no live ray there is no render launch."""
+    live_idx, live_rays = cull_rays(rays, occupancy)
+    compact = render_fn(live_rays) if live_idx.shape[0] else None
+    out = scatter_results(compact, live_idx, rays.shape[0], white_back, keys)
+    out["live"] = int(live_idx.shape[0])
+    out["live_idx"] = live_idx
+    return out
+
+
+@torch.no_grad()
+def render_rays_culled(models: List[torch.nn.Module], embeddings: List[torch.nn.Module], rays: torch.Tensor,
+                       occupancy: OccupancyGrid, N_samples: int = 64, use_disp: bool = False, N_importance: int = 0,
+                       white_back: bool = False, test_time: bool = True, *, perturb: float = 0,
+                       noise_std: float = 0) -> Dict[str, torch.Tensor]:
+    """``render_rays`` at inference with empty space skipped: the same keys, shapes and dtypes, plus ``'live'``
+    (the number of rays rendered) and ``'live_idx'`` (their indices, int64).  Live rays are bit-identical to
+    ``render_rays(..., perturb=0, noise_std=0)``; a culled ray gets the vacuum value, an approximation whose error
+    is bounded empirically, not proved (module docstring).  Inference only: ``perturb`` and ``noise_std`` must be
+    0 and no gradient is built; anything else is a ValueError, because training must see the background rays to
+    learn that they are empty."""
+    if float(perturb) != 0.0 or float(noise_std) != 0.0:
+        raise ValueError("render_rays_culled is inference only (perturb = 0, noise_std = 0): training must see the "
+                         "background rays to learn that they are empty")
+    r = _check_rays(rays, occupancy)
+
+    def fn(live):
+        return render_rays(list(models), list(embeddings), live, int(N_samples), use_disp, 0, 0, int(N_importance),
+                           1024 * 32, white_back, test_time=test_time, match_reference_rng=False)
+
+    return render_culled(fn, r, occupancy, result_keys(int(N_importance), bool(test_time)), bool(white_back))

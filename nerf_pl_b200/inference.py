@@ -12,6 +12,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
+from .culling import OccupancyGrid, result_keys, render_culled
 from .nerf import packed_weights
 from .rendering import render_rays
 from .sharded import render_rays_sharded
@@ -48,13 +49,17 @@ def to_uint8(img: torch.Tensor) -> torch.Tensor:
 @torch.no_grad()
 def batched_inference(models: Sequence[torch.nn.Module], embeddings: Sequence[torch.nn.Module],
                       rays: torch.Tensor, N_samples: int, N_importance: int, use_disp: bool,
-                      chunk: int = 1024 * 32, white_back: bool = False, sharded: bool = False
-                      ) -> Dict[str, torch.Tensor]:
+                      chunk: int = 1024 * 32, white_back: bool = False, sharded: bool = False,
+                      occupancy: Optional[OccupancyGrid] = None) -> Dict[str, torch.Tensor]:
     """Drop-in for eval.py:58-86 batched_inference(models, embeddings, rays, N_samples,
     N_importance, use_disp, chunk, white_back): perturb=0, noise_std=0, test_time=True.  The
     reference loops over 32768-ray chunks and concatenates; here the whole image is one launch
     (``chunk`` is ignored).  ``sharded=True`` splits the rays over the ranks of the default process
-    group and all-gathers the result (nerf_pl_b200.sharded)."""
+    group and all-gathers the result (nerf_pl_b200.sharded).  ``occupancy`` (an ``nb.occupancy_grid``; default None:
+    every ray is rendered) skips empty space: only the rays that cross an occupied cell are rendered, the others
+    get the vacuum value, and the result also holds ``'live'`` and ``'live_idx'`` (nerf_pl_b200.culling, which also
+    says what that does and does not guarantee).  With ``sharded`` the live rays are what is split, so the ranks
+    get equal work."""
     del chunk
 
     def fn(r):
@@ -62,24 +67,31 @@ def batched_inference(models: Sequence[torch.nn.Module], embeddings: Sequence[to
         return render_rays(list(models), list(embeddings), r, N_samples, use_disp, 0, 0, N_importance,
                            1024 * 32, white_back, test_time=True, match_reference_rng=False)
 
-    return render_rays_sharded(fn, rays) if sharded else fn(rays)
+    run = (lambda r: render_rays_sharded(fn, r)) if sharded else fn
+    if occupancy is None:
+        return run(rays)
+    return render_culled(run, rays, occupancy, result_keys(int(N_importance), True), bool(white_back))
 
 
 @torch.no_grad()
 def render_image(models, embeddings, H: int, W: int, focal: float, c2w, near: float, far: float,
                  N_samples: int = 64, N_importance: int = 64, use_disp: bool = False, white_back: bool = False,
-                 ndc: bool = False, sharded: bool = False, device=None) -> Dict[str, torch.Tensor]:
+                 ndc: bool = False, sharded: bool = False, device=None,
+                 occupancy: Optional[OccupancyGrid] = None) -> Dict[str, torch.Tensor]:
     """Pose -> rays -> fused render -> (H, W, 3) uint8 image + float maps, all on the device
-    (test.ipynb cell 2 / eval.py:117-128)."""
+    (test.ipynb cell 2 / eval.py:117-128).  ``occupancy``: as for ``batched_inference``; the result then also
+    holds ``'live'``."""
     rays = generate_rays(H, W, focal, c2w, near, far, ndc=ndc, device=device)
     res = batched_inference(models, embeddings, rays, N_samples, N_importance, use_disp, 1024 * 32, white_back,
-                            sharded=sharded)
+                            sharded=sharded, occupancy=occupancy)
     typ = "fine" if N_importance > 0 else "coarse"
     out = {"rays": rays, "opacity": res[f"opacity_{typ}"].view(H, W)}
     if f"rgb_{typ}" in res:
         out["rgb"] = res[f"rgb_{typ}"].view(H, W, 3)
         out["depth"] = res[f"depth_{typ}"].view(H, W)
         out["rgb_uint8"] = to_uint8(out["rgb"])
+    if occupancy is not None:
+        out["live"] = res["live"]
     return out
 
 
