@@ -145,21 +145,9 @@ SIGNATURES = {
                                       _vp, _vp]),
     "nerfb200_color_accumulate": (_i32, [_vp, _vp, _vp, _i64, _f32, _vp, _vp]),
     "nerfb200_color_finalize": (_i32, [_vp, _i64, _vp, _vp]),
-    "nerfb200_launch_count": (_i64, []),
-    "nerfb200_check_status": (_i32, []),
-    "nerfb200_sm_count": (_i32, []),
-}
-EXPORTS = tuple(SIGNATURES)     # tests check the library exports all of them
-
-# The same for the companion header include/nerf_pl_b200_mesh_normals.h (the vertex-normal colouring method), which
-# nerf_pl_b200.h includes at its end.
-MESH_NORMALS_SIGNATURES = {
     "nerfb200_vertex_normals_workspace_bytes": (_sz, [_i64, _i64]),
     "nerfb200_vertex_normals": (_i32, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
     "nerfb200_normal_rays": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _vp, _vp]),
-}
-# And for include/nerf_pl_b200_occupancy.h (empty-space skipping at render time), included after it.
-OCCUPANCY_SIGNATURES = {
     "nerfb200_occupancy_workspace_bytes": (_sz, [_i64]),
     "nerfb200_occupancy_pack": (_i32, [_vp, _i64, _f64, _i32, _vp, _sz, _vp, _vp]),
     "nerfb200_occupancy_popcount": (_i32, [_vp, _i64, _vp, _vp]),
@@ -167,9 +155,11 @@ OCCUPANCY_SIGNATURES = {
     "nerfb200_cull_count": (_i32, [_vp, _i64, _vp, _i64, POINTER(_f64), _vp, _sz, _vp, POINTER(_i64), _vp]),
     "nerfb200_cull_emit": (_i32, [_vp, _i64, _vp, _vp, _sz, _vp, _vp, _vp]),
     "nerfb200_scatter_results": (_i32, [_P, _P, _vp, _i64, _i64, _i32, _vp]),
+    "nerfb200_launch_count": (_i64, []),
+    "nerfb200_check_status": (_i32, []),
+    "nerfb200_sm_count": (_i32, []),
 }
-HEADER_SIGNATURES = {"nerf_pl_b200.h": SIGNATURES, "nerf_pl_b200_mesh_normals.h": MESH_NORMALS_SIGNATURES,
-                     "nerf_pl_b200_occupancy.h": OCCUPANCY_SIGNATURES}
+EXPORTS = tuple(SIGNATURES)     # tests check the library exports all of them
 
 
 def _nvcc() -> str:
@@ -183,8 +173,7 @@ def needs_build() -> bool:
     if not os.path.exists(LIB_PATH):
         return True
     t = os.path.getmtime(LIB_PATH)
-    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS]
-    deps += [os.path.join(_HERE, "..", "include", h) for h in HEADER_SIGNATURES]
+    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS] + [os.path.join(_HERE, "..", "include", "nerf_pl_b200.h")]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
@@ -218,10 +207,9 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            for table in HEADER_SIGNATURES.values():
-                for name, (restype, argtypes) in table.items():
-                    fn = getattr(lib, name)
-                    fn.restype, fn.argtypes = restype, argtypes
+            for name, (restype, argtypes) in SIGNATURES.items():
+                fn = getattr(lib, name)
+                fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:
                 raise RuntimeError("libnerf_pl_b200.so ABI version mismatch")
             _lib = lib
@@ -258,3 +246,17 @@ def call(name: str, device, *args) -> None:
         with torch.cuda.device(device):
             rc = fn(*args, _stream_ptr())
     check(rc, name)
+
+
+def workspace(nbytes: int, device) -> torch.Tensor:
+    """Scratch of ``nbytes`` bytes (a *_workspace_bytes entry's answer) on ``device``; at least one byte, so that the
+    entries always see a non-NULL pointer."""
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
+def ranges_host(x_range, y_range, z_range):
+    """The ``ranges_host`` argument of the grid entries: {xmin, xmax, ymin, ymax, zmin, zmax} as 6 host doubles."""
+    vals = [float(v) for r in (x_range, y_range, z_range) for v in r]
+    if len(vals) != 6:
+        raise ValueError("x_range, y_range and z_range must each be (min, max)")
+    return (c_double * 6)(*vals)

@@ -3,7 +3,7 @@
 ``occupancy_grid`` turns a trained network into a bit field of occupied cells; ``cull_rays`` classifies rays
 against it and compacts the live ones; ``render_rays_culled`` renders only those with the ordinary fused kernel and
 scatters the results back over the value a ray through vacuum renders.  Every stage is an sm_90a kernel of
-``libnerf_pl_b200.so`` (csrc/occupancy_kernels.cuh, include/nerf_pl_b200_occupancy.h); the render kernel is not
+``libnerf_pl_b200.so`` (csrc/occupancy_kernels.cuh, include/nerf_pl_b200.h); the render kernel is not
 touched.  The reference has no counterpart: it evaluates every sample of every ray.
 
 What it guarantees.  A live ray is rendered by the same kernel on an ordinary ``(n_live, 8)`` tensor, and with
@@ -17,7 +17,7 @@ background rays to learn that they are empty.
 from __future__ import annotations
 
 import ctypes
-from typing import Callable, Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence
 
 import torch
 
@@ -25,13 +25,6 @@ from . import _lib
 from .rendering import render_rays
 
 RESULT_KEYS = ("rgb_coarse", "depth_coarse", "opacity_coarse", "rgb_fine", "depth_fine", "opacity_fine")
-
-
-def _ranges(x_range, y_range, z_range) -> Tuple[float, ...]:
-    vals = tuple(float(v) for r in (x_range, y_range, z_range) for v in r)
-    if len(vals) != 6:
-        raise ValueError("x_range, y_range and z_range must each be (min, max)")
-    return vals
 
 
 class OccupancyGrid:
@@ -51,7 +44,7 @@ class OccupancyGrid:
             raise ValueError(f"OccupancyGrid: bits must hold {words} 32-bit words")
         self.bits = bits.contiguous().view(torch.int32).reshape(-1)
         self.N = N
-        self.ranges = _ranges(x_range, y_range, z_range)
+        self.ranges = tuple(_lib.ranges_host(x_range, y_range, z_range))
         if any(self.ranges[2 * a] == self.ranges[2 * a + 1] for a in range(3)):
             raise ValueError("OccupancyGrid: every range needs min != max")
         self.dilate = int(dilate)
@@ -90,10 +83,6 @@ class OccupancyGrid:
         return cls(torch.as_tensor(state["bits"]).to(device), state["N"], r[0:2], r[2:4], r[4:6], state["dilate"])
 
 
-def _workspace(nbytes: int, device) -> torch.Tensor:
-    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
-
-
 @torch.no_grad()
 def pack_occupancy(sigma: torch.Tensor, x_range, y_range, z_range, sigma_threshold: float,
                    dilate: int = 1) -> OccupancyGrid:
@@ -109,7 +98,7 @@ def pack_occupancy(sigma: torch.Tensor, x_range, y_range, z_range, sigma_thresho
     nbytes = _lib.load().nerfb200_occupancy_workspace_bytes(N)
     if nbytes == 0:
         raise ValueError(f"pack_occupancy: N = {N} outside [2, 1625]")
-    ws = _workspace(nbytes, s.device)
+    ws = _lib.workspace(nbytes, s.device)
     bits = torch.empty(((N - 1) ** 3 + 31) // 32, dtype=torch.int32, device=s.device)
     _lib.call("nerfb200_occupancy_pack", s.device, s.data_ptr(), N, float(sigma_threshold), int(dilate), ws.data_ptr(),
               ws.numel(), bits.data_ptr())
@@ -151,7 +140,7 @@ def cull_rays(rays: torch.Tensor, occupancy: OccupancyGrid, return_flag: bool = 
     the per-ray uint8 flag.  Synchronises (the number of live rays sizes the outputs)."""
     r = _check_rays(rays, occupancy)
     dev, n = r.device, r.shape[0]
-    ws = _workspace(_lib.load().nerfb200_cull_workspace_bytes(n), dev)
+    ws = _lib.workspace(_lib.load().nerfb200_cull_workspace_bytes(n), dev)
     flag = torch.empty(n, dtype=torch.uint8, device=dev)
     n_live = ctypes.c_int64()
     _lib.call("nerfb200_cull_count", dev, r.data_ptr(), n, occupancy.bits.data_ptr(), occupancy.N,

@@ -25,13 +25,6 @@ from .nerf import Embedding, packed_weights
 from .rendering import render_rays
 
 
-def _ranges(x_range, y_range, z_range):
-    vals = [float(v) for r in (x_range, y_range, z_range) for v in r]
-    if len(vals) != 6:
-        raise ValueError("x_range, y_range and z_range must each be (min, max)")
-    return (ctypes.c_double * 6)(*vals)
-
-
 def _device_of(model: torch.nn.Module) -> torch.device:
     dev = next(model.parameters()).device
     if dev.type != "cuda":
@@ -45,10 +38,6 @@ def _cuda(t: torch.Tensor, what: str) -> torch.Tensor:
     return t
 
 
-def _workspace(nbytes: int, device) -> torch.Tensor:
-    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
-
-
 @torch.no_grad()
 def grid_positions(N: int, x_range, y_range, z_range, start: int = 0, count: Optional[int] = None,
                    device=None) -> torch.Tensor:
@@ -57,7 +46,8 @@ def grid_positions(N: int, x_range, y_range, z_range, start: int = 0, count: Opt
     device = torch.device("cuda") if device is None else torch.device(device)
     count = N ** 3 - start if count is None else count
     out = torch.empty(count, 3, dtype=torch.float32, device=device)
-    _lib.call("nerfb200_grid_positions", device, N, _ranges(x_range, y_range, z_range), start, count, out.data_ptr())
+    _lib.call("nerfb200_grid_positions", device, N, _lib.ranges_host(x_range, y_range, z_range), start, count,
+              out.data_ptr())
     return out
 
 
@@ -70,9 +60,9 @@ def sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk:
     out = torch.empty(N, N, N, dtype=torch.float32, device=dev)
     blob = packed_weights(model)
     chunk = int(min(chunk, N ** 3))
-    ws = _workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
-    _lib.call("nerfb200_sigma_grid", dev, blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk, ws.data_ptr(),
-              ws.numel(), out.data_ptr())
+    ws = _lib.workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
+    _lib.call("nerfb200_sigma_grid", dev, blob.data_ptr(), N, _lib.ranges_host(x_range, y_range, z_range), chunk,
+              ws.data_ptr(), ws.numel(), out.data_ptr())
     return out
 
 
@@ -88,7 +78,7 @@ def marching_cubes(sigma: torch.Tensor, threshold: float) -> Tuple[torch.Tensor,
     nbytes = _lib.load().nerfb200_mc_workspace_bytes(n0, n1, n2)
     if nbytes == 0:
         raise ValueError(f"marching_cubes: unsupported grid shape {tuple(s.shape)}")
-    ws = _workspace(nbytes, s.device)
+    ws = _lib.workspace(nbytes, s.device)
     counts = (ctypes.c_int64 * 2)()
     _lib.call("nerfb200_mc_count", s.device, s.data_ptr(), n0, n1, n2, float(threshold), ws.data_ptr(), ws.numel(),
               counts)
@@ -105,8 +95,8 @@ def to_world(vertices: torch.Tensor, N: int, x_range, y_range, z_range) -> torch
     x / y ranges (x takes y_range)."""
     v = _cuda(vertices, "vertices").detach().to(torch.float64).contiguous()
     out = torch.empty(v.shape[0], 3, dtype=torch.float32, device=v.device)
-    _lib.call("nerfb200_mesh_to_world", v.device, v.data_ptr(), v.shape[0], N, _ranges(x_range, y_range, z_range),
-              out.data_ptr())
+    _lib.call("nerfb200_mesh_to_world", v.device, v.data_ptr(), v.shape[0], N,
+              _lib.ranges_host(x_range, y_range, z_range), out.data_ptr())
     return out
 
 
@@ -118,7 +108,7 @@ def keep_largest_cluster(vertices: torch.Tensor, triangles: torch.Tensor) -> Tup
     t = _cuda(triangles, "triangles").detach().to(torch.int32).contiguous()
     if t.shape[0] == 0:
         return v[:0], t[:0]
-    ws = _workspace(_lib.load().nerfb200_mesh_cluster_workspace_bytes(v.shape[0], t.shape[0]), v.device)
+    ws = _lib.workspace(_lib.load().nerfb200_mesh_cluster_workspace_bytes(v.shape[0], t.shape[0]), v.device)
     counts = (ctypes.c_int64 * 2)()
     _lib.call("nerfb200_mesh_cluster_count", v.device, t.data_ptr(), t.shape[0], v.shape[0], ws.data_ptr(), ws.numel(),
               counts)
@@ -244,7 +234,7 @@ def vertex_normals(vertices: torch.Tensor, triangles: torch.Tensor) -> torch.Ten
     if nbytes == 0:
         raise ValueError(f"vertex_normals: unsupported mesh size (V = {n_v}, T = {n_t})")
     out = torch.empty(n_v, 3, dtype=torch.float64, device=v.device)
-    ws = _workspace(nbytes, v.device)
+    ws = _lib.workspace(nbytes, v.device)
     _lib.call("nerfb200_vertex_normals", v.device, v.data_ptr(), n_v, t.data_ptr(), n_t, ws.data_ptr(), ws.numel(),
               out.data_ptr())
     return out
@@ -309,8 +299,8 @@ def rgb_sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, ch
     out = torch.empty(N, N, N, 4, dtype=torch.float32, device=dev)
     blob = packed_weights(model)
     chunk = int(min(chunk, N ** 3))
-    ws = _workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
-    _lib.call("nerfb200_rgb_sigma_grid", dev, blob.data_ptr(), N, _ranges(x_range, y_range, z_range), chunk,
+    ws = _lib.workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
+    _lib.call("nerfb200_rgb_sigma_grid", dev, blob.data_ptr(), N, _lib.ranges_host(x_range, y_range, z_range), chunk,
               ws.data_ptr(), ws.numel(), out.data_ptr())
     return out
 
@@ -330,7 +320,7 @@ def pack_volume(rgbsigma: torch.Tensor, x_range) -> torch.Tensor:
     nbytes = _lib.load().nerfb200_volume_workspace_bytes(N)
     if nbytes == 0:
         raise ValueError(f"pack_volume: N = {N} outside [2, 1625]")
-    ws = _workspace(nbytes, g.device)
+    ws = _lib.workspace(nbytes, g.device)
     count = ctypes.c_int64()
     _lib.call("nerfb200_volume_count", g.device, g.data_ptr(), N, xmin, xmax, ws.data_ptr(), ws.numel(),
               ctypes.byref(count))

@@ -27,37 +27,40 @@ def test_header_symbols_exported(lib):
     declared = set(re.findall(r"\b(nerfb200_[a-z_0-9]+)\s*\(", hdr))
     declared -= {"nerfb200_render_args", "nerfb200_backward_args"}
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
+    assert "#define NERFB200_ABI_VERSION 3" in hdr
     for name in declared:
         assert hasattr(lib, name), name
 
 
 def _header_prototypes():
-    """{name: (return type, [argument declarations])} of every function include/nerf_pl_b200.h declares."""
+    """[(name, return type, [argument declarations])] of every function include/nerf_pl_b200.h declares, in order."""
     hdr = open(os.path.join(ROOT, "include", "nerf_pl_b200.h")).read()
     hdr = re.sub(r"/\*.*?\*/", " ", hdr, flags=re.S)
     hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
-    protos = {}
+    protos = []
     for decl in hdr.split(";"):
         m = re.search(r"(.*?)\b(nerfb200_\w+)\s*\((.*)\)\s*$", decl.strip(), re.S)
         if m:
             ret = " ".join(re.split(r"[{}]", m.group(1))[-1].split())
             args = [] if m.group(3).strip() == "void" else [" ".join(a.split()) for a in m.group(3).split(",")]
-            protos[m.group(2)] = (ret, args)
+            protos.append((m.group(2), ret, args))
     return protos
 
 
-def test_signature_table_matches_the_header():
-    """Every prototype of include/nerf_pl_b200.h against _lib.SIGNATURES: the same names, argument counts, argument
-    kinds and return types (a wrong width would silently corrupt the argument)."""
+def test_one_signature_table_matches_the_one_header(lib):
+    """Every prototype of include/nerf_pl_b200.h against _lib.SIGNATURES: the same names, declared once each, in the
+    same order, with the same argument counts, argument kinds and return types (a wrong width would silently corrupt
+    the argument); the loaded library's entries carry exactly those types."""
     protos = _header_prototypes()
-    assert len(protos) == 47
-    assert set(protos) == set(_lib.SIGNATURES), set(protos) ^ set(_lib.SIGNATURES)
-    assert list(protos) == list(_lib.EXPORTS)           # header order
+    names = [name for name, _, _ in protos]
+    assert len(names) == 57
+    assert len(set(names)) == len(names), sorted(n for n in names if names.count(n) > 1)
+    assert names == list(_lib.SIGNATURES) == list(_lib.EXPORTS)          # header order
     scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "size_t": ctypes.c_size_t,
                "float": ctypes.c_float, "double": ctypes.c_double}
     returns = {"int": ctypes.c_int32, "size_t": ctypes.c_size_t, "int64_t": ctypes.c_int64,
                "const char*": ctypes.c_char_p}
-    for name, (ret, args) in protos.items():
+    for name, ret, args in protos:
         restype, argtypes = _lib.SIGNATURES[name]
         assert restype is returns[ret], (name, ret, restype)
         assert len(argtypes) == len(args), (name, args, argtypes)
@@ -67,6 +70,8 @@ def test_signature_table_matches_the_header():
             else:
                 base = decl.replace("const ", "").rsplit(" ", 1)[0]
                 assert t is scalars[base], (name, decl, t)
+        fn = getattr(lib, name)
+        assert fn.restype is restype and list(fn.argtypes) == argtypes, name
 
 
 def test_call_appends_the_stream_and_maps_return_codes(monkeypatch):

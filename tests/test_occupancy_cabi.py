@@ -1,65 +1,18 @@
-"""CPU-side checks of the companion header include/nerf_pl_b200_occupancy.h (empty-space skipping at render time):
-its prototypes against _lib.OCCUPANCY_SIGNATURES, the library exports them, the main header includes it, and the
-argument checks that need no GPU."""
+"""CPU-side checks of the empty-space skipping entries: workspace sizes, the argument checks that need no GPU and the
+Python surface (their prototypes are checked with the rest of include/nerf_pl_b200.h in test_cabi.py)."""
 import ctypes
 import inspect
-import os
-import re
 
 import pytest
 
 import nerf_pl_b200 as nb
 from nerf_pl_b200 import _lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "nerf_pl_b200_occupancy.h")
-NEW = ("nerfb200_occupancy_workspace_bytes", "nerfb200_occupancy_pack", "nerfb200_occupancy_popcount",
-       "nerfb200_cull_workspace_bytes", "nerfb200_cull_count", "nerfb200_cull_emit", "nerfb200_scatter_results")
-
 
 @pytest.fixture(scope="module")
 def lib():
     _lib.build()
     return _lib.load()
-
-
-def _prototypes(path):
-    hdr = re.sub(r"/\*.*?\*/", " ", open(path).read(), flags=re.S)
-    hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
-    protos = {}
-    for decl in hdr.split(";"):
-        m = re.search(r"(.*?)\b(nerfb200_\w+)\s*\((.*)\)\s*$", decl.strip(), re.S)
-        if m:
-            ret = " ".join(re.split(r"[{}]", m.group(1))[-1].split())
-            protos[m.group(2)] = (ret, [" ".join(a.split()) for a in m.group(3).split(",")])
-    return protos
-
-
-def test_every_new_symbol_is_declared_exported_and_typed(lib):
-    protos = _prototypes(HEADER)
-    assert tuple(protos) == NEW == tuple(_lib.OCCUPANCY_SIGNATURES)
-    assert not set(protos) & (set(_lib.SIGNATURES) | set(_lib.MESH_NORMALS_SIGNATURES))
-    assert _lib.HEADER_SIGNATURES["nerf_pl_b200_occupancy.h"] is _lib.OCCUPANCY_SIGNATURES
-    scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "size_t": ctypes.c_size_t,
-               "double": ctypes.c_double}
-    returns = {"int": ctypes.c_int32, "size_t": ctypes.c_size_t}
-    for name, (ret, args) in protos.items():
-        restype, argtypes = _lib.OCCUPANCY_SIGNATURES[name]
-        assert restype is returns[ret], name
-        assert len(argtypes) == len(args), name
-        for decl, t in zip(args, argtypes):
-            if "*" in decl or "[" in decl:
-                assert t is ctypes.c_void_p or issubclass(t, ctypes._Pointer), (name, decl)
-            else:
-                assert t is scalars[decl.replace("const ", "").rsplit(" ", 1)[0]], (name, decl)
-        fn = getattr(lib, name)
-        assert fn.restype is restype and list(fn.argtypes) == argtypes
-
-
-def test_main_header_includes_the_companion_and_keeps_its_version():
-    main = open(os.path.join(ROOT, "include", "nerf_pl_b200.h")).read()
-    assert '#include "nerf_pl_b200_occupancy.h"' in main
-    assert "#define NERFB200_ABI_VERSION 3" in main
 
 
 def test_occupancy_pack_argument_checks(lib):
