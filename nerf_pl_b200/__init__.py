@@ -9,6 +9,7 @@ from .data import DeviceRayBatches
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
 from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, normal_rays, normal_vertex_colors, pack_volume,
                    query_rgb_sigma, rgb_sigma_grid, sigma_grid, vertex_normals, write_ply, write_vol)
+from .metrics import ssim, visualize_depth
 from .optim import FusedAdam
 from .rendering import render_rays, render_rays_host, render_rays_loss, sample_pdf, searchsorted, volume_render
 from .training import CapturedTrainStep, nerf_forward_train
@@ -21,5 +22,6 @@ __all__ = [
     "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
     "vertex_normals", "normal_rays", "normal_vertex_colors",
     "OccupancyGrid", "occupancy_grid", "pack_occupancy", "cull_rays", "scatter_results", "render_rays_culled",
+    "ssim", "visualize_depth",
 ]
 __version__ = "0.1.0"

@@ -22,7 +22,8 @@ if os.environ.get("NERFB200_LIB"):          # a library built elsewhere (e.g. wi
     LIB_PATH = os.path.abspath(os.environ["NERFB200_LIB"])
 SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
-           "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh"]
+           "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h"]
+INCLUDES = ["nerf_pl_b200.h", "nerf_pl_b200_metrics.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -161,6 +162,14 @@ SIGNATURES = {
 }
 EXPORTS = tuple(SIGNATURES)     # tests check the library exports all of them
 
+# The entries of the companion header include/nerf_pl_b200_metrics.h, in header order (its own tests check it).
+METRICS_SIGNATURES = {
+    "nerfb200_ssim_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64]),
+    "nerfb200_ssim": (_i32, [_vp, POINTER(_i64), _vp, POINTER(_i64), _i64, _i64, _i64, _i64, _i32, _vp, _sz, _vp, _vp]),
+    "nerfb200_visualize_depth_workspace_bytes": (_sz, [_i64, _i64]),
+    "nerfb200_visualize_depth": (_i32, [_vp, _i64, _i64, _i64, _i64, _vp, _sz, _vp, _vp]),
+}
+
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
@@ -173,7 +182,7 @@ def needs_build() -> bool:
     if not os.path.exists(LIB_PATH):
         return True
     t = os.path.getmtime(LIB_PATH)
-    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS] + [os.path.join(_HERE, "..", "include", "nerf_pl_b200.h")]
+    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS] + [os.path.join(_HERE, "..", "include", f) for f in INCLUDES]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
@@ -207,7 +216,7 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (restype, argtypes) in SIGNATURES.items():
+            for name, (restype, argtypes) in (*SIGNATURES.items(), *METRICS_SIGNATURES.items()):
                 fn = getattr(lib, name)
                 fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:

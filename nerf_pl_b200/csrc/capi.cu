@@ -11,10 +11,12 @@
 #include <vector>
 
 #include "../../include/nerf_pl_b200.h"
+#include "../../include/nerf_pl_b200_metrics.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
 #include "occupancy_kernels.cuh"
+#include "metrics_kernels.cuh"
 
 #include <thrust/iterator/transform_iterator.h>
 
@@ -866,6 +868,33 @@ int cull_prepare(const float* rays, int64_t n, void* ws, size_t bytes, CullParam
   p->rays = rays; p->n = n;
   p->bits = nullptr; p->flag = nullptr; p->live_idx = nullptr; p->live_rays = nullptr;
   return 0;
+}
+
+// ------------------------------------------------------------------ image metrics (kernels: metrics_kernels.cuh)
+
+// The product of `k` extents, each >= 1, or -1 when one is < 1 or the product exceeds 2^48 elements.
+long long image_elems(const int64_t* ext, int k) {
+  long long n = 1;
+  for (int a = 0; a < k; ++a) {
+    if (ext[a] < 1 || ext[a] > (1LL << 48) / n) return -1;
+    n *= ext[a];
+  }
+  return n;
+}
+
+// The SSIM workspace of n pixels: one double per tile.
+size_t ssim_carve(long long n, void* base, double** partial) {
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  *partial = c.take<double>(ceil_div(n, kSsimTile));
+  return c.off;
+}
+
+// The visualize_depth workspace of n pixels: the (min, max) pairs of the first pass, one per block.
+int depth_minmax_blocks(long long n) { return grid_blocks(n, kDepthThreads * kDepthItemsPerThread, kDepthMinMaxCtas); }
+size_t depth_viz_carve(long long n, void* base, float2** partial) {
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  *partial = c.take<float2>(depth_minmax_blocks(n));
+  return c.off;
 }
 
 }  // namespace
@@ -1815,6 +1844,73 @@ int nerfb200_scatter_results(const float* const src_host[6], float* const dst_ho
   p.live_idx = reinterpret_cast<const long long*>(live_idx);
   p.n_live = n_live; p.n = n_rays; p.bg = white_back ? 1.f : 0.f;
   return launch("scatter_results launch", scatter_results_kernel, grid_blocks(n_rays, 256), 256, 0, stream, p);
+}
+
+// ---- image metrics (include/nerf_pl_b200_metrics.h; kernels: metrics_kernels.cuh)
+size_t nerfb200_ssim_workspace_bytes(int64_t b, int64_t c, int64_t h, int64_t w) {
+  const int64_t ext[4] = {b, c, h, w};
+  const long long n = image_elems(ext, 4);
+  double* partial;
+  return n < 0 ? 0 : ssim_carve(n, nullptr, &partial);
+}
+
+int nerfb200_ssim(const float* pred, const int64_t pred_strides_host[4], const float* gt,
+                  const int64_t gt_strides_host[4], int64_t b, int64_t c, int64_t h, int64_t w, int32_t reduction,
+                  void* ws, size_t bytes, float* out, void* stream) {
+  const int64_t ext[4] = {b, c, h, w};
+  const long long n = image_elems(ext, 4);
+  if (n < 0) return fail(NERFB200_EINVAL, "ssim: b, c, h and w must be >= 1 (and at most 2^48 pixels)");
+  if (reduction != NERFB200_SSIM_MEAN && reduction != NERFB200_SSIM_SUM && reduction != NERFB200_SSIM_NONE)
+    return fail(NERFB200_EINVAL, "ssim: reduction must be NERFB200_SSIM_MEAN, _SUM or _NONE");
+  if (!pred || !gt || !pred_strides_host || !gt_strides_host || !out) return fail(NERFB200_EINVAL, "ssim: NULL argument");
+  SsimParams p;
+  for (int a = 0; a < 4; ++a) {
+    if (pred_strides_host[a] < 0 || gt_strides_host[a] < 0) return fail(NERFB200_EINVAL, "ssim: negative stride");
+    p.xs[a] = pred_strides_host[a];
+    p.ys[a] = gt_strides_host[a];
+  }
+  p.x = pred; p.y = gt; p.C = c; p.H = h; p.W = w; p.n = n;
+  // kornia's window: exp(-x^2 / (2 sigma^2)) at x = -1, 0, 1 with sigma = 1.5, normalised to sum 1
+  const double e = std::exp(-1.0 / (2.0 * 1.5 * 1.5));
+  p.g[0] = e / (1.0 + 2.0 * e);
+  p.g[1] = 1.0 / (1.0 + 2.0 * e);
+  p.map = nullptr; p.partial = nullptr;
+  const long long tiles = ceil_div(n, kSsimTile);
+  if (reduction == NERFB200_SSIM_NONE) {
+    p.map = out;
+    return launch("ssim launch", ssim_kernel, grid_blocks(tiles, 1), kSsimTile, 0, stream, p);
+  }
+  if (!ws) return fail(NERFB200_EINVAL, "ssim: NULL workspace");
+  if (bytes < ssim_carve(n, ws, &p.partial))
+    return fail(NERFB200_EINVAL, "ssim: workspace smaller than nerfb200_ssim_workspace_bytes");
+  TRY(launch("ssim launch", ssim_kernel, grid_blocks(tiles, 1), kSsimTile, 0, stream, p));
+  const double denom = reduction == NERFB200_SSIM_MEAN ? static_cast<double>(n) : 1.0;
+  return launch("ssim finish launch", ssim_finish_kernel, 1, kSsimFinishThreads, 0, stream, p.partial, tiles, denom,
+                out);
+}
+
+size_t nerfb200_visualize_depth_workspace_bytes(int64_t h, int64_t w) {
+  const int64_t ext[2] = {h, w};
+  const long long n = image_elems(ext, 2);
+  float2* partial;
+  return n < 0 ? 0 : depth_viz_carve(n, nullptr, &partial);
+}
+
+int nerfb200_visualize_depth(const float* depth, int64_t h, int64_t w, int64_t stride_h, int64_t stride_w, void* ws,
+                             size_t bytes, float* out, void* stream) {
+  const int64_t ext[2] = {h, w};
+  const long long n = image_elems(ext, 2);
+  if (n < 0) return fail(NERFB200_EINVAL, "visualize_depth: h and w must be >= 1 (and at most 2^48 pixels)");
+  if (stride_h < 0 || stride_w < 0) return fail(NERFB200_EINVAL, "visualize_depth: negative stride");
+  if (!depth || !ws || !out) return fail(NERFB200_EINVAL, "visualize_depth: NULL argument");
+  DepthVizParams p;
+  if (bytes < depth_viz_carve(n, ws, &p.partial))
+    return fail(NERFB200_EINVAL, "visualize_depth: workspace smaller than nerfb200_visualize_depth_workspace_bytes");
+  p.depth = depth; p.H = h; p.W = w; p.sh = stride_h; p.sw = stride_w; p.out = out;
+  p.n_partial = depth_minmax_blocks(n);
+  TRY(launch("visualize_depth min/max launch", depth_minmax_kernel, p.n_partial, kDepthThreads, 0, stream, p));
+  return launch("visualize_depth colour launch", depth_color_kernel, grid_blocks(n, kDepthThreads), kDepthThreads, 0,
+                stream, p);
 }
 
 }  // extern "C"
