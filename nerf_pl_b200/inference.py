@@ -114,7 +114,15 @@ def mse_psnr(results: Dict[str, torch.Tensor], targets: torch.Tensor) -> Dict[st
     Returns {'loss': mse_coarse (+ mse_fine), 'psnr': of rgb_fine if present else rgb_coarse}."""
     rc, rf = results.get("rgb_coarse"), results.get("rgb_fine")
     ref = rf if rf is not None else rc
-    if ref is None or not ref.is_cuda:
+    if ref is None:
+        raise ValueError("results must hold CUDA rgb_coarse and/or rgb_fine")
+    # the C entry takes its row count from targets: every shape is checked here, before anything is launched
+    if targets.dim() != 2 or targets.shape[1] != 3:
+        raise ValueError(f"targets must be (N_rays, 3), got {tuple(targets.shape)}")
+    for name, v in (("rgb_coarse", rc), ("rgb_fine", rf)):
+        if v is not None and v.shape != targets.shape:
+            raise ValueError(f"{name} must have the shape of targets {tuple(targets.shape)}, got {tuple(v.shape)}")
+    if not ref.is_cuda:
         raise ValueError("results must hold CUDA rgb_coarse and/or rgb_fine")
     t = targets.detach().to(torch.float32).contiguous()
     out = torch.empty(4, dtype=torch.float32, device=ref.device)

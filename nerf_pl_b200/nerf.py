@@ -163,8 +163,10 @@ class Embedding(nn.Module):
         self.logscale = logscale
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        # embed_kernel reads (n, 3) rows and takes at most 16 frequencies; every other input goes through torch ops
         fused = (x.is_cuda and self.logscale and self.in_channels == 3 and x.dtype == torch.float32
-                 and x.dim() == 2 and not (torch.is_grad_enabled() and x.requires_grad))
+                 and x.dim() == 2 and x.shape[-1] == 3 and self.N_freqs <= 16
+                 and not (torch.is_grad_enabled() and x.requires_grad))
         if fused:
             xc = x.contiguous()
             out = torch.empty(xc.shape[0], self.out_channels, dtype=torch.float32, device=x.device)

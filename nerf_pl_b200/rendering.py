@@ -96,12 +96,17 @@ def sample_pdf(bins: torch.Tensor, weights: torch.Tensor, N_importance: int, det
     ``u`` may be given to reproduce a specific random draw."""
     if abs(eps - 1e-5) > 1e-12:
         raise ValueError("nerf_pl_b200.sample_pdf implements the reference default eps=1e-5")
+    # the C entry gets only sizes: every shape is checked here, before anything is launched
+    if weights.dim() != 2:
+        raise ValueError("weights must be (N_rays, N_samples_)")
+    n_rays, n_w = weights.shape
+    if tuple(bins.shape) != (n_rays, n_w + 1):
+        raise ValueError("bins must be (N_rays, N_samples_+1)")
+    if u is not None and tuple(u.shape) != (n_rays, N_importance):
+        raise ValueError(f"u must be (N_rays, N_importance) = ({n_rays}, {N_importance}), got {tuple(u.shape)}")
     if not bins.is_cuda:
         raise RuntimeError("nerf_pl_b200.sample_pdf runs on CUDA tensors only (no CPU fallback)")
     _require_fp32("sample_pdf", bins, weights, u)
-    n_rays, n_w = weights.shape
-    if bins.shape != (n_rays, n_w + 1):
-        raise ValueError("bins must be (N_rays, N_samples_+1)")
     if u is None:
         if det:
             u = torch.linspace(0, 1, N_importance, device=bins.device).expand(n_rays, N_importance)
@@ -120,10 +125,17 @@ def volume_render(sigmas: torch.Tensor, rgbs: Optional[torch.Tensor], z_vals: to
                   white_back: bool = False):
     """Alpha-compositing quadrature (reference models/rendering.py:143-170).
     Returns (weights, rgb | None, depth | None, opacity)."""
+    # the C entry gets only sizes: every shape is checked here, before anything is launched
+    if sigmas.dim() != 2:
+        raise ValueError("sigmas must be (N_rays, N_samples)")
+    n, S = sigmas.shape
+    for name, t, shape in (("rgbs", rgbs, (n, S, 3)), ("z_vals", z_vals, (n, S)), ("dirs", dirs, (n, 3)),
+                           ("noise", noise, (n, S))):
+        if t is not None and tuple(t.shape) != shape:
+            raise ValueError(f"{name} must be {shape} for sigmas of shape {(n, S)}, got {tuple(t.shape)}")
     if not sigmas.is_cuda:
         raise RuntimeError("nerf_pl_b200.volume_render runs on CUDA tensors only (no CPU fallback)")
     _require_fp32("volume_render", sigmas, rgbs, z_vals, dirs, noise)
-    n, S = sigmas.shape
     dev = sigmas.device
     f32 = dict(dtype=torch.float32, device=dev)
     weights = torch.empty(n, S, **f32)

@@ -113,11 +113,18 @@ def nerf_forward(w: Dict[str, np.ndarray], x: np.ndarray, sigma_only: bool = Fal
 # ------------------------------------------------------------------ torchsearchsorted
 def searchsorted(a: np.ndarray, v: np.ndarray, side: str = "left") -> np.ndarray:
     """Row-wise np.searchsorted with single-row broadcasting
-    (torchsearchsorted/src/torchsearchsorted/utils.py:4-15, searchsorted.py:23-35)."""
+    (torchsearchsorted/src/torchsearchsorted/utils.py:4-15, searchsorted.py:23-35).  A NaN in ``v`` gives 0, as the
+    reference's CUDA kernel gives it (every comparison with NaN is false, so its search ends left of a[0]); numpy
+    itself sorts NaN above +inf."""
     nrow = max(a.shape[0], v.shape[0])
     out = np.empty((nrow, v.shape[1]), dtype=np.int64)
-    for r in range(nrow):
-        out[r] = np.searchsorted(a[0 if a.shape[0] == 1 else r], v[0 if v.shape[0] == 1 else r], side=side)
+    if a.shape[0] == 1:                 # one sorted row for every query: one call
+        res = np.searchsorted(a[0], v.reshape(-1), side=side).reshape(v.shape)
+        out[:] = res
+    else:
+        for r in range(nrow):
+            out[r] = np.searchsorted(a[r], v[0 if v.shape[0] == 1 else r], side=side)
+    out[np.broadcast_to(np.isnan(v), out.shape)] = 0
     return out
 
 

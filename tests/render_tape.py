@@ -239,6 +239,41 @@ def composite64(sigma, z, dirs, rgb=None, noise=None, noise_std=0.0, white_back=
     return w, c, (w * zz).sum(1), opac
 
 
+def composite_errors(sig, rgb, z, d, noise, noise_std, white_back, w, c, dp, op) -> dict:
+    """The device's volume_render outputs w (R, S), c (R, 3) | None, dp (R) | None, op (R) against float64 on its
+    inputs: weights in units of weight_units(S) against composite64 (the last sample apart), opacity / rgb / depth in
+    units of sum_bar_units against float64 sums of the device's own weights.  Returns {metric: worst value}; compare
+    with BARS["weights"], BARS["weights_last"] and BARS["sums"]."""
+    S = np.asarray(sig).shape[1]
+    w64, _, _, _ = composite64(sig, z, d, None, noise, noise_std)
+    dw = np.abs(np.asarray(w, F64) - w64) / weight_units(S)
+    wd = np.asarray(w, F64)
+    opac = wd.sum(1)
+    e = {"weights": float(dw[:, :-1].max()) if S > 1 else 0.0, "weights_last": float(dw[:, -1].max()),
+         "opacity": float((np.abs(op - opac) / sum_bar_units(S, np.abs(wd).sum(1))).max())}
+    if c is not None:
+        col = (wd[..., None] * rgb).sum(1)
+        absc = np.abs(wd[..., None] * rgb).sum(1)
+        extra = 0.0
+        if white_back:
+            col, absc = col + (1 - opac)[:, None], absc + np.abs(wd).sum(1)[:, None]
+            extra = 2 * U32 * (np.abs(col) + 1)
+        e["rgb"] = float((np.abs(c - col) / sum_bar_units(S, absc, extra)).max())
+        e["depth"] = float((np.abs(dp - (wd * np.asarray(z, F64)).sum(1))
+                            / sum_bar_units(S, np.abs(wd * np.asarray(z, F64)).sum(1))).max())
+    return e
+
+
+def composite_violations(e: dict) -> list:
+    """The metrics of `composite_errors` above their BARS."""
+    bad = []
+    for k, v in e.items():
+        bar = BARS["weights_last" if k == "weights_last" else "weights" if k == "weights" else "sums"]
+        if not v <= bar:
+            bad.append(f"{k}: {v:.3g} > {bar}")
+    return bad
+
+
 def check_resampling(z_dev, w_coarse, z_coarse, u, defect: Optional[str] = None) -> dict:
     """The fine depths z_dev (R, S + K) the kernel returned, against `z_fine` on its own coarse weights and depths
     (bitwise), and the emulated new depths against `sample_pdf64`.  Returns {'differ': elements of z_dev that are not

@@ -384,22 +384,8 @@ def test_volume_render_vs_float64(S, noise_std, wb, dev):
     T = lambda a: None if a is None else torch.from_numpy(a).to(dev)
     w, c, dp, op = [x.cpu().numpy() for x in nb.volume_render(T(sig), T(rgb), T(z), T(d), T(nz), noise_std, wb)]
     w64, _, _, _ = rt.composite64(sig, z, d, None, nz, noise_std)
-    dw = np.abs(w - w64) / rt.weight_units(S)
-    wd = w.astype(F64)
-    opac = wd.sum(1)
-    col = (wd[..., None] * rgb).sum(1)
-    absc = np.abs(wd[..., None] * rgb).sum(1)
-    extra = 0.0
-    if wb:
-        col, absc = col + (1 - opac)[:, None], absc + wd.sum(1)[:, None]
-        extra = 2 * U32 * (np.abs(col) + 1)
-    e = {"weights": float(dw[:, :-1].max()), "weights_last": float(dw[:, -1].max()),
-         "opacity": float((np.abs(op - opac) / rt.sum_bar_units(S, wd.sum(1))).max()),
-         "rgb": float((np.abs(c - col) / rt.sum_bar_units(S, absc, extra)).max()),
-         "depth": float((np.abs(dp - (wd * z).sum(1)) / rt.sum_bar_units(S, np.abs(wd * z).sum(1))).max())}
+    e = rt.composite_errors(sig, rgb, z, d, nz, noise_std, wb, w, c, dp, op)
     print(f"\nvolume_render S {S} noise {noise_std}: " + " ".join(f"{k} {v:.3g}" for k, v in e.items()))
     assert np.all(np.isfinite(w)) and w[0, 0] == 1 and np.all(w[1] == 0)
     np.testing.assert_allclose(op, w64.sum(1), rtol=0, atol=S * 4 * U32)     # weights sum to the opacity
-    for k, v in e.items():
-        bar = rt.BARS["weights_last" if k == "weights_last" else "weights" if k == "weights" else "sums"]
-        assert v <= bar, (k, v)
+    assert not rt.composite_violations(e), rt.composite_violations(e)
