@@ -224,8 +224,8 @@ int nerfb200_nerf_forward_train(const float* x, int64_t n, int64_t x_stride, con
  * params: the live 24 fp32 parameters (state_dict order); writes the 24 gradient tensors `grads`
  * (overwritten, not accumulated).  All kernels are sm_90a code on `stream`: gradient seed, rgb head,
  * wgmma dgrad chain, wgmma split-K wgrad (with the direction slice of dir_encoding), reduction,
- * unfolding.  A per-sample gradient outside its layer's fp16 range is reported like the render
- * backward's (status 102: nerfb200_check_status / the next call). */
+ * unfolding.  A per-sample gradient outside its layer's fp16 range (status 102) or not finite (status 103)
+ * is reported like the render backward's (nerfb200_check_status / the next call). */
 int nerfb200_nerf_backward(const float* g_out, int64_t n, const void* packed, const float* const params[24], void* ws,
                            float* const grads[24], void* stream);
 

@@ -78,6 +78,7 @@ struct CompBwdParams {
   float* dsigma;
   float* dprergb;
   unsigned* amax_bits;      // [2]: max |d sigma|, max |d rgb_pre| as float bits (scale selection) or null
+  int* status;              // device status word: 103 when a per-sample gradient is not finite
 };
 
 __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompBwdParams p) {
@@ -86,6 +87,7 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompBwdParams 
   const long long ray = static_cast<long long>(blockIdx.x) * wpb + (threadIdx.x >> 5);
   const int S = p.S, P = S >> 5;
   float amax = 0.f, amax_rgb = 0.f;
+  bool nonfinite = false;
   if (ray < p.n_rays) {
     const float* rr = p.rays + ray * p.ray_stride;
     const float dx = rr[3], dy = rr[4], dz = rr[5];
@@ -153,15 +155,20 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompBwdParams 
       const float ds = pos[q] ? dalpha * de[q] : 0.f;
       p.dsigma[g0 + i] = ds;
       amax = fmaxf(amax, fabsf(ds));
+      nonfinite |= !isfinite(ds);
       const float* c = p.rgb + (g0 + i) * 3;
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) {
         const float dp = wgt[q] * g[ch] * c[ch] * (1.f - c[ch]);
         p.dprergb[(g0 + i) * 3 + ch] = dp;
         amax_rgb = fmaxf(amax_rgb, fabsf(dp));
+        nonfinite |= !isfinite(dp);
       }
     }
   }
+  // A non-finite ray, colour or upstream gradient: the reference's gradients are NaN everywhere, but fmaxf above
+  // drops NaN and the wgrad sums of the biases never see it, so say so instead of returning finite bias gradients.
+  if (__any_sync(0xffffffffu, nonfinite) && lane == 0) report_fault(p.status, 103);
   // padding rows carry no gradient
   const long long n = static_cast<long long>(p.n_rays) * S;
   if (blockIdx.x == gridDim.x - 1)
@@ -192,10 +199,12 @@ struct MlpSeedParams {
   float* dsigma;            // (n_pad)
   float* dprergb;           // (n_pad, 3)
   unsigned* amax_bits;      // [2]: max |d sigma|, max |d rgb_pre| as float bits
+  int* status;              // device status word: 103 when a per-sample gradient is not finite
 };
 __global__ void __launch_bounds__(256) mlp_seed_kernel(const MlpSeedParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   float amax = 0.f, amax_rgb = 0.f;
+  bool nonfinite = false;
   if (i < p.n) {
     const float4 g = __ldg(reinterpret_cast<const float4*>(p.g) + i);
     const float gc[3] = {g.x, g.y, g.z};
@@ -205,9 +214,11 @@ __global__ void __launch_bounds__(256) mlp_seed_kernel(const MlpSeedParams p) {
       const float dp = gc[ch] * c * (1.f - c);
       p.dprergb[i * 3 + ch] = dp;
       amax_rgb = fmaxf(amax_rgb, fabsf(dp));
+      nonfinite |= !isfinite(dp);
     }
     p.dsigma[i] = g.w;
     amax = fabsf(g.w);
+    nonfinite |= !isfinite(g.w);
   } else if (i < p.n_pad) {
     p.dsigma[i] = 0.f;
     p.dprergb[3 * i] = 0.f; p.dprergb[3 * i + 1] = 0.f; p.dprergb[3 * i + 2] = 0.f;
@@ -218,6 +229,7 @@ __global__ void __launch_bounds__(256) mlp_seed_kernel(const MlpSeedParams p) {
     amax_rgb = fmaxf(amax_rgb, __shfl_xor_sync(0xffffffffu, amax_rgb, o));
   }
   const int lane = threadIdx.x & 31;
+  if (__any_sync(0xffffffffu, nonfinite) && lane == 0) report_fault(p.status, 103);   // as composite_bwd_kernel
   if (lane == 0 && amax > 0.f && amax < 3e38f) atomicMax(p.amax_bits, __float_as_uint(amax));
   if (lane == 0 && amax_rgb > 0.f && amax_rgb < 3e38f) atomicMax(p.amax_bits + 1, __float_as_uint(amax_rgb));
 }

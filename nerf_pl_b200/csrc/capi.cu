@@ -159,7 +159,8 @@ int device_info(DeviceInfo** out) {
 }
 
 // A kernel of an EARLIER call on this device reported a device-side fault (misaligned shared
-// memory, code 101; a training backward whose per-sample gradients overflowed fp16, code 102)
+// memory, code 101; a training backward whose per-sample gradients overflowed fp16, code 102; one whose per-sample
+// gradients were not finite, code 103)
 // through the internal status word: surface it on this call and clear it.
 // (The word lives in mapped pinned host memory, so this is a plain host read, no synchronisation;
 // callers that want the fault of THIS call pass their own `status` word or call
@@ -172,6 +173,9 @@ int check_sticky_status(DeviceInfo* d) {
   if (st == 102)
     return fail(NERFB200_EDEVICE, "an earlier training backward reported device status 102: a per-sample "
                 "gradient exceeded the fp16 range of its layer's scale, its weight gradients are wrong");
+  if (st == 103)
+    return fail(NERFB200_EDEVICE, "an earlier training backward reported device status 103: a per-sample gradient "
+                "was not finite (a non-finite ray, input, output or upstream gradient), its weight gradients are wrong");
   return fail(NERFB200_EDEVICE, "an earlier nerf_pl_b200 kernel reported device status %d", st);
 }
 
@@ -1247,6 +1251,7 @@ int nerfb200_nerf_backward(const float* g_out, int64_t n, const void* packed, co
   sd.n = n; sd.n_pad = pb.n_pad;
   sd.g = g_out; sd.rgb = pb.rgb; sd.dsigma = pb.dsigma; sd.dprergb = pb.dprergb;
   sd.amax_bits = L.amax;
+  sd.status = d->status;
   const char* what = "nerf_backward launches";
   TRY(launch(what, mlp_seed_kernel, static_cast<int>(ceil_div(pb.n_pad, 256)), 256, 0, stream, sd));
   const float* const* const p2[2] = {params, params};
@@ -1395,6 +1400,7 @@ int nerfb200_render_backward(const nerfb200_backward_args* b, void* stream_v) {
     cp.rgb_out = rgb_out[ps]; cp.target = b->target; cp.loss_grad = b->loss_grad;
     cp.dsigma = L.pass[ps].dsigma; cp.dprergb = L.pass[ps].dprergb;
     cp.amax_bits = L.amax + 2 * ps;
+    cp.status = d->status;
     TRY(launch(what, composite_bwd_kernel, (L.n_rays + 3) / 4, 128, 0, stream, cp));
   }
   return backward_tail(L, params, grads, net, a->rays, a->ray_stride, d, stream, what);

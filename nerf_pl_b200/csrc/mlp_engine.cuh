@@ -204,6 +204,13 @@ __device__ __forceinline__ uint32_t cvt_f16x2_relu(float lo, float hi) {
   asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
+// torch.relu in fp32: max(v, 0) that keeps a NaN (fmaxf returns 0 for it, which would hand a NaN point a finite
+// sigma / rgb made of the biases alone).  Bitwise fmaxf(v, 0.f) for every other v.
+__device__ __forceinline__ float relu_keep_nan(float v) {
+  float d;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(d) : "f"(v));
+  return d;
+}
 __device__ __forceinline__ uint32_t cvt_f16x2(float lo, float hi) {
   uint32_t d;
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
@@ -233,8 +240,8 @@ __device__ __forceinline__ void epi_hidden(WgCtx& c, int l, const float (&acc)[1
     for (int s = 0; s < 2; ++s) {
       const float v0 = acc[4 * j + 2 * s] + b.x, v1 = acc[4 * j + 2 * s + 1] + b.y;
       if (kSigma) {
-        sig[s] = fmaf(fmaxf(v0, 0.f), w.x, sig[s]);
-        sig[s] = fmaf(fmaxf(v1, 0.f), w.y, sig[s]);
+        sig[s] = fmaf(relu_keep_nan(v0), w.x, sig[s]);
+        sig[s] = fmaf(relu_keep_nan(v1), w.y, sig[s]);
       }
       if (kSave)
         mk[s][j >> 4] |= ((__float_as_uint(v0) >> 31) << (2 * (j & 15))) | ((__float_as_uint(v1) >> 31) << (2 * (j & 15) + 1));
@@ -269,8 +276,8 @@ __device__ __forceinline__ void epi_dir(WgCtx& c, const float (&acc)[128], const
 #pragma unroll
     for (int s = 0; s < 2; ++s) {
       const float2 b = *reinterpret_cast<const float2*>(dbias[s] + n);
-      const float v0 = fmaxf(acc[4 * j + 2 * s] + b.x, 0.f);
-      const float v1 = fmaxf(acc[4 * j + 2 * s + 1] + b.y, 0.f);
+      const float v0 = relu_keep_nan(acc[4 * j + 2 * s] + b.x);
+      const float v1 = relu_keep_nan(acc[4 * j + 2 * s + 1] + b.y);
       rgb[s][0] = fmaf(v1, wr.y, fmaf(v0, wr.x, rgb[s][0]));
       rgb[s][1] = fmaf(v1, wg.y, fmaf(v0, wg.x, rgb[s][1]));
       rgb[s][2] = fmaf(v1, wb.y, fmaf(v0, wb.x, rgb[s][2]));

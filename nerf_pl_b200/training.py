@@ -334,8 +334,8 @@ def nerf_forward_train(model: torch.nn.Module, x: torch.Tensor) -> torch.Tensor:
 
     Raises ``ValueError`` for what the kernels do not do: ``x.requires_grad`` (no gradient with respect to the
     input), a non-default architecture, ``x`` not of shape (B, 90); ``RuntimeError`` for CPU tensors.  A backward
-    whose per-sample gradients exceed their layer's fp16 range is reported (device status 102) by the next library
-    call or ``nerfb200_check_status``."""
+    whose per-sample gradients exceed their layer's fp16 range (device status 102), or are not finite (status 103: a
+    non-finite input or upstream gradient), is reported by the next library call or ``nerfb200_check_status``."""
     if not x.is_cuda:
         raise RuntimeError("nerf_pl_b200.nerf_forward_train runs on CUDA tensors only (no CPU fallback)")
     if x.requires_grad:

@@ -111,18 +111,21 @@ def run_case(name, dev, emb):
     return run_render(dict(DEFAULTS, **CASES[name]), 200 + list(CASES).index(name), dev, emb)
 
 
-def run_render(c, seed, dev, emb):
-    """The three renders of configuration `c` (DEFAULTS' keys) on rays and random numbers drawn from `seed`."""
+def run_render(c, seed, dev, emb, rays=None, rnd=None):
+    """The three renders of configuration `c` (DEFAULTS' keys) on rays and random numbers drawn from `seed`; `rays`
+    (n, 8) and `rnd` (numpy random tensors keyed as render_rays' randoms) replace the drawn ones when given."""
     n, S, K = c["n"], c["S"], c["K"]
-    rays = _rays(c, seed)
+    rays = _rays(c, seed) if rays is None else rays
     rs = np.random.RandomState(seed)
     target = rs.uniform(0, 1, (n, 3)).astype(F32)
     rnd_np = {}
-    if c["perturb"] > 0:
+    if rnd is not None:
+        rnd_np = dict(rnd)
+    elif c["perturb"] > 0:
         rnd_np["perturb_rand"] = rs.rand(n, S).astype(F32)
         if K:
             rnd_np["u_rand"] = rs.rand(n, K).astype(F32)
-    if c["noise_std"] > 0:
+    if c["noise_std"] > 0 and rnd is None:
         rnd_np["noise_coarse"] = rs.randn(n, S).astype(F32)
         if K:
             rnd_np["noise_fine"] = rs.randn(n, S + K).astype(F32)
