@@ -5,7 +5,7 @@ signatures, executed by hand-written wgmma (sm_90a) CUDA kernels through a C-ABI
 from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_forward_torch, nerf_parameters,
                    packed_weights)
 from .culling import OccupancyGrid, cull_rays, occupancy_grid, pack_occupancy, render_rays_culled, scatter_results
-from .data import DeviceRayBatches
+from .data import DeviceRayBatches, DeviceViewBatches
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
 from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, normal_rays, normal_vertex_colors, pack_volume,
                    query_rgb_sigma, rgb_sigma_grid, sigma_grid, vertex_normals, write_ply, write_vol)
@@ -13,6 +13,7 @@ from .metrics import ssim, visualize_depth
 from .optim import FusedAdam
 from .rendering import render_rays, render_rays_host, render_rays_loss, sample_pdf, searchsorted, volume_render
 from .training import CapturedTrainStep, nerf_forward_train
+from .views import Views, read_blender_views, read_llff_views
 
 __all__ = [
     "Embedding", "NeRF", "render_rays", "render_rays_loss", "render_rays_host", "FusedAdam", "invalidate_packed", "sample_pdf", "searchsorted", "volume_render",
@@ -23,5 +24,6 @@ __all__ = [
     "vertex_normals", "normal_rays", "normal_vertex_colors",
     "OccupancyGrid", "occupancy_grid", "pack_occupancy", "cull_rays", "scatter_results", "render_rays_culled",
     "ssim", "visualize_depth",
+    "DeviceViewBatches", "Views", "read_blender_views", "read_llff_views",
 ]
 __version__ = "0.1.0"

@@ -23,7 +23,7 @@ if os.environ.get("NERFB200_LIB"):          # a library built elsewhere (e.g. wi
 SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
            "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h"]
-INCLUDES = ["nerf_pl_b200.h", "nerf_pl_b200_metrics.h"]
+INCLUDES = ["nerf_pl_b200.h", "nerf_pl_b200_metrics.h", "nerf_pl_b200_views.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -170,6 +170,12 @@ METRICS_SIGNATURES = {
     "nerfb200_visualize_depth": (_i32, [_vp, _i64, _i64, _i64, _i64, _vp, _sz, _vp, _vp]),
 }
 
+# The entries of the companion header include/nerf_pl_b200_views.h, in header order (its own tests check it).
+VIEWS_SIGNATURES = {
+    "nerfb200_view_batch": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _f32, _f32, _f32, _i32, _vp, _i64, _vp, _vp,
+                                   _vp]),
+}
+
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
@@ -216,7 +222,8 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (restype, argtypes) in (*SIGNATURES.items(), *METRICS_SIGNATURES.items()):
+            for name, (restype, argtypes) in (*SIGNATURES.items(), *METRICS_SIGNATURES.items(),
+                                              *VIEWS_SIGNATURES.items()):
                 fn = getattr(lib, name)
                 fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:

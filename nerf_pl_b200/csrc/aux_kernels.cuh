@@ -400,6 +400,43 @@ __global__ void composite_kernel(const float* __restrict__ sigmas, const float* 
 // rotate by c2w[:, :3], normalise, origin = c2w[:, 3]) and optionally get_ndc_rays (:75-92, as
 // datasets/llff.py:236-241 applies it: near plane 1.0, then near/far columns 0/1).
 // Writes the (H*W, 8) ray rows [o, d, near, far] the renderer consumes, so rays never cross PCIe.
+//
+// pixel_ray is the per-pixel body, shared with view_batch_kernel (below): pixel (row j, column i) of an H x W view
+// with pose c2w (row-major (3, 4)) -> its ray row, written as two float4 to `out` (16-byte aligned).
+__device__ __forceinline__ void pixel_ray(int i, int j, int H, int W, float focal, const float* c2w, float near_in,
+                                          float far_in, int ndc, float* out_row) {
+  const float dx = __fdiv_rn(static_cast<float>(i) - 0.5f * W, focal);
+  const float dy = -__fdiv_rn(static_cast<float>(j) - 0.5f * H, focal);
+  const float dz = -1.f;
+  float d[3], o[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    d[r] = __fadd_rn(__fadd_rn(__fmul_rn(dx, c2w[4 * r + 0]), __fmul_rn(dy, c2w[4 * r + 1])),
+                     __fmul_rn(dz, c2w[4 * r + 2]));
+    o[r] = c2w[4 * r + 3];
+  }
+  const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
+#pragma unroll
+  for (int r = 0; r < 3; ++r) d[r] = __fdiv_rn(d[r], nrm);
+  float near = near_in, far = far_in;
+  if (ndc) {
+    const float n1 = 1.0f;                                   // llff.py:238 near plane at 1.0
+    const float tt = -__fdiv_rn(__fadd_rn(n1, o[2]), d[2]);
+#pragma unroll
+    for (int r = 0; r < 3; ++r) o[r] = __fadd_rn(o[r], __fmul_rn(tt, d[r]));
+    const float ox_oz = __fdiv_rn(o[0], o[2]), oy_oz = __fdiv_rn(o[1], o[2]);
+    const float sx = -1.f / (W / (2.f * focal)), sy = -1.f / (H / (2.f * focal));
+    const float o0 = sx * ox_oz, o1 = sy * oy_oz, o2 = 1.f + 2.f * n1 / o[2];
+    const float d0 = sx * (__fdiv_rn(d[0], d[2]) - ox_oz), d1 = sy * (__fdiv_rn(d[1], d[2]) - oy_oz);
+    const float d2 = 1.f - o2;
+    o[0] = o0; o[1] = o1; o[2] = o2; d[0] = d0; d[1] = d1; d[2] = d2;
+    near = 0.f; far = 1.f;
+  }
+  float4* out = reinterpret_cast<float4*>(out_row);
+  out[0] = make_float4(o[0], o[1], o[2], d[0]);
+  out[1] = make_float4(d[1], d[2], near, far);
+}
+
 struct RayGenParams {
   int H, W;
   float focal;
@@ -413,36 +450,67 @@ __global__ void generate_rays_kernel(const RayGenParams p) {
   for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int j = static_cast<int>(idx / p.W), i = static_cast<int>(idx - static_cast<long long>(j) * p.W);
-    const float dx = __fdiv_rn(static_cast<float>(i) - 0.5f * p.W, p.focal);
-    const float dy = -__fdiv_rn(static_cast<float>(j) - 0.5f * p.H, p.focal);
-    const float dz = -1.f;
-    float d[3], o[3];
+    pixel_ray(i, j, p.H, p.W, p.focal, p.c2w, p.near, p.far, p.ndc, p.rays + idx * 8);
+  }
+}
+
+// ------------------------------------------------ training batches from the views (datasets/blender.py:47-69,
+// datasets/llff.py:221-253)
+// The reference concatenates every training view's rays and colours into all_rays / all_rgbs, view-major, pixels
+// row-major.  Here pixel id p of that order is decoded (64-bit) into (view, row, column): the ray comes from the
+// view's pose through pixel_ray, the colour from the view's uint8 pixel as T.ToTensor() makes it (a division by
+// 255, not a multiplication by 1/255: torch's CPU div rounds the quotient once), blended onto white for RGBA
+// (blender.py:58: rgb * a + (1 - a), three torch ops, three roundings).  An id outside [0, V*H*W) reads nothing
+// and gives a NaN row.
+struct ViewBatchParams {
+  const uint8_t* images;   // (V, H, W, C) uint8
+  long long V;
+  int H, W, C;             // C: 3 (RGB) or 4 (RGBA)
+  const float* c2w;        // (V, 3, 4)
+  float focal, near, far;
+  int ndc;
+  const long long* ids;    // (n,)
+  long long n;
+  float* rays;             // (n, 8), 16-byte aligned
+  float* rgbs;             // (n, 3)
+};
+__global__ void view_batch_kernel(const ViewBatchParams p) {
+  const long long hw = static_cast<long long>(p.H) * p.W;
+  const long long total = p.V * hw;
+  for (long long k = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; k < p.n;
+       k += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long id = __ldg(p.ids + k);
+    float* ray = p.rays + k * 8;
+    float* rgb = p.rgbs + k * 3;
+    if (id < 0 || id >= total) {
+      const float nan = __int_as_float(0x7fffffff);
+      float4* out = reinterpret_cast<float4*>(ray);
+      out[0] = make_float4(nan, nan, nan, nan);
+      out[1] = out[0];
+      rgb[0] = rgb[1] = rgb[2] = nan;
+      continue;
+    }
+    const long long v = id / hw, rem = id - v * hw;
+    const int j = static_cast<int>(rem / p.W), i = static_cast<int>(rem - static_cast<long long>(j) * p.W);
+    float c2w[12];
+    const float4* pose = reinterpret_cast<const float4*>(p.c2w + v * 12);
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
-      d[r] = __fadd_rn(__fadd_rn(__fmul_rn(dx, p.c2w[4 * r + 0]), __fmul_rn(dy, p.c2w[4 * r + 1])),
-                       __fmul_rn(dz, p.c2w[4 * r + 2]));
-      o[r] = p.c2w[4 * r + 3];
+      const float4 row = __ldg(pose + r);
+      c2w[4 * r + 0] = row.x; c2w[4 * r + 1] = row.y; c2w[4 * r + 2] = row.z; c2w[4 * r + 3] = row.w;
     }
-    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
+    pixel_ray(i, j, p.H, p.W, p.focal, c2w, p.near, p.far, p.ndc, ray);
+    const uint8_t* px = p.images + id * p.C;
+    float c[3];
 #pragma unroll
-    for (int r = 0; r < 3; ++r) d[r] = __fdiv_rn(d[r], nrm);
-    float near = p.near, far = p.far;
-    if (p.ndc) {
-      const float n1 = 1.0f;                                   // llff.py:238 near plane at 1.0
-      const float tt = -__fdiv_rn(__fadd_rn(n1, o[2]), d[2]);
+    for (int ch = 0; ch < 3; ++ch) c[ch] = __fdiv_rn(static_cast<float>(__ldg(px + ch)), 255.f);
+    if (p.C == 4) {
+      const float a = __fdiv_rn(static_cast<float>(__ldg(px + 3)), 255.f);
+      const float bg = __fsub_rn(1.f, a);
 #pragma unroll
-      for (int r = 0; r < 3; ++r) o[r] = __fadd_rn(o[r], __fmul_rn(tt, d[r]));
-      const float ox_oz = __fdiv_rn(o[0], o[2]), oy_oz = __fdiv_rn(o[1], o[2]);
-      const float sx = -1.f / (p.W / (2.f * p.focal)), sy = -1.f / (p.H / (2.f * p.focal));
-      const float o0 = sx * ox_oz, o1 = sy * oy_oz, o2 = 1.f + 2.f * n1 / o[2];
-      const float d0 = sx * (__fdiv_rn(d[0], d[2]) - ox_oz), d1 = sy * (__fdiv_rn(d[1], d[2]) - oy_oz);
-      const float d2 = 1.f - o2;
-      o[0] = o0; o[1] = o1; o[2] = o2; d[0] = d0; d[1] = d1; d[2] = d2;
-      near = 0.f; far = 1.f;
+      for (int ch = 0; ch < 3; ++ch) c[ch] = __fadd_rn(__fmul_rn(c[ch], a), bg);
     }
-    float4* out = reinterpret_cast<float4*>(p.rays + idx * 8);
-    out[0] = make_float4(o[0], o[1], o[2], d[0]);
-    out[1] = make_float4(d[1], d[2], near, far);
+    rgb[0] = c[0]; rgb[1] = c[1]; rgb[2] = c[2];
   }
 }
 

@@ -12,6 +12,7 @@
 
 #include "../../include/nerf_pl_b200.h"
 #include "../../include/nerf_pl_b200_metrics.h"
+#include "../../include/nerf_pl_b200_views.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
@@ -1332,6 +1333,25 @@ int nerfb200_generate_rays(int32_t H, int32_t W, float focal, const float c2w_ho
   for (int i = 0; i < 12; ++i) p.c2w[i] = c2w_host[i];
   return launch("generate_rays launch", generate_rays_kernel, grid_blocks(static_cast<long long>(H) * W, 256), 256, 0,
                 stream, p);
+}
+
+int nerfb200_view_batch(const uint8_t* images, int64_t V, int32_t H, int32_t W, int32_t C, const float* c2w,
+                        float focal, float near, float far, int32_t ndc, const int64_t* ids, int64_t n, float* rays,
+                        float* rgbs, void* stream) {
+  if (V < 1 || H < 1 || W < 1 || n < 0) return fail(NERFB200_EINVAL, "view_batch: bad V / H / W / n");
+  if (C != 3 && C != 4) return fail(NERFB200_EINVAL, "view_batch: C must be 3 (RGB) or 4 (RGBA)");
+  if (!(focal > 0.f)) return fail(NERFB200_EINVAL, "view_batch: focal must be > 0");
+  // V * H * W * C bytes must be addressable with 64-bit ids
+  if (V > INT64_MAX / (static_cast<int64_t>(H) * W * C)) return fail(NERFB200_EINVAL, "view_batch: V * H * W * C overflows");
+  if (n == 0) return 0;
+  if (!images || !c2w || !ids || !rays || !rgbs) return fail(NERFB200_EINVAL, "view_batch: NULL argument");
+  if ((reinterpret_cast<uintptr_t>(rays) | reinterpret_cast<uintptr_t>(c2w)) & 15)
+    return fail(NERFB200_EINVAL, "view_batch: rays and c2w must be 16-byte aligned");
+  ViewBatchParams p;
+  p.images = images; p.V = V; p.H = H; p.W = W; p.C = C;
+  p.c2w = c2w; p.focal = focal; p.near = near; p.far = far; p.ndc = ndc;
+  p.ids = reinterpret_cast<const long long*>(ids); p.n = n; p.rays = rays; p.rgbs = rgbs;
+  return launch("view_batch launch", view_batch_kernel, grid_blocks(n, 256), 256, 0, stream, p);
 }
 
 int nerfb200_to_uint8(const float* src, int64_t n, uint8_t* dst, void* stream) {

@@ -28,7 +28,7 @@ import torch
 from . import _lib
 from .nerf import (_EXPECTED_SHAPES, _aligned_buffer, nerf_forward_fused, nerf_parameters, packed_weights,
                    packed_weights_pair)
-from .data import DeviceRayBatches, next_step_schedule
+from .data import _EpochBatches, next_step_schedule
 from .rendering import _draw_randoms, _ptr, _render_args
 
 
@@ -370,7 +370,7 @@ class CapturedTrainStep:
     """The reference's training step (train.py:103-117 with the optimiser step) captured once as a CUDA graph and
     replayed by ``step()``: no Python, no host-side kernel launches and no host synchronisation per step.
 
-    ``models`` (coarse[, fine]) are trained on ``batches`` (a ``DeviceRayBatches``) by ``optimizer``, a
+    ``models`` (coarse[, fine]) are trained on ``batches`` (a ``DeviceRayBatches`` or ``DeviceViewBatches``) by ``optimizer``, a
     ``FusedAdam(capturable=True)`` over their parameters; the other arguments are ``render_rays_loss``'s.  Each
     replay gathers the next batch from a device-resident epoch permutation at a device-side offset, renders it with
     the loss fused in, runs the backward and the Adam update.  Only full batches are used (``drop_last`` semantics:
@@ -401,8 +401,8 @@ class CapturedTrainStep:
         if not (isinstance(optimizer, FusedAdam) and optimizer.capturable):
             raise ValueError("CapturedTrainStep needs FusedAdam(..., capturable=True): a non-capturable step reads "
                              "its step count on the host and would replay step 1 forever")
-        if not isinstance(batches, DeviceRayBatches):
-            raise TypeError("batches must be a nerf_pl_b200.DeviceRayBatches")
+        if not isinstance(batches, _EpochBatches):
+            raise TypeError("batches must be a nerf_pl_b200.DeviceRayBatches or DeviceViewBatches")
         S_c, K = int(N_samples), int(N_importance)
         if K > 0 and len(models) < 2:
             raise ValueError("N_importance > 0 needs a fine model (models[1])")
