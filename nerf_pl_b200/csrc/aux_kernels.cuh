@@ -142,7 +142,16 @@ struct MlpParams {
   // the render path's training workspace (PassBufs: enc, act, mask, d, sigma, rgb; one pass, one sample per row)
   PassBufs tr;
   uint8_t* xdir;           // tiled (n_pad, 64) fp16: the direction rows of the direction layer's extra K slice
+  // compacted-sample mode (row_ray non-null, plain instantiation): row i is the sample at depth row_z[i] of ray
+  // row_ray[i] of `rays`, encoded by encode_row as the render kernel encodes it; with sigma_only = 0 its direction
+  // bias is the 128 floats at dirbias + row_ray[i] * kSkipDirStride (csrc/sample_skip_kernels.cuh), as the render
+  // kernel's per-ray dirbias.  x is unused.
+  const int* row_ray;
+  const float* row_z;
+  const float* rays;       // (., 8) [o, d, near, far]
+  const float* dirbias;
 };
+constexpr int kSkipDirStride = 2 * kDirW;   // per ray: the coarse network's direction bias, then the fine one's
 
 // kSave: also stores per sample the encoded input rows, the 8 activations and their ReLU sign bits, the direction-layer
 // output, the direction rows and raw sigma / rgb.  The returned values are those of the plain instantiation, bit for bit
@@ -162,11 +171,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
   const int lane = threadIdx.x & 31;
   const long long n_tiles = (p.n + 127) / 128;
   const bool so = p.sigma_only != 0;
+  const bool rows = !kSave && p.row_ray != nullptr;
   if (warp < kConsumerWarp0) {
     regs_dec<kRegsAux>();
     if (warp == kProducerWarp && lane == 0) {
       RingState rs;
-      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) produce_tile(rs, smem, bars, p.net, so, !so);
+      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) produce_tile(rs, smem, bars, p.net, so, !so && !rows);
     }
   } else {
     regs_inc<kRegsConsumer>();
@@ -190,7 +200,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
         const int row = 64 * c.wg + (t >> 1);
         const long long gi = min(tile * 128 + row, p.n - 1);
         const float* xr = p.x + gi * p.x_stride;
-        if (p.raw_xyz) {
+        if (rows) {
+          // a sample of a ray, as the render kernel encodes it (its helper warps' encode_row)
+          const float* ray = p.rays + static_cast<long long>(__ldg(p.row_ray + gi)) * 8;
+          const float o[3] = {__ldg(ray), __ldg(ray + 1), __ldg(ray + 2)};
+          const float d[3] = {__ldg(ray + 3), __ldg(ray + 4), __ldg(ray + 5)};
+          const float z = __ldg(p.row_z + gi);
+          for (int part = (t & 1) * 2; part < (t & 1) * 2 + 2; ++part) encode_row(enc, row, part, o, d, z);
+        } else if (p.raw_xyz) {
           // dense-grid sigma query (extract_color_mesh.py:127-140): encode the raw position here
           const float o[3] = {__ldg(xr), __ldg(xr + 1), __ldg(xr + 2)};
           const float zero[3] = {0.f, 0.f, 0.f};
@@ -217,7 +234,15 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
       const DirSrc ds = p.raw_xyz ? DirSrc{kZeroDirRow.v, 0, tile * 128, p.n, nullptr}
                                   : DirSrc{p.x, p.x_stride, tile * 128, p.n, kSave ? p.xdir : nullptr};
       float sig[2], rgb[2][3];
-      if (kSave) {
+      if (rows) {
+        const float* rbias[2];
+#pragma unroll
+        for (int s = 0; s < 2; ++s)
+          rbias[s] = p.dirbias + static_cast<long long>(__ldg(p.row_ray + min(tile * 128 + c.row[s], p.n - 1))) *
+                                     kSkipDirStride;
+        if (so) wg_tile<true, false, false>(c, kSmemEnc, rbias, nullptr, sig, rgb);
+        else wg_tile<false, false, false>(c, kSmemEnc, rbias, nullptr, sig, rgb);
+      } else if (kSave) {
 #pragma unroll
         for (int s = 0; s < 2; ++s) c.grow[s] = (tile * 128 + c.row[s] < p.n) ? tile * 128 + c.row[s] : -1;
         wg_tile<false, true, true>(c, kSmemEnc, dbias, &ds, sig, rgb);

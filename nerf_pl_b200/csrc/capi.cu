@@ -13,11 +13,13 @@
 #include "../../include/nerf_pl_b200.h"
 #include "../../include/nerf_pl_b200_metrics.h"
 #include "../../include/nerf_pl_b200_views.h"
+#include "../../include/nerf_pl_b200_samples.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
 #include "occupancy_kernels.cuh"
 #include "metrics_kernels.cuh"
+#include "sample_skip_kernels.cuh"
 
 #include <thrust/iterator/transform_iterator.h>
 
@@ -872,6 +874,53 @@ int cull_prepare(const float* rays, int64_t n, void* ws, size_t bytes, CullParam
   if (bytes < cull_carve(n, ws, p)) return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_cull_workspace_bytes", who);
   p->rays = rays; p->n = n;
   p->bits = nullptr; p->flag = nullptr; p->live_idx = nullptr; p->live_rays = nullptr;
+  return 0;
+}
+
+// ------------------------------------------------------------------ per-sample skipping (kernels: sample_skip_kernels.cuh)
+constexpr long long kSkipMaxRays = 1LL << 22;   // rows (n * S_f) and ray indices stay in int32
+
+bool samples_shape_ok(long long n, int Sc, int K) {
+  return n >= 0 && n <= kSkipMaxRays && (Sc == 32 || Sc == 64 || Sc == 128) && K >= 0 && K % 32 == 0 &&
+         Sc + K <= kMaxSf;
+}
+
+// The workspace of n rays: per-ray masks, counts, offsets, fine depths and direction biases, and the compacted rows
+// of the larger pass with their MLP outputs (16 bytes per row).
+size_t samples_carve(long long n, int Sc, int K, void* base, SkipParams* p) {
+  const long long Sf = Sc + K, rows = n * Sf;
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  p->mask[0] = c.take<uint32_t>(n * kSkipMaskWords);
+  p->mask[1] = c.take<uint32_t>(n * kSkipMaskWords);
+  p->cnt = c.take<int>(n + 1);
+  p->ofs = c.take<long long>(n + 1);
+  p->zf = c.take<float>(n * Sf);
+  p->dirbias = c.take<float>(n * kSkipDirStride);
+  p->row_ray = c.take<int>(rows);
+  p->row_z = c.take<float>(rows);
+  p->mlp_out = c.take<float>(rows * 4);
+  return c.off;
+}
+
+// The compacted-row MLP of one pass over `rows` rows (mlp_forward_kernel's compacted-sample mode).
+int samples_mlp(const SkipParams& sp, int pass, long long rows, bool sigma_only, void* stream) {
+  MlpParams m{};
+  m.n = rows;
+  m.net = sp.net[pass];
+  m.sigma_only = sigma_only;
+  m.out = const_cast<float*>(sp.mlp_out);
+  m.row_ray = sp.row_ray;
+  m.row_z = sp.row_z;
+  m.rays = sp.rays;
+  m.dirbias = sp.dirbias + pass * kDirW;
+  return launch_mlp(m, nullptr, stream, pass ? "render_samples fine mlp launch" : "render_samples coarse mlp launch");
+}
+
+// Scan the per-ray counts of the current pass and read the total back.
+int samples_scan(const SkipParams& sp, cudaStream_t s, long long* total) {
+  TRY(launch("render_samples scan launch", cull_scan_kernel, 1, 1024, 0, s, sp.cnt, sp.ofs, static_cast<long long>(sp.n)));
+  CUDA_TRY(cudaMemcpyAsync(total, sp.ofs + sp.n, sizeof(*total), cudaMemcpyDeviceToHost, s), "render_samples readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "render_samples readback");
   return 0;
 }
 
@@ -1870,6 +1919,89 @@ int nerfb200_scatter_results(const float* const src_host[6], float* const dst_ho
   p.live_idx = reinterpret_cast<const long long*>(live_idx);
   p.n_live = n_live; p.n = n_rays; p.bg = white_back ? 1.f : 0.f;
   return launch("scatter_results launch", scatter_results_kernel, grid_blocks(n_rays, 256), 256, 0, stream, p);
+}
+
+// ---- per-sample skipping (include/nerf_pl_b200_samples.h; kernels: sample_skip_kernels.cuh)
+size_t nerfb200_samples_workspace_bytes(int64_t n_rays, int32_t n_samples, int32_t n_importance) {
+  SkipParams p;
+  return samples_shape_ok(n_rays, n_samples, n_importance) ? samples_carve(n_rays, n_samples, n_importance, nullptr, &p)
+                                                           : 0;
+}
+
+int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t bytes, int64_t* live_samples_host,
+                            void* stream) {
+  if (!a || !live_samples_host) return fail(NERFB200_EINVAL, "render_samples: NULL argument");
+  if (!samples_shape_ok(a->n_rays, a->n_samples, a->n_importance))
+    return fail(NERFB200_EUNSUPPORTED, "render_samples: needs N_samples in {32, 64, 128}, N_importance a multiple of "
+                "32, N_samples + N_importance <= 192 and 0 <= n_rays <= 2^22");
+  if (a->N < 2 || a->N > kVolMaxN) return fail(NERFB200_EINVAL, "render_samples: N must be in [2, 1625]");
+  SkipParams p{};
+  for (int ax = 0; ax < 3; ++ax) {
+    const double lo = a->ranges[2 * ax], hi = a->ranges[2 * ax + 1];
+    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
+      return fail(NERFB200_EINVAL, "render_samples: every range must be finite with min != max");
+    p.grid.lo[ax] = lo;
+    p.grid.scale[ax] = static_cast<double>(a->N - 1) / (hi - lo);
+  }
+  live_samples_host[0] = live_samples_host[1] = 0;
+  if (a->n_rays == 0) return 0;
+  const bool fine = a->n_importance > 0, coarse_rgb = a->test_time == 0;
+  if (!a->rays || !a->packed_coarse || !a->bits || !a->opacity_coarse || !ws)
+    return fail(NERFB200_EINVAL, "render_samples: NULL argument");
+  if (coarse_rgb && (!a->rgb_coarse || !a->depth_coarse))
+    return fail(NERFB200_EINVAL, "render_samples: rgb_coarse / depth_coarse is NULL with test_time=0");
+  if (fine && (!a->packed_fine || !a->rgb_fine || !a->depth_fine || !a->opacity_fine))
+    return fail(NERFB200_EINVAL, "render_samples: packed_fine / fine outputs are NULL with N_importance>0");
+  if ((reinterpret_cast<uintptr_t>(a->rays) | reinterpret_cast<uintptr_t>(a->packed_coarse) |
+       reinterpret_cast<uintptr_t>(a->packed_fine) | reinterpret_cast<uintptr_t>(a->samples_coarse) |
+       reinterpret_cast<uintptr_t>(a->samples_fine)) & 15)
+    return fail(NERFB200_EINVAL, "render_samples: rays, packed images and samples must be 16-byte aligned");
+  if (bytes < samples_carve(a->n_rays, a->n_samples, a->n_importance, ws, &p))
+    return fail(NERFB200_EINVAL, "render_samples: workspace smaller than nerfb200_samples_workspace_bytes");
+  DeviceInfo* d = nullptr;
+  TRY(device_info(&d));
+  p.rays = a->rays; p.n = static_cast<int>(a->n_rays); p.live_flag = a->live_flag;
+  p.Sc = a->n_samples; p.K = a->n_importance; p.use_disp = a->use_disp; p.white_back = a->white_back;
+  p.test_time = a->test_time;
+  p.grid.bits = a->bits; p.grid.M = a->N - 1;
+  p.net[0] = static_cast<const uint8_t*>(a->packed_coarse);
+  p.net[1] = static_cast<const uint8_t*>(a->packed_fine);
+  if (a->mask_coarse) p.mask[0] = a->mask_coarse;
+  if (a->mask_fine) p.mask[1] = a->mask_fine;
+  p.rgb_coarse = a->rgb_coarse; p.depth_coarse = a->depth_coarse; p.opacity_coarse = a->opacity_coarse;
+  p.rgb_fine = a->rgb_fine; p.depth_fine = a->depth_fine; p.opacity_fine = a->opacity_fine;
+  p.z_fine = a->z_fine; p.weights_coarse = a->weights_coarse; p.weights_fine = a->weights_fine;
+  p.samples[0] = a->samples_coarse; p.samples[1] = a->samples_fine;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int ray_blocks = grid_blocks(ceil_div(p.n, kSkipWarps), 1);
+  // coarse pass
+  TRY(launch("render_samples classify launch", skip_classify_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
+  long long n_c = 0, n_f = 0;
+  TRY(samples_scan(p, s, &n_c));
+  bool have_bias = false;
+  if (n_c > 0) {
+    TRY(launch("render_samples emit launch", skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, 0));
+    if (coarse_rgb) {
+      TRY(launch("render_samples dir_bias launch", skip_dir_bias_kernel, grid_blocks(p.n, 1), kDirW, 0, s, p, 0,
+                 fine ? 2 : 1));
+      have_bias = true;
+    }
+    TRY(samples_mlp(p, 0, n_c, !coarse_rgb, s));
+  }
+  TRY(launch("render_samples coarse stage launch", skip_coarse_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
+  live_samples_host[0] = n_c;
+  if (!fine) return 0;
+  // fine pass
+  TRY(samples_scan(p, s, &n_f));
+  if (n_f > 0) {
+    TRY(launch("render_samples emit launch", skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, 1));
+    if (!have_bias)
+      TRY(launch("render_samples dir_bias launch", skip_dir_bias_kernel, grid_blocks(p.n, 1), kDirW, 0, s, p, 1, 2));
+    TRY(samples_mlp(p, 1, n_f, false, s));
+  }
+  TRY(launch("render_samples fine stage launch", skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
+  live_samples_host[1] = n_f;
+  return 0;
 }
 
 // ---- image metrics (include/nerf_pl_b200_metrics.h; kernels: metrics_kernels.cuh)

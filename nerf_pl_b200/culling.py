@@ -6,6 +6,12 @@ scatters the results back over the value a ray through vacuum renders.  Every st
 ``libnerf_pl_b200.so`` (csrc/occupancy_kernels.cuh, include/nerf_pl_b200.h); the render kernel is not
 touched.  The reference has no counterpart: it evaluates every sample of every ray.
 
+``skip="samples"`` (``render_rays_culled``, ``batched_inference``, ``render_image``) goes one step further: inside a
+live ray, a sample whose point lies in no occupied cell gets sigma = 0 and is not evaluated
+(csrc/sample_skip_kernels.cuh, include/nerf_pl_b200_samples.h; DESIGN.md "Skipping empty samples").  The evaluated
+samples have the fused kernel's sigma and rgb bit for bit, and a ray with nothing to skip renders bit for bit as
+``render_rays`` renders it; a ray with skipped samples is an approximation, like a culled ray.
+
 What it guarantees.  A live ray is rendered by the same kernel on an ordinary ``(n_live, 8)`` tensor, and with
 ``perturb = noise_std = 0`` a ray's result does not depend on its row: live pixels are bit-identical to the
 unculled render.  A culled pixel is *approximated* by the vacuum value.  The cell walk is exact and the dilation
@@ -22,6 +28,7 @@ from typing import Callable, Dict, List, Optional, Sequence
 import torch
 
 from . import _lib
+from .nerf import packed_weights
 from .rendering import render_rays
 
 RESULT_KEYS = ("rgb_coarse", "depth_coarse", "opacity_coarse", "rgb_fine", "depth_fine", "opacity_fine")
@@ -193,21 +200,150 @@ def render_culled(render_fn: Callable[[torch.Tensor], Dict[str, torch.Tensor]], 
     return out
 
 
+# Rays per nerfb200_render_samples call: the workspace is about 6.4 KB per ray at 64 + 128 samples (210 MB per
+# chunk), and each chunk costs two read-backs of a sample count.  Tests lower it to show that results do not depend
+# on it.
+_SAMPLE_CHUNK = 1 << 15
+
+SKIP_MODES = ("rays", "samples")
+
+
+def check_skip(skip: str, occupancy) -> None:
+    """``skip`` must name a mode, and ``"samples"`` needs a grid."""
+    if skip not in SKIP_MODES:
+        raise ValueError(f"skip must be one of {SKIP_MODES}, got {skip!r}")
+    if skip == "samples" and occupancy is None:
+        raise ValueError("skip='samples' needs an occupancy grid")
+
+
+@torch.no_grad()
+def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupancy: OccupancyGrid, N_samples: int,
+                   use_disp: bool, N_importance: int, white_back: bool, test_time: bool,
+                   live_flag: Optional[torch.Tensor] = None, extras: bool = False,
+                   per_sample: bool = False) -> Dict[str, torch.Tensor]:
+    """Render every ray of ``rays`` (n, 8) with empty samples skipped (module docstring), in chunks of
+    ``_SAMPLE_CHUNK`` rays.  Returns ``render_rays``' keys for ``test_time`` / ``N_importance``, ``extras`` as
+    ``render_rays`` gives them, and ``'live_samples'``: (evaluated coarse samples, evaluated fine samples).
+    ``live_flag`` (n) uint8: a ray whose flag is 0 has every sample skipped.  ``per_sample`` adds
+    ``'samples_coarse'`` / ``'samples_fine'`` (n, S, 4: rgb and sigma, 0 where skipped) and ``'mask_coarse'`` /
+    ``'mask_fine'`` (n, 6) int32 (bit b of word w: sample 32 w + b evaluated).  Synchronises twice per chunk."""
+    S_c, K = int(N_samples), int(N_importance)
+    S_f = S_c + K
+    if K > 0 and len(models) < 2:
+        raise ValueError("N_importance > 0 needs a fine model (models[1])")
+    lib = _lib.load()
+    rays = rays.detach().to(torch.float32).contiguous()
+    dev, n = rays.device, rays.shape[0]
+    chunk = max(1, min(int(_SAMPLE_CHUNK), n))
+    nbytes = lib.nerfb200_samples_workspace_bytes(chunk, S_c, K)
+    if nbytes == 0:
+        raise ValueError("skip='samples' supports N_samples in {32, 64, 128} and N_importance a multiple of 32 with "
+                         "N_samples + N_importance <= 192")
+    f32 = dict(dtype=torch.float32, device=dev)
+    out = {k: torch.empty((n, 3) if k.startswith("rgb") else (n,), **f32) for k in result_keys(K, bool(test_time))}
+    opt = {}
+    if extras:
+        opt["weights_coarse"] = torch.empty(n, S_c, **f32)
+        if K > 0:
+            opt["z_fine"] = torch.empty(n, S_f, **f32)
+            opt["weights_fine"] = torch.empty(n, S_f, **f32)
+    if per_sample:
+        opt["samples_coarse"] = torch.empty(n, S_c, 4, **f32)
+        opt["mask_coarse"] = torch.empty(n, 6, dtype=torch.int32, device=dev)
+        if K > 0:
+            opt["samples_fine"] = torch.empty(n, S_f, 4, **f32)
+            opt["mask_fine"] = torch.empty(n, 6, dtype=torch.int32, device=dev)
+    flag = None if live_flag is None else live_flag.to(torch.uint8).contiguous()
+    packed = (packed_weights(models[0]), packed_weights(models[1]) if K > 0 else None)
+    ws = _lib.workspace(nbytes, dev)
+    counts = [0, 0]
+    got = (ctypes.c_int64 * 2)()
+    for lo in range(0, n, chunk):
+        m = min(chunk, n - lo)
+        ptr = lambda t: None if t is None else t.data_ptr() + lo * t.stride(0) * t.element_size()  # noqa: E731
+        args = _lib.SamplesArgs(
+            rays=ptr(rays), n_rays=m, live_flag=ptr(flag), packed_coarse=packed[0].data_ptr(),
+            packed_fine=None if packed[1] is None else packed[1].data_ptr(), n_samples=S_c, n_importance=K,
+            use_disp=int(bool(use_disp)), white_back=int(bool(white_back)), test_time=int(bool(test_time)),
+            bits=occupancy.bits.data_ptr(), N=occupancy.N, ranges=_lib.ranges_host(*[occupancy.ranges[2 * a:2 * a + 2]
+                                                                                       for a in range(3)]),
+            **{k: ptr(out.get(k)) for k in RESULT_KEYS}, **{k: ptr(t) for k, t in opt.items()})
+        _lib.call("nerfb200_render_samples", dev, ctypes.byref(args), ws.data_ptr(), ws.numel(), got)
+        counts[0] += got[0]
+        counts[1] += got[1]
+    if extras:
+        out["weights_coarse"] = opt["weights_coarse"]
+        if K > 0:
+            out["z_vals_fine"] = opt["z_fine"]
+            out["weights_fine"] = opt["weights_fine"]
+    if per_sample:
+        out.update({k: v for k, v in opt.items() if k.startswith(("samples", "mask"))})
+    out["live_samples"] = tuple(counts)
+    return out
+
+
+def render_culled_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupancy: OccupancyGrid,
+                          N_samples: int, use_disp: bool, N_importance: int, white_back: bool, test_time: bool,
+                          extras: bool = False, sharded: bool = False) -> Dict[str, torch.Tensor]:
+    """cull -> ``render_samples(live rays)`` -> scatter, with ``'live'``, ``'live_idx'`` and ``'live_samples'``.
+    With ``extras`` every ray goes through ``render_samples``, the culled ones with every sample skipped, so that the
+    extra tensors are full size; their results are then the vacuum value as well.  ``sharded`` splits the live rays
+    over the ranks (``render_rays_sharded``); ``'live_samples'`` then counts this rank's samples."""
+    r = _check_rays(rays, occupancy)
+    keys = result_keys(int(N_importance), bool(test_time))
+    counts = [0, 0]
+
+    def fn(live, flag=None):
+        res = render_samples(models, live, occupancy, N_samples, use_disp, N_importance, white_back, test_time,
+                             live_flag=flag, extras=extras)
+        ls = res.pop("live_samples")
+        counts[0] += ls[0]
+        counts[1] += ls[1]
+        return res
+
+    if extras:
+        live_idx, _, flag = cull_rays(r, occupancy, return_flag=True)
+        out = fn(r, flag)
+    else:
+        from .sharded import render_rays_sharded
+        run = (lambda x: render_rays_sharded(fn, x)) if sharded else fn
+        live_idx, live_rays = cull_rays(r, occupancy)
+        compact = run(live_rays) if live_idx.shape[0] else None
+        out = scatter_results(compact, live_idx, r.shape[0], white_back, keys)
+    out["live"] = int(live_idx.shape[0])
+    out["live_idx"] = live_idx
+    out["live_samples"] = tuple(counts)
+    return out
+
+
 @torch.no_grad()
 def render_rays_culled(models: List[torch.nn.Module], embeddings: List[torch.nn.Module], rays: torch.Tensor,
                        occupancy: OccupancyGrid, N_samples: int = 64, use_disp: bool = False, N_importance: int = 0,
                        white_back: bool = False, test_time: bool = True, *, perturb: float = 0,
-                       noise_std: float = 0) -> Dict[str, torch.Tensor]:
+                       noise_std: float = 0, skip: str = "rays", extras: bool = False) -> Dict[str, torch.Tensor]:
     """``render_rays`` at inference with empty space skipped: the same keys, shapes and dtypes, plus ``'live'``
     (the number of rays rendered) and ``'live_idx'`` (their indices, int64).  Live rays are bit-identical to
     ``render_rays(..., perturb=0, noise_std=0)``; a culled ray gets the vacuum value, an approximation whose error
     is bounded empirically, not proved (module docstring).  Inference only: ``perturb`` and ``noise_std`` must be
     0 and no gradient is built; anything else is a ValueError, because training must see the background rays to
-    learn that they are empty."""
+    learn that they are empty.
+
+    ``skip="samples"`` also skips the empty samples of the live rays (module docstring; DESIGN.md "Skipping empty
+    samples"): faster, no longer bit-identical, and the result holds ``'live_samples'`` (evaluated coarse, fine
+    samples).  ``extras=True`` (with ``"samples"``) adds ``weights_coarse``, ``weights_fine`` and ``z_vals_fine`` as
+    ``render_rays`` does.  It synchronises twice per chunk of ``_SAMPLE_CHUNK`` live rays."""
     if float(perturb) != 0.0 or float(noise_std) != 0.0:
         raise ValueError("render_rays_culled is inference only (perturb = 0, noise_std = 0): training must see the "
                          "background rays to learn that they are empty")
+    check_skip(skip, occupancy)
+    if extras and skip != "samples":
+        raise ValueError("extras=True needs skip='samples' (render_rays(..., extras=True) renders every ray)")
     r = _check_rays(rays, occupancy)
+    if skip == "samples":
+        from .rendering import _check_render_inputs
+        _check_render_inputs("render_rays_culled", models, embeddings, int(N_importance), r)
+        return render_culled_samples(list(models), r, occupancy, int(N_samples), use_disp, int(N_importance),
+                                     white_back, test_time, extras=extras)
 
     def fn(live):
         return render_rays(list(models), list(embeddings), live, int(N_samples), use_disp, 0, 0, int(N_importance),
