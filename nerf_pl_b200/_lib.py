@@ -22,8 +22,10 @@ if os.environ.get("NERFB200_LIB"):          # a library built elsewhere (e.g. wi
     LIB_PATH = os.path.abspath(os.environ["NERFB200_LIB"])
 SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
-           "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h", "sample_skip_kernels.cuh"]
-INCLUDES = ["nerf_pl_b200.h", "nerf_pl_b200_metrics.h", "nerf_pl_b200_views.h", "nerf_pl_b200_samples.h"]
+           "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h", "sample_skip_kernels.cuh",
+           "train_skip_kernels.cuh"]
+INCLUDES = ["nerf_pl_b200.h", "nerf_pl_b200_metrics.h", "nerf_pl_b200_views.h", "nerf_pl_b200_samples.h",
+            "nerf_pl_b200_train_samples.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -127,6 +129,52 @@ class SamplesArgs(ctypes.Structure):
     ]
 
 
+class TrainSamplesArgs(ctypes.Structure):
+    """Mirror of ``nerfb200_train_samples_args`` (include/nerf_pl_b200_train_samples.h)."""
+
+    _fields_ = [
+        ("rays", c_void_p),
+        ("n_rays", c_int64),
+        ("packed_coarse", c_void_p),
+        ("packed_fine", c_void_p),
+        ("n_samples", c_int32),
+        ("n_importance", c_int32),
+        ("use_disp", c_int32),
+        ("white_back", c_int32),
+        ("perturb", c_float),
+        ("noise_std", c_float),
+        ("perturb_rand", c_void_p),
+        ("noise_coarse", c_void_p),
+        ("u_rand", c_void_p),
+        ("noise_fine", c_void_p),
+        ("rng_seed", ctypes.c_uint64),
+        ("rng_in_kernel", c_int32),
+        ("bits", c_void_p),
+        ("N", c_int64),
+        ("ranges", c_double * 6),
+        ("target", c_void_p),
+        ("rgb_coarse", c_void_p),
+        ("depth_coarse", c_void_p),
+        ("opacity_coarse", c_void_p),
+        ("rgb_fine", c_void_p),
+        ("depth_fine", c_void_p),
+        ("opacity_fine", c_void_p),
+        ("loss_out", c_void_p),
+        ("z_coarse", c_void_p),
+        ("z_fine", c_void_p),
+        ("weights_coarse", c_void_p),
+        ("weights_fine", c_void_p),
+        ("samples_coarse", c_void_p),
+        ("samples_fine", c_void_p),
+        ("mask_coarse", c_void_p),
+        ("mask_fine", c_void_p),
+        ("dsigma_coarse", c_void_p),
+        ("dsigma_fine", c_void_p),
+        ("dprergb_coarse", c_void_p),
+        ("dprergb_fine", c_void_p),
+    ]
+
+
 _vp, _i32, _i64, _f32, _f64, _sz = c_void_p, c_int32, c_int64, c_float, c_double, c_size_t
 _P, _RA, _BA = POINTER(c_void_p), POINTER(RenderArgs), POINTER(BackwardArgs)
 
@@ -215,6 +263,14 @@ SAMPLES_SIGNATURES = {
     "nerfb200_render_samples": (_i32, [POINTER(SamplesArgs), _vp, _sz, POINTER(_i64), _vp]),
 }
 
+# The entries of the companion header include/nerf_pl_b200_train_samples.h, in header order (its own tests check it).
+TRAIN_SAMPLES_SIGNATURES = {
+    "nerfb200_train_samples_workspace_bytes": (_sz, [_i64, _i32, _i32]),
+    "nerfb200_train_samples_forward": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_train_samples_backward": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp, _P, _P, _P, _P,
+                                                _vp]),
+}
+
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
@@ -262,7 +318,8 @@ def load() -> ctypes.CDLL:
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
             for name, (restype, argtypes) in (*SIGNATURES.items(), *METRICS_SIGNATURES.items(),
-                                              *VIEWS_SIGNATURES.items(), *SAMPLES_SIGNATURES.items()):
+                                              *VIEWS_SIGNATURES.items(), *SAMPLES_SIGNATURES.items(),
+                                              *TRAIN_SAMPLES_SIGNATURES.items()):
                 fn = getattr(lib, name)
                 fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:

@@ -150,13 +150,20 @@ struct MlpParams {
   const float* row_z;
   const float* rays;       // (., 8) [o, d, near, far]
   const float* dirbias;
+  // compacted-sample training mode (kRowsSave): the fp16 direction row of each ray, (., 64) [Embedding(3, 4)(d), 0..]
+  const __half* dirrow;
 };
 constexpr int kSkipDirStride = 2 * kDirW;   // per ray: the coarse network's direction bias, then the fine one's
 
 // kSave: also stores per sample the encoded input rows, the 8 activations and their ReLU sign bits, the direction-layer
 // output, the direction rows and raw sigma / rgb.  The returned values are those of the plain instantiation, bit for bit
 // (the save mode only adds stores).
-template <bool kSave>
+// kRowsSave (with kSave): the compacted-sample mode with the same stores, for training with empty samples skipped
+// (csrc/train_skip_kernels.cuh).  The direction still enters through the per-ray fp32 bias, so the values are the
+// compacted-sample mode's; xdir receives the row's ray's direction row, so that the direction-slice wgrad GEMM yields
+// gW_dir[:, 256:283].  Padding rows of the last tile are stored as copies of row n - 1 (their gradient is 0), so every
+// row below n_pad is written by this launch whatever an earlier, longer launch left in the workspace.
+template <bool kSave, bool kRowsSave = false>
 __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   Scratch* sc = reinterpret_cast<Scratch*>(smem + kSmemScratch);
@@ -171,7 +178,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
   const int lane = threadIdx.x & 31;
   const long long n_tiles = (p.n + 127) / 128;
   const bool so = p.sigma_only != 0;
-  const bool rows = !kSave && p.row_ray != nullptr;
+  const bool rows = kRowsSave || (!kSave && p.row_ray != nullptr);
   if (warp < kConsumerWarp0) {
     regs_dec<kRegsAux>();
     if (warp == kProducerWarp && lane == 0) {
@@ -202,11 +209,26 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
         const float* xr = p.x + gi * p.x_stride;
         if (rows) {
           // a sample of a ray, as the render kernel encodes it (its helper warps' encode_row)
-          const float* ray = p.rays + static_cast<long long>(__ldg(p.row_ray + gi)) * 8;
+          const long long ri = __ldg(p.row_ray + gi);
+          const float* ray = p.rays + ri * 8;
           const float o[3] = {__ldg(ray), __ldg(ray + 1), __ldg(ray + 2)};
           const float d[3] = {__ldg(ray + 3), __ldg(ray + 4), __ldg(ray + 5)};
           const float z = __ldg(p.row_z + gi);
           for (int part = (t & 1) * 2; part < (t & 1) * 2 + 2; ++part) encode_row(enc, row, part, o, d, z);
+          if (kRowsSave) {
+            // the row's two threads (adjacent lanes) wrote interleaved columns; each then stores its four 16-byte
+            // chunks of the encoded row and of the ray's direction row, in the tile's swizzle
+            __syncwarp();
+            uint8_t* dst = p.tr.enc + tile * 16384;
+            uint8_t* xd = p.xdir + tile * 16384;
+            const uint4* dr = reinterpret_cast<const uint4*>(p.dirrow + ri * 64);
+#pragma unroll
+            for (int cc = 0; cc < 4; ++cc) {
+              const uint32_t off = sw128_off(row, ((t & 1) * 4 + cc) * 8);
+              *reinterpret_cast<uint4*>(dst + off) = *reinterpret_cast<const uint4*>(enc + off);
+              *reinterpret_cast<uint4*>(xd + off) = __ldg(dr + (t & 1) * 4 + cc);
+            }
+          }
         } else if (p.raw_xyz) {
           // dense-grid sigma query (extract_color_mesh.py:127-140): encode the raw position here
           const float o[3] = {__ldg(xr), __ldg(xr + 1), __ldg(xr + 2)};
@@ -240,8 +262,15 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
         for (int s = 0; s < 2; ++s)
           rbias[s] = p.dirbias + static_cast<long long>(__ldg(p.row_ray + min(tile * 128 + c.row[s], p.n - 1))) *
                                      kSkipDirStride;
-        if (so) wg_tile<true, false, false>(c, kSmemEnc, rbias, nullptr, sig, rgb);
-        else wg_tile<false, false, false>(c, kSmemEnc, rbias, nullptr, sig, rgb);
+        if (kRowsSave) {
+#pragma unroll
+          for (int s = 0; s < 2; ++s) c.grow[s] = tile * 128 + c.row[s];
+          wg_tile<false, false, true>(c, kSmemEnc, rbias, nullptr, sig, rgb);
+        } else if (so) {
+          wg_tile<true, false, false>(c, kSmemEnc, rbias, nullptr, sig, rgb);
+        } else {
+          wg_tile<false, false, false>(c, kSmemEnc, rbias, nullptr, sig, rgb);
+        }
       } else if (kSave) {
 #pragma unroll
         for (int s = 0; s < 2; ++s) c.grow[s] = (tile * 128 + c.row[s] < p.n) ? tile * 128 + c.row[s] : -1;

@@ -14,12 +14,14 @@
 #include "../../include/nerf_pl_b200_metrics.h"
 #include "../../include/nerf_pl_b200_views.h"
 #include "../../include/nerf_pl_b200_samples.h"
+#include "../../include/nerf_pl_b200_train_samples.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
 #include "occupancy_kernels.cuh"
 #include "metrics_kernels.cuh"
 #include "sample_skip_kernels.cuh"
+#include "train_skip_kernels.cuh"
 
 #include <thrust/iterator/transform_iterator.h>
 
@@ -141,6 +143,8 @@ int device_info(DeviceInfo** out) {
                                   static_cast<int>(kSmemTotal)), "smem attr mlp");
     CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kSmemTotal)), "smem attr mlp(save)");
+    CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kSmemTotal)), "smem attr mlp(save rows)");
     CUDA_TRY(cudaFuncSetAttribute(chain_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kChSmemTotal)), "smem attr chain");
     CUDA_TRY(cudaFuncSetAttribute(chain_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -922,6 +926,152 @@ int samples_scan(const SkipParams& sp, cudaStream_t s, long long* total) {
   CUDA_TRY(cudaMemcpyAsync(total, sp.ofs + sp.n, sizeof(*total), cudaMemcpyDeviceToHost, s), "render_samples readback");
   CUDA_TRY(cudaStreamSynchronize(s), "render_samples readback");
   return 0;
+}
+
+// The grid of both per-sample skipping entries: N in [2, kVolMaxN], every range finite with min != max.
+int skip_grid(const uint32_t* bits, int64_t N, const double* ranges, SkipGrid* g, const char* who) {
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
+  for (int ax = 0; ax < 3; ++ax) {
+    const double lo = ranges[2 * ax], hi = ranges[2 * ax + 1];
+    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
+      return fail(NERFB200_EINVAL, "%s: every range must be finite with min != max", who);
+    g->lo[ax] = lo;
+    g->scale[ax] = static_cast<double>(N - 1) / (hi - lo);
+  }
+  g->bits = bits;
+  g->M = N - 1;
+  return 0;
+}
+
+// ------------------------------------------------------------------ training with empty samples skipped
+// (kernels: train_skip_kernels.cuh).  One workspace per batch shape, sized for every sample evaluated: the per-ray
+// buffers, the compacted rows of the larger pass, then one NeRF.forward training workspace per network carved for
+// that worst case.  A step's layout keeps the carved addresses and takes its own row count (train_skip_net_layout),
+// so nothing is reallocated or re-zeroed between steps; the forward uploads the step's wgrad plans.
+struct TrainSkipWs {
+  TrainSkipParams t;
+  uint8_t* net_ws[2];
+  long long cap[2];             // rows of each network with every sample evaluated
+};
+
+size_t train_skip_carve(long long n, int Sc, int K, void* base, int sm_count, TrainSkipWs* w) {
+  const long long Sf = Sc + K, rows = n * Sf;
+  Carver c{static_cast<uint8_t*>(base), 0, 1024};
+  SkipParams& p = w->t.s;
+  p.mask[0] = c.take<uint32_t>(n * kSkipMaskWords);
+  p.mask[1] = c.take<uint32_t>(n * kSkipMaskWords);
+  p.cnt = c.take<int>(n + 1);
+  w->t.ofs[0] = c.take<long long>(n + 1);
+  w->t.ofs[1] = c.take<long long>(n + 1);
+  w->t.zc = c.take<float>(n * Sc);
+  p.zf = c.take<float>(n * Sf);
+  p.dirbias = c.take<float>(n * kSkipDirStride);
+  w->t.dirrow = c.take<__half>(n * 64);
+  p.row_ray = c.take<int>(rows);
+  p.row_z = c.take<float>(rows);
+  p.mlp_out = c.take<float>(rows * 4);
+  w->net_ws[0] = w->net_ws[1] = nullptr;
+  w->cap[0] = w->cap[1] = 0;
+  for (int ps = 0; ps < (K > 0 ? 2 : 1); ++ps) {
+    w->cap[ps] = n * (ps ? Sf : Sc);
+    TrainLayout L;
+    make_train_layout(&L, nullptr, true, w->cap[ps], 1, 0, sm_count);
+    w->net_ws[ps] = c.take(L.bytes);
+  }
+  return c.off;
+}
+
+// The NeRF.forward training layout of `rows` rows inside a workspace carved for `cap` rows.  Every buffer keeps its
+// worst-case address; the row count, the padded row count (the stride of the activation layers), the head kernel's
+// pseudo-rays and the wgrad plan are the step's.  The plan of fewer rows needs no more CTAs, pieces or head blocks
+// than the carved one.
+void train_skip_net_layout(TrainLayout* L, uint8_t* base, long long cap, long long rows, int sm_count) {
+  make_train_layout(L, base, true, cap, 1, 0, sm_count);
+  PassBufs& b = L->pass[0];
+  b.n = rows;
+  b.n_pad = (rows + 127) / 128 * 128;
+  L->n_rays = static_cast<int>(b.n_pad / kMlpPseudoRay);
+  L->head_grid = (L->n_rays + kHeadWarps - 1) / kHeadWarps;
+  plan_wgrad(L, sm_count, nullptr, nullptr);
+}
+
+// Upload the wgrad plan of a step's layout (called right after a count read-back, when the stream is idle).
+int train_skip_upload_plan(TrainLayout& L, int sm_count, cudaStream_t s) {
+  std::vector<WgradJob> jobs(kMaxWgJobs);
+  std::vector<int> cta_first(kMaxWgCtas + 1, 0);
+  plan_wgrad(&L, sm_count, jobs.data(), cta_first.data());
+  CUDA_TRY(cudaMemcpyAsync(L.jobs_dev, jobs.data(), sizeof(WgradJob) * L.n_jobs, cudaMemcpyHostToDevice, s),
+           "train_samples job table upload");
+  CUDA_TRY(cudaMemcpyAsync(L.cta_first_dev, cta_first.data(), sizeof(int) * (L.n_cta + 1), cudaMemcpyHostToDevice, s),
+           "train_samples cta table upload");
+  return 0;
+}
+
+// The argument checks of both entries, and the step's parameters and workspace carve.
+int train_skip_setup(const nerfb200_train_samples_args* a, void* ws, size_t bytes, int sm_count, TrainSkipWs* w,
+                     const char* who) {
+  if (!a) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (!samples_shape_ok(a->n_rays, a->n_samples, a->n_importance) || a->n_rays < 1)
+    return fail(NERFB200_EUNSUPPORTED, "%s: needs N_samples in {32, 64, 128}, N_importance a multiple of 32, "
+                "N_samples + N_importance <= 192 and 1 <= n_rays <= 2^22", who);
+  std::memset(w, 0, sizeof(*w));
+  TrainSkipParams& t = w->t;
+  SkipParams& p = t.s;
+  TRY(skip_grid(a->bits, a->N, a->ranges, &p.grid, who));
+  const bool fine = a->n_importance > 0;
+  if (!a->rays || !a->packed_coarse || !a->bits || !a->target || !a->loss_out || !a->rgb_coarse || !a->depth_coarse ||
+      !a->opacity_coarse || !ws)
+    return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (fine && (!a->packed_fine || !a->rgb_fine || !a->depth_fine || !a->opacity_fine))
+    return fail(NERFB200_EINVAL, "%s: packed_fine / fine outputs are NULL with N_importance>0", who);
+  if (a->rng_in_kernel < 0 || a->rng_in_kernel > 2) return fail(NERFB200_EINVAL, "%s: rng_in_kernel must be 0, 1 or 2", who);
+  if (a->rng_in_kernel == 2 && !a->rng_seed) return fail(NERFB200_EINVAL, "%s: rng_in_kernel = 2 needs rng_seed", who);
+  if (!(a->perturb >= 0.f) || !(a->noise_std >= 0.f)) return fail(NERFB200_EINVAL, "%s: perturb / noise_std < 0", who);
+  if (a->perturb > 0.f && !a->rng_in_kernel && (!a->perturb_rand || (fine && !a->u_rand)))
+    return fail(NERFB200_EINVAL, "%s: perturb>0 needs perturb_rand and u_rand", who);
+  if (a->noise_std > 0.f && (!a->noise_coarse || (fine && !a->noise_fine)))
+    return fail(NERFB200_EINVAL, "%s: noise_std>0 needs noise_coarse and noise_fine", who);
+  if ((reinterpret_cast<uintptr_t>(a->rays) | reinterpret_cast<uintptr_t>(a->packed_coarse) |
+       reinterpret_cast<uintptr_t>(a->packed_fine) | reinterpret_cast<uintptr_t>(a->samples_coarse) |
+       reinterpret_cast<uintptr_t>(a->samples_fine)) & 15)
+    return fail(NERFB200_EINVAL, "%s: rays, packed images and samples must be 16-byte aligned", who);
+  if (reinterpret_cast<uintptr_t>(ws) & 1023) return fail(NERFB200_EINVAL, "%s: workspace must be 1024-byte aligned", who);
+  if (bytes < train_skip_carve(a->n_rays, a->n_samples, a->n_importance, ws, sm_count, w))
+    return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_train_samples_workspace_bytes", who);
+  p.rays = a->rays; p.n = static_cast<int>(a->n_rays);
+  p.Sc = a->n_samples; p.K = a->n_importance; p.use_disp = a->use_disp; p.white_back = a->white_back;
+  p.net[0] = static_cast<const uint8_t*>(a->packed_coarse);
+  p.net[1] = static_cast<const uint8_t*>(a->packed_fine);
+  p.rgb_coarse = a->rgb_coarse; p.depth_coarse = a->depth_coarse; p.opacity_coarse = a->opacity_coarse;
+  p.rgb_fine = a->rgb_fine; p.depth_fine = a->depth_fine; p.opacity_fine = a->opacity_fine;
+  p.z_fine = a->z_fine; p.weights_coarse = a->weights_coarse; p.weights_fine = a->weights_fine;
+  p.samples[0] = a->samples_coarse; p.samples[1] = a->samples_fine;
+  t.perturb = a->perturb; t.noise_std = a->noise_std;
+  t.perturb_rand = a->perturb_rand; t.u_rand = a->u_rand;
+  t.noise[0] = a->noise_coarse; t.noise[1] = a->noise_fine;
+  t.rng_seed = a->rng_seed; t.rng_in_kernel = a->rng_in_kernel;
+  t.z_coarse = a->z_coarse;
+  return 0;
+}
+
+// The training MLP of one network over the step's compacted rows (mlp_forward_kernel<true, true>).
+int train_skip_mlp(const TrainSkipParams& t, const TrainLayout& L, int pass, long long rows, const DeviceInfo* d,
+                   cudaStream_t s) {
+  MlpParams m{};
+  m.n = rows;
+  m.net = t.s.net[pass];
+  m.out = const_cast<float*>(t.s.mlp_out);
+  m.status = d->status;
+  m.tr = L.pass[0];
+  m.xdir = L.xdir;
+  m.row_ray = t.s.row_ray;
+  m.row_z = t.s.row_z;
+  m.rays = t.s.rays;
+  m.dirbias = t.s.dirbias + pass * kDirW;
+  m.dirrow = t.dirrow;
+  const long long tiles = ceil_div(rows, 128);
+  return launch(pass ? "train_samples fine mlp launch" : "train_samples coarse mlp launch", mlp_forward_kernel<true, true>,
+                static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count), kThreads, kSmemTotal, s, m);
 }
 
 // ------------------------------------------------------------------ image metrics (kernels: metrics_kernels.cuh)
@@ -1934,15 +2084,8 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
   if (!samples_shape_ok(a->n_rays, a->n_samples, a->n_importance))
     return fail(NERFB200_EUNSUPPORTED, "render_samples: needs N_samples in {32, 64, 128}, N_importance a multiple of "
                 "32, N_samples + N_importance <= 192 and 0 <= n_rays <= 2^22");
-  if (a->N < 2 || a->N > kVolMaxN) return fail(NERFB200_EINVAL, "render_samples: N must be in [2, 1625]");
   SkipParams p{};
-  for (int ax = 0; ax < 3; ++ax) {
-    const double lo = a->ranges[2 * ax], hi = a->ranges[2 * ax + 1];
-    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
-      return fail(NERFB200_EINVAL, "render_samples: every range must be finite with min != max");
-    p.grid.lo[ax] = lo;
-    p.grid.scale[ax] = static_cast<double>(a->N - 1) / (hi - lo);
-  }
+  TRY(skip_grid(a->bits, a->N, a->ranges, &p.grid, "render_samples"));
   live_samples_host[0] = live_samples_host[1] = 0;
   if (a->n_rays == 0) return 0;
   const bool fine = a->n_importance > 0, coarse_rgb = a->test_time == 0;
@@ -1963,7 +2106,6 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
   p.rays = a->rays; p.n = static_cast<int>(a->n_rays); p.live_flag = a->live_flag;
   p.Sc = a->n_samples; p.K = a->n_importance; p.use_disp = a->use_disp; p.white_back = a->white_back;
   p.test_time = a->test_time;
-  p.grid.bits = a->bits; p.grid.M = a->N - 1;
   p.net[0] = static_cast<const uint8_t*>(a->packed_coarse);
   p.net[1] = static_cast<const uint8_t*>(a->packed_fine);
   if (a->mask_coarse) p.mask[0] = a->mask_coarse;
@@ -2001,6 +2143,126 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
   }
   TRY(launch("render_samples fine stage launch", skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
   live_samples_host[1] = n_f;
+  return 0;
+}
+
+// ---- training with empty samples skipped (include/nerf_pl_b200_train_samples.h; kernels: train_skip_kernels.cuh)
+size_t nerfb200_train_samples_workspace_bytes(int64_t n_rays, int32_t n_samples, int32_t n_importance) {
+  if (!samples_shape_ok(n_rays, n_samples, n_importance) || n_rays < 1) return 0;
+  TrainSkipWs w;
+  return train_skip_carve(n_rays, n_samples, n_importance, nullptr, nerfb200_sm_count(), &w);
+}
+
+int nerfb200_train_samples_forward(const nerfb200_train_samples_args* a, void* ws, size_t bytes,
+                                   int64_t* live_samples_host, void* stream) {
+  if (!live_samples_host) return fail(NERFB200_EINVAL, "train_samples_forward: NULL argument");
+  TrainSkipWs w;
+  TRY(train_skip_setup(a, ws, bytes, nerfb200_sm_count(), &w, "train_samples_forward"));
+  DeviceInfo* d = nullptr;
+  TRY(device_info(&d));
+  TRY(check_sticky_status(d));
+  TrainSkipParams& t = w.t;
+  const bool fine = t.s.K > 0;
+  const long long n = t.s.n;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int ray_blocks = grid_blocks(ceil_div(n, kSkipWarps), 1);
+  const char* what = "train_samples_forward launches";
+  live_samples_host[0] = live_samples_host[1] = 0;
+  // coarse pass
+  TRY(launch(what, train_skip_classify_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+  TRY(launch(what, skip_dir_bias_kernel, grid_blocks(n, 1), kDirW, 0, s, t.s, 0, fine ? 2 : 1));
+  t.s.ofs = t.ofs[0];
+  long long rows[2] = {0, 0};
+  TRY(samples_scan(t.s, s, &rows[0]));
+  TrainLayout L[2];
+  if (rows[0] > 0) {
+    train_skip_net_layout(&L[0], w.net_ws[0], w.cap[0], rows[0], d->sm_count);
+    if (!fine) TRY(train_skip_upload_plan(L[0], d->sm_count, s));
+    TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 0));
+    TRY(train_skip_mlp(t, L[0], 0, rows[0], d, s));
+  }
+  TRY(launch(what, train_skip_coarse_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+  if (fine) {
+    t.s.ofs = t.ofs[1];
+    TRY(samples_scan(t.s, s, &rows[1]));
+    if (rows[0] > 0) TRY(train_skip_upload_plan(L[0], d->sm_count, s));
+    if (rows[1] > 0) {
+      train_skip_net_layout(&L[1], w.net_ws[1], w.cap[1], rows[1], d->sm_count);
+      TRY(train_skip_upload_plan(L[1], d->sm_count, s));
+      TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 1));
+      TRY(train_skip_mlp(t, L[1], 1, rows[1], d, s));
+    }
+    TRY(launch(what, train_skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+  }
+  // losses.py / metrics.py on the results, one block in a fixed order
+  TRY(launch(what, mse_psnr_kernel, 1, 1024, 0, s, t.s.rgb_coarse, fine ? t.s.rgb_fine : nullptr, a->target, n * 3,
+             a->loss_out));
+  uint32_t* const mask_out[2] = {a->mask_coarse, a->mask_fine};
+  for (int ps = 0; ps < (fine ? 2 : 1); ++ps)
+    if (mask_out[ps])
+      CUDA_TRY(cudaMemcpyAsync(mask_out[ps], t.s.mask[ps], sizeof(uint32_t) * n * kSkipMaskWords,
+                               cudaMemcpyDeviceToDevice, s), "train_samples mask copy");
+  live_samples_host[0] = rows[0];
+  live_samples_host[1] = rows[1];
+  return 0;
+}
+
+int nerfb200_train_samples_backward(const nerfb200_train_samples_args* a, void* ws, size_t bytes,
+                                    const int64_t* live_samples_host, const float* loss_grad,
+                                    const float* const params_coarse[24], const float* const params_fine[24],
+                                    float* const grads_coarse[24], float* const grads_fine[24], void* stream) {
+  if (!live_samples_host) return fail(NERFB200_EINVAL, "train_samples_backward: NULL argument");
+  TrainSkipWs w;
+  TRY(train_skip_setup(a, ws, bytes, nerfb200_sm_count(), &w, "train_samples_backward"));
+  const TrainSkipParams& t = w.t;
+  const int n_net = t.s.K > 0 ? 2 : 1;
+  const float* const* const params[2] = {params_coarse, params_fine};
+  float* const* const grads[2] = {grads_coarse, grads_fine};
+  for (int ps = 0; ps < n_net; ++ps) {
+    if (live_samples_host[ps] < 0 || live_samples_host[ps] > w.cap[ps])
+      return fail(NERFB200_EINVAL, "train_samples_backward: live sample count out of range");
+    if (live_samples_host[ps] == 0) continue;
+    if (!params[ps] || !grads[ps]) return fail(NERFB200_EINVAL, "train_samples_backward: params / grads tables are NULL");
+    for (int i = 0; i < kNumParams; ++i)
+      if (!params[ps][i] || !grads[ps][i])
+        return fail(NERFB200_EINVAL, "train_samples_backward: NULL parameter / gradient tensor");
+  }
+  DeviceInfo* d = nullptr;
+  TRY(device_info(&d));
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const char* what = "train_samples_backward launches";
+  for (int ps = 0; ps < n_net; ++ps) {
+    const long long rows = live_samples_host[ps];
+    if (rows == 0) continue;
+    TrainLayout L;
+    train_skip_net_layout(&L, w.net_ws[ps], w.cap[ps], rows, d->sm_count);
+    const PassBufs& pb = L.pass[0];
+    TrainSkipBwdParams bp;
+    bp.n_rays = t.s.n; bp.S = ps ? t.s.Sc + t.s.K : t.s.Sc;
+    bp.n_rows = rows; bp.n_pad = pb.n_pad;
+    bp.rays = t.s.rays; bp.z = ps ? t.s.zf : t.zc;
+    bp.mask = t.s.mask[ps]; bp.ofs = t.ofs[ps];
+    bp.sigma = pb.sigma; bp.rgb = pb.rgb;
+    bp.noise = t.noise_std > 0.f ? t.noise[ps] : nullptr;
+    bp.noise_std = t.noise_std; bp.white_back = t.s.white_back;
+    bp.rgb_out = ps ? t.s.rgb_fine : t.s.rgb_coarse;
+    bp.target = a->target; bp.loss_grad = loss_grad;
+    bp.dsigma = pb.dsigma; bp.dprergb = pb.dprergb;
+    bp.amax_bits = L.amax;
+    bp.status = d->status;
+    TRY(launch(what, train_skip_bwd_kernel, grid_blocks(ceil_div(t.s.n, kSkipWarps), 1), kSkipWarps * 32, 0, s, bp));
+    float* const ds_out = ps ? a->dsigma_fine : a->dsigma_coarse;
+    float* const dp_out = ps ? a->dprergb_fine : a->dprergb_coarse;
+    if (ds_out)
+      CUDA_TRY(cudaMemcpyAsync(ds_out, pb.dsigma, sizeof(float) * rows, cudaMemcpyDeviceToDevice, s), "dsigma copy");
+    if (dp_out)
+      CUDA_TRY(cudaMemcpyAsync(dp_out, pb.dprergb, sizeof(float) * 3 * rows, cudaMemcpyDeviceToDevice, s),
+               "dprergb copy");
+    const float* const* const p2[2] = {params[ps], params[ps]};
+    float* const* const g2[2] = {grads[ps], grads[ps]};
+    const uint8_t* const net[2] = {t.s.net[ps], t.s.net[ps]};
+    TRY(backward_tail(L, p2, g2, net, nullptr, 0, d, s, what));
+  }
   return 0;
 }
 

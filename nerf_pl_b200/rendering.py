@@ -408,21 +408,35 @@ def render_rays_loss(models: List[torch.nn.Module],
                      white_back: bool = False,
                      *,
                      randoms: Optional[Dict[str, torch.Tensor]] = None,
-                     match_reference_rng: bool = True) -> Dict[str, torch.Tensor]:
+                     match_reference_rng: bool = True,
+                     occupancy=None) -> Dict[str, torch.Tensor]:
     """One training-step forward with the loss fused into the render launch: the reference's
     ``results = render_rays(...)`` (train.py:55-64), ``loss = MSELoss(results, rgbs)``
     (losses.py:9-14) and ``psnr(results['rgb_fine'], rgbs)`` (metrics.py:12-13, train.py:107-112) as
     ONE kernel.  Returns the render_rays result dict plus ``loss`` (differentiable scalar),
     ``psnr``, ``mse_coarse``, ``mse_fine``; ``loss.backward()`` runs the fused sm_90a backward with
-    the gradient seed 2 (rgb - rgbs) / (3 N) formed inside the compositing-backward kernel."""
+    the gradient seed 2 (rgb - rgbs) / (3 N) formed inside the compositing-backward kernel.
+
+    ``occupancy`` (a ``nerf_pl_b200.OccupancyGrid``) skips the empty samples of every ray (``train_skip.py``,
+    DESIGN.md "Training with empty samples skipped"): the result gains ``'live_samples'`` (evaluated coarse, fine
+    samples) and only ``loss`` carries a gradient.  It needs the render kernel's shapes and at most 2^22 rays
+    (ValueError), and a grid on the rays' device (RuntimeError); each step synchronises twice."""
     del chunk
     _check_render_inputs("render_rays_loss", models, embeddings, N_importance, rays)
     n, S_c, K = rays.shape[0], int(N_samples), int(N_importance)
     if n == 0:
         raise ValueError("empty ray batch")
+    if occupancy is not None:
+        from .train_skip import check_grid, check_shape
+        check_shape(n, S_c, K)
+        check_grid(occupancy, rays)
     rays_c = rays.detach().to(torch.float32).contiguous()
     pr, nc, ur, nf, seed = _resolve_randoms(randoms, n, S_c, K, float(perturb), float(noise_std), rays.device,
                                             match_reference_rng)
+    if occupancy is not None:
+        from .train_skip import render_rays_train_skip
+        return render_rays_train_skip(models, rays_c, S_c, use_disp, float(perturb), float(noise_std), K, white_back,
+                                      pr, nc, ur, nf, rgbs, occupancy, rng_seed=seed)
     from .training import render_rays_train
     return render_rays_train(models, rays_c, S_c, use_disp, float(perturb), float(noise_std), K, white_back,
                              pr, nc, ur, nf, target=rgbs, rng_seed=seed)
