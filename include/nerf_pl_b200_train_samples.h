@@ -77,9 +77,15 @@ size_t nerfb200_train_samples_workspace_bytes(int64_t n_rays, int32_t n_samples,
 
 /* The forward.  n_samples in {32, 64, 128}, n_importance a multiple of 32, their sum <= 192, 1 <= n_rays <= 2^22.
  * ws: 1024-byte aligned, held until the backward.  live_samples_host[2] receives the evaluated coarse and fine
- * sample counts.  Synchronises the stream twice (each count sizes the launches after it). */
+ * sample counts.  Synchronises the stream once, to read them back when the last pass's count is known; no launch is
+ * sized from them. */
 int nerfb200_train_samples_forward(const nerfb200_train_samples_args* args, void* ws, size_t bytes,
                                    int64_t* live_samples_host, void* stream);
+
+/* The same forward without the read-back: live_samples_dev[2] (device) receives the counts.  No launch is sized from
+ * a count on the host, and nothing is synchronised or read from host memory, so a CUDA graph can capture it. */
+int nerfb200_train_samples_forward_dev(const nerfb200_train_samples_args* args, void* ws, size_t bytes,
+                                       int64_t* live_samples_dev, void* stream);
 
 /* The backward of the forward that used `args`, `ws` and returned live_samples_host: the gradients of the 24
  * parameters of each network (the tables of nerfb200_backward_args) for the seed loss_grad (a device scalar dL/dloss
@@ -89,6 +95,14 @@ int nerfb200_train_samples_backward(const nerfb200_train_samples_args* args, voi
                                     const int64_t* live_samples_host, const float* loss_grad,
                                     const float* const params_coarse[24], const float* const params_fine[24],
                                     float* const grads_coarse[24], float* const grads_fine[24], void* stream);
+
+/* The backward of either forward with the counts the workspace holds (no host counts): capturable as the forward_dev
+ * entry.  Every network's gradients are written, exact zeros for one with no evaluated sample, so both tables must be
+ * complete.  The optional per-row outputs receive the first live_samples rows of each pass. */
+int nerfb200_train_samples_backward_dev(const nerfb200_train_samples_args* args, void* ws, size_t bytes,
+                                        const float* loss_grad, const float* const params_coarse[24],
+                                        const float* const params_fine[24], float* const grads_coarse[24],
+                                        float* const grads_fine[24], void* stream);
 
 #ifdef __cplusplus
 }

@@ -267,8 +267,10 @@ SAMPLES_SIGNATURES = {
 TRAIN_SAMPLES_SIGNATURES = {
     "nerfb200_train_samples_workspace_bytes": (_sz, [_i64, _i32, _i32]),
     "nerfb200_train_samples_forward": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_train_samples_forward_dev": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp]),
     "nerfb200_train_samples_backward": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp, _P, _P, _P, _P,
                                                 _vp]),
+    "nerfb200_train_samples_backward_dev": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, _vp, _P, _P, _P, _P, _vp]),
 }
 
 

@@ -152,6 +152,8 @@ struct MlpParams {
   const float* dirbias;
   // compacted-sample training mode (kRowsSave): the fp16 direction row of each ray, (., 64) [Embedding(3, 4)(d), 0..]
   const __half* dirrow;
+  // and the row count: *n_dev rows (the launch is sized for p.n, the carved worst case); tr.n_pad is derived from it
+  const long long* n_dev;
 };
 constexpr int kSkipDirStride = 2 * kDirW;   // per ray: the coarse network's direction bias, then the fine one's
 
@@ -162,7 +164,8 @@ constexpr int kSkipDirStride = 2 * kDirW;   // per ray: the coarse network's dir
 // (csrc/train_skip_kernels.cuh).  The direction still enters through the per-ray fp32 bias, so the values are the
 // compacted-sample mode's; xdir receives the row's ray's direction row, so that the direction-slice wgrad GEMM yields
 // gW_dir[:, 256:283].  Padding rows of the last tile are stored as copies of row n - 1 (their gradient is 0), so every
-// row below n_pad is written by this launch whatever an earlier, longer launch left in the workspace.
+// row below n_pad is written by this launch whatever an earlier, longer launch left in the workspace.  Its row count is
+// read on the device (n_dev), so a CUDA graph can capture the launch; CTAs past the count's tiles write nothing.
 template <bool kSave, bool kRowsSave = false>
 __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -176,7 +179,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
   __syncthreads();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const long long n_tiles = (p.n + 127) / 128;
+  const long long n_rows = kRowsSave ? *p.n_dev : 0;     // (kRowsSave ? n_rows : p.n) is the row count
+  const long long n_tiles = ((kRowsSave ? n_rows : p.n) + 127) / 128;
   const bool so = p.sigma_only != 0;
   const bool rows = kRowsSave || (!kSave && p.row_ray != nullptr);
   if (warp < kConsumerWarp0) {
@@ -198,14 +202,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
       c.save_act = p.tr.act;
       c.save_mask = p.tr.mask;
       c.save_d = p.tr.d;
-      c.save_n = p.tr.n_pad;
+      c.save_n = kRowsSave ? n_tiles * 128 : p.tr.n_pad;
     }
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       // this warpgroup's 64 rows of the ENC tile: two threads per row (the previous tile's MMAs that read
       // them have completed: every layer ends with wgmma.wait_group 0)
       {
         const int row = 64 * c.wg + (t >> 1);
-        const long long gi = min(tile * 128 + row, p.n - 1);
+        const long long gi = min(tile * 128 + row, (kRowsSave ? n_rows : p.n) - 1);
         const float* xr = p.x + gi * p.x_stride;
         if (rows) {
           // a sample of a ray, as the render kernel encodes it (its helper warps' encode_row)
@@ -260,7 +264,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
         const float* rbias[2];
 #pragma unroll
         for (int s = 0; s < 2; ++s)
-          rbias[s] = p.dirbias + static_cast<long long>(__ldg(p.row_ray + min(tile * 128 + c.row[s], p.n - 1))) *
+          rbias[s] = p.dirbias + static_cast<long long>(__ldg(p.row_ray + min(tile * 128 + c.row[s],
+                                                                             (kRowsSave ? n_rows : p.n) - 1))) *
                                      kSkipDirStride;
         if (kRowsSave) {
 #pragma unroll
@@ -284,7 +289,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           const long long gi = tile * 128 + c.row[s];
-          if (gi >= p.n) continue;
+          if (gi >= (kRowsSave ? n_rows : p.n)) continue;
           const float sg = c.cst[kF32BSigma] + sig[s];
           if (so && !kSave) {
             p.out[gi] = sg;

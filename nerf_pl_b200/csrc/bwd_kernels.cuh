@@ -322,109 +322,120 @@ struct HeadBwdParams {
 
 // (A two-role variant - one warp streaming d, a second one h8, 24 warps per SM instead of 16 - measured 128 us
 // against 88 us for this one: more warps in flight did not help, the extra address streams hurt.)
-__global__ void __launch_bounds__(kHeadWarps * 32) head_bwd_kernel(const HeadBwdParams p) {
-  __shared__ float red[kHeadWarps][kHeadPartFloats];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long unit = static_cast<long long>(blockIdx.x) * kHeadWarps + warp;     // (pass, ray)
-  const int ps = unit >= p.n_rays ? 1 : 0;
-  const long long ray = unit - (ps ? p.n_rays : 0);
-  const bool active = ray < p.n_rays && ps < p.n_pass;
-  float gw[3][4], gb[3] = {0.f, 0.f, 0.f}, rs[4] = {0.f, 0.f, 0.f, 0.f};
-  float gs[8], gsb = 0.f;       // sigma head: this lane's 8 columns of h8 (one 16-byte chunk), sum of dsigma
-#pragma unroll
-  for (int c = 0; c < 3; ++c)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) gw[c][i] = 0.f;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) gs[i] = 0.f;
-  if (active) {
-    const PassBufs& pb = p.pass[ps];
-    const int S = pb.S;
-    const float scale = p.lscale[ps * kLevels];
-    float w[3][4];
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) w[c][i] = p.w_rgb[ps][c * 128 + 4 * lane + i];
-    if (ps == 0 && lane < 15 && p.direnc != nullptr) {     // Embedding(3,4)(rays_d) exactly as render_kernel.cuh setup_group
-      const int cc = lane / 5, kk = lane % 5;
-      const float dv = p.rays[ray * p.ray_stride + 3 + cc];
-      float* de = p.direnc + ray * 28;
-      if (kk == 4) {
-        de[cc] = dv;
-      } else {
-        float sn, cs;
-        sincosf(__fmul_rn(static_cast<float>(1 << kk), dv), &sn, &cs);
-        de[3 + 6 * kk + cc] = sn;
-        de[3 + 6 * kk + 3 + cc] = cs;
-      }
-    }
-    // lane's 4 columns: column block lane / 16, 16-byte chunk (lane % 16) / 2, half (lane & 1)
-    const uint32_t fb = lane >> 4, ch = (lane & 15) >> 1, hf = (lane & 1) * 8;
-    const uint8_t* h8 = pb.act + 7ll * pb.n_pad * 512;
-    const long long g0 = ray * S;
-#pragma unroll 8
-    for (int i = 0; i < S; ++i) {
-      const long long g = g0 + i;
-      const unsigned long long off = tiled_block_off(static_cast<unsigned long long>(g >> 6), fb, 2) + (g & 63) * 128 +
-                                     ((ch ^ static_cast<uint32_t>(g & 7)) << 4) + hf;
-      const uint2 dv2 = __ldg(reinterpret_cast<const uint2*>(pb.d + off));
-      // h8 row: 32 lanes x 16 bytes, lane = (column block lane / 8, chunk lane % 8)
-      const uint4 hv = __ldg(reinterpret_cast<const uint4*>(
-          h8 + tiled_block_off(static_cast<unsigned long long>(g >> 6), lane >> 3, 4) + (g & 63) * 128 +
-          (((lane & 7u) ^ static_cast<uint32_t>(g & 7)) << 4)));
-      const float ds = __ldg(pb.dsigma + g);
-      {
-        const float2 a0 = __half22float2(*reinterpret_cast<const __half2*>(&hv.x));
-        const float2 a1 = __half22float2(*reinterpret_cast<const __half2*>(&hv.y));
-        const float2 a2 = __half22float2(*reinterpret_cast<const __half2*>(&hv.z));
-        const float2 a3 = __half22float2(*reinterpret_cast<const __half2*>(&hv.w));
-        gs[0] = fmaf(ds, a0.x, gs[0]); gs[1] = fmaf(ds, a0.y, gs[1]); gs[2] = fmaf(ds, a1.x, gs[2]); gs[3] = fmaf(ds, a1.y, gs[3]);
-        gs[4] = fmaf(ds, a2.x, gs[4]); gs[5] = fmaf(ds, a2.y, gs[5]); gs[6] = fmaf(ds, a3.x, gs[6]); gs[7] = fmaf(ds, a3.y, gs[7]);
-        gsb += ds;
-      }
-      const float q0 = __ldg(pb.dprergb + 3 * g), q1 = __ldg(pb.dprergb + 3 * g + 1), q2 = __ldg(pb.dprergb + 3 * g + 2);
-      const float2 d01 = __half22float2(*reinterpret_cast<const __half2*>(&dv2.x));
-      const float2 d23 = __half22float2(*reinterpret_cast<const __half2*>(&dv2.y));
-      const float dv[4] = {d01.x, d01.y, d23.x, d23.y};
-      float val[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        gw[0][k] = fmaf(q0, dv[k], gw[0][k]);
-        gw[1][k] = fmaf(q1, dv[k], gw[1][k]);
-        gw[2][k] = fmaf(q2, dv[k], gw[2][k]);
-        val[k] = (dv[k] > 0.f) ? fmaf(q0, w[0][k], fmaf(q1, w[1][k], q2 * w[2][k])) : 0.f;
-        rs[k] += val[k];
-      }
-      gb[0] += q0; gb[1] += q1; gb[2] += q2;
-      *reinterpret_cast<uint2*>(pb.dd + off) = make_uint2(cvt_bwd_x2(val[0] * scale, val[1] * scale),
-                                                          cvt_bwd_x2(val[2] * scale, val[3] * scale));
-    }
-    if (p.raysum[ps] != nullptr)
-      *reinterpret_cast<float4*>(p.raysum[ps] + ray * 128 + 4 * lane) = make_float4(rs[0], rs[1], rs[2], rs[3]);
+// The body of head_bwd_kernel and of head_bwd_dev_kernel over a HeadBwdParams `p`.  A macro rather than a device
+// function: the plain kernel then compiles to the instructions it had before the planned variant existed.
+#define NERFB200_HEAD_BWD_BODY                                                                                                      \
+  __shared__ float red[kHeadWarps][kHeadPartFloats];                                                                                \
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;                                                                       \
+  const long long unit = static_cast<long long>(blockIdx.x) * kHeadWarps + warp;  /* (pass, ray) */                                 \
+  const int ps = unit >= p.n_rays ? 1 : 0;                                                                                          \
+  const long long ray = unit - (ps ? p.n_rays : 0);                                                                                 \
+  const bool active = ray < p.n_rays && ps < p.n_pass;                                                                              \
+  float gw[3][4], gb[3] = {0.f, 0.f, 0.f}, rs[4] = {0.f, 0.f, 0.f, 0.f};                                                            \
+  float gs[8], gsb = 0.f;  /* sigma head: this lane's 8 columns of h8 (one 16-byte chunk), sum of dsigma */                         \
+_Pragma("unroll")                                                                                                                   \
+  for (int c = 0; c < 3; ++c)                                                                                                       \
+_Pragma("unroll")                                                                                                                   \
+    for (int i = 0; i < 4; ++i) gw[c][i] = 0.f;                                                                                     \
+_Pragma("unroll")                                                                                                                   \
+  for (int i = 0; i < 8; ++i) gs[i] = 0.f;                                                                                          \
+  if (active) {                                                                                                                     \
+    const PassBufs& pb = p.pass[ps];                                                                                                \
+    const int S = pb.S;                                                                                                             \
+    const float scale = p.lscale[ps * kLevels];                                                                                     \
+    float w[3][4];                                                                                                                  \
+_Pragma("unroll")                                                                                                                   \
+    for (int c = 0; c < 3; ++c)                                                                                                     \
+_Pragma("unroll")                                                                                                                   \
+      for (int i = 0; i < 4; ++i) w[c][i] = p.w_rgb[ps][c * 128 + 4 * lane + i];                                                    \
+    if (ps == 0 && lane < 15 && p.direnc != nullptr) {  /* Embedding(3,4)(rays_d) exactly as render_kernel.cuh setup_group */       \
+      const int cc = lane / 5, kk = lane % 5;                                                                                       \
+      const float dv = p.rays[ray * p.ray_stride + 3 + cc];                                                                         \
+      float* de = p.direnc + ray * 28;                                                                                              \
+      if (kk == 4) {                                                                                                                \
+        de[cc] = dv;                                                                                                                \
+      } else {                                                                                                                      \
+        float sn, cs;                                                                                                               \
+        sincosf(__fmul_rn(static_cast<float>(1 << kk), dv), &sn, &cs);                                                              \
+        de[3 + 6 * kk + cc] = sn;                                                                                                   \
+        de[3 + 6 * kk + 3 + cc] = cs;                                                                                               \
+      }                                                                                                                             \
+    }                                                                                                                               \
+    /* lane's 4 columns: column block lane / 16, 16-byte chunk (lane % 16) / 2, half (lane & 1) */                                  \
+    const uint32_t fb = lane >> 4, ch = (lane & 15) >> 1, hf = (lane & 1) * 8;                                                      \
+    const uint8_t* h8 = pb.act + 7ll * pb.n_pad * 512;                                                                              \
+    const long long g0 = ray * S;                                                                                                   \
+_Pragma("unroll 8")                                                                                                                 \
+    for (int i = 0; i < S; ++i) {                                                                                                   \
+      const long long g = g0 + i;                                                                                                   \
+      const unsigned long long off = tiled_block_off(static_cast<unsigned long long>(g >> 6), fb, 2) + (g & 63) * 128 +             \
+                                     ((ch ^ static_cast<uint32_t>(g & 7)) << 4) + hf;                                               \
+      const uint2 dv2 = __ldg(reinterpret_cast<const uint2*>(pb.d + off));                                                          \
+      /* h8 row: 32 lanes x 16 bytes, lane = (column block lane / 8, chunk lane % 8) */                                             \
+      const uint4 hv = __ldg(reinterpret_cast<const uint4*>(                                                                        \
+          h8 + tiled_block_off(static_cast<unsigned long long>(g >> 6), lane >> 3, 4) + (g & 63) * 128 +                            \
+          (((lane & 7u) ^ static_cast<uint32_t>(g & 7)) << 4)));                                                                    \
+      const float ds = __ldg(pb.dsigma + g);                                                                                        \
+      {                                                                                                                             \
+        const float2 a0 = __half22float2(*reinterpret_cast<const __half2*>(&hv.x));                                                 \
+        const float2 a1 = __half22float2(*reinterpret_cast<const __half2*>(&hv.y));                                                 \
+        const float2 a2 = __half22float2(*reinterpret_cast<const __half2*>(&hv.z));                                                 \
+        const float2 a3 = __half22float2(*reinterpret_cast<const __half2*>(&hv.w));                                                 \
+        gs[0] = fmaf(ds, a0.x, gs[0]); gs[1] = fmaf(ds, a0.y, gs[1]); gs[2] = fmaf(ds, a1.x, gs[2]); gs[3] = fmaf(ds, a1.y, gs[3]); \
+        gs[4] = fmaf(ds, a2.x, gs[4]); gs[5] = fmaf(ds, a2.y, gs[5]); gs[6] = fmaf(ds, a3.x, gs[6]); gs[7] = fmaf(ds, a3.y, gs[7]); \
+        gsb += ds;                                                                                                                  \
+      }                                                                                                                             \
+      const float q0 = __ldg(pb.dprergb + 3 * g), q1 = __ldg(pb.dprergb + 3 * g + 1), q2 = __ldg(pb.dprergb + 3 * g + 2);           \
+      const float2 d01 = __half22float2(*reinterpret_cast<const __half2*>(&dv2.x));                                                 \
+      const float2 d23 = __half22float2(*reinterpret_cast<const __half2*>(&dv2.y));                                                 \
+      const float dv[4] = {d01.x, d01.y, d23.x, d23.y};                                                                             \
+      float val[4];                                                                                                                 \
+_Pragma("unroll")                                                                                                                   \
+      for (int k = 0; k < 4; ++k) {                                                                                                 \
+        gw[0][k] = fmaf(q0, dv[k], gw[0][k]);                                                                                       \
+        gw[1][k] = fmaf(q1, dv[k], gw[1][k]);                                                                                       \
+        gw[2][k] = fmaf(q2, dv[k], gw[2][k]);                                                                                       \
+        val[k] = (dv[k] > 0.f) ? fmaf(q0, w[0][k], fmaf(q1, w[1][k], q2 * w[2][k])) : 0.f;                                          \
+        rs[k] += val[k];                                                                                                            \
+      }                                                                                                                             \
+      gb[0] += q0; gb[1] += q1; gb[2] += q2;                                                                                        \
+      *reinterpret_cast<uint2*>(pb.dd + off) = make_uint2(cvt_bwd_x2(val[0] * scale, val[1] * scale),                               \
+                                                          cvt_bwd_x2(val[2] * scale, val[3] * scale));                              \
+    }                                                                                                                               \
+    if (p.raysum[ps] != nullptr)                                                                                                    \
+      *reinterpret_cast<float4*>(p.raysum[ps] + ray * 128 + 4 * lane) = make_float4(rs[0], rs[1], rs[2], rs[3]);                    \
+  }                                                                                                                                 \
+  /* per-block partial of gW_rgb / gb_rgb: warps in fixed order */                                                                  \
+_Pragma("unroll")                                                                                                                   \
+  for (int c = 0; c < 3; ++c)                                                                                                       \
+_Pragma("unroll")                                                                                                                   \
+    for (int k = 0; k < 4; ++k) red[warp][c * 128 + 4 * lane + k] = gw[c][k];                                                       \
+  if (lane < 4) red[warp][kHeadPartRgbB + lane] = (lane < 3) ? gb[lane] : 0.f;                                                      \
+_Pragma("unroll")                                                                                                                   \
+  for (int k = 0; k < 8; ++k) red[warp][kHeadPartSigW + 8 * lane + k] = gs[k];                                                      \
+  if (lane < 4) red[warp][kHeadPartSigB + lane] = (lane == 0) ? gsb : 0.f;                                                          \
+  __syncthreads();                                                                                                                  \
+  /* a block's warps all belong to one pass unless it straddles the boundary: sum per pass */                                       \
+  for (int q = 0; q < p.n_pass; ++q) {                                                                                              \
+    float* out = p.part[q] + static_cast<long long>(blockIdx.x) * kHeadPartFloats;                                                  \
+    for (int i = threadIdx.x; i < kHeadPartFloats; i += blockDim.x) {                                                               \
+      float acc = 0.f;                                                                                                              \
+      for (int wv = 0; wv < kHeadWarps; ++wv) {                                                                                     \
+        const long long u = static_cast<long long>(blockIdx.x) * kHeadWarps + wv;                                                   \
+        if ((u >= p.n_rays ? 1 : 0) == q) acc += red[wv][i];                                                                        \
+      }                                                                                                                             \
+      out[i] = acc;                                                                                                                 \
+    }                                                                                                                               \
   }
-  // per-block partial of gW_rgb / gb_rgb: warps in fixed order
-#pragma unroll
-  for (int c = 0; c < 3; ++c)
-#pragma unroll
-    for (int k = 0; k < 4; ++k) red[warp][c * 128 + 4 * lane + k] = gw[c][k];
-  if (lane < 4) red[warp][kHeadPartRgbB + lane] = (lane < 3) ? gb[lane] : 0.f;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) red[warp][kHeadPartSigW + 8 * lane + k] = gs[k];
-  if (lane < 4) red[warp][kHeadPartSigB + lane] = (lane == 0) ? gsb : 0.f;
-  __syncthreads();
-  // a block's warps all belong to one pass unless it straddles the boundary: sum per pass
-  for (int q = 0; q < p.n_pass; ++q) {
-    float* out = p.part[q] + static_cast<long long>(blockIdx.x) * kHeadPartFloats;
-    for (int i = threadIdx.x; i < kHeadPartFloats; i += blockDim.x) {
-      float acc = 0.f;
-      for (int wv = 0; wv < kHeadWarps; ++wv) {
-        const long long u = static_cast<long long>(blockIdx.x) * kHeadWarps + wv;
-        if ((u >= p.n_rays ? 1 : 0) == q) acc += red[wv][i];
-      }
-      out[i] = acc;
-    }
-  }
+
+__global__ void __launch_bounds__(kHeadWarps * 32) head_bwd_kernel(const HeadBwdParams p) { NERFB200_HEAD_BWD_BODY }
+// The same with its parameters planned on the device (capi.cu train_skip_plan_kernel): launched at the grid of the
+// carved worst case, the blocks past the plan's *grid return without writing.
+__global__ void __launch_bounds__(kHeadWarps * 32) head_bwd_dev_kernel(const HeadBwdParams* __restrict__ pp,
+                                                                        const int* __restrict__ grid) {
+  if (static_cast<int>(blockIdx.x) >= *grid) return;
+  const HeadBwdParams& p = *pp;
+  NERFB200_HEAD_BWD_BODY
 }
 
 // gW_dir[n][256 + j] = sum_rays raysum[ray][n] dir_enc[ray][j]: block = 128 threads (n), blockIdx.x = ray slice,
@@ -553,7 +564,7 @@ __device__ __forceinline__ float chain_epi(const WgCtx& c, uint8_t* dpre, const 
 }
 
 template <bool kProbe>
-__global__ void __launch_bounds__(kThreads, 1) chain_bwd_kernel(const ChainParams p) {
+__device__ __forceinline__ void chain_bwd_body(const ChainParams& p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   ChainScratch* sc = reinterpret_cast<ChainScratch*>(smem + kChScratch);
   Barriers* bars = &sc->bars;
@@ -667,6 +678,14 @@ __global__ void __launch_bounds__(kThreads, 1) chain_bwd_kernel(const ChainParam
         }
     }
   }
+}
+template <bool kProbe>
+__global__ void __launch_bounds__(kThreads, 1) chain_bwd_kernel(const ChainParams p) { chain_bwd_body<kProbe>(p); }
+// The same with its parameters planned on the device: launched at the grid of the carved worst case, a CTA whose
+// first visit is past the plan's tiles visits none.
+template <bool kProbe>
+__global__ void __launch_bounds__(kThreads, 1) chain_bwd_dev_kernel(const ChainParams* __restrict__ p) {
+  chain_bwd_body<kProbe>(*p);
 }
 
 // ------------------------------------------------------------------------------------ wgrad
@@ -892,8 +911,7 @@ struct ReduceTable {
   ReduceItem it[kMaxReduceItems];
 };
 
-__global__ void __launch_bounds__(256) wgrad_reduce_kernel(const __grid_constant__ ReduceTable tab) {
-  const ReduceItem& it = tab.it[blockIdx.y];
+__device__ __forceinline__ void reduce_item(const ReduceItem& it) {
   const int total = it.rows * it.cols;
   const float mul = (it.mul != nullptr) ? *it.mul : 1.f;
   if (it.by_warp) {        // fixed order: lane l sums partials l, l + 32, ...; then a butterfly over the lanes
@@ -923,6 +941,13 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const __grid_constant
     for (int s = 0; s < it.n_split; ++s) acc += src[s * it.split_stride];
     it.out[static_cast<long long>(r) * it.out_ld + it.out_col0 + c] = acc * mul;
   }
+}
+__global__ void __launch_bounds__(256) wgrad_reduce_kernel(const __grid_constant__ ReduceTable tab) {
+  reduce_item(tab.it[blockIdx.y]);
+}
+// The same over a table planned on the device (its item count, the grid's y, does not depend on the plan).
+__global__ void __launch_bounds__(256) wgrad_reduce_dev_kernel(const ReduceTable* __restrict__ tab) {
+  reduce_item(tab->it[blockIdx.y]);
 }
 
 // Chain rule through the pack-time folding (layout.h): W' = Wd[:, :256] Wf, b' = Wd[:, :256] bf + bd

@@ -149,6 +149,10 @@ int device_info(DeviceInfo** out) {
                                   static_cast<int>(kChSmemTotal)), "smem attr chain");
     CUDA_TRY(cudaFuncSetAttribute(chain_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kChSmemTotal)), "smem attr chain (probe)");
+    CUDA_TRY(cudaFuncSetAttribute(chain_bwd_dev_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kChSmemTotal)), "smem attr chain (planned)");
+    CUDA_TRY(cudaFuncSetAttribute(chain_bwd_dev_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kChSmemTotal)), "smem attr chain (planned probe)");
     CUDA_TRY(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kWgSmemTotal)), "smem attr wgrad");
     // one cdf of n_weights + 1 floats per warp: above the 48 KB default from n_weights = 3072
@@ -259,9 +263,9 @@ struct TrainLayout {
   size_t bytes;
 };
 
-void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first);
+__host__ __device__ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first);
 
-void job_shape(int kind, int* a_fb, int* b_fb) {
+__host__ __device__ void job_shape(int kind, int* a_fb, int* b_fb) {
   *a_fb = (kind == kJ9 || kind == kJDir) ? 2 : 4;
   *b_fb = (kind == kJ1 || kind == kJ5a || kind == kJDir) ? 1 : 4;
 }
@@ -333,8 +337,9 @@ void make_train_layout(TrainLayout* L, uint8_t* base, bool mlp, int64_t n, int n
 }
 
 // The wgrad plan of a layout: CTA counts per (pass, layer) (always), and when `jobs` / `cta_first` are
-// given the host image of the piece table and of the per-CTA piece ranges.
-void job_operands(const TrainLayout& L, int ps, int k, const uint8_t** A, const uint8_t** B) {
+// given the image of the piece table and of the per-CTA piece ranges (host memory for the plain paths, the
+// workspace's tables for train_skip_plan_kernel).
+__host__ __device__ void job_operands(const TrainLayout& L, int ps, int k, const uint8_t** A, const uint8_t** B) {
   const PassBufs& b = L.pass[ps];
   const size_t lay = static_cast<size_t>(b.n_pad) * 512;
   switch (k) {
@@ -351,7 +356,7 @@ void job_operands(const TrainLayout& L, int ps, int k, const uint8_t** A, const 
   }
 }
 
-void fill_piece(TrainLayout* L, WgradJob* jobs, int piece, int cta, int ps, int k, long long c0, long long c1,
+__host__ __device__ void fill_piece(TrainLayout* L, WgradJob* jobs, int piece, int cta, int ps, int k, long long c0, long long c1,
                 int step, bool add) {
   if (!jobs) return;
   int a_fb, b_fb;
@@ -369,7 +374,7 @@ void fill_piece(TrainLayout* L, WgradJob* jobs, int piece, int cta, int ps, int 
   j.bias_out = (k == kJ5b || k == kJDir) ? nullptr : slot + 256 * 256;
 }
 
-void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
+__host__ __device__ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
   if (n_cta > kMaxWgCtas) n_cta = kMaxWgCtas;
   const int kinds = L->n_kinds;
   long long total = 0;
@@ -388,7 +393,7 @@ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
   int used = 0;
   for (int ps = 0; ps < L->n_pass; ++ps)
     for (int k = 0; k < kinds; ++k) {
-      const double share = static_cast<double>(work[ps][k]) * n_cta / static_cast<double>(total);
+      const double share = total > 0 ? static_cast<double>(work[ps][k]) * n_cta / static_cast<double>(total) : 0.0;
       int n = static_cast<int>(share);
       if (n < 1) n = 1;
       n_of[ps][k] = n;
@@ -414,8 +419,8 @@ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
   int n_cta_used = 0;
   for (int ps = 0; ps < L->n_pass; ++ps)
     for (int k = 0; k < kinds; ++k)
-      n_cta_used += static_cast<int>(std::min<long long>(n_of[ps][k], L->pass[ps].n_pad / 64));
-  const int max_pieces = kMaxWgJobs / n_cta_used;        // per CTA
+      n_cta_used += static_cast<int>(n_of[ps][k] < L->pass[ps].n_pad / 64 ? n_of[ps][k] : L->pass[ps].n_pad / 64);
+  const int max_pieces = n_cta_used > 0 ? kMaxWgJobs / n_cta_used : kMaxWgJobs;        // per CTA
   int piece = 0, cta = 0;
   for (int ps = 0; ps < L->n_pass; ++ps)
     for (int k = 0; k < kinds; ++k) {
@@ -423,12 +428,21 @@ void plan_wgrad(TrainLayout* L, int n_cta, WgradJob* jobs, int* cta_first) {
       int g = n_of[ps][k];
       if (g > chunks) g = static_cast<int>(chunks);
       L->first_cta[ps][k] = cta;
+      // CTA j's share, ceil((chunks - j) / g) chunks, is q + 1 for j < r and q for the others (chunks = q g + r): the
+      // divisions are per GEMM, not per CTA (train_skip_plan_kernel runs this on one device thread)
+      const long long q = g > 0 ? chunks / g : 0, r = g > 0 ? chunks - q * g : 0;
+      long long len_of[2];
+      for (int e = 0; e < 2; ++e) {
+        const long long want = (q + 1 - e + max_pieces - 1) / max_pieces;
+        len_of[e] = want > kWgPieceChunks ? want : kWgPieceChunks;
+      }
       for (int j = 0; j < g; ++j, ++cta) {
-        const long long mine = (chunks - j + g - 1) / g;
-        const long long len = std::max<long long>(kWgPieceChunks, (mine + max_pieces - 1) / max_pieces);
+        const int e = j < r ? 0 : 1;
+        const long long mine = q + 1 - e, len = len_of[e];
         if (cta_first) cta_first[cta] = piece;
         for (long long s = 0; s < mine; s += len, ++piece)
-          fill_piece(L, jobs, piece, cta, ps, k, j + s * g, std::min(chunks, j + (s + len) * g), g, s > 0);
+          fill_piece(L, jobs, piece, cta, ps, k, j + s * g, chunks < j + (s + len) * g ? chunks : j + (s + len) * g, g,
+                     s > 0);
       }
       L->n_split[ps][k] = g;
     }
@@ -455,39 +469,59 @@ Arena g_arena[64];
 std::mutex g_host_call_mu;
 std::mutex g_arena_mu;   // separate from g_mu: the host entry calls nerfb200_render_rays (device_info locks g_mu)
 
-// Step 3 of a training backward: the chain kernel's probe pass over pt0 + pt1 tiles spread evenly over each pass, the
-// phase-1 scales, then the real pass over all t0 + t1 tiles (the probe's first).  cp: everything but the visit order.
-int launch_chain(ChainParams& cp, long long t0, long long t1, long long pt0, long long pt1, ScaleParams& sp, int sm_count,
-                 cudaStream_t stream, const char* what) {
-  const long long span[2] = {t0, t1}, pt[2] = {pt0, pt1};
-  auto gcd = [](long long x, long long y) {
-    while (y != 0) { const long long r = x % y; x = y; y = r; }
-    return x;
-  };
+// Step 3 of a training backward: the chain kernel's probe pass over pt0 + pt1 tiles spread evenly over each pass, then
+// (after the phase-1 scales) the real pass over all t0 + t1 tiles, the probe's first.  The parameters of both launches
+// from a layout, on the host for the plain paths and on the device for train_skip_plan_kernel.
+__host__ __device__ void chain_plan(const TrainLayout& L, const uint8_t* const net[2], int* status, int sm_count,
+                                    ChainParams* probe, ChainParams* real) {
+  ChainParams& cp = *probe;
+  const int q1 = L.n_pass > 1 ? 1 : 0;
+  cp.n_pass = L.n_pass;
+  cp.pass[0] = L.pass[0]; cp.pass[1] = L.pass[1];
+  cp.net[0] = net[0]; cp.net[1] = net[1];
+  cp.lscale = L.lscale;
+  cp.lamax = L.lamax;
+  cp.status = status;
+  const long long t0 = L.pass[0].n_pad / 128, t1 = q1 ? L.pass[1].n_pad / 128 : 0;
+  const long long n_probe = q1 ? (sm_count + 1) / 2 : sm_count;      // probe tiles per pass, at most
+  const long long span[2] = {t0, t1}, pt[2] = {t0 < n_probe ? t0 : n_probe, t1 < n_probe ? t1 : n_probe};
   for (int ps = 0; ps < 2; ++ps) {
     long long s = (pt[ps] > 0 && span[ps] > pt[ps]) ? span[ps] / pt[ps] : 1;
-    while (span[ps] > 1 && gcd(s, span[ps]) != 1) ++s;
+    for (;;) {                    // the smallest stride from span / probe tiles up that is coprime to the span
+      long long x = s, y = span[ps];
+      while (y != 0) { const long long r = x % y; x = y; y = r; }
+      if (span[ps] <= 1 || x == 1) break;
+      ++s;
+    }
     cp.span[ps] = span[ps] > 0 ? span[ps] : 1;
     cp.stride[ps] = s;
+    cp.tiles[ps] = cp.head[ps] = pt[ps];
   }
-  cp.tiles[0] = cp.head[0] = pt0;
-  cp.tiles[1] = cp.head[1] = pt1;
-  const int pc = static_cast<int>(pt0 + pt1);
-  TRY(launch(what, chain_bwd_kernel<true>, pc, kThreads, kChSmemTotal, stream, cp));
-  sp.phase = 1;
-  TRY(launch(what, bwd_scale_kernel, 1, 128, 0, stream, sp));
-  cp.head[0] = pt0;
-  cp.head[1] = pt1;
-  cp.tiles[0] = t0;
-  cp.tiles[1] = t1;
-  const long long total = t0 + t1;
-  const int ctas = static_cast<int>(total < sm_count ? total : sm_count);
-  return launch(what, chain_bwd_kernel<false>, ctas, kThreads, kChSmemTotal, stream, cp);
+  *real = cp;
+  real->tiles[0] = t0;
+  real->tiles[1] = t1;
+}
+
+// Step 2: the head kernel's parameters (host and device, as chain_plan).
+__host__ __device__ void head_plan(const TrainLayout& L, const float* w_rgb0, const float* w_rgb1, const float* rays,
+                                   long long ray_stride, HeadBwdParams* hp) {
+  hp->n_rays = L.n_rays; hp->n_pass = L.n_pass;
+  hp->pass[0] = L.pass[0]; hp->pass[1] = L.pass[1];
+  if (!rays) {
+    hp->pass[0].S = kMlpPseudoRay;
+    hp->pass[1] = hp->pass[0];
+  }
+  hp->w_rgb[0] = w_rgb0; hp->w_rgb[1] = w_rgb1;
+  hp->lscale = L.lscale;
+  hp->rays = rays; hp->ray_stride = ray_stride;
+  hp->raysum[0] = L.raysum[0]; hp->raysum[1] = L.raysum[1];
+  hp->direnc = L.direnc;
+  hp->part[0] = L.head_part[0]; hp->part[1] = L.head_part[1];
 }
 
 // Step 5: the reduction items of pass ps that both training backwards share (wgrad GEMMs of layers 1..8 and of the
 // folded W', the head partials), appended to `tab`.  g: the pass's 24 gradient tensors.
-void add_reduce_items(ReduceTable& tab, const TrainLayout& L, int ps, float* const* g) {
+__host__ __device__ void add_reduce_items(ReduceTable& tab, const TrainLayout& L, int ps, float* const* g) {
   auto add = [&](const float* part, long long stride, int n_split, float* out, const float* mul, int rows, int cols,
                  int part_ld, int out_ld, int out_col0, int transposed = 0) {
     ReduceItem& it = tab.it[tab.n++];
@@ -539,13 +573,24 @@ int init_train_workspace(TrainLayout& L, void* ws, int sm_count, cudaStream_t st
   return 0;
 }
 
+// The count-dependent launch parameters of one network's backward tail when training with empty samples skipped,
+// written into the workspace by train_skip_plan_kernel from the device's sample count.
+struct TrainSkipPlan {
+  HeadBwdParams head;
+  int head_grid;
+  ChainParams probe, chain;
+  ReduceTable tab;
+};
+
 // Steps 2-6 of both training backwards, once step 1 has left each pass's per-sample d sigma / d rgb_pre and their
 // maxima in the workspace.  params / grads / net: per pass.  rays: the render path's rays, whose directions the head
 // kernel embeds for the per-ray direction part of gW_dir; null for a direct NeRF.forward call, whose head kernel walks
-// pseudo-rays of 64 samples and whose direction part is the wgrad GEMM kJDir.
+// pseudo-rays of 64 samples and whose direction part is the wgrad GEMM kJDir.  plan: null, or the device plan of a
+// layout carved for more rows (training with empty samples skipped): every launch then has the grid of L, the carved
+// worst case, and the count-dependent kernels read their parameters from the plan.
 int backward_tail(const TrainLayout& L, const float* const* const params[2], float* const* const grads[2],
                   const uint8_t* const net[2], const float* rays, long long ray_stride, const DeviceInfo* d,
-                  cudaStream_t stream, const char* what) {
+                  cudaStream_t stream, const char* what, const TrainSkipPlan* plan = nullptr) {
   const int q1 = L.n_pass > 1 ? 1 : 0;        // table entry of the second pass: a single pass fills both slots
   ScaleParams sp;
   sp.n_pass = L.n_pass; sp.phase = 0;
@@ -555,19 +600,11 @@ int backward_tail(const TrainLayout& L, const float* const* const params[2], flo
   TRY(launch(what, bwd_scale_kernel, 1, 128, 0, stream, sp));
   // 2. rgb head, ReLU of the direction layer (both passes in one launch), direction part of gW_dir
   HeadBwdParams hp;
-  hp.n_rays = L.n_rays; hp.n_pass = L.n_pass;
-  hp.pass[0] = L.pass[0]; hp.pass[1] = L.pass[1];
-  if (!rays) {
-    hp.pass[0].S = kMlpPseudoRay;
-    hp.pass[1] = hp.pass[0];
-  }
-  hp.w_rgb[0] = params[0][22]; hp.w_rgb[1] = params[q1][22];
-  hp.lscale = L.lscale;
-  hp.rays = rays; hp.ray_stride = ray_stride;
-  hp.raysum[0] = L.raysum[0]; hp.raysum[1] = L.raysum[1];
-  hp.direnc = L.direnc;
-  hp.part[0] = L.head_part[0]; hp.part[1] = L.head_part[1];
-  TRY(launch(what, head_bwd_kernel, L.head_grid, kHeadWarps * 32, 0, stream, hp));
+  head_plan(L, params[0][22], params[q1][22], rays, ray_stride, &hp);
+  if (plan)
+    TRY(launch(what, head_bwd_dev_kernel, L.head_grid, kHeadWarps * 32, 0, stream, &plan->head, &plan->head_grid));
+  else
+    TRY(launch(what, head_bwd_kernel, L.head_grid, kHeadWarps * 32, 0, stream, hp));
   if (rays) {
     DirGradParams dp;
     dp.n_rays = L.n_rays;
@@ -582,16 +619,21 @@ int backward_tail(const TrainLayout& L, const float* const* const params[2], flo
   // Both launches visit the tiles of a pass in the order j -> j * stride mod span (stride coprime to span, about
   // span / probe tiles), the real pass the probe's tiles first, so its first wave finds them in L2.  A tile the
   // probe did not see can still exceed its level's range: the wgrad kernel reports that (status 102).
-  ChainParams cp;
-  cp.n_pass = L.n_pass;
-  cp.pass[0] = L.pass[0]; cp.pass[1] = L.pass[1];
-  cp.net[0] = net[0]; cp.net[1] = net[1];
-  cp.lscale = L.lscale;
-  cp.lamax = L.lamax;
-  cp.status = d->status;
-  const long long t0 = L.pass[0].n_pad / 128, t1 = q1 ? L.pass[1].n_pad / 128 : 0;
-  const long long probe = q1 ? (d->sm_count + 1) / 2 : d->sm_count;      // probe tiles per pass, at most
-  TRY(launch_chain(cp, t0, t1, t0 < probe ? t0 : probe, t1 < probe ? t1 : probe, sp, d->sm_count, stream, what));
+  ChainParams probe, cp;
+  chain_plan(L, net, d->status, d->sm_count, &probe, &cp);
+  const int probe_ctas = static_cast<int>(probe.tiles[0] + probe.tiles[1]);
+  const long long total = cp.tiles[0] + cp.tiles[1];
+  const int ctas = static_cast<int>(total < d->sm_count ? total : d->sm_count);
+  if (plan)
+    TRY(launch(what, chain_bwd_dev_kernel<true>, probe_ctas, kThreads, kChSmemTotal, stream, &plan->probe));
+  else
+    TRY(launch(what, chain_bwd_kernel<true>, probe_ctas, kThreads, kChSmemTotal, stream, probe));
+  sp.phase = 1;
+  TRY(launch(what, bwd_scale_kernel, 1, 128, 0, stream, sp));
+  if (plan)
+    TRY(launch(what, chain_bwd_dev_kernel<false>, ctas, kThreads, kChSmemTotal, stream, &plan->chain));
+  else
+    TRY(launch(what, chain_bwd_kernel<false>, ctas, kThreads, kChSmemTotal, stream, cp));
   // 4. split-K wgrad (wgmma)
   TRY(launch(what, wgrad_kernel, L.n_cta, kWgThreads, kWgSmemTotal, stream, L.jobs_dev, L.cta_first_dev, d->status));
   // 5. partial sums -> gradient tensors (fixed order), 6. unfold W'
@@ -599,7 +641,10 @@ int backward_tail(const TrainLayout& L, const float* const* const params[2], flo
   tab.n = 0;
   for (int ps = 0; ps < L.n_pass; ++ps) add_reduce_items(tab, L, ps, grads[ps]);
   // latency-bound: 64 blocks per item (16 measured 40 us)
-  TRY(launch(what, wgrad_reduce_kernel, dim3(64, tab.n), 256, 0, stream, tab));
+  if (plan)
+    TRY(launch(what, wgrad_reduce_dev_kernel, dim3(64, tab.n), 256, 0, stream, &plan->tab));
+  else
+    TRY(launch(what, wgrad_reduce_kernel, dim3(64, tab.n), 256, 0, stream, tab));
   UnfoldParams up;
   for (int ps = 0; ps < 2; ++ps) {
     const int q = ps ? q1 : 0;
@@ -945,12 +990,17 @@ int skip_grid(const uint32_t* bits, int64_t N, const double* ranges, SkipGrid* g
 
 // ------------------------------------------------------------------ training with empty samples skipped
 // (kernels: train_skip_kernels.cuh).  One workspace per batch shape, sized for every sample evaluated: the per-ray
-// buffers, the compacted rows of the larger pass, then one NeRF.forward training workspace per network carved for
-// that worst case.  A step's layout keeps the carved addresses and takes its own row count (train_skip_net_layout),
-// so nothing is reallocated or re-zeroed between steps; the forward uploads the step's wgrad plans.
+// buffers, the compacted rows of the larger pass, then per network a NeRF.forward training workspace carved for that
+// worst case and the device plan of its backward.  Nothing is reallocated or re-zeroed between steps, and no launch
+// is sized on the host from a step's sample count: each pass's count stays on the device (the total of its scan),
+// the compacted-row MLP reads it, and train_skip_plan_kernel turns it into the backward's layout, wgrad tables, head /
+// chain parameters and reduction table.  Every launch has the grid of the carved worst case, so the step can be
+// captured in a CUDA graph.
 struct TrainSkipWs {
   TrainSkipParams t;
   uint8_t* net_ws[2];
+  TrainSkipPlan* plan[2];
+  long long* live;              // [2] the eager forward's counts, read back once
   long long cap[2];             // rows of each network with every sample evaluated
 };
 
@@ -970,41 +1020,70 @@ size_t train_skip_carve(long long n, int Sc, int K, void* base, int sm_count, Tr
   p.row_ray = c.take<int>(rows);
   p.row_z = c.take<float>(rows);
   p.mlp_out = c.take<float>(rows * 4);
+  w->live = c.take<long long>(2);
   w->net_ws[0] = w->net_ws[1] = nullptr;
+  w->plan[0] = w->plan[1] = nullptr;
   w->cap[0] = w->cap[1] = 0;
   for (int ps = 0; ps < (K > 0 ? 2 : 1); ++ps) {
     w->cap[ps] = n * (ps ? Sf : Sc);
     TrainLayout L;
     make_train_layout(&L, nullptr, true, w->cap[ps], 1, 0, sm_count);
     w->net_ws[ps] = c.take(L.bytes);
+    w->plan[ps] = c.take<TrainSkipPlan>(1);
   }
   return c.off;
 }
 
-// The NeRF.forward training layout of `rows` rows inside a workspace carved for `cap` rows.  Every buffer keeps its
-// worst-case address; the row count, the padded row count (the stride of the activation layers), the head kernel's
-// pseudo-rays and the wgrad plan are the step's.  The plan of fewer rows needs no more CTAs, pieces or head blocks
-// than the carved one.
-void train_skip_net_layout(TrainLayout* L, uint8_t* base, long long cap, long long rows, int sm_count) {
-  make_train_layout(L, base, true, cap, 1, 0, sm_count);
+// The NeRF.forward training layout of `rows` rows inside a layout carved for more: every buffer keeps its worst-case
+// address; the row count, the padded row count (the stride of the activation layers) and the head kernel's
+// pseudo-rays and blocks are the step's.  With the wgrad plan (plan_wgrad) this plan of fewer rows needs no more
+// CTAs, pieces or head blocks than the carved one.
+__host__ __device__ void train_skip_rows(TrainLayout* L, long long rows) {
   PassBufs& b = L->pass[0];
   b.n = rows;
   b.n_pad = (rows + 127) / 128 * 128;
   L->n_rays = static_cast<int>(b.n_pad / kMlpPseudoRay);
   L->head_grid = (L->n_rays + kHeadWarps - 1) / kHeadWarps;
-  plan_wgrad(L, sm_count, nullptr, nullptr);
 }
 
-// Upload the wgrad plan of a step's layout (called right after a count read-back, when the stream is idle).
-int train_skip_upload_plan(TrainLayout& L, int sm_count, cudaStream_t s) {
-  std::vector<WgradJob> jobs(kMaxWgJobs);
-  std::vector<int> cta_first(kMaxWgCtas + 1, 0);
-  plan_wgrad(&L, sm_count, jobs.data(), cta_first.data());
-  CUDA_TRY(cudaMemcpyAsync(L.jobs_dev, jobs.data(), sizeof(WgradJob) * L.n_jobs, cudaMemcpyHostToDevice, s),
-           "train_samples job table upload");
-  CUDA_TRY(cudaMemcpyAsync(L.cta_first_dev, cta_first.data(), sizeof(int) * (L.n_cta + 1), cudaMemcpyHostToDevice, s),
-           "train_samples cta table upload");
-  return 0;
+// The backward plans of the networks from their evaluated rows, block ps for network ps (one thread each): the step's
+// layout, its wgrad piece table and CTA ranges in the workspace's tables (the CTAs past the step's own up to the carved
+// count get empty ranges), the head and chain parameters and the reduction table, each from the planner the host uses
+// for the plain paths.  The plan is built in local memory and stored once.
+struct TrainSkipPlanArgs {
+  TrainLayout L[2];             // carved for each network's worst case
+  const long long* rows[2];     // device: the pass's evaluated rows (null: no plan for that network)
+  const float* params[2][24];
+  float* grads[2][24];
+  const uint8_t* net[2];
+  TrainSkipPlan* out[2];
+  int sm_count;
+  int* status;
+};
+
+__global__ void __launch_bounds__(32) train_skip_plan_kernel(const TrainSkipPlanArgs a) {
+  __shared__ TrainSkipPlan o;
+  const int ps = blockIdx.x;
+  if (a.rows[ps] == nullptr) return;
+  if (threadIdx.x == 0) {
+    TrainLayout L = a.L[ps];
+    const int cap_ctas = L.n_cta;
+    train_skip_rows(&L, *a.rows[ps]);
+    plan_wgrad(&L, a.sm_count, L.jobs_dev, L.cta_first_dev);
+    for (int b = L.n_cta + 1; b <= cap_ctas; ++b) L.cta_first_dev[b] = L.n_jobs;
+    head_plan(L, a.params[ps][22], a.params[ps][22], nullptr, 0, &o.head);
+    o.head_grid = L.head_grid;
+    const uint8_t* const net[2] = {a.net[ps], a.net[ps]};
+    chain_plan(L, net, a.status, a.sm_count, &o.probe, &o.chain);
+    o.tab.n = 0;
+    add_reduce_items(o.tab, L, 0, a.grads[ps]);
+  }
+  __syncwarp();
+  // the warp stores the plan
+  static_assert(sizeof(TrainSkipPlan) % 8 == 0, "plan words");
+  const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&o);
+  unsigned long long* dst = reinterpret_cast<unsigned long long*>(a.out[ps]);
+  for (int i = threadIdx.x; i < static_cast<int>(sizeof(TrainSkipPlan) / 8); i += 32) dst[i] = src[i];
 }
 
 // The argument checks of both entries, and the step's parameters and workspace carve.
@@ -1054,11 +1133,15 @@ int train_skip_setup(const nerfb200_train_samples_args* a, void* ws, size_t byte
   return 0;
 }
 
-// The training MLP of one network over the step's compacted rows (mlp_forward_kernel<true, true>).
-int train_skip_mlp(const TrainSkipParams& t, const TrainLayout& L, int pass, long long rows, const DeviceInfo* d,
-                   cudaStream_t s) {
+// The training MLP of one network over the pass's compacted rows (mlp_forward_kernel<true, true>), at the grid of
+// the carved worst case; the kernel reads the row count from the pass's scan.
+int train_skip_mlp(const TrainSkipWs& w, int pass, const DeviceInfo* d, cudaStream_t s) {
+  const TrainSkipParams& t = w.t;
+  TrainLayout L;
+  make_train_layout(&L, w.net_ws[pass], true, w.cap[pass], 1, 0, d->sm_count);
   MlpParams m{};
-  m.n = rows;
+  m.n = w.cap[pass];
+  m.n_dev = t.ofs[pass] + t.s.n;
   m.net = t.s.net[pass];
   m.out = const_cast<float*>(t.s.mlp_out);
   m.status = d->status;
@@ -1069,9 +1152,127 @@ int train_skip_mlp(const TrainSkipParams& t, const TrainLayout& L, int pass, lon
   m.rays = t.s.rays;
   m.dirbias = t.s.dirbias + pass * kDirW;
   m.dirrow = t.dirrow;
-  const long long tiles = ceil_div(rows, 128);
+  const long long tiles = ceil_div(m.n, 128);
   return launch(pass ? "train_samples fine mlp launch" : "train_samples coarse mlp launch", mlp_forward_kernel<true, true>,
                 static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count), kThreads, kSmemTotal, s, m);
+}
+
+// The forward of both entries, every launch at the grid of the carved worst case.  live_dev[2] receives the
+// evaluated coarse and fine sample counts as soon as the last scan has them; with live_host (the eager entry) they
+// are also read back there, once.  That read-back is not left to the end: the host then enqueues the rest of the
+// forward and returns to queue the backward while the GPU runs the last MLP, as it did when it read each count before
+// sizing the launches after it.
+int train_skip_forward(const nerfb200_train_samples_args* a, const TrainSkipWs& w, long long* live_dev,
+                       int64_t* live_host, const DeviceInfo* d, cudaStream_t s) {
+  TrainSkipParams t = w.t;
+  const bool fine = t.s.K > 0;
+  const long long n = t.s.n;
+  const int ray_blocks = grid_blocks(ceil_div(n, kSkipWarps), 1);
+  const char* what = "train_samples_forward launches";
+  auto counts = [&]() -> int {
+    TRY(launch(what, train_skip_counts_kernel, 1, 32, 0, s, t.ofs[0] + n, fine ? t.ofs[1] + n : nullptr, live_dev));
+    if (!live_host) return 0;
+    long long live[2];
+    CUDA_TRY(cudaMemcpyAsync(live, live_dev, sizeof(live), cudaMemcpyDeviceToHost, s), "train_samples readback");
+    CUDA_TRY(cudaStreamSynchronize(s), "train_samples readback");
+    live_host[0] = live[0];
+    live_host[1] = live[1];
+    return 0;
+  };
+  // coarse pass
+  TRY(launch(what, train_skip_classify_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+  TRY(launch(what, skip_dir_bias_kernel, grid_blocks(n, 1), kDirW, 0, s, t.s, 0, fine ? 2 : 1));
+  t.s.ofs = t.ofs[0];
+  TRY(launch(what, cull_scan_kernel, 1, 1024, 0, s, t.s.cnt, t.s.ofs, n));
+  if (!fine) TRY(counts());
+  TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 0));
+  TRY(train_skip_mlp(w, 0, d, s));
+  TRY(launch(what, train_skip_coarse_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+  if (fine) {
+    t.s.ofs = t.ofs[1];
+    TRY(launch(what, cull_scan_kernel, 1, 1024, 0, s, t.s.cnt, t.s.ofs, n));
+    TRY(counts());
+    TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 1));
+    TRY(train_skip_mlp(w, 1, d, s));
+    TRY(launch(what, train_skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+  }
+  // losses.py / metrics.py on the results, one block in a fixed order
+  TRY(launch(what, mse_psnr_kernel, 1, 1024, 0, s, t.s.rgb_coarse, fine ? t.s.rgb_fine : nullptr, a->target, n * 3,
+             a->loss_out));
+  uint32_t* const mask_out[2] = {a->mask_coarse, a->mask_fine};
+  for (int ps = 0; ps < (fine ? 2 : 1); ++ps)
+    if (mask_out[ps])
+      CUDA_TRY(cudaMemcpyAsync(mask_out[ps], t.s.mask[ps], sizeof(uint32_t) * n * kSkipMaskWords,
+                               cudaMemcpyDeviceToDevice, s), "train_samples mask copy");
+  return 0;
+}
+
+// The backward of the networks with run[ps]: one plan launch for all of them from the device counts, then per network
+// the sparse compositing backward, the optional per-row copies and the tail, every launch at the grid of the carved
+// worst case.
+int train_skip_backward(const nerfb200_train_samples_args* a, const TrainSkipWs& w, const bool run[2],
+                        const float* loss_grad, const float* const* const params[2], float* const* const grads[2],
+                        const DeviceInfo* d, cudaStream_t s) {
+  const TrainSkipParams& t = w.t;
+  const char* what = "train_samples_backward launches";
+  const int n_net = t.s.K > 0 ? 2 : 1;
+  TrainLayout L[2];
+  TrainSkipPlanArgs pa;
+  std::memset(&pa, 0, sizeof(pa));
+  for (int ps = 0; ps < n_net; ++ps) {
+    if (!run[ps]) continue;
+    make_train_layout(&L[ps], w.net_ws[ps], true, w.cap[ps], 1, 0, d->sm_count);
+    pa.L[ps] = L[ps];
+    pa.rows[ps] = t.ofs[ps] + t.s.n;
+    for (int i = 0; i < kNumParams; ++i) {
+      pa.params[ps][i] = params[ps][i];
+      pa.grads[ps][i] = grads[ps][i];
+    }
+    pa.net[ps] = t.s.net[ps];
+    pa.out[ps] = w.plan[ps];
+  }
+  pa.sm_count = d->sm_count;
+  pa.status = d->status;
+  TRY(launch(what, train_skip_plan_kernel, n_net, 32, 0, s, pa));
+  for (int ps = 0; ps < n_net; ++ps) {
+    if (!run[ps]) continue;
+    const long long* rows = pa.rows[ps];
+    const PassBufs& pb = L[ps].pass[0];
+    TrainSkipBwdParams bp;
+    bp.n_rays = t.s.n; bp.S = ps ? t.s.Sc + t.s.K : t.s.Sc;
+    bp.n_rows = rows;
+    bp.rays = t.s.rays; bp.z = ps ? t.s.zf : t.zc;
+    bp.mask = t.s.mask[ps]; bp.ofs = t.ofs[ps];
+    bp.sigma = pb.sigma; bp.rgb = pb.rgb;
+    bp.noise = t.noise_std > 0.f ? t.noise[ps] : nullptr;
+    bp.noise_std = t.noise_std; bp.white_back = t.s.white_back;
+    bp.rgb_out = ps ? t.s.rgb_fine : t.s.rgb_coarse;
+    bp.target = a->target; bp.loss_grad = loss_grad;
+    bp.dsigma = pb.dsigma; bp.dprergb = pb.dprergb;
+    bp.amax_bits = L[ps].amax;
+    bp.status = d->status;
+    TRY(launch(what, train_skip_bwd_kernel, grid_blocks(ceil_div(t.s.n, kSkipWarps), 1), kSkipWarps * 32, 0, s, bp));
+    float* const ds_out = ps ? a->dsigma_fine : a->dsigma_coarse;
+    float* const dp_out = ps ? a->dprergb_fine : a->dprergb_coarse;
+    if (ds_out)
+      TRY(launch(what, train_skip_copy_rows_kernel, grid_blocks(w.cap[ps], 256), 256, 0, s, pb.dsigma, ds_out, rows, 1));
+    if (dp_out)
+      TRY(launch(what, train_skip_copy_rows_kernel, grid_blocks(3 * w.cap[ps], 256), 256, 0, s, pb.dprergb, dp_out,
+                 rows, 3));
+    const float* const* const p2[2] = {params[ps], params[ps]};
+    float* const* const g2[2] = {grads[ps], grads[ps]};
+    const uint8_t* const net[2] = {t.s.net[ps], t.s.net[ps]};
+    TRY(backward_tail(L[ps], p2, g2, net, nullptr, 0, d, s, what, w.plan[ps]));
+  }
+  return 0;
+}
+
+// The parameter / gradient tables of network ps (every tensor non-null).
+int train_skip_tables_ok(const float* const* params, float* const* grads) {
+  if (!params || !grads) return fail(NERFB200_EINVAL, "train_samples_backward: params / grads tables are NULL");
+  for (int i = 0; i < kNumParams; ++i)
+    if (!params[i] || !grads[i]) return fail(NERFB200_EINVAL, "train_samples_backward: NULL parameter / gradient tensor");
+  return 0;
 }
 
 // ------------------------------------------------------------------ image metrics (kernels: metrics_kernels.cuh)
@@ -2161,50 +2362,21 @@ int nerfb200_train_samples_forward(const nerfb200_train_samples_args* a, void* w
   DeviceInfo* d = nullptr;
   TRY(device_info(&d));
   TRY(check_sticky_status(d));
-  TrainSkipParams& t = w.t;
-  const bool fine = t.s.K > 0;
-  const long long n = t.s.n;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int ray_blocks = grid_blocks(ceil_div(n, kSkipWarps), 1);
-  const char* what = "train_samples_forward launches";
   live_samples_host[0] = live_samples_host[1] = 0;
-  // coarse pass
-  TRY(launch(what, train_skip_classify_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
-  TRY(launch(what, skip_dir_bias_kernel, grid_blocks(n, 1), kDirW, 0, s, t.s, 0, fine ? 2 : 1));
-  t.s.ofs = t.ofs[0];
-  long long rows[2] = {0, 0};
-  TRY(samples_scan(t.s, s, &rows[0]));
-  TrainLayout L[2];
-  if (rows[0] > 0) {
-    train_skip_net_layout(&L[0], w.net_ws[0], w.cap[0], rows[0], d->sm_count);
-    if (!fine) TRY(train_skip_upload_plan(L[0], d->sm_count, s));
-    TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 0));
-    TRY(train_skip_mlp(t, L[0], 0, rows[0], d, s));
-  }
-  TRY(launch(what, train_skip_coarse_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
-  if (fine) {
-    t.s.ofs = t.ofs[1];
-    TRY(samples_scan(t.s, s, &rows[1]));
-    if (rows[0] > 0) TRY(train_skip_upload_plan(L[0], d->sm_count, s));
-    if (rows[1] > 0) {
-      train_skip_net_layout(&L[1], w.net_ws[1], w.cap[1], rows[1], d->sm_count);
-      TRY(train_skip_upload_plan(L[1], d->sm_count, s));
-      TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 1));
-      TRY(train_skip_mlp(t, L[1], 1, rows[1], d, s));
-    }
-    TRY(launch(what, train_skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
-  }
-  // losses.py / metrics.py on the results, one block in a fixed order
-  TRY(launch(what, mse_psnr_kernel, 1, 1024, 0, s, t.s.rgb_coarse, fine ? t.s.rgb_fine : nullptr, a->target, n * 3,
-             a->loss_out));
-  uint32_t* const mask_out[2] = {a->mask_coarse, a->mask_fine};
-  for (int ps = 0; ps < (fine ? 2 : 1); ++ps)
-    if (mask_out[ps])
-      CUDA_TRY(cudaMemcpyAsync(mask_out[ps], t.s.mask[ps], sizeof(uint32_t) * n * kSkipMaskWords,
-                               cudaMemcpyDeviceToDevice, s), "train_samples mask copy");
-  live_samples_host[0] = rows[0];
-  live_samples_host[1] = rows[1];
-  return 0;
+  return train_skip_forward(a, w, w.live, live_samples_host, d, s);
+}
+
+int nerfb200_train_samples_forward_dev(const nerfb200_train_samples_args* a, void* ws, size_t bytes,
+                                       int64_t* live_samples_dev, void* stream) {
+  if (!live_samples_dev) return fail(NERFB200_EINVAL, "train_samples_forward_dev: NULL argument");
+  TrainSkipWs w;
+  TRY(train_skip_setup(a, ws, bytes, nerfb200_sm_count(), &w, "train_samples_forward_dev"));
+  DeviceInfo* d = nullptr;
+  TRY(device_info(&d));
+  TRY(check_sticky_status(d));
+  return train_skip_forward(a, w, reinterpret_cast<long long*>(live_samples_dev), nullptr, d,
+                            static_cast<cudaStream_t>(stream));
 }
 
 int nerfb200_train_samples_backward(const nerfb200_train_samples_args* a, void* ws, size_t bytes,
@@ -2214,56 +2386,35 @@ int nerfb200_train_samples_backward(const nerfb200_train_samples_args* a, void* 
   if (!live_samples_host) return fail(NERFB200_EINVAL, "train_samples_backward: NULL argument");
   TrainSkipWs w;
   TRY(train_skip_setup(a, ws, bytes, nerfb200_sm_count(), &w, "train_samples_backward"));
-  const TrainSkipParams& t = w.t;
-  const int n_net = t.s.K > 0 ? 2 : 1;
+  const int n_net = w.t.s.K > 0 ? 2 : 1;
   const float* const* const params[2] = {params_coarse, params_fine};
   float* const* const grads[2] = {grads_coarse, grads_fine};
   for (int ps = 0; ps < n_net; ++ps) {
     if (live_samples_host[ps] < 0 || live_samples_host[ps] > w.cap[ps])
       return fail(NERFB200_EINVAL, "train_samples_backward: live sample count out of range");
-    if (live_samples_host[ps] == 0) continue;
-    if (!params[ps] || !grads[ps]) return fail(NERFB200_EINVAL, "train_samples_backward: params / grads tables are NULL");
-    for (int i = 0; i < kNumParams; ++i)
-      if (!params[ps][i] || !grads[ps][i])
-        return fail(NERFB200_EINVAL, "train_samples_backward: NULL parameter / gradient tensor");
+    if (live_samples_host[ps] > 0) TRY(train_skip_tables_ok(params[ps], grads[ps]));
   }
   DeviceInfo* d = nullptr;
   TRY(device_info(&d));
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const char* what = "train_samples_backward launches";
-  for (int ps = 0; ps < n_net; ++ps) {
-    const long long rows = live_samples_host[ps];
-    if (rows == 0) continue;
-    TrainLayout L;
-    train_skip_net_layout(&L, w.net_ws[ps], w.cap[ps], rows, d->sm_count);
-    const PassBufs& pb = L.pass[0];
-    TrainSkipBwdParams bp;
-    bp.n_rays = t.s.n; bp.S = ps ? t.s.Sc + t.s.K : t.s.Sc;
-    bp.n_rows = rows; bp.n_pad = pb.n_pad;
-    bp.rays = t.s.rays; bp.z = ps ? t.s.zf : t.zc;
-    bp.mask = t.s.mask[ps]; bp.ofs = t.ofs[ps];
-    bp.sigma = pb.sigma; bp.rgb = pb.rgb;
-    bp.noise = t.noise_std > 0.f ? t.noise[ps] : nullptr;
-    bp.noise_std = t.noise_std; bp.white_back = t.s.white_back;
-    bp.rgb_out = ps ? t.s.rgb_fine : t.s.rgb_coarse;
-    bp.target = a->target; bp.loss_grad = loss_grad;
-    bp.dsigma = pb.dsigma; bp.dprergb = pb.dprergb;
-    bp.amax_bits = L.amax;
-    bp.status = d->status;
-    TRY(launch(what, train_skip_bwd_kernel, grid_blocks(ceil_div(t.s.n, kSkipWarps), 1), kSkipWarps * 32, 0, s, bp));
-    float* const ds_out = ps ? a->dsigma_fine : a->dsigma_coarse;
-    float* const dp_out = ps ? a->dprergb_fine : a->dprergb_coarse;
-    if (ds_out)
-      CUDA_TRY(cudaMemcpyAsync(ds_out, pb.dsigma, sizeof(float) * rows, cudaMemcpyDeviceToDevice, s), "dsigma copy");
-    if (dp_out)
-      CUDA_TRY(cudaMemcpyAsync(dp_out, pb.dprergb, sizeof(float) * 3 * rows, cudaMemcpyDeviceToDevice, s),
-               "dprergb copy");
-    const float* const* const p2[2] = {params[ps], params[ps]};
-    float* const* const g2[2] = {grads[ps], grads[ps]};
-    const uint8_t* const net[2] = {t.s.net[ps], t.s.net[ps]};
-    TRY(backward_tail(L, p2, g2, net, nullptr, 0, d, s, what));
-  }
-  return 0;
+  const bool run[2] = {live_samples_host[0] > 0, n_net > 1 && live_samples_host[1] > 0};
+  if (!run[0] && !run[1]) return 0;
+  return train_skip_backward(a, w, run, loss_grad, params, grads, d, static_cast<cudaStream_t>(stream));
+}
+
+int nerfb200_train_samples_backward_dev(const nerfb200_train_samples_args* a, void* ws, size_t bytes,
+                                        const float* loss_grad, const float* const params_coarse[24],
+                                        const float* const params_fine[24], float* const grads_coarse[24],
+                                        float* const grads_fine[24], void* stream) {
+  TrainSkipWs w;
+  TRY(train_skip_setup(a, ws, bytes, nerfb200_sm_count(), &w, "train_samples_backward_dev"));
+  const int n_net = w.t.s.K > 0 ? 2 : 1;
+  const float* const* const params[2] = {params_coarse, params_fine};
+  float* const* const grads[2] = {grads_coarse, grads_fine};
+  for (int ps = 0; ps < n_net; ++ps) TRY(train_skip_tables_ok(params[ps], grads[ps]));
+  DeviceInfo* d = nullptr;
+  TRY(device_info(&d));
+  const bool run[2] = {true, n_net > 1};
+  return train_skip_backward(a, w, run, loss_grad, params, grads, d, static_cast<cudaStream_t>(stream));
 }
 
 // ---- image metrics (include/nerf_pl_b200_metrics.h; kernels: metrics_kernels.cuh)

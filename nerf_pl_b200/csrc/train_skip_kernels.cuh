@@ -226,10 +226,11 @@ __global__ void __launch_bounds__(kSkipWarps * 32) train_skip_fine_stage_kernel(
 // composite_bwd_kernel's arithmetic (the fused MSE seed, white_back, noise, the ReLU mask) on one ray per warp, with
 // sigma / rgb of an evaluated sample read from its compacted row and sigma = 0, rgb = 0 (no noise) for a skipped one.
 // d sigma / d rgb_pre go to the evaluated rows only; rows n_rows .. n_pad - 1 (padding of the last MLP tile) get 0.
+// n_rows is read on the device (the pass's total in ofs), n_pad is its multiple of 128.
 // Also the amax words of the scale selection and status 103 for a non-finite per-sample gradient.
 struct TrainSkipBwdParams {
   int n_rays, S;
-  long long n_rows, n_pad;
+  const long long* n_rows;      // device: the evaluated rows of the pass
   const float* rays;            // (n_rays, 8)
   const float* z;               // (n_rays, S) depths of the pass
   const uint32_t* mask;         // (n_rays, kSkipMaskWords)
@@ -342,7 +343,8 @@ __global__ void __launch_bounds__(kSkipWarps * 32) train_skip_bwd_kernel(const T
     }
   }
   if (__any_sync(0xffffffffu, nonfinite) && lane == 0) report_fault(p.status, 103);
-  for (long long i = p.n_rows + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < p.n_pad;
+  const long long n_rows = *p.n_rows, n_pad = (n_rows + 127) / 128 * 128;
+  for (long long i = n_rows + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_pad;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     p.dsigma[i] = 0.f;
     p.dprergb[3 * i] = 0.f; p.dprergb[3 * i + 1] = 0.f; p.dprergb[3 * i + 2] = 0.f;
@@ -354,6 +356,23 @@ __global__ void __launch_bounds__(kSkipWarps * 32) train_skip_bwd_kernel(const T
   }
   if (lane == 0 && amax > 0.f && amax < 3e38f) atomicMax(p.amax_bits, __float_as_uint(amax));
   if (lane == 0 && amax_rgb > 0.f && amax_rgb < 3e38f) atomicMax(p.amax_bits + 1, __float_as_uint(amax_rgb));
+}
+
+// The evaluated sample counts of both passes (the totals of their scans; 0 for the fine pass without one).
+__global__ void train_skip_counts_kernel(const long long* c0, const long long* c1, long long* out) {
+  if (threadIdx.x == 0) {
+    out[0] = *c0;
+    out[1] = c1 != nullptr ? *c1 : 0;
+  }
+}
+
+// dst[0 .. *rows * width) = src[...]: the optional per-row outputs of the backward, exactly the evaluated rows.
+__global__ void train_skip_copy_rows_kernel(const float* __restrict__ src, float* __restrict__ dst,
+                                            const long long* __restrict__ rows, int width) {
+  const long long total = *rows * width;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    dst[i] = src[i];
 }
 
 }  // namespace nerfb200

@@ -420,7 +420,8 @@ def render_rays_loss(models: List[torch.nn.Module],
     ``occupancy`` (a ``nerf_pl_b200.OccupancyGrid``) skips the empty samples of every ray (``train_skip.py``,
     DESIGN.md "Training with empty samples skipped"): the result gains ``'live_samples'`` (evaluated coarse, fine
     samples) and only ``loss`` carries a gradient.  It needs the render kernel's shapes and at most 2^22 rays
-    (ValueError), and a grid on the rays' device (RuntimeError); each step synchronises twice."""
+    (ValueError), and a grid on the rays' device (RuntimeError); each step synchronises once, to read back
+    ``live_samples`` (``CapturedTrainStep(..., occupancy=grid)`` replays the step without synchronising)."""
     del chunk
     _check_render_inputs("render_rays_loss", models, embeddings, N_importance, rays)
     n, S_c, K = rays.shape[0], int(N_samples), int(N_importance)

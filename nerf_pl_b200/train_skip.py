@@ -9,9 +9,13 @@ that appears in a cell the grid calls empty is trained from the next rebuild on.
 
 forward : ``nerfb200_train_samples_forward`` (include/nerf_pl_b200_train_samples.h): perturbed depths and
           classification, the compacted rows of each network through the save-mode MLP, compositing with noise, the
-          random resampling and the merge, the loss.  Two read-backs of a sample count per step.
-backward: ``nerfb200_train_samples_backward``: the compositing backward over the sparse sample lists, then per
-          network the backward of a direct ``NeRF.forward`` call (chain, wgrad, reduction, unfold).
+          random resampling and the merge, the loss.  Every launch is sized for the worst case and reads the
+          step's sample counts on the device; the eager call reads the two counts back once at the end.
+backward: ``nerfb200_train_samples_backward``: per network, a plan kernel turns the device count into the launch
+          parameters, then the compositing backward over the sparse sample lists and the backward of a direct
+          ``NeRF.forward`` call (chain, wgrad, reduction, unfold).
+capturable mode (``live_samples=`` a device tensor): the ``_dev`` entries, which neither synchronise nor read host
+          memory, so ``CapturedTrainStep(occupancy=grid)`` replays the step as one CUDA graph.
 """
 from __future__ import annotations
 
@@ -40,6 +44,7 @@ class SkipTrainWorkspace:
         nbytes = int(_lib.load().nerfb200_train_samples_workspace_bytes(n, S_c, K))
         if nbytes == 0:
             raise ValueError("invalid training shape")
+        self.key = (dev.index, n, S_c, K)
         self.buf = _aligned_buffer(nbytes, dev)
         self.buf.zero_()
         self.bytes = nbytes
@@ -102,7 +107,10 @@ class SkipRenderFunction(torch.autograd.Function):
             blob_c, blob_f = packed_weights_pair(models[0], models[1])
         else:
             blob_c, blob_f = packed_weights(models[0]), None
-        lease = _Lease(SkipTrainWorkspace.acquire(dev, n, S_c, K))
+        own, live_dev = cfg.get("workspace"), cfg.get("live_out")
+        if own is not None and own.key != (dev.index, n, S_c, K):
+            raise ValueError("the given training workspace is of another shape")
+        lease = _Lease(own if own is not None else SkipTrainWorkspace.acquire(dev, n, S_c, K))
         seed = cfg.get("rng_seed")
         if seed is None:
             rng = dict(rng_seed=0, rng_in_kernel=0)
@@ -118,16 +126,22 @@ class SkipRenderFunction(torch.autograd.Function):
             u_rand=_ptr(ur), noise_fine=_ptr(nf), bits=grid.bits.data_ptr(), N=grid.N,
             ranges=(ctypes.c_double * 6)(*grid.ranges), target=target.data_ptr(), loss_out=loss_out.data_ptr(),
             **dict(zip(_OUTPUTS, [o.data_ptr() for o in out])), **{k: _ptr(t) for k, t in extras.items()}, **rng)
-        live = (ctypes.c_int64 * 2)()
-        _lib.call("nerfb200_train_samples_forward", dev, ctypes.byref(args), lease.ws.buf.data_ptr(), lease.ws.bytes,
-                  live)
+        if live_dev is None:
+            live = (ctypes.c_int64 * 2)()
+            _lib.call("nerfb200_train_samples_forward", dev, ctypes.byref(args), lease.ws.buf.data_ptr(),
+                      lease.ws.bytes, live)
+            cfg["live_samples"] = (int(live[0]), int(live[1]))
+        else:
+            live = None
+            _lib.call("nerfb200_train_samples_forward_dev", dev, ctypes.byref(args), lease.ws.buf.data_ptr(),
+                      lease.ws.bytes, ctypes.cast(live_dev.data_ptr(), ctypes.POINTER(ctypes.c_int64)))
+            cfg["live_samples"] = live_dev
         ctx.args, ctx.live, ctx.lease, ctx.K = args, live, lease, K
         # what the args point to (detached aliases of the outputs: see FusedRenderFunction)
         ctx.keep = (rays, pr, nc, ur, nf, target, [o.detach() for o in out], blob_c, blob_f, grid.bits, seed)
         ctx.n_params = len(params)
         ctx.save_for_backward(*params)
         ctx.set_materialize_grads(False)
-        cfg["live_samples"] = (int(live[0]), int(live[1]))
         return tuple(out) + (loss_out,)
 
     @staticmethod
@@ -147,14 +161,18 @@ class SkipRenderFunction(torch.autograd.Function):
         dev = params[0].device
         grads, tables = _grad_buffers(params, dev)
         nets = 2 if ctx.K > 0 else 1
-        for ps in range(nets):
-            if ctx.live[ps] == 0:                # no evaluated sample: nothing launched for this network
-                for t in grads[24 * ps:24 * ps + 24]:
-                    t.zero_()
         (pc, gc) = tables[0]
         pf, gf = tables[1] if nets > 1 else (None, None)
-        _lib.call("nerfb200_train_samples_backward", dev, ctypes.byref(ctx.args), lease.ws.buf.data_ptr(),
-                  lease.ws.bytes, ctx.live, g4.data_ptr() + 8, pc, pf, gc, gf)
+        if ctx.live is None:                     # capturable: the device path writes every network's gradients
+            _lib.call("nerfb200_train_samples_backward_dev", dev, ctypes.byref(ctx.args), lease.ws.buf.data_ptr(),
+                      lease.ws.bytes, g4.data_ptr() + 8, pc, pf, gc, gf)
+        else:
+            for ps in range(nets):
+                if ctx.live[ps] == 0:            # no evaluated sample: nothing launched for this network
+                    for t in grads[24 * ps:24 * ps + 24]:
+                        t.zero_()
+            _lib.call("nerfb200_train_samples_backward", dev, ctypes.byref(ctx.args), lease.ws.buf.data_ptr(),
+                      lease.ws.bytes, ctx.live, g4.data_ptr() + 8, pc, pf, gc, gf)
         lease.release()
         ctx.keep = ctx.args = None
         if nets == 1:
@@ -163,16 +181,26 @@ class SkipRenderFunction(torch.autograd.Function):
 
 
 def render_rays_train_skip(models, rays, N_samples, use_disp, perturb, noise_std, N_importance, white_back, pr, nc, ur,
-                           nf, target, occupancy, rng_seed=None, extras: bool = False) -> Dict[str, torch.Tensor]:
+                           nf, target, occupancy, rng_seed=None, extras: bool = False,
+                           workspace: Optional[SkipTrainWorkspace] = None,
+                           live_samples: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
     """``render_rays_train`` with empty samples skipped: the result keys of ``render_rays_loss`` plus
     ``'live_samples'`` (evaluated coarse, fine samples).  ``extras`` adds, for tests: ``z_vals_coarse``,
     ``z_vals_fine``, ``weights_coarse``, ``weights_fine``, ``samples_coarse`` / ``samples_fine`` (n, S, 4: network
     rgb and sigma, 0 where skipped) and ``mask_coarse`` / ``mask_fine`` ((n, 6) int32, bit b of word w: sample
     32 w + b evaluated), and ``dsigma_coarse`` / ``dsigma_fine`` (n S) and ``dprergb_coarse`` / ``dprergb_fine``
     (n S, 3), which ``loss.backward()`` fills in their first ``live_samples`` rows with the per-row d loss / d sigma
-    and d loss / d (rgb before the sigmoid) of the evaluated samples, ray-major in depth-index order."""
+    and d loss / d (rgb before the sigmoid) of the evaluated samples, ray-major in depth-index order.
+
+    ``live_samples`` (a device int64 tensor of 2 elements) selects the capturable mode: no host synchronisation, the
+    counts are written into that tensor, which is also the result's ``'live_samples'``, and the backward writes
+    every network's gradients itself (exact zeros for a network with no evaluated sample).  ``workspace`` is a
+    ``SkipTrainWorkspace`` of this shape that the caller owns (outside the pool), as ``render_rays_train`` takes."""
     S_c, K = int(N_samples), int(N_importance)
     n, dev = rays.shape[0], rays.device
+    if live_samples is not None and (live_samples.dtype != torch.int64 or live_samples.numel() != 2
+                                     or live_samples.device != dev or not live_samples.is_contiguous()):
+        raise ValueError("live_samples must be a contiguous int64 tensor of 2 elements on the rays' device")
     f32 = dict(dtype=torch.float32, device=dev)
     ex = {}
     if extras:
@@ -187,7 +215,7 @@ def render_rays_train_skip(models, rays, N_samples, use_disp, perturb, noise_std
                       dsigma_fine=torch.zeros(n * (S_c + K), **f32), dprergb_fine=torch.zeros(n * (S_c + K), 3, **f32))
     cfg = dict(models=list(models), occupancy=occupancy, N_samples=S_c, N_importance=K, use_disp=bool(use_disp),
                perturb=float(perturb), noise_std=float(noise_std), white_back=bool(white_back), rng_seed=rng_seed,
-               extras=ex)
+               extras=ex, workspace=workspace, live_out=live_samples)
     params = _params_of(models, K)
     target = target.detach().to(torch.float32).contiguous()
     if target.shape != (n, 3):

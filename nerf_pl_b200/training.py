@@ -391,11 +391,17 @@ class CapturedTrainStep:
     The gradients of every parameter the optimizer holds are set to None before the warm-up and before the capture,
     so parameters outside ``models`` (the fine model when ``N_importance == 0``, other groups) are neither warmed up
     nor updated by the replays.  Between replays the models' ``.grad`` are the graph's own buffers.  ``launches_per_step`` is the number of
-    library kernels one replay runs (counted while capturing)."""
+    library kernels one replay runs (counted while capturing).
+
+    ``occupancy`` (a ``nerf_pl_b200.OccupancyGrid``) captures the step with empty samples skipped, as
+    ``render_rays_loss(..., occupancy=grid)`` computes it.  The step copies the grid's bits into a buffer it owns
+    and uses a ``SkipTrainWorkspace`` of its own; ``set_occupancy(grid)`` copies a rebuilt grid of the same ``N``,
+    ranges and ``dilate`` into that buffer between replays, and ``live_samples`` is the device int64 pair of the last
+    replay's evaluated coarse and fine sample counts."""
 
     def __init__(self, models, batches, optimizer, N_samples: int = 64, use_disp: bool = False, perturb: float = 1.0,
                  noise_std: float = 1.0, N_importance: int = 64, white_back: bool = False, randoms=None,
-                 warmup: int = 3):
+                 warmup: int = 3, occupancy=None):
         from .optim import FusedAdam
         global _CAPTURED_SEEDS
         if not (isinstance(optimizer, FusedAdam) and optimizer.capturable):
@@ -433,7 +439,18 @@ class CapturedTrainStep:
             self.seed_word = torch.tensor(s, dtype=torch.int64, device=dev)
         elif randoms is not None:
             raise ValueError("randoms must be None, 'kernel' or {'seed': int}")
-        self.workspace = TrainWorkspace(dev, B, S_c, K)
+        self._grid = None
+        if occupancy is None:
+            self.workspace = TrainWorkspace(dev, B, S_c, K)
+        else:
+            from .culling import OccupancyGrid
+            from .train_skip import SkipTrainWorkspace, check_shape
+            check_shape(B, S_c, K)
+            self._check_grid(occupancy, dev)
+            r = occupancy.ranges
+            self._grid = OccupancyGrid(occupancy.bits.clone(), occupancy.N, r[0:2], r[2:4], r[4:6], occupancy.dilate)
+            self.workspace = SkipTrainWorkspace(dev, B, S_c, K)
+            self._live = torch.zeros(2, dtype=torch.int64, device=dev)
         self._perm = batches.next_permutation().clone()
         self._offset = torch.zeros((), dtype=torch.int64, device=dev)
         self._arange = torch.arange(B, device=dev)
@@ -453,9 +470,15 @@ class CapturedTrainStep:
             nf = torch.randn(B, S_c + K, device=idx.device) if c["noise_std"] > 0 and K > 0 else None
         else:
             pr, nc, ur, nf = _draw_randoms(B, S_c, K, c["perturb"], c["noise_std"], idx.device, False)
-        res = render_rays_train(self.models, batch["rays"], S_c, c["use_disp"], c["perturb"], c["noise_std"], K,
-                                c["white_back"], pr, nc, ur, nf, target=batch["rgbs"], rng_seed=self.seed_word,
-                                workspace=self.workspace)
+        if self._grid is None:
+            res = render_rays_train(self.models, batch["rays"], S_c, c["use_disp"], c["perturb"], c["noise_std"], K,
+                                    c["white_back"], pr, nc, ur, nf, target=batch["rgbs"], rng_seed=self.seed_word,
+                                    workspace=self.workspace)
+        else:
+            from .train_skip import render_rays_train_skip
+            res = render_rays_train_skip(self.models, batch["rays"], S_c, c["use_disp"], c["perturb"], c["noise_std"],
+                                         K, c["white_back"], pr, nc, ur, nf, batch["rgbs"], self._grid,
+                                         rng_seed=self.seed_word, workspace=self.workspace, live_samples=self._live)
         res["loss"].backward()
         self.optimizer.step()
         self._offset.add_(B)
@@ -505,6 +528,32 @@ class CapturedTrainStep:
         except Exception as e:
             raise RuntimeError(f"CapturedTrainStep: capturing the training step failed: {e}") from e
         self.launches_per_step = int(lib.nerfb200_launch_count() - n0)
+
+    @staticmethod
+    def _check_grid(grid, dev) -> None:
+        from .culling import OccupancyGrid
+        if not isinstance(grid, OccupancyGrid):
+            raise ValueError("occupancy must be a nerf_pl_b200.OccupancyGrid")
+        if grid.device != dev:
+            raise RuntimeError(f"the occupancy grid is on {grid.device}, the step trains on {dev}")
+
+    @property
+    def live_samples(self) -> Optional[torch.Tensor]:
+        """The last replay's evaluated (coarse, fine) sample counts, a device int64 tensor (None without a grid)."""
+        return None if self._grid is None else self._live
+
+    def set_occupancy(self, grid) -> None:
+        """Copy a rebuilt grid's bits into the step's own grid buffer (stream-ordered before the next replay).  The
+        graph holds N, the ranges and dilate by value: a grid that differs in any of them is a ValueError."""
+        if self._grid is None:
+            raise ValueError("this step was captured without occupancy=")
+        self._check_grid(grid, self._grid.device)
+        g = self._grid
+        if (grid.N, tuple(grid.ranges), grid.dilate) != (g.N, tuple(g.ranges), g.dilate):
+            raise ValueError("set_occupancy needs a grid of the captured N, ranges and dilate "
+                             f"({g.N}, {tuple(g.ranges)}, {g.dilate}); got ({grid.N}, {tuple(grid.ranges)}, "
+                             f"{grid.dilate})")
+        g.bits.copy_(grid.bits)
 
     def step(self):
         """Replay one training step; returns the device scalars (loss, psnr) of this step."""
