@@ -6,6 +6,7 @@ from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_
                    packed_weights)
 from .culling import OccupancyGrid, cull_rays, occupancy_grid, pack_occupancy, render_rays_culled, scatter_results
 from .data import DeviceRayBatches, DeviceViewBatches
+from .density_grid import DensityGrid
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
 from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, normal_rays, normal_vertex_colors, pack_volume,
                    query_rgb_sigma, rgb_sigma_grid, sigma_grid, vertex_normals, write_ply, write_vol)
@@ -23,6 +24,7 @@ __all__ = [
     "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
     "vertex_normals", "normal_rays", "normal_vertex_colors",
     "OccupancyGrid", "occupancy_grid", "pack_occupancy", "cull_rays", "scatter_results", "render_rays_culled",
+    "DensityGrid",
     "ssim", "visualize_depth",
     "DeviceViewBatches", "Views", "read_blender_views", "read_llff_views",
 ]

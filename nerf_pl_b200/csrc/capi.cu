@@ -15,6 +15,7 @@
 #include "../../include/nerf_pl_b200_views.h"
 #include "../../include/nerf_pl_b200_samples.h"
 #include "../../include/nerf_pl_b200_train_samples.h"
+#include "../../include/nerf_pl_b200_density.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
@@ -22,6 +23,7 @@
 #include "metrics_kernels.cuh"
 #include "sample_skip_kernels.cuh"
 #include "train_skip_kernels.cuh"
+#include "density_kernels.cuh"
 
 #include <thrust/iterator/transform_iterator.h>
 
@@ -925,6 +927,34 @@ int cull_prepare(const float* rays, int64_t n, void* ws, size_t bytes, CullParam
   p->bits = nullptr; p->flag = nullptr; p->live_idx = nullptr; p->live_rays = nullptr;
   return 0;
 }
+
+// ------------------------------------------------------------------ the density grid (kernels: density_kernels.cuh)
+
+// The workspace of an update of C cells, `chunk` (<= C) at a time: the chunk's points and sigma, then the two
+// byte-per-cell buffers of occupancy_carve.
+size_t density_carve(long long C, long long chunk, void* base, float** xyz, float** sigma, uint8_t* buf[2]) {
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  *xyz = c.take<float>(chunk * 3);
+  *sigma = c.take<float>(chunk);
+  c.off += occupancy_carve(C, base ? static_cast<uint8_t*>(base) + c.off : nullptr, buf);
+  return c.off;
+}
+
+// N in [2, 1625] and every range finite with min != max.
+int density_box(int64_t N, const double* ranges, DensityBox* b, const char* who) {
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
+  if (!ranges) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  for (int a = 0; a < 3; ++a) {
+    const double lo = ranges[2 * a], hi = ranges[2 * a + 1];
+    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
+      return fail(NERFB200_EINVAL, "%s: every range must be finite with min != max", who);
+    b->lo[a] = lo;
+    b->hi[a] = hi;
+  }
+  b->M = N - 1;
+  return 0;
+}
+
 
 // ------------------------------------------------------------------ per-sample skipping (kernels: sample_skip_kernels.cuh)
 constexpr long long kSkipMaxRays = 1LL << 22;   // rows (n * S_f) and ray indices stay in int32
@@ -2483,5 +2513,68 @@ int nerfb200_visualize_depth(const float* depth, int64_t h, int64_t w, int64_t s
   return launch("visualize_depth colour launch", depth_color_kernel, grid_blocks(n, kDepthThreads), kDepthThreads, 0,
                 stream, p);
 }
+
+// ---- the density grid (kernels: density_kernels.cuh)
+size_t nerfb200_density_workspace_bytes(int64_t N, int64_t chunk) {
+  if (N < 2 || N > kVolMaxN || chunk < 1) return 0;
+  const long long C = (N - 1) * (N - 1) * (N - 1);
+  float *xyz, *sigma;
+  uint8_t* buf[2];
+  return density_carve(C, chunk < C ? chunk : C, nullptr, &xyz, &sigma, buf);
+}
+
+int nerfb200_density_points(int64_t N, const double ranges_host[6], const int64_t* key_dev, int64_t start,
+                            int64_t count, float* xyz, void* stream) {
+  DensityBox b;
+  TRY(density_box(N, ranges_host, &b, "density_points"));
+  const long long C = b.M * b.M * b.M;
+  if (start < 0 || count < 0 || start > C || count > C - start)
+    return fail(NERFB200_EINVAL, "density_points: cells [start, start + count) outside the grid");
+  if (count == 0) return 0;
+  if (!key_dev || !xyz) return fail(NERFB200_EINVAL, "density_points: NULL argument");
+  return launch("density_points launch", density_points_kernel, grid_blocks(count, 256), 256, 0, stream, b,
+                reinterpret_cast<const long long*>(key_dev), static_cast<long long>(start), static_cast<long long>(count),
+                xyz);
+}
+
+int nerfb200_density_update(const void* packed, int64_t N, const double ranges_host[6], double sigma_threshold,
+                            float decay, int32_t dilate, int64_t chunk, int64_t* key_dev, float* density,
+                            uint32_t* bits, void* ws, size_t bytes, void* stream) {
+  DensityBox b;
+  TRY(density_box(N, ranges_host, &b, "density_update"));
+  if (sigma_threshold != sigma_threshold) return fail(NERFB200_EINVAL, "density_update: sigma_threshold is NaN");
+  if (!(decay >= 0.f && decay <= 1.f)) return fail(NERFB200_EINVAL, "density_update: decay must be in [0, 1]");
+  if (dilate < 0) return fail(NERFB200_EINVAL, "density_update: dilate < 0");
+  if (chunk < 1) return fail(NERFB200_EINVAL, "density_update: chunk < 1");
+  if (!packed || !key_dev || !density || !bits || !ws) return fail(NERFB200_EINVAL, "density_update: NULL argument");
+  if (bytes < nerfb200_density_workspace_bytes(N, chunk))
+    return fail(NERFB200_EINVAL, "density_update: workspace smaller than nerfb200_density_workspace_bytes");
+  const long long M = b.M, C = M * M * M, ch = chunk < C ? chunk : C;
+  float *xyz, *sigma;
+  uint8_t* buf[2];
+  density_carve(C, ch, ws, &xyz, &sigma, buf);
+  uint8_t *a = buf[0], *o = buf[1];
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  long long* key = reinterpret_cast<long long*>(key_dev);
+  for (long long c0 = 0; c0 < C; c0 += ch) {
+    const long long n = C - c0 < ch ? C - c0 : ch;
+    TRY(nerfb200_density_points(N, ranges_host, key_dev, c0, n, xyz, stream));
+    TRY(nerfb200_query_sigma(xyz, n, 3, packed, sigma, stream));
+    TRY(launch("density decay launch", density_decay_kernel, grid_blocks(n, 256), 256, 0, s, sigma, c0, n, decay,
+               sigma_threshold, density, a, c0 + n == C ? key : nullptr));
+  }
+  // the dilation and packing of nerfb200_occupancy_pack
+  const int radius = static_cast<int>(dilate < M - 1 ? dilate : M - 1);
+  if (radius > 0) {
+    const long long stride[3] = {1, M, M * M};
+    for (int ax = 0; ax < 3; ++ax) {
+      TRY(launch("density dilate launch", occ_dilate_axis_kernel, grid_blocks(C, 256), 256, 0, s, a, o, M, stride[ax],
+                 radius));
+      std::swap(a, o);
+    }
+  }
+  return launch("density pack launch", occ_pack_kernel, grid_blocks(C, 256), 256, 0, s, a, C, bits);
+}
+
 
 }  // extern "C"

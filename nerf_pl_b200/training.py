@@ -397,11 +397,18 @@ class CapturedTrainStep:
     ``render_rays_loss(..., occupancy=grid)`` computes it.  The step copies the grid's bits into a buffer it owns
     and uses a ``SkipTrainWorkspace`` of its own; ``set_occupancy(grid)`` copies a rebuilt grid of the same ``N``,
     ranges and ``dilate`` into that buffer between replays, and ``live_samples`` is the device int64 pair of the last
-    replay's evaluated coarse and fine sample counts."""
+    replay's evaluated coarse and fine sample counts.
+
+    ``occupancy`` may also be a ``nerf_pl_b200.DensityGrid``, which the step then keeps current itself: the grid's
+    ``update`` from the last trained model (the fine one, or the coarse one when ``N_importance == 0``) is captured
+    as a second graph, and ``step()`` replays it before the training step whenever ``steps % update_every == 0``
+    (so replay 0 starts from a refreshed grid).  The training graph reads the density grid's own bits, and
+    ``set_occupancy`` raises.  The warm-up also runs the update and restores the grid's density, bits and key.
+    ``launches_per_update`` is the number of library kernels one update replay runs."""
 
     def __init__(self, models, batches, optimizer, N_samples: int = 64, use_disp: bool = False, perturb: float = 1.0,
                  noise_std: float = 1.0, N_importance: int = 64, white_back: bool = False, randoms=None,
-                 warmup: int = 3, occupancy=None):
+                 warmup: int = 3, occupancy=None, update_every: Optional[int] = None):
         from .optim import FusedAdam
         global _CAPTURED_SEEDS
         if not (isinstance(optimizer, FusedAdam) and optimizer.capturable):
@@ -439,7 +446,17 @@ class CapturedTrainStep:
             self.seed_word = torch.tensor(s, dtype=torch.int64, device=dev)
         elif randoms is not None:
             raise ValueError("randoms must be None, 'kernel' or {'seed': int}")
-        self._grid = None
+        from .density_grid import DensityGrid
+        self._grid = self.density_grid = None
+        self.update_every = None
+        if isinstance(occupancy, DensityGrid):
+            if update_every is None or int(update_every) != update_every or int(update_every) < 1:
+                raise ValueError(f"occupancy=DensityGrid needs update_every, an int >= 1 (got {update_every!r})")
+            self.update_every = int(update_every)
+            self.density_grid = occupancy
+            occupancy = occupancy.grid              # the training graph reads the density grid's own bits
+        elif update_every is not None:
+            raise ValueError("update_every needs occupancy=DensityGrid (a grid the step maintains itself)")
         if occupancy is None:
             self.workspace = TrainWorkspace(dev, B, S_c, K)
         else:
@@ -448,7 +465,8 @@ class CapturedTrainStep:
             check_shape(B, S_c, K)
             self._check_grid(occupancy, dev)
             r = occupancy.ranges
-            self._grid = OccupancyGrid(occupancy.bits.clone(), occupancy.N, r[0:2], r[2:4], r[4:6], occupancy.dilate)
+            self._grid = occupancy if self.density_grid is not None else \
+                OccupancyGrid(occupancy.bits.clone(), occupancy.N, r[0:2], r[2:4], r[4:6], occupancy.dilate)
             self.workspace = SkipTrainWorkspace(dev, B, S_c, K)
             self._live = torch.zeros(2, dtype=torch.int64, device=dev)
         self._perm = batches.next_permutation().clone()
@@ -496,11 +514,15 @@ class CapturedTrainStep:
             saved_st = [{k: v.clone() for k, v in opt.state[p].items()} if len(opt.state.get(p, {})) else None
                         for p in self.params]
             saved_seed = None if self.seed_word is None else self.seed_word.clone()
+            dg = self.density_grid
+            saved_dg = None if dg is None else (dg._density.clone(), dg.bits.clone(), dg.key.clone())
         opt.sync_lr()
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             for _ in range(max(warmup, 1)):
+                if dg is not None:
+                    dg.update(self.models[-1])
                 opt.zero_grad(set_to_none=True)     # every parameter the optimizer holds: no stale gradient steps
                 self._offset.zero_()        # every warm-up step takes the first batch: never past the permutation
                 self._body()
@@ -518,8 +540,22 @@ class CapturedTrainStep:
             self._offset.zero_()
             if saved_seed is not None:
                 self.seed_word.copy_(saved_seed)
+            if saved_dg is not None:
+                for t, v in zip((dg._density, dg.bits, dg.key), saved_dg):
+                    t.copy_(v)
         opt.zero_grad(set_to_none=True)     # captured: only the models' parameters get gradients, hence updates
         lib = _lib.load()
+        self.update_graph = None
+        self.launches_per_update = 0
+        if dg is not None:
+            self.update_graph = torch.cuda.CUDAGraph()
+            n0 = lib.nerfb200_launch_count()
+            try:
+                with torch.cuda.graph(self.update_graph):
+                    dg.update(self.models[-1])
+            except Exception as e:
+                raise RuntimeError(f"CapturedTrainStep: capturing the density grid update failed: {e}") from e
+            self.launches_per_update = int(lib.nerfb200_launch_count() - n0)
         self.graph = torch.cuda.CUDAGraph()
         n0 = lib.nerfb200_launch_count()
         try:
@@ -547,6 +583,8 @@ class CapturedTrainStep:
         graph holds N, the ranges and dilate by value: a grid that differs in any of them is a ValueError."""
         if self._grid is None:
             raise ValueError("this step was captured without occupancy=")
+        if self.density_grid is not None:
+            raise ValueError("this step maintains its DensityGrid itself (update_every); set_occupancy does not apply")
         self._check_grid(grid, self._grid.device)
         g = self._grid
         if (grid.N, tuple(grid.ranges), grid.dilate) != (g.N, tuple(g.ranges), g.dilate):
@@ -563,6 +601,8 @@ class CapturedTrainStep:
             self._offset.zero_()
             self.epoch = epoch
         self.optimizer.sync_lr()
+        if self.update_graph is not None and self.steps % self.update_every == 0:
+            self.update_graph.replay()
         self.graph.replay()
         self.steps += 1
         return self._loss, self._psnr
