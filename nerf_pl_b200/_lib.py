@@ -23,9 +23,9 @@ if os.environ.get("NERFB200_LIB"):          # a library built elsewhere (e.g. wi
 SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
            "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h", "sample_skip_kernels.cuh",
-           "train_skip_kernels.cuh", "density_kernels.cuh"]
+           "train_skip_kernels.cuh", "density_kernels.cuh", "masked_grid_kernels.cuh"]
 INCLUDES = ["nerf_pl_b200.h", "nerf_pl_b200_metrics.h", "nerf_pl_b200_views.h", "nerf_pl_b200_samples.h",
-            "nerf_pl_b200_train_samples.h", "nerf_pl_b200_density.h"]
+            "nerf_pl_b200_train_samples.h", "nerf_pl_b200_density.h", "nerf_pl_b200_masked_grid.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -280,6 +280,15 @@ DENSITY_SIGNATURES = {
     "nerfb200_density_update": (_i32, [_vp, _i64, POINTER(_f64), _f64, _f32, _i32, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
+# The entries of the companion header include/nerf_pl_b200_masked_grid.h, in header order (its own tests check it).
+MASKED_GRID_SIGNATURES = {
+    "nerfb200_masked_grid_workspace_bytes": (_sz, [_i64]),
+    "nerfb200_sigma_grid_masked": (_i32, [_vp, _i64, POINTER(_f64), _vp, _i64, POINTER(_f64), _i64, _vp, _sz, _vp,
+                                          POINTER(_i64), _vp]),
+    "nerfb200_rgb_sigma_grid_masked": (_i32, [_vp, _i64, POINTER(_f64), _vp, _i64, POINTER(_f64), _i64, _vp, _sz, _vp,
+                                              POINTER(_i64), _vp]),
+}
+
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
@@ -328,7 +337,8 @@ def load() -> ctypes.CDLL:
             lib = ctypes.CDLL(LIB_PATH)
             for name, (restype, argtypes) in (*SIGNATURES.items(), *METRICS_SIGNATURES.items(),
                                               *VIEWS_SIGNATURES.items(), *SAMPLES_SIGNATURES.items(),
-                                              *TRAIN_SAMPLES_SIGNATURES.items(), *DENSITY_SIGNATURES.items()):
+                                              *TRAIN_SAMPLES_SIGNATURES.items(), *DENSITY_SIGNATURES.items(),
+                                              *MASKED_GRID_SIGNATURES.items()):
                 fn = getattr(lib, name)
                 fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:

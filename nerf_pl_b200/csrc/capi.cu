@@ -16,6 +16,7 @@
 #include "../../include/nerf_pl_b200_samples.h"
 #include "../../include/nerf_pl_b200_train_samples.h"
 #include "../../include/nerf_pl_b200_density.h"
+#include "../../include/nerf_pl_b200_masked_grid.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
@@ -24,6 +25,7 @@
 #include "sample_skip_kernels.cuh"
 #include "train_skip_kernels.cuh"
 #include "density_kernels.cuh"
+#include "masked_grid_kernels.cuh"
 
 #include <thrust/iterator/transform_iterator.h>
 
@@ -1015,6 +1017,73 @@ int skip_grid(const uint32_t* bits, int64_t N, const double* ranges, SkipGrid* g
   }
   g->bits = bits;
   g->M = N - 1;
+  return 0;
+}
+
+// ------------------------------------------------------------------ grids through an occupancy grid
+// (kernels: masked_grid_kernels.cuh)
+
+// The workspace of one chunk of `chunk` points: the tile counts, their scan and CUB's scratch, then the compacted
+// positions, indices and query outputs.  The outputs are sized for four channels, so one size serves both entries.
+size_t masked_grid_carve(long long chunk, void* base, MaskedGridParams* p, CubScratch* s) {
+  const long long tiles = ceil_div(chunk, kMaskTile);
+  size_t tb = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tb, static_cast<const unsigned long long*>(nullptr),
+                                static_cast<unsigned long long*>(nullptr), static_cast<int>(tiles + 1));
+  s->temp_bytes = tb;
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  p->tcnt = c.take<unsigned long long>(tiles + 1);
+  p->tofs = c.take<unsigned long long>(tiles + 1);
+  s->temp = c.take(s->temp_bytes);
+  p->xyz = c.take<float>(chunk * 3);
+  p->idx = c.take<long long>(chunk);
+  p->vals = c.take<float>(chunk * 4);
+  return c.off;
+}
+
+// Both masked grids (channels 1 or 4), after the entry's own checks of N and the output.  Per chunk: classify, scan,
+// one read-back of the evaluated count; with points to evaluate, emit, the point query and the scatter.
+int masked_grid(const void* packed, int64_t N, const double* ranges, const uint32_t* bits, int64_t occ_N,
+                const double* occ_ranges, int64_t chunk, void* ws, size_t bytes, float* out, int64_t* evaluated_host,
+                int channels, void* stream, const char* who) {
+  if (chunk < 1) return fail(NERFB200_EINVAL, "%s: chunk < 1", who);
+  if (!packed || !ranges || !bits || !occ_ranges || !ws || !out || !evaluated_host)
+    return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  MaskedGridParams p{};
+  TRY(skip_grid(bits, occ_N, occ_ranges, &p.occ, who));
+  CubScratch sc;
+  if (bytes < masked_grid_carve(chunk, ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_masked_grid_workspace_bytes(chunk)", who);
+  for (int a = 0; a < 3; ++a) { p.lo[a] = ranges[2 * a]; p.hi[a] = ranges[2 * a + 1]; }
+  p.N = N;
+  p.channels = channels;
+  p.out = out;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long total = N * N * N;
+  long long evaluated = 0;
+  for (long long s0 = 0; s0 < total; s0 += chunk) {
+    p.start = s0;
+    p.count = total - s0 < chunk ? total - s0 : chunk;
+    const long long tiles = ceil_div(p.count, kMaskTile);
+    CUDA_TRY(cudaMemsetAsync(p.tcnt + tiles, 0, sizeof(unsigned long long), s), "masked grid memset");
+    TRY(launch("masked grid classify launch", masked_grid_classify_kernel, grid_blocks(tiles * kMaskThreads, 256),
+               kMaskThreads, 0, s, p));
+    size_t tb = sc.temp_bytes;
+    TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, p.tcnt, p.tofs, static_cast<int>(tiles + 1), s),
+                   "masked grid scan"));
+    unsigned long long h = 0;
+    CUDA_TRY(cudaMemcpyAsync(&h, p.tofs + tiles, sizeof(h), cudaMemcpyDeviceToHost, s), "masked grid readback");
+    CUDA_TRY(cudaStreamSynchronize(s), "masked grid readback");
+    if (h == 0) continue;
+    const long long n = static_cast<long long>(h);
+    TRY(launch("masked grid emit launch", masked_grid_emit_kernel, grid_blocks(tiles * kMaskThreads, 256), kMaskThreads,
+               0, s, p));
+    TRY(channels == 4 ? nerfb200_query_rgb_sigma(p.xyz, n, 3, packed, p.vals, stream)
+                      : nerfb200_query_sigma(p.xyz, n, 3, packed, p.vals, stream));
+    TRY(launch("masked grid scatter launch", masked_grid_scatter_kernel, grid_blocks(n, 256), 256, 0, s, p, n));
+    evaluated += n;
+  }
+  *evaluated_host = evaluated;
   return 0;
 }
 
@@ -2574,6 +2643,32 @@ int nerfb200_density_update(const void* packed, int64_t N, const double ranges_h
     }
   }
   return launch("density pack launch", occ_pack_kernel, grid_blocks(C, 256), 256, 0, s, a, C, bits);
+}
+
+// ---- grids through an occupancy grid (kernels: masked_grid_kernels.cuh)
+size_t nerfb200_masked_grid_workspace_bytes(int64_t chunk) {
+  if (chunk < 1) return 0;
+  MaskedGridParams p;
+  CubScratch sc;
+  return masked_grid_carve(chunk, nullptr, &p, &sc);
+}
+
+int nerfb200_sigma_grid_masked(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
+                               int64_t occ_N, const double occ_ranges_host[6], int64_t chunk, void* ws, size_t bytes,
+                               float* sigma_out, int64_t* evaluated_host, void* stream) {
+  if (N < 2) return fail(NERFB200_EINVAL, "sigma_grid_masked: N < 2");
+  return masked_grid(packed, N, ranges_host, bits, occ_N, occ_ranges_host, chunk, ws, bytes, sigma_out, evaluated_host,
+                     1, stream, "sigma_grid_masked");
+}
+
+int nerfb200_rgb_sigma_grid_masked(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
+                                   int64_t occ_N, const double occ_ranges_host[6], int64_t chunk, void* ws,
+                                   size_t bytes, float* rgbsigma_out, int64_t* evaluated_host, void* stream) {
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "rgb_sigma_grid_masked: N not in [2, 1625]");
+  if (reinterpret_cast<uintptr_t>(rgbsigma_out) & 15)
+    return fail(NERFB200_EINVAL, "rgb_sigma_grid_masked: out must be 16-byte aligned");
+  return masked_grid(packed, N, ranges_host, bits, occ_N, occ_ranges_host, chunk, ws, bytes, rgbsigma_out,
+                     evaluated_host, 4, stream, "rgb_sigma_grid_masked");
 }
 
 

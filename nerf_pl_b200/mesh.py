@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .culling import OccupancyGrid, render_rays_culled
 from .inference import to_uint8
 from .nerf import Embedding, packed_weights
 from .rendering import render_rays
@@ -51,11 +52,47 @@ def grid_positions(N: int, x_range, y_range, z_range, start: int = 0, count: Opt
     return out
 
 
+def _check_occupancy(occupancy, dev: torch.device) -> OccupancyGrid:
+    if not isinstance(occupancy, OccupancyGrid):
+        raise ValueError("occupancy must be a nerf_pl_b200.OccupancyGrid (for a DensityGrid pass its .grid)")
+    if occupancy.device != dev:
+        raise RuntimeError(f"the occupancy grid is on {occupancy.device}, the model on {dev}")
+    return occupancy
+
+
+def _masked_grid(entry: str, model: torch.nn.Module, N: int, ranges, occupancy, chunk: int, channels: int):
+    """The grid of ``entry`` (nerfb200_sigma_grid_masked or nerfb200_rgb_sigma_grid_masked): (grid, evaluated)."""
+    dev = _device_of(model)
+    occ = _check_occupancy(occupancy, dev)
+    out = torch.empty((N, N, N) if channels == 1 else (N, N, N, channels), dtype=torch.float32, device=dev)
+    blob = packed_weights(model)
+    chunk = int(min(chunk, N ** 3))
+    nbytes = _lib.load().nerfb200_masked_grid_workspace_bytes(chunk)
+    if nbytes == 0:
+        raise ValueError(f"chunk = {chunk} must be >= 1")
+    ws = _lib.workspace(nbytes, dev)
+    evaluated = ctypes.c_int64()
+    _lib.call(entry, dev, blob.data_ptr(), N, ranges, occ.bits.data_ptr(), occ.N, (ctypes.c_double * 6)(*occ.ranges),
+              chunk, ws.data_ptr(), ws.numel(), out.data_ptr(), ctypes.byref(evaluated))
+    return out, int(evaluated.value)
+
+
 @torch.no_grad()
-def sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk: int = 1 << 21) -> torch.Tensor:
+def sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk: int = 1 << 21, *,
+               occupancy: Optional[OccupancyGrid] = None, return_evaluated: bool = False):
     """(N, N, N) fp32 ``max(sigma, 0)`` of ``model`` on the reference's grid (extract_color_mesh.py:113-140):
     ``sigma[i, j, k] = max(sigma(x_j, y_i, z_k), 0)`` (np.meshgrid's 'xy' indexing).  ``chunk`` points are
-    queried per launch; the scratch is their positions only."""
+    queried per launch; the scratch is their positions only.
+
+    ``occupancy`` (an ``OccupancyGrid``; for a ``DensityGrid`` its ``.grid``) evaluates only the lattice points that
+    lie in the closed box of an occupied cell, the rule of ``skip="samples"``: those get the value above bit for bit,
+    every other point gets +0.0 (DESIGN.md "Grids through an occupancy grid").  Its N and box are independent of the
+    mesh grid's.  It synchronises once per chunk.  ``return_evaluated`` returns (grid, number of evaluated points;
+    N^3 without a grid)."""
+    if occupancy is not None:
+        out, evaluated = _masked_grid("nerfb200_sigma_grid_masked", model, int(N),
+                                      _lib.ranges_host(x_range, y_range, z_range), occupancy, chunk, 1)
+        return (out, evaluated) if return_evaluated else out
     dev = _device_of(model)
     out = torch.empty(N, N, N, dtype=torch.float32, device=dev)
     blob = packed_weights(model)
@@ -63,7 +100,7 @@ def sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk:
     ws = _lib.workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
     _lib.call("nerfb200_sigma_grid", dev, blob.data_ptr(), N, _lib.ranges_host(x_range, y_range, z_range), chunk,
               ws.data_ptr(), ws.numel(), out.data_ptr())
-    return out
+    return (out, N ** 3) if return_evaluated else out
 
 
 @torch.no_grad()
@@ -121,9 +158,12 @@ def keep_largest_cluster(vertices: torch.Tensor, triangles: torch.Tensor) -> Tup
 
 @torch.no_grad()
 def extract_mesh(model: torch.nn.Module, N_grid: int, x_range, y_range, z_range, sigma_threshold: float,
-                 keep_largest: bool = True) -> Tuple[torch.Tensor, torch.Tensor]:
-    """extract_color_mesh.py:113-171: world vertices (V, 3) fp32 and triangles (T, 3) int32 on the device."""
-    sigma = sigma_grid(model, N_grid, x_range, y_range, z_range)
+                 keep_largest: bool = True, *,
+                 occupancy: Optional[OccupancyGrid] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """extract_color_mesh.py:113-171: world vertices (V, 3) fp32 and triangles (T, 3) int32 on the device.
+    ``occupancy``: the sigma grid is ``sigma_grid(..., occupancy=occupancy)``, so density the grid calls empty
+    never reaches marching cubes."""
+    sigma = sigma_grid(model, N_grid, x_range, y_range, z_range, occupancy=occupancy)
     vidx, tris = marching_cubes(sigma, sigma_threshold)
     del sigma
     verts = to_world(vidx, N_grid, x_range, y_range, z_range)
@@ -172,15 +212,21 @@ def project_view(vertices: torch.Tensor, image: torch.Tensor, pose, focal: float
 @torch.no_grad()
 def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: torch.Tensor, poses: Sequence,
                        focal: float, near: float, N_samples: int = 64, occ_threshold: float = 0.2,
-                       white_back: bool = False, return_opacities: bool = False):
+                       white_back: bool = False, return_opacities: bool = False, *,
+                       occupancy: Optional[OccupancyGrid] = None):
     """extract_color_mesh.py:206-284 (the default colour-averaging method) on the device.
 
     vertices (V, 3) fp32 world; images (n_views, H, W, 3) uint8 CUDA; poses: n_views (3, 4) camera-to-world;
     focal: the dataset focal (K is float32 with principal point (W/2, H/2)); near: ``dataset.bounds.min()``.
     Per view: project + bilinear sample + occlusion rays, the fused ``render_rays`` with ``model`` as the only
     network (N_importance = 0, test_time), and a float64 accumulation in view order.  Returns (V, 3) uint8
-    (and the per-view opacities (n_views, V) when ``return_opacities``)."""
+    (and the per-view opacities (n_views, V) when ``return_opacities``).
+
+    ``occupancy``: each view's occlusion rays are rendered by ``render_rays_culled(..., skip="samples")`` on that grid
+    instead, so density in cells it calls empty does not occlude a vertex."""
     v = _cuda(vertices, "vertices").detach().to(torch.float32).contiguous()
+    if occupancy is not None:
+        _check_occupancy(occupancy, _device_of(model))
     imgs = _cuda(images, "images").contiguous()
     if imgs.dtype != torch.uint8 or imgs.dim() != 4 or imgs.shape[3] != 3:
         raise ValueError("images must be (n_views, H, W, 3) uint8")
@@ -192,8 +238,12 @@ def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: t
     opac = []
     for idx in range(imgs.shape[0]):
         colors, depth, rays = project_view(v, imgs[idx], poses[idx], focal, near)
-        res = render_rays([model], emb, rays, N_samples, False, 0, 0, 0, 1024 * 32, white_back, test_time=True,
-                          match_reference_rng=False)
+        if occupancy is None:
+            res = render_rays([model], emb, rays, N_samples, False, 0, 0, 0, 1024 * 32, white_back, test_time=True,
+                              match_reference_rng=False)
+        else:
+            res = render_rays_culled([model], emb, rays, occupancy, N_samples, False, 0, white_back, True,
+                                     skip="samples")
         opacity = res["opacity_coarse"].contiguous()
         if return_opacities:
             opac.append(opacity)
@@ -260,20 +310,29 @@ def normal_rays(vertices: torch.Tensor, normals: torch.Tensor, near: float, far:
 @torch.no_grad()
 def normal_vertex_colors(nerf_coarse: torch.nn.Module, nerf_fine: torch.nn.Module, vertices: torch.Tensor,
                          triangles: torch.Tensor, near: float, far: float, N_samples: int = 64,
-                         N_importance: int = 64, near_t: float = 1.0, white_back: bool = False) -> torch.Tensor:
+                         N_importance: int = 64, near_t: float = 1.0, white_back: bool = False, *,
+                         occupancy: Optional[OccupancyGrid] = None) -> torch.Tensor:
     """extract_color_mesh.py:187-203 and 280-281 (``--use_vertex_normal``) on the device: (V, 3) uint8 vertex colours
     ``(rgb_fine * 255).astype(uint8)`` of rays that start at ``v - n * near * near_t`` and run along the open3d
     vertex normal n.  One ``vertex_normals``, one ``normal_rays``, one fused ``render_rays`` of all V rays with both
     networks (test_time, perturb 0, noise 0), and ``to_uint8``.  near / far: ``dataset.bounds.min()`` / ``.max()``;
-    white_back: ``dataset.white_back``."""
-    _device_of(nerf_coarse)
+    white_back: ``dataset.white_back``.  ``occupancy``: the rays are rendered by ``render_rays_culled(...,
+    skip="samples")`` on that grid instead, so density in cells it calls empty does not tint the colours."""
+    dev = _device_of(nerf_coarse)
     _device_of(nerf_fine)
+    if occupancy is not None:
+        _check_occupancy(occupancy, dev)
     if int(N_importance) <= 0:
         raise ValueError("normal_vertex_colors needs N_importance > 0 (the colours are rgb_fine)")
     normals = vertex_normals(vertices, triangles)
     rays = normal_rays(vertices, normals, near, far, near_t)
-    res = render_rays([nerf_coarse, nerf_fine], [Embedding(3, 10), Embedding(3, 4)], rays, int(N_samples), False, 0, 0,
-                      int(N_importance), 1024 * 32, bool(white_back), test_time=True, match_reference_rng=False)
+    emb = [Embedding(3, 10), Embedding(3, 4)]
+    if occupancy is None:
+        res = render_rays([nerf_coarse, nerf_fine], emb, rays, int(N_samples), False, 0, 0, int(N_importance),
+                          1024 * 32, bool(white_back), test_time=True, match_reference_rng=False)
+    else:
+        res = render_rays_culled([nerf_coarse, nerf_fine], emb, rays, occupancy, int(N_samples), False,
+                                 int(N_importance), bool(white_back), True, skip="samples")
     return to_uint8(res["rgb_fine"])
 
 
@@ -291,10 +350,20 @@ def query_rgb_sigma(model: torch.nn.Module, xyz: torch.Tensor) -> torch.Tensor:
 
 
 @torch.no_grad()
-def rgb_sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk: int = 1 << 21) -> torch.Tensor:
+def rgb_sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk: int = 1 << 21, *,
+                   occupancy: Optional[OccupancyGrid] = None, return_evaluated: bool = False):
     """(N, N, N, 4) fp32 [sigmoid rgb, raw sigma] of ``model`` on the grid of ``sigma_grid`` with the direction
     (0, 0, 0): extract_mesh.ipynb's ``rgbsigma`` ("Search for tight bounds"), reshaped.  Raw sigma: no
-    ``max(sigma, 0)``.  ``chunk`` points are queried per launch; the scratch is their positions only."""
+    ``max(sigma, 0)``.  ``chunk`` points are queried per launch; the scratch is their positions only.
+
+    ``occupancy`` and ``return_evaluated`` as for ``sigma_grid``: an evaluated point gets the four channels above bit
+    for bit, every other point (0, 0, 0, 0), which ``pack_volume`` drops (alpha 0)."""
+    if occupancy is not None:
+        if not 2 <= int(N) <= 1625:
+            raise ValueError(f"rgb_sigma_grid: N = {N} outside [2, 1625]")
+        out, evaluated = _masked_grid("nerfb200_rgb_sigma_grid_masked", model, int(N),
+                                      _lib.ranges_host(x_range, y_range, z_range), occupancy, chunk, 4)
+        return (out, evaluated) if return_evaluated else out
     dev = _device_of(model)
     out = torch.empty(N, N, N, 4, dtype=torch.float32, device=dev)
     blob = packed_weights(model)
@@ -302,7 +371,7 @@ def rgb_sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, ch
     ws = _lib.workspace(_lib.load().nerfb200_sigma_grid_workspace_bytes(chunk), dev)
     _lib.call("nerfb200_rgb_sigma_grid", dev, blob.data_ptr(), N, _lib.ranges_host(x_range, y_range, z_range), chunk,
               ws.data_ptr(), ws.numel(), out.data_ptr())
-    return out
+    return (out, N ** 3) if return_evaluated else out
 
 
 @torch.no_grad()
