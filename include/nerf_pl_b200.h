@@ -444,6 +444,265 @@ int nerfb200_check_status(void);
 /* Device properties the launcher uses: SM count of the current device (0 if none). */
 int nerfb200_sm_count(void);
 
+
+/* ==== image metrics of the reference's eval and validation loop, on the device ====================
+ * Definitions and their provenance: DESIGN.md "Image metrics". */
+
+/* ---- SSIM -----------------------------------------------------------------------------------
+ * Replaces: metrics.py:15-20 ssim(image_pred, image_gt, reduction) = 1 - 2 * kornia.losses.ssim(pred, gt, 3,
+ * reduction), kornia 0.2.0's published definition: a 3 x 3 window (outer product of the normalised size-3 Gaussian,
+ * sigma 1.5), zero padding 1, per channel; mu, sigma^2 and sigma12 as filter(x*y) - mu_x*mu_y; C1 = 0.01^2,
+ * C2 = 0.03^2; loss = clamp(1 - ssim_map, 0, 1) / 2.  Every pixel's moments and ssim_map are computed in double.
+ *
+ * pred, gt: (b, c, h, w) fp32 with element strides pred_strides_host / gt_strides_host (4 HOST int64 each, >= 0),
+ * b, c, h, w >= 1.  reduction:
+ *   NERFB200_SSIM_MEAN / NERFB200_SSIM_SUM: out is ONE device float, 1 - 2 * (mean / sum of the loss); the sum is
+ *     taken in double in a fixed order, so the result does not depend on the grid.  Needs the workspace; does not
+ *     synchronise.
+ *   NERFB200_SSIM_NONE: out is the contiguous (b, c, h, w) map 1 - 2 * loss; ws may be NULL. */
+#define NERFB200_SSIM_MEAN 0
+#define NERFB200_SSIM_SUM 1
+#define NERFB200_SSIM_NONE 2
+size_t nerfb200_ssim_workspace_bytes(int64_t b, int64_t c, int64_t h, int64_t w);
+int nerfb200_ssim(const float* pred, const int64_t pred_strides_host[4], const float* gt,
+                  const int64_t gt_strides_host[4], int64_t b, int64_t c, int64_t h, int64_t w, int32_t reduction,
+                  void* ws, size_t bytes, float* out, void* stream);
+
+/* ---- depth visualisation ----------------------------------------------------------------------
+ * Replaces: utils/visualization.py:6-18 visualize_depth(depth) with the default cmap=cv2.COLORMAP_JET, bit for
+ * bit: nan_to_num (NaN -> 0, +-inf -> +-FLT_MAX), y = (x - min) / (max - min + 1e-8f) in fp32, uint8(255 * y) by
+ * truncation, OpenCV's JET table (csrc/jet_lut.h), u8 / 255.  depth: (h, w) fp32 with element strides stride_h,
+ * stride_w (>= 0); out: contiguous (3, h, w) fp32 in cv2's channel order (channel 0 = blue), as the reference
+ * returns it.  A map holding both +inf and -inf is outside the contract.  Two launches, no synchronisation. */
+size_t nerfb200_visualize_depth_workspace_bytes(int64_t h, int64_t w);
+int nerfb200_visualize_depth(const float* depth, int64_t h, int64_t w, int64_t stride_h, int64_t stride_w, void* ws,
+                             size_t bytes, float* out, void* stream);
+
+/* ==== training batches generated on the device from the dataset's views ===========================
+ * Definitions and their exactness argument: DESIGN.md "Training batches from the views". */
+
+/* ---- one training batch from the views --------------------------------------------------------
+ * Replaces: the all_rays / all_rgbs buffers of datasets/blender.py:47-69 and datasets/llff.py:221-253 and the
+ * DataLoader's gather from them.  Row k of the batch is pixel ids[k] of the reference's concatenation order
+ * (view-major, pixels row-major): p = (v * H + j) * W + i, 0 <= p < V * H * W (an id outside gives a NaN row).
+ *   images: (V, H, W, C) uint8, C = 3 (RGB) or 4 (RGBA);  c2w: (V, 3, 4) fp32 poses, 16-byte aligned.
+ *   rays:   (n, 8) fp32 [o(3) d(3) near far], 16-byte aligned: nerfb200_generate_rays' row of pixel (j, i) of view v
+ *           (ndc != 0: the forward-facing NDC warp of llff.py:236-241, near/far columns 0/1).
+ *   rgbs:   (n, 3) fp32: u8 / 255 (T.ToTensor()); with C = 4, rgb * a + (1 - a) (blender.py:58).
+ * V, H, W >= 1, focal > 0, n >= 0.  One launch; reads nothing on the host, so it can be captured in a graph. */
+int nerfb200_view_batch(const uint8_t* images, int64_t V, int32_t H, int32_t W, int32_t C, const float* c2w,
+                        float focal, float near, float far, int32_t ndc, const int64_t* ids, int64_t n, float* rays,
+                        float* rgbs, void* stream);
+
+/* ==== rendering with empty samples skipped (inference) ============================================
+ * Definition and guarantees: DESIGN.md "Skipping empty samples". */
+
+/* One render of n_rays rays with perturb = noise_std = 0 in which a sample is evaluated only when its point
+ * o + d z (rounded as the render kernel rounds it) lies in the closed box of an occupied cell of the occupancy grid
+ * (bits, N, ranges_host: as nerfb200_cull_count).  A skipped sample has sigma = 0.  A ray with a non-finite value or
+ * far <= near, and a pass whose interval lengths delta |d| are not all finite, is evaluated at every sample.
+ * Compositing, the inverse-CDF resampling (u = linspace(0, 1, N_importance)) and the merge are the render kernel's.
+ *   rays: (n_rays, 8) fp32, 16-byte aligned.  live_flag: nullable (n_rays) uint8; a ray whose flag is 0 has every
+ *   sample skipped.  Results: as nerfb200_render_args (rgb / depth_coarse only with test_time = 0, the fine ones
+ *   with n_importance > 0); z_fine (n, S_f), weights_coarse (n, S_c), weights_fine (n, S_f) optional.
+ *   samples_coarse (n, S_c, 4) / samples_fine (n, S_f, 4), optional, 16-byte aligned: rgb and sigma of every sample,
+ *   0 where skipped (rgb 0 in the coarse pass with test_time).  mask_coarse / mask_fine, optional (n, 6) uint32:
+ *   bit b of word w set iff sample 32 w + b is evaluated.  live_samples_host[2] receives the evaluated coarse and
+ *   fine sample counts.
+ * n_samples in {32, 64, 128}, n_importance a multiple of 32, their sum <= 192, 0 <= n_rays <= 2^22.  Synchronises
+ * the stream twice (each sample count sizes the launches after it); no MLP launch for a pass without an evaluated
+ * sample. */
+typedef struct nerfb200_samples_args {
+  const float* rays;
+  int64_t n_rays;
+  const uint8_t* live_flag;
+  const void* packed_coarse;
+  const void* packed_fine;
+  int32_t n_samples;
+  int32_t n_importance;
+  int32_t use_disp;
+  int32_t white_back;
+  int32_t test_time;
+  const uint32_t* bits;
+  int64_t N;
+  double ranges[6];
+  float* rgb_coarse;
+  float* depth_coarse;
+  float* opacity_coarse;
+  float* rgb_fine;
+  float* depth_fine;
+  float* opacity_fine;
+  float* z_fine;
+  float* weights_coarse;
+  float* weights_fine;
+  float* samples_coarse;
+  float* samples_fine;
+  uint32_t* mask_coarse;
+  uint32_t* mask_fine;
+} nerfb200_samples_args;
+
+/* Workspace bytes of nerfb200_render_samples for n_rays rays (0 for an unsupported shape). */
+size_t nerfb200_samples_workspace_bytes(int64_t n_rays, int32_t n_samples, int32_t n_importance);
+
+int nerfb200_render_samples(const nerfb200_samples_args* args, void* ws, size_t bytes, int64_t* live_samples_host,
+                            void* stream);
+
+/* ==== the training step with empty samples skipped ===============================================
+ * Definition and guarantees: DESIGN.md "Training with empty samples skipped". */
+
+/* One training step's render + loss over n_rays rays in which a sample is evaluated only when its point lies in an
+ * occupied cell of the occupancy grid (bits, N, ranges: as nerfb200_render_samples).  The coarse depths are the
+ * render kernel's stratified depths with the perturb jitter; perturb_rand / u_rand (or rng_in_kernel and rng_seed,
+ * with the meaning they have in nerfb200_render_args) and noise_coarse / noise_fine are the render kernel's random
+ * inputs.  An evaluated sample gets the network's sigma + noise * noise_std, a skipped one sigma = 0 (no noise), so
+ * its weight is 0 and it gets no gradient.  A ray with a non-finite value or far <= near, and a pass whose interval
+ * lengths delta |d| are not all finite, is evaluated at every sample.  Compositing, white_back, the inverse-CDF
+ * resampling with the render kernel's sorted random u (linspace with perturb = 0) and the merge run on those weights.
+ *   rays (n_rays, 8) fp32 and target (n_rays, 3), 16-byte aligned.  Results: the six outputs of nerfb200_render_args
+ * (the fine ones with n_importance > 0), loss_out[4] as its fused loss epilogue (mse_coarse, mse_fine, their sum,
+ * psnr of the finest pass), reduced in an order that does not depend on the launch.  Optional (null = not written):
+ * z_coarse (n, S_c), z_fine (n, S_f), weights_coarse / weights_fine, samples_coarse / samples_fine (n, S, 4: raw
+ * network rgb and sigma, 0 where skipped; 16-byte aligned), mask_coarse / mask_fine (n, 6) uint32 (bit b of word w:
+ * sample 32 w + b evaluated).  The backward fills, when given: dsigma_coarse / dsigma_fine (rows) and dprergb_coarse /
+ * dprergb_fine (rows, 3), the per-row d loss / d sigma and d loss / d (rgb before the sigmoid) of the evaluated
+ * samples, rows in ray-major, depth-index order (live_samples_host rows per pass). */
+typedef struct nerfb200_train_samples_args {
+  const float* rays;
+  int64_t n_rays;
+  const void* packed_coarse;
+  const void* packed_fine;
+  int32_t n_samples;
+  int32_t n_importance;
+  int32_t use_disp;
+  int32_t white_back;
+  float perturb;
+  float noise_std;
+  const float* perturb_rand;
+  const float* noise_coarse;
+  const float* u_rand;
+  const float* noise_fine;
+  uint64_t rng_seed;
+  int32_t rng_in_kernel;
+  const uint32_t* bits;
+  int64_t N;
+  double ranges[6];
+  const float* target;
+  float* rgb_coarse;
+  float* depth_coarse;
+  float* opacity_coarse;
+  float* rgb_fine;
+  float* depth_fine;
+  float* opacity_fine;
+  float* loss_out;
+  float* z_coarse;
+  float* z_fine;
+  float* weights_coarse;
+  float* weights_fine;
+  float* samples_coarse;
+  float* samples_fine;
+  uint32_t* mask_coarse;
+  uint32_t* mask_fine;
+  float* dsigma_coarse;
+  float* dsigma_fine;
+  float* dprergb_coarse;
+  float* dprergb_fine;
+} nerfb200_train_samples_args;
+
+/* Workspace bytes for n_rays rays: sized for every sample evaluated, so one workspace serves every step of a batch
+ * shape (0 for an unsupported shape).  Zero it once before its first use; it is never re-zeroed. */
+size_t nerfb200_train_samples_workspace_bytes(int64_t n_rays, int32_t n_samples, int32_t n_importance);
+
+/* The forward.  n_samples in {32, 64, 128}, n_importance a multiple of 32, their sum <= 192, 1 <= n_rays <= 2^22.
+ * ws: 1024-byte aligned, held until the backward.  live_samples_host[2] receives the evaluated coarse and fine
+ * sample counts.  Synchronises the stream once, to read them back when the last pass's count is known; no launch is
+ * sized from them. */
+int nerfb200_train_samples_forward(const nerfb200_train_samples_args* args, void* ws, size_t bytes,
+                                   int64_t* live_samples_host, void* stream);
+
+/* The same forward without the read-back: live_samples_dev[2] (device) receives the counts.  No launch is sized from
+ * a count on the host, and nothing is synchronised or read from host memory, so a CUDA graph can capture it. */
+int nerfb200_train_samples_forward_dev(const nerfb200_train_samples_args* args, void* ws, size_t bytes,
+                                       int64_t* live_samples_dev, void* stream);
+
+/* The backward of the forward that used `args`, `ws` and returned live_samples_host: the gradients of the 24
+ * parameters of each network (the tables of nerfb200_backward_args) for the seed loss_grad (a device scalar dL/dloss
+ * of loss_out[2], or null for 1).  A network with no evaluated sample launches nothing and its gradients are not
+ * written (they are 0).  Non-finite per-sample gradients are reported as device status 103. */
+int nerfb200_train_samples_backward(const nerfb200_train_samples_args* args, void* ws, size_t bytes,
+                                    const int64_t* live_samples_host, const float* loss_grad,
+                                    const float* const params_coarse[24], const float* const params_fine[24],
+                                    float* const grads_coarse[24], float* const grads_fine[24], void* stream);
+
+/* The backward of either forward with the counts the workspace holds (no host counts): capturable as the forward_dev
+ * entry.  Every network's gradients are written, exact zeros for one with no evaluated sample, so both tables must be
+ * complete.  The optional per-row outputs receive the first live_samples rows of each pass. */
+int nerfb200_train_samples_backward_dev(const nerfb200_train_samples_args* args, void* ws, size_t bytes,
+                                        const float* loss_grad, const float* const params_coarse[24],
+                                        const float* const params_fine[24], float* const grads_coarse[24],
+                                        float* const grads_fine[24], void* stream);
+
+/* ==== the density grid: an occupancy grid kept current during training ============================
+ * Definition and guarantees: DESIGN.md "Keeping the grid current during training".
+ *
+ * The grid has the occupancy grid's conventions (nerfb200_occupancy_pack): N points per axis over ranges_host
+ * {xmin, xmax, ymin, ymax, zmin, zmax} (each finite with min != max; a reversed range is allowed), M = N - 1 cells
+ * per axis, cell c = (cz * M + cy) * M + cx, bit c % 32 of word c / 32, the bits past the last cell 0.  Its state is
+ * density (M^3 float32, in cell order), bits (ceil(M^3 / 32) uint32 words) and key (one int64 in device memory).
+ * An update from the packed network f with key s:
+ *   1. u_a = the render kernel's in-kernel uniform (rng_in_kernel) of key s, ray c, element a, stream 2; a = 0, 1, 2;
+ *   2. p_a = float32(lo_a + (double(cell_a) + double(u_a)) * ((hi_a - lo_a) / M)), every double operation rounded
+ *      on its own;
+ *   3. sigma_c = nerfb200_query_sigma(f, p);
+ *   4. density_c = fmaxf(float32(decay * density_c), sigma_c > 0 ? sigma_c : 0) (a NaN sigma counts as 0);
+ *   5. cell c is occupied iff double(density_c) > sigma_threshold; the set is dilated by `dilate` cells (Chebyshev)
+ *      and packed into bits;
+ *   6. key = key + 1, so that update k of a grid seeded with s uses s + k. */
+
+/* Workspace bytes of an update of an N-point grid, `chunk` cells at a time (0 for N outside [2, 1625] or
+ * chunk < 1).  A chunk larger than the grid is taken as the grid. */
+size_t nerfb200_density_workspace_bytes(int64_t N, int64_t chunk);
+
+/* Steps 1-2 for cells [start, start + count) with the key *key_dev: xyz (count, 3) fp32. */
+int nerfb200_density_points(int64_t N, const double ranges_host[6], const int64_t* key_dev, int64_t start,
+                            int64_t count, float* xyz, void* stream);
+
+/* One whole update (steps 1-6) from the packed image of nerfb200_pack_weights, `chunk` cells at a time.
+ * sigma_threshold must not be NaN, decay must be in [0, 1], dilate >= 0; ws: nerfb200_density_workspace_bytes(N,
+ * chunk) bytes.  Every launch has a size fixed by (N, chunk): nothing is synchronised, allocated or read back, so a
+ * CUDA graph can capture the call; a replay reads the key where the previous one left it. */
+int nerfb200_density_update(const void* packed, int64_t N, const double ranges_host[6], double sigma_threshold,
+                            float decay, int32_t dilate, int64_t chunk, int64_t* key_dev, float* density,
+                            uint32_t* bits, void* ws, size_t bytes, void* stream);
+
+/* ==== mesh and Unity-volume grids through an occupancy grid =======================================
+ * Definition and guarantees: DESIGN.md "Grids through an occupancy grid".
+ *
+ * The mesh grid is nerfb200_sigma_grid's: N points per axis over ranges_host, flat point p = (i * N + j) * N + k at
+ * the fp32 position (x_j, y_i, z_k) of nerfb200_grid_positions.  The occupancy grid is nerfb200_cull_count's: bits
+ * (one bit per cell, cell (cz * M + cy) * M + cx, M = occ_N - 1) over occ_ranges_host (each finite with
+ * min != max; a reversed range is allowed).  The two grids' N and ranges are independent.  A lattice point is
+ * *evaluated* iff its position lies in the closed box of an occupied cell (the rule of nerfb200_render_samples: a
+ * point on a shared face, edge or corner checks every cell that touches it; outside the box or NaN it is empty).
+ *
+ * Per chunk of `chunk` lattice points: classify, scan, compact the evaluated positions, query them with
+ * nerfb200_query_sigma / nerfb200_query_rgb_sigma, scatter.  Each chunk reads its evaluated count back once, so the
+ * calls synchronise.  *evaluated_host receives the number of evaluated points. */
+
+/* Workspace bytes of either entry at `chunk` points per chunk (0 for chunk < 1). */
+size_t nerfb200_masked_grid_workspace_bytes(int64_t chunk);
+
+/* sigma_out (N^3) fp32: an evaluated point gets nerfb200_sigma_grid's value bit for bit, max(sigma, 0); every
+ * other point gets +0.0.  N >= 2, occ_N in [2, 1625], chunk >= 1; ws: nerfb200_masked_grid_workspace_bytes(chunk). */
+int nerfb200_sigma_grid_masked(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
+                               int64_t occ_N, const double occ_ranges_host[6], int64_t chunk, void* ws, size_t bytes,
+                               float* sigma_out, int64_t* evaluated_host, void* stream);
+
+/* rgbsigma_out (N^3, 4) fp32, 16-byte aligned: an evaluated point gets nerfb200_rgb_sigma_grid's four channels bit
+ * for bit; every other point gets (0, 0, 0, 0).  N in [2, 1625]; otherwise as nerfb200_sigma_grid_masked. */
+int nerfb200_rgb_sigma_grid_masked(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
+                                   int64_t occ_N, const double occ_ranges_host[6], int64_t chunk, void* ws,
+                                   size_t bytes, float* rgbsigma_out, int64_t* evaluated_host, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

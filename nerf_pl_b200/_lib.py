@@ -24,8 +24,7 @@ SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
            "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h", "sample_skip_kernels.cuh",
            "train_skip_kernels.cuh", "density_kernels.cuh", "masked_grid_kernels.cuh"]
-INCLUDES = ["nerf_pl_b200.h", "nerf_pl_b200_metrics.h", "nerf_pl_b200_views.h", "nerf_pl_b200_samples.h",
-            "nerf_pl_b200_train_samples.h", "nerf_pl_b200_density.h", "nerf_pl_b200_masked_grid.h"]
+INCLUDES = ["nerf_pl_b200.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -97,7 +96,7 @@ class BackwardArgs(ctypes.Structure):
 
 
 class SamplesArgs(ctypes.Structure):
-    """Mirror of ``nerfb200_samples_args`` (include/nerf_pl_b200_samples.h)."""
+    """Mirror of ``nerfb200_samples_args`` (include/nerf_pl_b200.h)."""
 
     _fields_ = [
         ("rays", c_void_p),
@@ -130,7 +129,7 @@ class SamplesArgs(ctypes.Structure):
 
 
 class TrainSamplesArgs(ctypes.Structure):
-    """Mirror of ``nerfb200_train_samples_args`` (include/nerf_pl_b200_train_samples.h)."""
+    """Mirror of ``nerfb200_train_samples_args`` (include/nerf_pl_b200.h)."""
 
     _fields_ = [
         ("rays", c_void_p),
@@ -177,6 +176,7 @@ class TrainSamplesArgs(ctypes.Structure):
 
 _vp, _i32, _i64, _f32, _f64, _sz = c_void_p, c_int32, c_int64, c_float, c_double, c_size_t
 _P, _RA, _BA = POINTER(c_void_p), POINTER(RenderArgs), POINTER(BackwardArgs)
+_SA, _TA = POINTER(SamplesArgs), POINTER(TrainSamplesArgs)
 
 # Every entry include/nerf_pl_b200.h declares, in header order: name -> (restype, argtypes); tests check it against
 # the header's prototypes.  Pointers and arrays are c_void_p or POINTER(...).  The entries that take a stream take it
@@ -240,54 +240,35 @@ SIGNATURES = {
     "nerfb200_launch_count": (_i64, []),
     "nerfb200_check_status": (_i32, []),
     "nerfb200_sm_count": (_i32, []),
-}
-EXPORTS = tuple(SIGNATURES)     # tests check the library exports all of them
-
-# The entries of the companion header include/nerf_pl_b200_metrics.h, in header order (its own tests check it).
-METRICS_SIGNATURES = {
+    # image metrics
     "nerfb200_ssim_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64]),
     "nerfb200_ssim": (_i32, [_vp, POINTER(_i64), _vp, POINTER(_i64), _i64, _i64, _i64, _i64, _i32, _vp, _sz, _vp, _vp]),
     "nerfb200_visualize_depth_workspace_bytes": (_sz, [_i64, _i64]),
     "nerfb200_visualize_depth": (_i32, [_vp, _i64, _i64, _i64, _i64, _vp, _sz, _vp, _vp]),
-}
-
-# The entries of the companion header include/nerf_pl_b200_views.h, in header order (its own tests check it).
-VIEWS_SIGNATURES = {
+    # training batches from the views
     "nerfb200_view_batch": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _f32, _f32, _f32, _i32, _vp, _i64, _vp, _vp,
                                    _vp]),
-}
-
-# The entries of the companion header include/nerf_pl_b200_samples.h, in header order (its own tests check it).
-SAMPLES_SIGNATURES = {
+    # rendering with empty samples skipped
     "nerfb200_samples_workspace_bytes": (_sz, [_i64, _i32, _i32]),
-    "nerfb200_render_samples": (_i32, [POINTER(SamplesArgs), _vp, _sz, POINTER(_i64), _vp]),
-}
-
-# The entries of the companion header include/nerf_pl_b200_train_samples.h, in header order (its own tests check it).
-TRAIN_SAMPLES_SIGNATURES = {
+    "nerfb200_render_samples": (_i32, [_SA, _vp, _sz, POINTER(_i64), _vp]),
+    # the training step with empty samples skipped
     "nerfb200_train_samples_workspace_bytes": (_sz, [_i64, _i32, _i32]),
-    "nerfb200_train_samples_forward": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp]),
-    "nerfb200_train_samples_forward_dev": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp]),
-    "nerfb200_train_samples_backward": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, POINTER(_i64), _vp, _P, _P, _P, _P,
-                                                _vp]),
-    "nerfb200_train_samples_backward_dev": (_i32, [POINTER(TrainSamplesArgs), _vp, _sz, _vp, _P, _P, _P, _P, _vp]),
-}
-
-# The entries of the companion header include/nerf_pl_b200_density.h, in header order (its own tests check it).
-DENSITY_SIGNATURES = {
+    "nerfb200_train_samples_forward": (_i32, [_TA, _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_train_samples_forward_dev": (_i32, [_TA, _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_train_samples_backward": (_i32, [_TA, _vp, _sz, POINTER(_i64), _vp, _P, _P, _P, _P, _vp]),
+    "nerfb200_train_samples_backward_dev": (_i32, [_TA, _vp, _sz, _vp, _P, _P, _P, _P, _vp]),
+    # the density grid
     "nerfb200_density_workspace_bytes": (_sz, [_i64, _i64]),
     "nerfb200_density_points": (_i32, [_i64, POINTER(_f64), _vp, _i64, _i64, _vp, _vp]),
     "nerfb200_density_update": (_i32, [_vp, _i64, POINTER(_f64), _f64, _f32, _i32, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
-}
-
-# The entries of the companion header include/nerf_pl_b200_masked_grid.h, in header order (its own tests check it).
-MASKED_GRID_SIGNATURES = {
+    # grids through an occupancy grid
     "nerfb200_masked_grid_workspace_bytes": (_sz, [_i64]),
     "nerfb200_sigma_grid_masked": (_i32, [_vp, _i64, POINTER(_f64), _vp, _i64, POINTER(_f64), _i64, _vp, _sz, _vp,
                                           POINTER(_i64), _vp]),
     "nerfb200_rgb_sigma_grid_masked": (_i32, [_vp, _i64, POINTER(_f64), _vp, _i64, POINTER(_f64), _i64, _vp, _sz, _vp,
                                               POINTER(_i64), _vp]),
 }
+EXPORTS = tuple(SIGNATURES)     # tests check the library exports all of them
 
 
 def _nvcc() -> str:
@@ -335,10 +316,7 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (restype, argtypes) in (*SIGNATURES.items(), *METRICS_SIGNATURES.items(),
-                                              *VIEWS_SIGNATURES.items(), *SAMPLES_SIGNATURES.items(),
-                                              *TRAIN_SAMPLES_SIGNATURES.items(), *DENSITY_SIGNATURES.items(),
-                                              *MASKED_GRID_SIGNATURES.items()):
+            for name, (restype, argtypes) in SIGNATURES.items():
                 fn = getattr(lib, name)
                 fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:

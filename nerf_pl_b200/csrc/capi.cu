@@ -11,12 +11,6 @@
 #include <vector>
 
 #include "../../include/nerf_pl_b200.h"
-#include "../../include/nerf_pl_b200_metrics.h"
-#include "../../include/nerf_pl_b200_views.h"
-#include "../../include/nerf_pl_b200_samples.h"
-#include "../../include/nerf_pl_b200_train_samples.h"
-#include "../../include/nerf_pl_b200_density.h"
-#include "../../include/nerf_pl_b200_masked_grid.h"
 #include "aux_kernels.cuh"
 #include "bwd_kernels.cuh"
 #include "mesh_kernels.cuh"
@@ -942,16 +936,22 @@ size_t density_carve(long long C, long long chunk, void* base, float** xyz, floa
   return c.off;
 }
 
-// N in [2, 1625] and every range finite with min != max.
-int density_box(int64_t N, const double* ranges, DensityBox* b, const char* who) {
+// The lattice of the density grid and of the per-sample skipping entries' occupancy grid: N in [2, 1625] points per
+// axis and every range finite with min != max.
+int grid_box_ok(int64_t N, const double* ranges, const char* who) {
   if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
   if (!ranges) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  for (int a = 0; a < 3; ++a) {
-    const double lo = ranges[2 * a], hi = ranges[2 * a + 1];
-    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
+  for (int a = 0; a < 6; a += 2)
+    if (!std::isfinite(ranges[a]) || !std::isfinite(ranges[a + 1]) || ranges[a] == ranges[a + 1])
       return fail(NERFB200_EINVAL, "%s: every range must be finite with min != max", who);
-    b->lo[a] = lo;
-    b->hi[a] = hi;
+  return 0;
+}
+
+int density_box(int64_t N, const double* ranges, DensityBox* b, const char* who) {
+  TRY(grid_box_ok(N, ranges, who));
+  for (int a = 0; a < 3; ++a) {
+    b->lo[a] = ranges[2 * a];
+    b->hi[a] = ranges[2 * a + 1];
   }
   b->M = N - 1;
   return 0;
@@ -1005,15 +1005,12 @@ int samples_scan(const SkipParams& sp, cudaStream_t s, long long* total) {
   return 0;
 }
 
-// The grid of both per-sample skipping entries: N in [2, kVolMaxN], every range finite with min != max.
+// The occupancy grid of the per-sample skipping entries and the masked grids.
 int skip_grid(const uint32_t* bits, int64_t N, const double* ranges, SkipGrid* g, const char* who) {
-  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
+  TRY(grid_box_ok(N, ranges, who));
   for (int ax = 0; ax < 3; ++ax) {
-    const double lo = ranges[2 * ax], hi = ranges[2 * ax + 1];
-    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
-      return fail(NERFB200_EINVAL, "%s: every range must be finite with min != max", who);
-    g->lo[ax] = lo;
-    g->scale[ax] = static_cast<double>(N - 1) / (hi - lo);
+    g->lo[ax] = ranges[2 * ax];
+    g->scale[ax] = static_cast<double>(N - 1) / (ranges[2 * ax + 1] - ranges[2 * ax]);
   }
   g->bits = bits;
   g->M = N - 1;
@@ -1088,15 +1085,16 @@ int masked_grid(const void* packed, int64_t N, const double* ranges, const uint3
 }
 
 // ------------------------------------------------------------------ training with empty samples skipped
-// (kernels: train_skip_kernels.cuh).  One workspace per batch shape, sized for every sample evaluated: the per-ray
-// buffers, the compacted rows of the larger pass, then per network a NeRF.forward training workspace carved for that
-// worst case and the device plan of its backward.  Nothing is reallocated or re-zeroed between steps, and no launch
-// is sized on the host from a step's sample count: each pass's count stays on the device (the total of its scan),
-// the compacted-row MLP reads it, and train_skip_plan_kernel turns it into the backward's layout, wgrad tables, head /
-// chain parameters and reduction table.  Every launch has the grid of the carved worst case, so the step can be
-// captured in a CUDA graph.
+// (kernels: sample_skip_kernels.cuh, train_skip_kernels.cuh).  One workspace per batch shape, sized for every sample
+// evaluated: the per-ray buffers, the compacted rows of the larger pass, then per network a NeRF.forward training
+// workspace carved for that worst case and the device plan of its backward.  Nothing is reallocated or re-zeroed
+// between steps, and no launch is sized on the host from a step's sample count: each pass's count stays on the device
+// (the total of its scan), the compacted-row MLP reads it, and train_skip_plan_kernel turns it into the backward's
+// layout, wgrad tables, head / chain parameters and reduction table.  Every launch has the grid of the carved worst
+// case, so the step can be captured in a CUDA graph.
 struct TrainSkipWs {
-  TrainSkipParams t;
+  SkipParams p;                 // p.ofs: the offsets of the pass a launch works on (ofs[pass] below)
+  long long* ofs[2];            // (n + 1) exclusive scans of the evaluated samples of each pass
   uint8_t* net_ws[2];
   TrainSkipPlan* plan[2];
   long long* live;              // [2] the eager forward's counts, read back once
@@ -1106,16 +1104,16 @@ struct TrainSkipWs {
 size_t train_skip_carve(long long n, int Sc, int K, void* base, int sm_count, TrainSkipWs* w) {
   const long long Sf = Sc + K, rows = n * Sf;
   Carver c{static_cast<uint8_t*>(base), 0, 1024};
-  SkipParams& p = w->t.s;
+  SkipParams& p = w->p;
   p.mask[0] = c.take<uint32_t>(n * kSkipMaskWords);
   p.mask[1] = c.take<uint32_t>(n * kSkipMaskWords);
   p.cnt = c.take<int>(n + 1);
-  w->t.ofs[0] = c.take<long long>(n + 1);
-  w->t.ofs[1] = c.take<long long>(n + 1);
-  w->t.zc = c.take<float>(n * Sc);
+  w->ofs[0] = c.take<long long>(n + 1);
+  w->ofs[1] = c.take<long long>(n + 1);
+  p.zc = c.take<float>(n * Sc);
   p.zf = c.take<float>(n * Sf);
   p.dirbias = c.take<float>(n * kSkipDirStride);
-  w->t.dirrow = c.take<__half>(n * 64);
+  p.dirrow = c.take<__half>(n * 64);
   p.row_ray = c.take<int>(rows);
   p.row_z = c.take<float>(rows);
   p.mlp_out = c.take<float>(rows * 4);
@@ -1193,8 +1191,7 @@ int train_skip_setup(const nerfb200_train_samples_args* a, void* ws, size_t byte
     return fail(NERFB200_EUNSUPPORTED, "%s: needs N_samples in {32, 64, 128}, N_importance a multiple of 32, "
                 "N_samples + N_importance <= 192 and 1 <= n_rays <= 2^22", who);
   std::memset(w, 0, sizeof(*w));
-  TrainSkipParams& t = w->t;
-  SkipParams& p = t.s;
+  SkipParams& p = w->p;
   TRY(skip_grid(a->bits, a->N, a->ranges, &p.grid, who));
   const bool fine = a->n_importance > 0;
   if (!a->rays || !a->packed_coarse || !a->bits || !a->target || !a->loss_out || !a->rgb_coarse || !a->depth_coarse ||
@@ -1224,33 +1221,33 @@ int train_skip_setup(const nerfb200_train_samples_args* a, void* ws, size_t byte
   p.rgb_fine = a->rgb_fine; p.depth_fine = a->depth_fine; p.opacity_fine = a->opacity_fine;
   p.z_fine = a->z_fine; p.weights_coarse = a->weights_coarse; p.weights_fine = a->weights_fine;
   p.samples[0] = a->samples_coarse; p.samples[1] = a->samples_fine;
-  t.perturb = a->perturb; t.noise_std = a->noise_std;
-  t.perturb_rand = a->perturb_rand; t.u_rand = a->u_rand;
-  t.noise[0] = a->noise_coarse; t.noise[1] = a->noise_fine;
-  t.rng_seed = a->rng_seed; t.rng_in_kernel = a->rng_in_kernel;
-  t.z_coarse = a->z_coarse;
+  p.perturb = a->perturb; p.noise_std = a->noise_std;
+  p.perturb_rand = a->perturb_rand; p.u_rand = a->u_rand;
+  p.noise[0] = a->noise_coarse; p.noise[1] = a->noise_fine;
+  p.rng_seed = a->rng_seed; p.rng_in_kernel = a->rng_in_kernel;
+  p.z_coarse = a->z_coarse;
   return 0;
 }
 
 // The training MLP of one network over the pass's compacted rows (mlp_forward_kernel<true, true>), at the grid of
 // the carved worst case; the kernel reads the row count from the pass's scan.
 int train_skip_mlp(const TrainSkipWs& w, int pass, const DeviceInfo* d, cudaStream_t s) {
-  const TrainSkipParams& t = w.t;
+  const SkipParams& p = w.p;
   TrainLayout L;
   make_train_layout(&L, w.net_ws[pass], true, w.cap[pass], 1, 0, d->sm_count);
   MlpParams m{};
   m.n = w.cap[pass];
-  m.n_dev = t.ofs[pass] + t.s.n;
-  m.net = t.s.net[pass];
-  m.out = const_cast<float*>(t.s.mlp_out);
+  m.n_dev = w.ofs[pass] + p.n;
+  m.net = p.net[pass];
+  m.out = const_cast<float*>(p.mlp_out);
   m.status = d->status;
   m.tr = L.pass[0];
   m.xdir = L.xdir;
-  m.row_ray = t.s.row_ray;
-  m.row_z = t.s.row_z;
-  m.rays = t.s.rays;
-  m.dirbias = t.s.dirbias + pass * kDirW;
-  m.dirrow = t.dirrow;
+  m.row_ray = p.row_ray;
+  m.row_z = p.row_z;
+  m.rays = p.rays;
+  m.dirbias = p.dirbias + pass * kDirW;
+  m.dirrow = p.dirrow;
   const long long tiles = ceil_div(m.n, 128);
   return launch(pass ? "train_samples fine mlp launch" : "train_samples coarse mlp launch", mlp_forward_kernel<true, true>,
                 static_cast<int>(tiles < d->sm_count ? tiles : d->sm_count), kThreads, kSmemTotal, s, m);
@@ -1263,13 +1260,13 @@ int train_skip_mlp(const TrainSkipWs& w, int pass, const DeviceInfo* d, cudaStre
 // sizing the launches after it.
 int train_skip_forward(const nerfb200_train_samples_args* a, const TrainSkipWs& w, long long* live_dev,
                        int64_t* live_host, const DeviceInfo* d, cudaStream_t s) {
-  TrainSkipParams t = w.t;
-  const bool fine = t.s.K > 0;
-  const long long n = t.s.n;
+  SkipParams p = w.p;
+  const bool fine = p.K > 0;
+  const long long n = p.n;
   const int ray_blocks = grid_blocks(ceil_div(n, kSkipWarps), 1);
   const char* what = "train_samples_forward launches";
   auto counts = [&]() -> int {
-    TRY(launch(what, train_skip_counts_kernel, 1, 32, 0, s, t.ofs[0] + n, fine ? t.ofs[1] + n : nullptr, live_dev));
+    TRY(launch(what, train_skip_counts_kernel, 1, 32, 0, s, w.ofs[0] + n, fine ? w.ofs[1] + n : nullptr, live_dev));
     if (!live_host) return 0;
     long long live[2];
     CUDA_TRY(cudaMemcpyAsync(live, live_dev, sizeof(live), cudaMemcpyDeviceToHost, s), "train_samples readback");
@@ -1279,29 +1276,29 @@ int train_skip_forward(const nerfb200_train_samples_args* a, const TrainSkipWs& 
     return 0;
   };
   // coarse pass
-  TRY(launch(what, train_skip_classify_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
-  TRY(launch(what, skip_dir_bias_kernel, grid_blocks(n, 1), kDirW, 0, s, t.s, 0, fine ? 2 : 1));
-  t.s.ofs = t.ofs[0];
-  TRY(launch(what, cull_scan_kernel, 1, 1024, 0, s, t.s.cnt, t.s.ofs, n));
+  TRY(launch(what, skip_classify_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
+  TRY(launch(what, skip_dir_bias_kernel, grid_blocks(n, 1), kDirW, 0, s, p, 0, fine ? 2 : 1));
+  p.ofs = w.ofs[0];
+  TRY(launch(what, cull_scan_kernel, 1, 1024, 0, s, p.cnt, p.ofs, n));
   if (!fine) TRY(counts());
-  TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 0));
+  TRY(launch(what, skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, 0));
   TRY(train_skip_mlp(w, 0, d, s));
-  TRY(launch(what, train_skip_coarse_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+  TRY(launch(what, skip_coarse_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
   if (fine) {
-    t.s.ofs = t.ofs[1];
-    TRY(launch(what, cull_scan_kernel, 1, 1024, 0, s, t.s.cnt, t.s.ofs, n));
+    p.ofs = w.ofs[1];
+    TRY(launch(what, cull_scan_kernel, 1, 1024, 0, s, p.cnt, p.ofs, n));
     TRY(counts());
-    TRY(launch(what, train_skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, t, 1));
+    TRY(launch(what, skip_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, 1));
     TRY(train_skip_mlp(w, 1, d, s));
-    TRY(launch(what, train_skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, t));
+    TRY(launch(what, skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
   }
   // losses.py / metrics.py on the results, one block in a fixed order
-  TRY(launch(what, mse_psnr_kernel, 1, 1024, 0, s, t.s.rgb_coarse, fine ? t.s.rgb_fine : nullptr, a->target, n * 3,
+  TRY(launch(what, mse_psnr_kernel, 1, 1024, 0, s, p.rgb_coarse, fine ? p.rgb_fine : nullptr, a->target, n * 3,
              a->loss_out));
   uint32_t* const mask_out[2] = {a->mask_coarse, a->mask_fine};
   for (int ps = 0; ps < (fine ? 2 : 1); ++ps)
     if (mask_out[ps])
-      CUDA_TRY(cudaMemcpyAsync(mask_out[ps], t.s.mask[ps], sizeof(uint32_t) * n * kSkipMaskWords,
+      CUDA_TRY(cudaMemcpyAsync(mask_out[ps], p.mask[ps], sizeof(uint32_t) * n * kSkipMaskWords,
                                cudaMemcpyDeviceToDevice, s), "train_samples mask copy");
   return 0;
 }
@@ -1312,9 +1309,9 @@ int train_skip_forward(const nerfb200_train_samples_args* a, const TrainSkipWs& 
 int train_skip_backward(const nerfb200_train_samples_args* a, const TrainSkipWs& w, const bool run[2],
                         const float* loss_grad, const float* const* const params[2], float* const* const grads[2],
                         const DeviceInfo* d, cudaStream_t s) {
-  const TrainSkipParams& t = w.t;
+  const SkipParams& p = w.p;
   const char* what = "train_samples_backward launches";
-  const int n_net = t.s.K > 0 ? 2 : 1;
+  const int n_net = p.K > 0 ? 2 : 1;
   TrainLayout L[2];
   TrainSkipPlanArgs pa;
   std::memset(&pa, 0, sizeof(pa));
@@ -1322,12 +1319,12 @@ int train_skip_backward(const nerfb200_train_samples_args* a, const TrainSkipWs&
     if (!run[ps]) continue;
     make_train_layout(&L[ps], w.net_ws[ps], true, w.cap[ps], 1, 0, d->sm_count);
     pa.L[ps] = L[ps];
-    pa.rows[ps] = t.ofs[ps] + t.s.n;
+    pa.rows[ps] = w.ofs[ps] + p.n;
     for (int i = 0; i < kNumParams; ++i) {
       pa.params[ps][i] = params[ps][i];
       pa.grads[ps][i] = grads[ps][i];
     }
-    pa.net[ps] = t.s.net[ps];
+    pa.net[ps] = p.net[ps];
     pa.out[ps] = w.plan[ps];
   }
   pa.sm_count = d->sm_count;
@@ -1338,19 +1335,19 @@ int train_skip_backward(const nerfb200_train_samples_args* a, const TrainSkipWs&
     const long long* rows = pa.rows[ps];
     const PassBufs& pb = L[ps].pass[0];
     TrainSkipBwdParams bp;
-    bp.n_rays = t.s.n; bp.S = ps ? t.s.Sc + t.s.K : t.s.Sc;
+    bp.n_rays = p.n; bp.S = ps ? p.Sc + p.K : p.Sc;
     bp.n_rows = rows;
-    bp.rays = t.s.rays; bp.z = ps ? t.s.zf : t.zc;
-    bp.mask = t.s.mask[ps]; bp.ofs = t.ofs[ps];
+    bp.rays = p.rays; bp.z = ps ? p.zf : p.zc;
+    bp.mask = p.mask[ps]; bp.ofs = w.ofs[ps];
     bp.sigma = pb.sigma; bp.rgb = pb.rgb;
-    bp.noise = t.noise_std > 0.f ? t.noise[ps] : nullptr;
-    bp.noise_std = t.noise_std; bp.white_back = t.s.white_back;
-    bp.rgb_out = ps ? t.s.rgb_fine : t.s.rgb_coarse;
+    bp.noise = p.noise_std > 0.f ? p.noise[ps] : nullptr;
+    bp.noise_std = p.noise_std; bp.white_back = p.white_back;
+    bp.rgb_out = ps ? p.rgb_fine : p.rgb_coarse;
     bp.target = a->target; bp.loss_grad = loss_grad;
     bp.dsigma = pb.dsigma; bp.dprergb = pb.dprergb;
     bp.amax_bits = L[ps].amax;
     bp.status = d->status;
-    TRY(launch(what, train_skip_bwd_kernel, grid_blocks(ceil_div(t.s.n, kSkipWarps), 1), kSkipWarps * 32, 0, s, bp));
+    TRY(launch(what, train_skip_bwd_kernel, grid_blocks(ceil_div(p.n, kSkipWarps), 1), kSkipWarps * 32, 0, s, bp));
     float* const ds_out = ps ? a->dsigma_fine : a->dsigma_coarse;
     float* const dp_out = ps ? a->dprergb_fine : a->dprergb_coarse;
     if (ds_out)
@@ -1360,7 +1357,7 @@ int train_skip_backward(const nerfb200_train_samples_args* a, const TrainSkipWs&
                  rows, 3));
     const float* const* const p2[2] = {params[ps], params[ps]};
     float* const* const g2[2] = {grads[ps], grads[ps]};
-    const uint8_t* const net[2] = {t.s.net[ps], t.s.net[ps]};
+    const uint8_t* const net[2] = {p.net[ps], p.net[ps]};
     TRY(backward_tail(L[ps], p2, g2, net, nullptr, 0, d, s, what, w.plan[ps]));
   }
   return 0;
@@ -2371,7 +2368,7 @@ int nerfb200_scatter_results(const float* const src_host[6], float* const dst_ho
   return launch("scatter_results launch", scatter_results_kernel, grid_blocks(n_rays, 256), 256, 0, stream, p);
 }
 
-// ---- per-sample skipping (include/nerf_pl_b200_samples.h; kernels: sample_skip_kernels.cuh)
+// ---- per-sample skipping (kernels: sample_skip_kernels.cuh)
 size_t nerfb200_samples_workspace_bytes(int64_t n_rays, int32_t n_samples, int32_t n_importance) {
   SkipParams p;
   return samples_shape_ok(n_rays, n_samples, n_importance) ? samples_carve(n_rays, n_samples, n_importance, nullptr, &p)
@@ -2446,7 +2443,7 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
   return 0;
 }
 
-// ---- training with empty samples skipped (include/nerf_pl_b200_train_samples.h; kernels: train_skip_kernels.cuh)
+// ---- training with empty samples skipped (kernels: sample_skip_kernels.cuh, train_skip_kernels.cuh)
 size_t nerfb200_train_samples_workspace_bytes(int64_t n_rays, int32_t n_samples, int32_t n_importance) {
   if (!samples_shape_ok(n_rays, n_samples, n_importance) || n_rays < 1) return 0;
   TrainSkipWs w;
@@ -2485,7 +2482,7 @@ int nerfb200_train_samples_backward(const nerfb200_train_samples_args* a, void* 
   if (!live_samples_host) return fail(NERFB200_EINVAL, "train_samples_backward: NULL argument");
   TrainSkipWs w;
   TRY(train_skip_setup(a, ws, bytes, nerfb200_sm_count(), &w, "train_samples_backward"));
-  const int n_net = w.t.s.K > 0 ? 2 : 1;
+  const int n_net = w.p.K > 0 ? 2 : 1;
   const float* const* const params[2] = {params_coarse, params_fine};
   float* const* const grads[2] = {grads_coarse, grads_fine};
   for (int ps = 0; ps < n_net; ++ps) {
@@ -2506,7 +2503,7 @@ int nerfb200_train_samples_backward_dev(const nerfb200_train_samples_args* a, vo
                                         float* const grads_fine[24], void* stream) {
   TrainSkipWs w;
   TRY(train_skip_setup(a, ws, bytes, nerfb200_sm_count(), &w, "train_samples_backward_dev"));
-  const int n_net = w.t.s.K > 0 ? 2 : 1;
+  const int n_net = w.p.K > 0 ? 2 : 1;
   const float* const* const params[2] = {params_coarse, params_fine};
   float* const* const grads[2] = {grads_coarse, grads_fine};
   for (int ps = 0; ps < n_net; ++ps) TRY(train_skip_tables_ok(params[ps], grads[ps]));
@@ -2516,7 +2513,7 @@ int nerfb200_train_samples_backward_dev(const nerfb200_train_samples_args* a, vo
   return train_skip_backward(a, w, run, loss_grad, params, grads, d, static_cast<cudaStream_t>(stream));
 }
 
-// ---- image metrics (include/nerf_pl_b200_metrics.h; kernels: metrics_kernels.cuh)
+// ---- image metrics (kernels: metrics_kernels.cuh)
 size_t nerfb200_ssim_workspace_bytes(int64_t b, int64_t c, int64_t h, int64_t w) {
   const int64_t ext[4] = {b, c, h, w};
   const long long n = image_elems(ext, 4);

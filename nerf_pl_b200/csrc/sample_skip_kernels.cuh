@@ -1,9 +1,14 @@
-// Per-sample empty-space skipping at render time (DESIGN.md "Skipping empty samples").  The live rays of a cull
-// (occupancy_kernels.cuh) are rendered sample by sample: a sample whose point lies in no occupied cell gets
-// sigma = 0 and is not evaluated, the others go through the MLP as compacted rows (mlp_forward_kernel's
-// compacted-sample mode).  Everything else reuses the render kernel's device functions (z_base, composite_ray,
+// Per-sample empty-space skipping (DESIGN.md "Skipping empty samples"), at render time and in training.  The rays of
+// a pass are rendered sample by sample: a sample whose point lies in no occupied cell gets sigma = 0 and is not
+// evaluated, the others go through the MLP as compacted rows (mlp_forward_kernel's compacted-sample mode, or its
+// training mode).  Everything else reuses the render kernel's device functions (z_base, composite_ray,
 // pdf_to_cdf_ray, inverse_cdf, merge_rank, dir_embed_term, dir_bias), so an evaluated sample has the fused kernel's
 // sigma / rgb bit for bit and a ray with nothing to skip renders as render_rays renders it.
+//
+// One set of per-ray kernels serves both callers; the render path is the training path with perturb = 0,
+// noise_std = 0 and no depth or direction-row store.  Training (train_skip_kernels.cuh) jitters the coarse depths
+// and keeps them in the workspace (zc), adds noise to the evaluated sigma, resamples with the render kernel's sorted
+// random u and writes the fp16 direction rows its MLP saves for the backward; rendering has test_time and live_flag.
 //
 // Per chunk of rays:  classify (coarse) -> scan -> [emit -> direction bias -> coarse MLP] -> coarse stage
 // (composite, resample, merge, classify fine) -> scan -> [emit -> fine MLP] -> fine stage (composite).
@@ -27,23 +32,57 @@ struct SkipParams {
   int n;
   const uint8_t* live_flag;     // nullable: a ray whose flag is 0 has every sample skipped
   int Sc, K, use_disp, white_back, test_time;
+  // training's randomness: perturb = noise_std = 0 is the render path
+  float perturb, noise_std;
+  const float* perturb_rand;    // (n, Sc), null with perturb = 0 or in-kernel random numbers
+  const float* noise[2];        // (n, Sc) / (n, Sf), null with noise_std = 0
+  const float* u_rand;          // (n, K), as perturb_rand
+  unsigned long long rng_seed;  // as RenderParams
+  int rng_in_kernel;
   SkipGrid grid;
   const uint8_t* net[2];        // packed images (coarse, fine)
   // workspace
   uint32_t* mask[2];            // (n, kSkipMaskWords) evaluated samples of the coarse / fine pass
   int* cnt;                     // (n) evaluated samples of the current pass
   long long* ofs;               // (n + 1) exclusive scan of cnt; ofs[n] the total
+  float* zc;                    // nullable (n, Sc) coarse depths, stored by the classification; null: z_base's
   float* zf;                    // (n, Sf) merged fine depths
   float* dirbias;               // (n, kSkipDirStride)
+  __half* dirrow;               // nullable (n, 64) fp16 direction rows of the training MLP
   int* row_ray;                 // (rows) compacted samples: ray, depth
   float* row_z;
   const float* mlp_out;         // (rows, 4) rgb + sigma, or (rows) sigma
   // results, nullable as render_rays' (RenderParams)
   float* rgb_coarse; float* depth_coarse; float* opacity_coarse;
   float* rgb_fine; float* depth_fine; float* opacity_fine;
-  float* z_fine; float* weights_coarse; float* weights_fine;
+  float* z_coarse; float* z_fine; float* weights_coarse; float* weights_fine;
   float* samples[2];            // optional (n, S, 4): rgb + sigma of every sample of the pass, 0 where skipped
 };
+
+__device__ __forceinline__ unsigned long long skip_key(const SkipParams& p) {
+  return p.rng_in_kernel == 2 ? *reinterpret_cast<const unsigned long long*>(p.rng_seed) : p.rng_seed;
+}
+
+// Coarse depths of ray r, sample i: render_rays_kernel's setup_group expression (models/rendering.py:189-204), the
+// uniform from the tensor or from Philox stream 0 with the render kernel's counters; z_base with perturb = 0.
+__device__ __forceinline__ float skip_z(const SkipParams& p, int r, int i, float nr, float fr) {
+  const int Sc = p.Sc;
+  const bool ud = p.use_disp != 0;
+  float z = z_base(nr, fr, i, Sc, ud);
+  if (p.perturb > 0.f) {
+    const float zl = (i > 0) ? z_base(nr, fr, i - 1, Sc, ud) : z;
+    const float zu = (i < Sc - 1) ? z_base(nr, fr, i + 1, Sc, ud) : z;
+    const float lower = (i > 0) ? __fmul_rn(0.5f, __fadd_rn(zl, z)) : z;
+    const float upper = (i < Sc - 1) ? __fmul_rn(0.5f, __fadd_rn(z, zu)) : z;
+    const float pu = p.rng_in_kernel ? philox_uniform(skip_key(p), static_cast<uint32_t>(r), static_cast<uint32_t>(i), 0u)
+                                     : __ldg(p.perturb_rand + static_cast<long long>(r) * Sc + i);
+    const float pr = __fmul_rn(p.perturb, pu);
+    z = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), pr));
+  }
+  return z;
+}
+
+__device__ __forceinline__ bool mask_bit(const uint32_t* m, int i) { return (m[i >> 5] >> (i & 31)) & 1u; }
 
 // Whether the point x lies in the closed box of an occupied cell.  In grid coordinates, compared in double; a
 // coordinate on a cell boundary belongs to both cells, so a point on a shared face, edge or corner checks every
@@ -157,27 +196,70 @@ __device__ __forceinline__ void expand_ray(const SkipParams& p, int r, int lane,
   }
 }
 
-// Coarse classification: the coarse depths of render_rays (z_base, perturb = 0), count per ray.
+// sigma + noise of the evaluated samples of one pass (composite_ray's expression); skipped samples keep sigma = 0.
+__device__ __forceinline__ void add_noise(const SkipParams& p, int pass, long long r, int lane, int S, const uint32_t* m,
+                                          float* sigma) {
+  if (p.noise_std <= 0.f) return;
+  const float* nz = p.noise[pass] + r * S;
+  for (int i = lane; i < S; i += 32)
+    if (mask_bit(m, i)) sigma[i] = __fadd_rn(sigma[i], __fmul_rn(__ldg(nz + i), p.noise_std));
+}
+
+// The results of pass `pass` of ray r: the weights (composite_ray left them in wts), the opacity and, with want_rgb,
+// the colour (on the white background with white_back) and the depth.
+__device__ __forceinline__ void store_pass(const SkipParams& p, int pass, long long r, int lane, int S, const RayOut& o,
+                                           bool want_rgb, const float* wts) {
+  float* const weights = pass ? p.weights_fine : p.weights_coarse;
+  if (weights != nullptr)
+    for (int i = lane; i < S; i += 32) weights[r * S + i] = wts[i];
+  if (lane == 0) {
+    const float add = (p.white_back != 0) ? __fsub_rn(1.f, o.opac) : 0.f;
+    (pass ? p.opacity_fine : p.opacity_coarse)[r] = o.opac;
+    if (want_rgb) {
+      float* const rgb = pass ? p.rgb_fine : p.rgb_coarse;
+      rgb[3 * r + 0] = o.r + add;
+      rgb[3 * r + 1] = o.g + add;
+      rgb[3 * r + 2] = o.b + add;
+      (pass ? p.depth_fine : p.depth_coarse)[r] = o.depth;
+    }
+  }
+}
+
+// Coarse classification: the coarse depths (skip_z; stored to zc and z_coarse when given), the count per ray and,
+// with dirrow, the fp16 direction row the training MLP stores for the direction-slice wgrad (Embedding(3, 4)(d) as
+// the render kernel computes it, columns 27..63 zero).
 __global__ void __launch_bounds__(kSkipWarps * 32) skip_classify_kernel(SkipParams p) {
   __shared__ float zs[kSkipWarps][kMaxSc];
+  __shared__ float de[kSkipWarps][28];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // n <= 2^22 (nerfb200_render_samples): int ray indices keep the loop state small across z_base's division calls
+  // n <= 2^22 (samples_shape_ok): int ray indices keep the loop state small across z_base's division calls
   for (int r = blockIdx.x * kSkipWarps + warp; r < p.n; r += gridDim.x * kSkipWarps) {
     // the depths first: the ray's other values are not live across those calls
     const float near = __ldg(p.rays + 8 * r + 6), far = __ldg(p.rays + 8 * r + 7);
-    for (int i = lane; i < p.Sc; i += 32) zs[warp][i] = z_base(near, far, i, p.Sc, p.use_disp != 0);
+    for (int i = lane; i < p.Sc; i += 32) {
+      const float z = skip_z(p, r, i, near, far);
+      zs[warp][i] = z;
+      if (p.zc != nullptr) p.zc[static_cast<long long>(r) * p.Sc + i] = z;
+      if (p.z_coarse != nullptr) p.z_coarse[static_cast<long long>(r) * p.Sc + i] = z;
+    }
+    if (p.dirrow != nullptr && lane < 15) dir_embed_term(lane, p.rays + 8 * r + 3, de[warp]);
     __syncwarp();
     const int c = classify_ray(p, load_skip_ray(p, r), r, lane, p.Sc, zs[warp], p.mask[0] + r * kSkipMaskWords);
     if (lane == 0) p.cnt[r] = c;
+    if (p.dirrow != nullptr) {
+      const float lo = (2 * lane < 27) ? de[warp][2 * lane] : 0.f, hi = (2 * lane + 1 < 27) ? de[warp][2 * lane + 1] : 0.f;
+      reinterpret_cast<__half2*>(p.dirrow + static_cast<long long>(r) * 64)[lane] = __floats2half2_rn(lo, hi);
+    }
     __syncwarp();
   }
 }
 
 // The rows of pass `pass`: evaluated sample i of ray r goes to row ofs[r] + (evaluated samples of r before i), so
-// the rows are ray-major and in depth-index order.
+// the rows are ray-major and in depth-index order.  The depths are zf's, or zc's (z_base's without zc) for pass 0.
 __global__ void __launch_bounds__(kSkipWarps * 32) skip_emit_kernel(SkipParams p, int pass) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = pass ? p.Sc + p.K : p.Sc;
+  const float* zb = pass ? p.zf : p.zc;
   for (long long r = static_cast<long long>(blockIdx.x) * kSkipWarps + warp; r < p.n;
        r += static_cast<long long>(gridDim.x) * kSkipWarps) {
     const uint32_t* m = p.mask[pass] + r * kSkipMaskWords;
@@ -189,7 +271,7 @@ __global__ void __launch_bounds__(kSkipWarps * 32) skip_emit_kernel(SkipParams p
       if ((b >> lane) & 1u) {
         const long long row = pos + __popc(b & ((1u << lane) - 1u));
         p.row_ray[row] = static_cast<int>(r);
-        p.row_z[row] = pass ? p.zf[r * S + i] : z_base(near, far, i, S, p.use_disp != 0);
+        p.row_z[row] = zb != nullptr ? zb[r * S + i] : z_base(near, far, i, S, p.use_disp != 0);
       }
       pos += __popc(b);
     }
@@ -211,9 +293,10 @@ __global__ void __launch_bounds__(kDirW) skip_dir_bias_kernel(SkipParams p, int 
   }
 }
 
-// Coarse stage of one ray per warp: expand, composite, results; then (N_importance > 0) the deterministic inverse-CDF
-// resampling, the merge and the classification of the fine samples.
-__global__ void __launch_bounds__(kSkipWarps * 32) skip_coarse_stage_kernel(SkipParams p) {
+// Coarse stage of one ray per warp: expand, noise, composite, results; then (K > 0) the inverse-CDF resampling with
+// the render kernel's u (sorted random numbers, linspace with perturb = 0), the merge and the fine classification.
+// The scratch allows 9 blocks per SM; the register bound keeps the training branches from allowing fewer.
+__global__ void __launch_bounds__(kSkipWarps * 32, 9) skip_coarse_stage_kernel(SkipParams p) {
   __shared__ SkipWarpScratch scr[kSkipWarps];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   SkipWarpScratch& w = scr[warp];
@@ -221,29 +304,53 @@ __global__ void __launch_bounds__(kSkipWarps * 32) skip_coarse_stage_kernel(Skip
   const bool want_rgb = p.test_time == 0;
   for (long long r = static_cast<long long>(blockIdx.x) * kSkipWarps + warp; r < p.n;
        r += static_cast<long long>(gridDim.x) * kSkipWarps) {
-    const float near = __ldg(p.rays + r * 8 + 6), far = __ldg(p.rays + r * 8 + 7);
-    for (int i = lane; i < Sc; i += 32) w.zc[i] = z_base(near, far, i, Sc, p.use_disp != 0);
-    expand_ray(p, static_cast<int>(r), lane, Sc, p.mask[0] + r * kSkipMaskWords, want_rgb, w, p.samples[0]);
+    const uint32_t* m = p.mask[0] + r * kSkipMaskWords;
+    if (p.zc != nullptr) {
+      for (int i = lane; i < Sc; i += 32) w.zc[i] = p.zc[r * Sc + i];
+    } else {
+      const float near = __ldg(p.rays + r * 8 + 6), far = __ldg(p.rays + r * 8 + 7);
+      for (int i = lane; i < Sc; i += 32) w.zc[i] = z_base(near, far, i, Sc, p.use_disp != 0);
+    }
+    expand_ray(p, static_cast<int>(r), lane, Sc, m, want_rgb, w, p.samples[0]);
+    add_noise(p, 0, r, lane, Sc, m, w.sigma);
     __syncwarp();
     const RayOut o = composite_ray(lane, Sc, w.zc, w.sigma, w.rgb[0], w.rgb[1], w.rgb[2], nullptr, 0.f,
                                    load_skip_ray(p, static_cast<int>(r)).dnorm, want_rgb, w.sigma);
     __syncwarp();
-    if (p.weights_coarse != nullptr)
-      for (int i = lane; i < Sc; i += 32) p.weights_coarse[r * Sc + i] = w.sigma[i];
-    if (lane == 0) {
-      const float add = (p.white_back != 0) ? __fsub_rn(1.f, o.opac) : 0.f;
-      p.opacity_coarse[r] = o.opac;
-      if (want_rgb) {
-        p.rgb_coarse[3 * r + 0] = o.r + add;
-        p.rgb_coarse[3 * r + 1] = o.g + add;
-        p.rgb_coarse[3 * r + 2] = o.b + add;
-        p.depth_coarse[r] = o.depth;
-      }
-    }
+    store_pass(p, 0, r, lane, Sc, o, want_rgb, w.sigma);
     if (K == 0) continue;
     pdf_to_cdf_ray(lane, Sc, w.sigma, w.cdf);
+    // u: render_rays_kernel's ranking (a u's slot is the number of u's before it in torch.sort's order); the u's
+    // are parked in w.zf, which the merge overwrites below
+    if (p.perturb > 0.f) {
+      const unsigned long long key = p.rng_in_kernel ? skip_key(p) : 0ull;
+      for (int j = lane; j < K; j += 32)
+        w.zf[j] = p.rng_in_kernel ? philox_uniform(key, static_cast<uint32_t>(r), static_cast<uint32_t>(j), 1u)
+                                  : __ldg(p.u_rand + r * K + j);
+    }
     __syncwarp();
-    for (int j = lane; j < K; j += 32) w.znew[j] = inverse_cdf(Sc, w.zc, w.cdf, linspace01(j, K));
+    for (int j = lane; j < K; j += 32) {
+      float uj;
+      int slot = j;
+      if (p.perturb > 0.f) {
+        uj = w.zf[j];
+        slot = 0;
+        if (p.rng_in_kernel) {       // philox_uniform is never NaN
+          for (int q = 0; q < K; ++q) {
+            const float uq = w.zf[q];
+            slot += (uq < uj) || (uq == uj && q < j);
+          }
+        } else {
+          for (int q = 0; q < K; ++q) {
+            const float uq = w.zf[q];
+            slot += sort_before(uq, uj) || (sort_tied(uq, uj) && q < j);
+          }
+        }
+      } else {
+        uj = linspace01(j, K);
+      }
+      w.znew[slot] = inverse_cdf(Sc, w.zc, w.cdf, uj);
+    }
     __syncwarp();
     bool inv = false;
     for (int i = lane; i < Sf; i += 32) inv |= merge_flag(i, Sc, w.zc, w.znew);
@@ -265,7 +372,7 @@ __global__ void __launch_bounds__(kSkipWarps * 32) skip_coarse_stage_kernel(Skip
   }
 }
 
-// Fine stage of one ray per warp: expand and composite the merged depths.
+// Fine stage of one ray per warp: expand, noise and composite the merged depths.
 __global__ void __launch_bounds__(kSkipWarps * 32) skip_fine_stage_kernel(SkipParams p) {
   __shared__ SkipWarpScratch scr[kSkipWarps];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -273,23 +380,15 @@ __global__ void __launch_bounds__(kSkipWarps * 32) skip_fine_stage_kernel(SkipPa
   const int Sf = p.Sc + p.K;
   for (long long r = static_cast<long long>(blockIdx.x) * kSkipWarps + warp; r < p.n;
        r += static_cast<long long>(gridDim.x) * kSkipWarps) {
-    const SkipRay s = load_skip_ray(p, static_cast<int>(r));
+    const uint32_t* m = p.mask[1] + r * kSkipMaskWords;
     for (int i = lane; i < Sf; i += 32) w.zf[i] = p.zf[r * Sf + i];
-    expand_ray(p, static_cast<int>(r), lane, Sf, p.mask[1] + r * kSkipMaskWords, true, w, p.samples[1]);
+    expand_ray(p, static_cast<int>(r), lane, Sf, m, true, w, p.samples[1]);
+    add_noise(p, 1, r, lane, Sf, m, w.sigma);
     __syncwarp();
-    const RayOut o = composite_ray(lane, Sf, w.zf, w.sigma, w.rgb[0], w.rgb[1], w.rgb[2], nullptr, 0.f, s.dnorm, true,
-                                   w.sigma);
+    const RayOut o = composite_ray(lane, Sf, w.zf, w.sigma, w.rgb[0], w.rgb[1], w.rgb[2], nullptr, 0.f,
+                                   load_skip_ray(p, static_cast<int>(r)).dnorm, true, w.sigma);
     __syncwarp();
-    if (p.weights_fine != nullptr)
-      for (int i = lane; i < Sf; i += 32) p.weights_fine[r * Sf + i] = w.sigma[i];
-    if (lane == 0) {
-      const float add = (p.white_back != 0) ? __fsub_rn(1.f, o.opac) : 0.f;
-      p.opacity_fine[r] = o.opac;
-      p.rgb_fine[3 * r + 0] = o.r + add;
-      p.rgb_fine[3 * r + 1] = o.g + add;
-      p.rgb_fine[3 * r + 2] = o.b + add;
-      p.depth_fine[r] = o.depth;
-    }
+    store_pass(p, 1, r, lane, Sf, o, true, w.sigma);
     __syncwarp();
   }
 }

@@ -6,223 +6,14 @@
 // nerfb200_nerf_backward's tail reads; the backward starts with train_skip_bwd_kernel, the compositing backward over
 // the sparse sample lists.
 //
-// Forward:  classify (perturbed depths, direction rows) -> scan -> [emit -> direction bias -> coarse MLP] -> coarse
-// stage (noise, composite, random resampling, merge, classify fine) -> scan -> [emit -> fine MLP] -> fine stage ->
-// loss (mse_psnr_kernel).  One warp per ray in grid-stride order: no result depends on the launch shape.
+// The forward runs the per-ray kernels of sample_skip_kernels.cuh with the training inputs set (perturb, noise, the
+// random u, the zc and dirrow workspace) and ends with the loss (mse_psnr_kernel).  This file holds what only training
+// has: the sparse compositing backward, the device copy of the sample counts and the per-row copies.
 #pragma once
 #include "sample_skip_kernels.cuh"
 
 namespace nerfb200 {
 
-struct TrainSkipParams {
-  SkipParams s;                 // s.ofs: the offsets of the pass a launch works on (ofs[pass] below)
-  float perturb, noise_std;
-  const float* perturb_rand;    // (n, Sc), null with perturb = 0 or in-kernel random numbers
-  const float* noise[2];        // (n, Sc) / (n, Sf), null with noise_std = 0
-  const float* u_rand;          // (n, K), as perturb_rand
-  unsigned long long rng_seed;  // as RenderParams
-  int rng_in_kernel;
-  float* zc;                    // (n, Sc) coarse depths (workspace)
-  __half* dirrow;               // (n, 64) fp16 direction rows (workspace)
-  long long* ofs[2];            // (n + 1) exclusive scans of the evaluated samples of each pass (workspace)
-  float* z_coarse;              // optional (n, Sc) copy of the coarse depths
-};
-
-__device__ __forceinline__ unsigned long long train_skip_key(const TrainSkipParams& t) {
-  return t.rng_in_kernel == 2 ? *reinterpret_cast<const unsigned long long*>(t.rng_seed) : t.rng_seed;
-}
-
-// Coarse depths of ray r, sample i: render_rays_kernel's setup_group expression (models/rendering.py:189-204), the
-// uniform from the tensor or from Philox stream 0 with the render kernel's counters.
-__device__ __forceinline__ float train_skip_z(const TrainSkipParams& t, int r, int i, float nr, float fr) {
-  const int Sc = t.s.Sc;
-  const bool ud = t.s.use_disp != 0;
-  float z = z_base(nr, fr, i, Sc, ud);
-  if (t.perturb > 0.f) {
-    const float zl = (i > 0) ? z_base(nr, fr, i - 1, Sc, ud) : z;
-    const float zu = (i < Sc - 1) ? z_base(nr, fr, i + 1, Sc, ud) : z;
-    const float lower = (i > 0) ? __fmul_rn(0.5f, __fadd_rn(zl, z)) : z;
-    const float upper = (i < Sc - 1) ? __fmul_rn(0.5f, __fadd_rn(z, zu)) : z;
-    const float pu = t.rng_in_kernel ? philox_uniform(train_skip_key(t), static_cast<uint32_t>(r), static_cast<uint32_t>(i), 0u)
-                                     : __ldg(t.perturb_rand + static_cast<long long>(r) * Sc + i);
-    const float pr = __fmul_rn(t.perturb, pu);
-    z = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), pr));
-  }
-  return z;
-}
-
-__device__ __forceinline__ bool mask_bit(const uint32_t* m, int i) { return (m[i >> 5] >> (i & 31)) & 1u; }
-
-// Per ray: the coarse depths, the coarse classification and count, and the fp16 direction row the training MLP
-// stores for the direction-slice wgrad (Embedding(3, 4)(d) as the render kernel computes it, columns 27..63 zero).
-__global__ void __launch_bounds__(kSkipWarps * 32) train_skip_classify_kernel(TrainSkipParams t) {
-  __shared__ float zs[kSkipWarps][kMaxSc];
-  __shared__ float de[kSkipWarps][28];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const SkipParams& p = t.s;
-  for (int r = blockIdx.x * kSkipWarps + warp; r < p.n; r += gridDim.x * kSkipWarps) {
-    const float near = __ldg(p.rays + 8 * r + 6), far = __ldg(p.rays + 8 * r + 7);
-    for (int i = lane; i < p.Sc; i += 32) {
-      const float z = train_skip_z(t, r, i, near, far);
-      zs[warp][i] = z;
-      t.zc[static_cast<long long>(r) * p.Sc + i] = z;
-      if (t.z_coarse != nullptr) t.z_coarse[static_cast<long long>(r) * p.Sc + i] = z;
-    }
-    if (lane < 15) dir_embed_term(lane, p.rays + 8 * r + 3, de[warp]);
-    __syncwarp();
-    const int c = classify_ray(p, load_skip_ray(p, r), r, lane, p.Sc, zs[warp], p.mask[0] + r * kSkipMaskWords);
-    if (lane == 0) p.cnt[r] = c;
-    const float lo = (2 * lane < 27) ? de[warp][2 * lane] : 0.f, hi = (2 * lane + 1 < 27) ? de[warp][2 * lane + 1] : 0.f;
-    reinterpret_cast<__half2*>(t.dirrow + static_cast<long long>(r) * 64)[lane] = __floats2half2_rn(lo, hi);
-    __syncwarp();
-  }
-}
-
-// The rows of pass `pass` (skip_emit_kernel's order), depths from the workspace.
-__global__ void __launch_bounds__(kSkipWarps * 32) train_skip_emit_kernel(TrainSkipParams t, int pass) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const SkipParams& p = t.s;
-  const int S = pass ? p.Sc + p.K : p.Sc;
-  const float* zb = pass ? p.zf : t.zc;
-  for (long long r = static_cast<long long>(blockIdx.x) * kSkipWarps + warp; r < p.n;
-       r += static_cast<long long>(gridDim.x) * kSkipWarps) {
-    const uint32_t* m = p.mask[pass] + r * kSkipMaskWords;
-    long long pos = p.ofs[r];
-    for (int k = 0; k < (S >> 5); ++k) {
-      const uint32_t b = m[k];
-      const int i = 32 * k + lane;
-      if ((b >> lane) & 1u) {
-        const long long row = pos + __popc(b & ((1u << lane) - 1u));
-        p.row_ray[row] = static_cast<int>(r);
-        p.row_z[row] = zb[r * S + i];
-      }
-      pos += __popc(b);
-    }
-  }
-}
-
-// sigma + noise of the evaluated samples of one pass (composite_ray's expression); skipped samples keep sigma = 0.
-__device__ __forceinline__ void add_noise(const TrainSkipParams& t, int pass, long long r, int lane, int S,
-                                          const uint32_t* m, float* sigma) {
-  if (t.noise_std <= 0.f) return;
-  const float* nz = t.noise[pass] + r * S;
-  for (int i = lane; i < S; i += 32)
-    if (mask_bit(m, i)) sigma[i] = __fadd_rn(sigma[i], __fmul_rn(__ldg(nz + i), t.noise_std));
-}
-
-// Coarse stage of one ray per warp: expand, noise, composite, results; then (K > 0) the inverse-CDF resampling with
-// the render kernel's u (sorted random numbers, linspace with perturb = 0), the merge and the fine classification.
-__global__ void __launch_bounds__(kSkipWarps * 32) train_skip_coarse_stage_kernel(TrainSkipParams t) {
-  __shared__ SkipWarpScratch scr[kSkipWarps];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  SkipWarpScratch& w = scr[warp];
-  const SkipParams& p = t.s;
-  const int Sc = p.Sc, K = p.K, Sf = Sc + K;
-  for (long long r = static_cast<long long>(blockIdx.x) * kSkipWarps + warp; r < p.n;
-       r += static_cast<long long>(gridDim.x) * kSkipWarps) {
-    const uint32_t* m = p.mask[0] + r * kSkipMaskWords;
-    for (int i = lane; i < Sc; i += 32) w.zc[i] = t.zc[r * Sc + i];
-    expand_ray(p, static_cast<int>(r), lane, Sc, m, true, w, p.samples[0]);
-    add_noise(t, 0, r, lane, Sc, m, w.sigma);
-    __syncwarp();
-    const RayOut o = composite_ray(lane, Sc, w.zc, w.sigma, w.rgb[0], w.rgb[1], w.rgb[2], nullptr, 0.f,
-                                   load_skip_ray(p, static_cast<int>(r)).dnorm, true, w.sigma);
-    __syncwarp();
-    if (p.weights_coarse != nullptr)
-      for (int i = lane; i < Sc; i += 32) p.weights_coarse[r * Sc + i] = w.sigma[i];
-    if (lane == 0) {
-      const float add = (p.white_back != 0) ? __fsub_rn(1.f, o.opac) : 0.f;
-      p.opacity_coarse[r] = o.opac;
-      p.rgb_coarse[3 * r + 0] = o.r + add;
-      p.rgb_coarse[3 * r + 1] = o.g + add;
-      p.rgb_coarse[3 * r + 2] = o.b + add;
-      p.depth_coarse[r] = o.depth;
-    }
-    if (K == 0) continue;
-    pdf_to_cdf_ray(lane, Sc, w.sigma, w.cdf);
-    // u: render_rays_kernel's ranking (a u's slot is the number of u's before it in torch.sort's order); the u's
-    // are parked in w.zf, which the merge overwrites below
-    if (t.perturb > 0.f) {
-      const unsigned long long key = t.rng_in_kernel ? train_skip_key(t) : 0ull;
-      for (int j = lane; j < K; j += 32)
-        w.zf[j] = t.rng_in_kernel ? philox_uniform(key, static_cast<uint32_t>(r), static_cast<uint32_t>(j), 1u)
-                                  : __ldg(t.u_rand + r * K + j);
-    }
-    __syncwarp();
-    for (int j = lane; j < K; j += 32) {
-      float uj;
-      int slot = j;
-      if (t.perturb > 0.f) {
-        uj = w.zf[j];
-        slot = 0;
-        if (t.rng_in_kernel) {       // philox_uniform is never NaN
-          for (int q = 0; q < K; ++q) {
-            const float uq = w.zf[q];
-            slot += (uq < uj) || (uq == uj && q < j);
-          }
-        } else {
-          for (int q = 0; q < K; ++q) {
-            const float uq = w.zf[q];
-            slot += sort_before(uq, uj) || (sort_tied(uq, uj) && q < j);
-          }
-        }
-      } else {
-        uj = linspace01(j, K);
-      }
-      w.znew[slot] = inverse_cdf(Sc, w.zc, w.cdf, uj);
-    }
-    __syncwarp();
-    bool inv = false;
-    for (int i = lane; i < Sf; i += 32) inv |= merge_flag(i, Sc, w.zc, w.znew);
-    const bool any_inv = __any_sync(0xffffffffu, inv);
-    for (int i = lane; i < Sf; i += 32) {
-      const float v = (i < Sc) ? w.zc[i] : w.znew[i - Sc];
-      w.zf[merge_rank(i, v, Sc, K, w.zc, w.znew, any_inv)] = v;
-    }
-    __syncwarp();
-    for (int i = lane; i < Sf; i += 32) {
-      p.zf[r * Sf + i] = w.zf[i];
-      if (p.z_fine != nullptr) p.z_fine[r * Sf + i] = w.zf[i];
-    }
-    const int c = classify_ray(p, load_skip_ray(p, static_cast<int>(r)), static_cast<int>(r), lane, Sf, w.zf,
-                               p.mask[1] + r * kSkipMaskWords);
-    if (lane == 0) p.cnt[r] = c;
-    __syncwarp();
-  }
-}
-
-// Fine stage of one ray per warp: expand, noise and composite the merged depths.
-__global__ void __launch_bounds__(kSkipWarps * 32) train_skip_fine_stage_kernel(TrainSkipParams t) {
-  __shared__ SkipWarpScratch scr[kSkipWarps];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  SkipWarpScratch& w = scr[warp];
-  const SkipParams& p = t.s;
-  const int Sf = p.Sc + p.K;
-  for (long long r = static_cast<long long>(blockIdx.x) * kSkipWarps + warp; r < p.n;
-       r += static_cast<long long>(gridDim.x) * kSkipWarps) {
-    const uint32_t* m = p.mask[1] + r * kSkipMaskWords;
-    for (int i = lane; i < Sf; i += 32) w.zf[i] = p.zf[r * Sf + i];
-    expand_ray(p, static_cast<int>(r), lane, Sf, m, true, w, p.samples[1]);
-    add_noise(t, 1, r, lane, Sf, m, w.sigma);
-    __syncwarp();
-    const RayOut o = composite_ray(lane, Sf, w.zf, w.sigma, w.rgb[0], w.rgb[1], w.rgb[2], nullptr, 0.f,
-                                   load_skip_ray(p, static_cast<int>(r)).dnorm, true, w.sigma);
-    __syncwarp();
-    if (p.weights_fine != nullptr)
-      for (int i = lane; i < Sf; i += 32) p.weights_fine[r * Sf + i] = w.sigma[i];
-    if (lane == 0) {
-      const float add = (p.white_back != 0) ? __fsub_rn(1.f, o.opac) : 0.f;
-      p.opacity_fine[r] = o.opac;
-      p.rgb_fine[3 * r + 0] = o.r + add;
-      p.rgb_fine[3 * r + 1] = o.g + add;
-      p.rgb_fine[3 * r + 2] = o.b + add;
-      p.depth_fine[r] = o.depth;
-    }
-    __syncwarp();
-  }
-}
-
-// ------------------------------------------------------------------ sparse compositing backward
 // composite_bwd_kernel's arithmetic (the fused MSE seed, white_back, noise, the ReLU mask) on one ray per warp, with
 // sigma / rgb of an evaluated sample read from its compacted row and sigma = 0, rgb = 0 (no noise) for a skipped one.
 // d sigma / d rgb_pre go to the evaluated rows only; rows n_rows .. n_pad - 1 (padding of the last MLP tile) get 0.

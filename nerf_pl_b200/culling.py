@@ -8,7 +8,7 @@ touched.  The reference has no counterpart: it evaluates every sample of every r
 
 ``skip="samples"`` (``render_rays_culled``, ``batched_inference``, ``render_image``) goes one step further: inside a
 live ray, a sample whose point lies in no occupied cell gets sigma = 0 and is not evaluated
-(csrc/sample_skip_kernels.cuh, include/nerf_pl_b200_samples.h; DESIGN.md "Skipping empty samples").  The evaluated
+(csrc/sample_skip_kernels.cuh, include/nerf_pl_b200.h; DESIGN.md "Skipping empty samples").  The evaluated
 samples have the fused kernel's sigma and rgb bit for bit, and a ray with nothing to skip renders bit for bit as
 ``render_rays`` renders it; a ray with skipped samples is an approximation, like a culled ray.
 

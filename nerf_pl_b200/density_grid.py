@@ -6,7 +6,7 @@ jittered point of the cell (the scheme of Instant-NGP-style occupancy grids), an
 density is above ``sigma_threshold``.  ``grid`` is an ``OccupancyGrid`` over the same bits tensor, so every consumer
 of a grid (``render_rays_culled``, ``skip="samples"``, ``render_rays_loss(occupancy=)``, ``CapturedTrainStep``)
 takes it as is.  An update is a fixed sequence of sm_90a launches with no host synchronisation and no allocation
-after the first call (csrc/density_kernels.cuh, include/nerf_pl_b200_density.h), so a CUDA graph can capture it;
+after the first call (csrc/density_kernels.cuh, include/nerf_pl_b200.h), so a CUDA graph can capture it;
 ``CapturedTrainStep(occupancy=grid, update_every=R)`` does.
 
 A fresh or reset grid has density 0 and every cell occupied: it skips nothing until its first update.

@@ -1,5 +1,5 @@
 """The reference's image metrics on the device: ``ssim`` (metrics.py:15-20) and ``visualize_depth``
-(utils/visualization.py:6-18), each one call into ``include/nerf_pl_b200_metrics.h``.  Definitions, provenance and
+(utils/visualization.py:6-18), each one call into ``include/nerf_pl_b200.h``.  Definitions, provenance and
 measured numbers: DESIGN.md "Image metrics"."""
 from __future__ import annotations
 

@@ -7,7 +7,7 @@ gradient.  An evaluated sample gets the network's sigma and rgb bit for bit as t
 them, then the noise.  Rebuild the grid from the fine network as training goes (INTEGRATION.md section 7): density
 that appears in a cell the grid calls empty is trained from the next rebuild on.
 
-forward : ``nerfb200_train_samples_forward`` (include/nerf_pl_b200_train_samples.h): perturbed depths and
+forward : ``nerfb200_train_samples_forward`` (include/nerf_pl_b200.h): perturbed depths and
           classification, the compacted rows of each network through the save-mode MLP, compositing with noise, the
           random resampling and the merge, the loss.  Every launch is sized for the worst case and reads the
           step's sample counts on the device; the eager call reads the two counts back once at the end.

@@ -1,5 +1,5 @@
 """Float64 numpy restatement of the density grid update (nerf_pl_b200.DensityGrid, csrc/density_kernels.cuh,
-include/nerf_pl_b200_density.h; DESIGN.md "Keeping the grid current during training").
+include/nerf_pl_b200.h; DESIGN.md "Keeping the grid current during training").
 
 For an N-point grid over ranges ((xmin, xmax), (ymin, ymax), (zmin, zmax)), M = N - 1 cells per axis and cell
 c = (cz * M + cy) * M + cx, one update from a network with key s is:

@@ -22,19 +22,29 @@ def lib():
     return _lib.load()
 
 
+HEADER = os.path.join(ROOT, "include", "nerf_pl_b200.h")
+# the argument structs the header declares and their ctypes mirrors
+MIRRORS = {"nerfb200_render_args": _lib.RenderArgs, "nerfb200_backward_args": _lib.BackwardArgs,
+           "nerfb200_samples_args": _lib.SamplesArgs, "nerfb200_train_samples_args": _lib.TrainSamplesArgs}
+
+
 def test_header_symbols_exported(lib):
-    hdr = open(os.path.join(ROOT, "include", "nerf_pl_b200.h")).read()
-    declared = set(re.findall(r"\b(nerfb200_[a-z_0-9]+)\s*\(", hdr))
-    declared -= {"nerfb200_render_args", "nerfb200_backward_args"}
+    hdr = open(HEADER).read()
+    declared = set(re.findall(r"\b(nerfb200_[a-z_0-9]+)\s*\(", hdr)) - set(MIRRORS)
+    assert len(declared) == 75
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
     assert "#define NERFB200_ABI_VERSION 3" in hdr
+    for k, v in (("MEAN", 0), ("SUM", 1), ("NONE", 2)):
+        assert f"#define NERFB200_SSIM_{k} {v}" in hdr
+    assert _lib.INCLUDES == ["nerf_pl_b200.h"]
+    assert sorted(_lib.HEADERS) == sorted(f for f in os.listdir(_lib.CSRC) if f != "capi.cu")
     for name in declared:
         assert hasattr(lib, name), name
 
 
 def _header_prototypes():
     """[(name, return type, [argument declarations])] of every function include/nerf_pl_b200.h declares, in order."""
-    hdr = open(os.path.join(ROOT, "include", "nerf_pl_b200.h")).read()
+    hdr = open(HEADER).read()
     hdr = re.sub(r"/\*.*?\*/", " ", hdr, flags=re.S)
     hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
     protos = []
@@ -47,31 +57,50 @@ def _header_prototypes():
     return protos
 
 
-def test_one_signature_table_matches_the_one_header(lib):
+# Pointer arguments whose memory is read or written on the host although their names do not end in `_host`.
+HOST_POINTERS = {("nerfb200_adam_step", "numel"), ("nerfb200_adam_step_dev", "numel"),
+                 ("nerfb200_train_samples_forward_dev", "live_samples_dev")}
+
+
+def test_one_signature_table_matches_all_75_entries_of_the_header(lib):
     """Every prototype of include/nerf_pl_b200.h against _lib.SIGNATURES: the same names, declared once each, in the
-    same order, with the same argument counts, argument kinds and return types (a wrong width would silently corrupt
-    the argument); the loaded library's entries carry exactly those types."""
+    same order, with the same argument counts, argument types and return types (a wrong width would silently corrupt
+    the argument); the loaded library's entries carry exactly those types.  A pointer is c_void_p (device memory),
+    except: an argument struct is a pointer to its mirror, a table of pointers is POINTER(c_void_p), and host memory
+    (an array, a name ending in `_host`, HOST_POINTERS) is a pointer to its scalar type."""
     protos = _header_prototypes()
     names = [name for name, _, _ in protos]
-    assert len(names) == 57
+    assert len(names) == 75
     assert len(set(names)) == len(names), sorted(n for n in names if names.count(n) > 1)
     assert names == list(_lib.SIGNATURES) == list(_lib.EXPORTS)          # header order
     scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "size_t": ctypes.c_size_t,
                "float": ctypes.c_float, "double": ctypes.c_double}
     returns = {"int": ctypes.c_int32, "size_t": ctypes.c_size_t, "int64_t": ctypes.c_int64,
                "const char*": ctypes.c_char_p}
+    host = set()
     for name, ret, args in protos:
         restype, argtypes = _lib.SIGNATURES[name]
         assert restype is returns[ret], (name, ret, restype)
         assert len(argtypes) == len(args), (name, args, argtypes)
         for decl, t in zip(args, argtypes):
-            if "*" in decl or "[" in decl:
-                assert t is ctypes.c_void_p or issubclass(t, ctypes._Pointer), (name, decl, t)
+            m = re.fullmatch(r"(?:const )?(\w+)((?:\s*\*\s*(?:const\s*)?)*)\s*(\w+)(\[\d+\])?", decl)
+            assert m, (name, decl)
+            base, stars, arg, array = m.group(1), m.group(2).count("*"), m.group(3), m.group(4)
+            if base in MIRRORS:
+                want = ctypes.POINTER(MIRRORS[base])
+            elif stars + bool(array) >= 2:
+                want = ctypes.POINTER(ctypes.c_void_p)
+            elif array or (stars and (arg.endswith("_host") or (name, arg) in HOST_POINTERS)):
+                want = ctypes.POINTER(scalars[base])
+                host.add((name, arg))
+            elif stars:
+                want = ctypes.c_void_p
             else:
-                base = decl.replace("const ", "").rsplit(" ", 1)[0]
-                assert t is scalars[base], (name, decl, t)
+                want = scalars[base]
+            assert t is want, (name, decl, t)
         fn = getattr(lib, name)
         assert fn.restype is restype and list(fn.argtypes) == argtypes, name
+    assert HOST_POINTERS <= host
 
 
 def test_call_appends_the_stream_and_maps_return_codes(monkeypatch):
@@ -116,7 +145,7 @@ def test_entries_are_called_through_lib_call():
 
 
 def test_abi_basics(lib):
-    assert lib.nerfb200_abi_version() == 3
+    assert lib.nerfb200_abi_version() == _lib.ABI_VERSION == 3
     # layout.h: 30 x 32 KiB + 5 x 16 KiB fp16 slices + fp32 tail, rounded to 1 KiB, + 30 backward slices
     fwd = 30 * 32768 + 5 * 16384 + 4 * (9 * 256 + 256 + 4 + 384 + 4 + 28 * 128)
     assert lib.nerfb200_packed_bytes() == (fwd + 1023) // 1024 * 1024 + 30 * 32768
@@ -127,21 +156,41 @@ def test_abi_basics(lib):
 
 
 def test_struct_mirrors_match_the_header(tmp_path):
-    """sizeof / offsetof of the argument structs as gcc lays out include/nerf_pl_b200.h == the ctypes mirrors."""
+    """sizeof / offsetof of the argument structs as gcc lays out include/nerf_pl_b200.h == the ctypes mirrors: four
+    offsets of nerfb200_render_args and every field of the two skipping structs."""
     import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    S, T = _lib.SamplesArgs, _lib.TrainSamplesArgs
+    exprs = ["sizeof(nerfb200_render_args)", "sizeof(nerfb200_backward_args)",
+             "offsetof(nerfb200_render_args, rng_seed)", "offsetof(nerfb200_render_args, rng_in_kernel)",
+             "offsetof(nerfb200_render_args, train_workspace)", "offsetof(nerfb200_render_args, perturb_rand)",
+             "sizeof(nerfb200_samples_args)", "sizeof(nerfb200_train_samples_args)"]
+    exprs += [f"offsetof(nerfb200_samples_args, {f})" for f, _ in S._fields_]
+    exprs += [f"offsetof(nerfb200_train_samples_args, {f})" for f, _ in T._fields_]
     src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "nerf_pl_b200.h"\n'
-                   'int main(void){printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(nerfb200_render_args), '
-                   'sizeof(nerfb200_backward_args), offsetof(nerfb200_render_args, rng_seed), '
-                   'offsetof(nerfb200_render_args, rng_in_kernel), offsetof(nerfb200_render_args, train_workspace), '
-                   'offsetof(nerfb200_render_args, perturb_rand));return 0;}\n')
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "nerf_pl_b200.h"\nint main(void){\n' +
+                   "".join(f'printf("%zu\\n", (size_t)({e}));\n' for e in exprs) + "return 0;}\n")
     exe = tmp_path / "sz"
-    subprocess.run(["gcc", "-I", os.path.join(root, "include"), str(src), "-o", str(exe)], check=True)
+    subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
     got = [int(x) for x in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
     R = _lib.RenderArgs
-    assert got == [ctypes.sizeof(R), ctypes.sizeof(_lib.BackwardArgs), R.rng_seed.offset, R.rng_in_kernel.offset,
-                   R.train_workspace.offset, R.perturb_rand.offset]
+    want = [ctypes.sizeof(R), ctypes.sizeof(_lib.BackwardArgs), R.rng_seed.offset, R.rng_in_kernel.offset,
+            R.train_workspace.offset, R.perturb_rand.offset, ctypes.sizeof(S), ctypes.sizeof(T)]
+    want += [getattr(S, f).offset for f, _ in S._fields_] + [getattr(T, f).offset for f, _ in T._fields_]
+    assert got == want
+
+
+def _struct_fields(name):
+    body = re.search(rf"typedef struct {name} \{{(.*?)\}}", open(HEADER).read(), re.S).group(1)
+    return [re.sub(r"\[.*\]", "", ln.strip().rstrip(";")).split()[-1].lstrip("*") for ln in body.splitlines()
+            if ln.strip()]
+
+
+def test_samples_args_fields_mirror_the_header():
+    assert _struct_fields("nerfb200_samples_args") == [f for f, _ in _lib.SamplesArgs._fields_]
+
+
+def test_train_samples_args_fields_mirror_the_header():
+    assert _struct_fields("nerfb200_train_samples_args") == [f for f, _ in _lib.TrainSamplesArgs._fields_]
 
 
 def test_training_workspace_layout(lib):

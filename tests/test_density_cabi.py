@@ -1,10 +1,7 @@
-"""The C ABI of the density grid: the companion header include/nerf_pl_b200_density.h against
-_lib.DENSITY_SIGNATURES, the workspace sizes, the argument errors the entries return before any launch, and the
+"""The C ABI of the density grid: the workspace sizes, the argument errors the entries return before any launch, and the
 argument errors of nb.DensityGrid and CapturedTrainStep(update_every=) that need no GPU."""
 import ctypes
 import math
-import os
-import re
 
 import pytest
 import torch
@@ -12,7 +9,6 @@ import torch
 import nerf_pl_b200 as nb
 from nerf_pl_b200 import _lib
 
-HEADER = os.path.join(os.path.dirname(__file__), "..", "include", "nerf_pl_b200_density.h")
 BOX = (ctypes.c_double * 6)(-1, 1, -1, 1, -1, 1)
 
 
@@ -20,45 +16,6 @@ BOX = (ctypes.c_double * 6)(-1, 1, -1, 1, -1, 1)
 def lib():
     _lib.build()
     return _lib.load()
-
-
-def _prototypes():
-    hdr = re.sub(r"/\*.*?\*/", " ", open(HEADER).read(), flags=re.S)
-    hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
-    protos = []
-    for decl in hdr.split(";"):
-        m = re.search(r"(\w[\w\s\*]*?)\b(nerfb200_\w+)\s*\((.*)\)\s*$", decl.strip(), re.S)
-        if m:
-            protos.append((m.group(2), " ".join(m.group(1).split()), [" ".join(a.split()) for a in m.group(3).split(",")]))
-    return protos
-
-
-def test_signature_table_matches_the_companion_header(lib):
-    protos = _prototypes()
-    names = [n for n, _, _ in protos]
-    assert names == list(_lib.DENSITY_SIGNATURES)
-    others = (_lib.SIGNATURES, _lib.METRICS_SIGNATURES, _lib.VIEWS_SIGNATURES, _lib.SAMPLES_SIGNATURES,
-              _lib.TRAIN_SAMPLES_SIGNATURES)
-    assert not set(names) & set().union(*others)
-    scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "size_t": ctypes.c_size_t, "int": ctypes.c_int32,
-               "double": ctypes.c_double, "float": ctypes.c_float}
-    for name, ret, args in protos:
-        restype, argtypes = _lib.DENSITY_SIGNATURES[name]
-        assert restype is scalars[ret], (name, ret)
-        assert len(argtypes) == len(args), (name, args)
-        for decl, t in zip(args, argtypes):
-            flat = decl.replace(" ", "")
-            if "ranges_host[6]" in flat:
-                assert t is ctypes.POINTER(ctypes.c_double), (name, decl)
-            elif "*" in decl:
-                assert t is ctypes.c_void_p, (name, decl, t)       # device pointers
-            else:
-                assert t is scalars[decl.replace("const ", "").rsplit(" ", 1)[0]], (name, decl, t)
-        fn = getattr(lib, name)
-        assert fn.restype is restype and list(fn.argtypes) == argtypes, name
-    assert '#include "nerf_pl_b200.h"' in open(HEADER).read()
-    assert "nerf_pl_b200_density.h" in _lib.INCLUDES and "density_kernels.cuh" in _lib.HEADERS
-    assert lib.nerfb200_abi_version() == 3
 
 
 def test_workspace_sizes(lib):

@@ -1,16 +1,14 @@
-"""The C ABI of the mesh grids taken through an occupancy grid: the companion header
-include/nerf_pl_b200_masked_grid.h against _lib.MASKED_GRID_SIGNATURES and the library's exports, the workspace
-sizes, and the argument errors the entries return before any launch."""
+"""The C ABI of the mesh grids taken through an occupancy grid: the arguments both entries take, the workspace sizes,
+and the argument errors the entries return before any launch."""
 import ctypes
 import math
-import os
-import re
 
 import pytest
 
 from nerf_pl_b200 import _lib
 
-HEADER = os.path.join(os.path.dirname(__file__), "..", "include", "nerf_pl_b200_masked_grid.h")
+from .test_cabi import _header_prototypes
+
 BOX = (ctypes.c_double * 6)(-1, 1, -1, 1, -1, 1)
 
 
@@ -20,52 +18,14 @@ def lib():
     return _lib.load()
 
 
-def _prototypes():
-    hdr = re.sub(r"/\*.*?\*/", " ", open(HEADER).read(), flags=re.S)
-    hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
-    protos = []
-    for decl in hdr.split(";"):
-        m = re.search(r"(\w[\w\s\*]*?)\b(nerfb200_\w+)\s*\((.*)\)\s*$", decl.strip(), re.S)
-        if m:
-            protos.append((m.group(2), " ".join(m.group(1).split()), [" ".join(a.split()) for a in m.group(3).split(",")]))
-    return protos
-
-
-def test_signature_table_matches_the_companion_header(lib):
-    protos = _prototypes()
-    names = [n for n, _, _ in protos]
-    assert names == list(_lib.MASKED_GRID_SIGNATURES) == ["nerfb200_masked_grid_workspace_bytes",
-                                                          "nerfb200_sigma_grid_masked",
-                                                          "nerfb200_rgb_sigma_grid_masked"]
-    others = (_lib.SIGNATURES, _lib.METRICS_SIGNATURES, _lib.VIEWS_SIGNATURES, _lib.SAMPLES_SIGNATURES,
-              _lib.TRAIN_SAMPLES_SIGNATURES, _lib.DENSITY_SIGNATURES)
-    assert not set(names) & set().union(*others)
-    scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "size_t": ctypes.c_size_t, "int": ctypes.c_int32,
-               "double": ctypes.c_double, "float": ctypes.c_float}
-    for name, ret, args in protos:
-        restype, argtypes = _lib.MASKED_GRID_SIGNATURES[name]
-        assert restype is scalars[ret], (name, ret)
-        assert len(argtypes) == len(args), (name, args)
-        for decl, t in zip(args, argtypes):
-            flat = decl.replace(" ", "")
-            if "ranges_host[6]" in flat:
-                assert t is ctypes.POINTER(ctypes.c_double), (name, decl)
-            elif flat == "int64_t*evaluated_host":
-                assert t is ctypes.POINTER(ctypes.c_int64), (name, decl)   # a host pointer
-            elif "*" in decl:
-                assert t is ctypes.c_void_p, (name, decl, t)               # device pointers
-            else:
-                assert t is scalars[decl.replace("const ", "").rsplit(" ", 1)[0]], (name, decl, t)
-        fn = getattr(lib, name)
-        assert fn.restype is restype and list(fn.argtypes) == argtypes, name
-    # both grid entries take the same arguments, the output's name aside
-    assert [a.split()[-1] for a in protos[1][2]] == [
+def test_both_grid_entries_take_the_same_arguments():
+    """The output's name aside."""
+    protos = {name: args for name, _, args in _header_prototypes()}
+    sigma, rgb = protos["nerfb200_sigma_grid_masked"], protos["nerfb200_rgb_sigma_grid_masked"]
+    assert [a.split()[-1] for a in sigma] == [
         "packed", "N", "ranges_host[6]", "bits", "occ_N", "occ_ranges_host[6]", "chunk", "ws", "bytes", "sigma_out",
         "evaluated_host", "stream"]
-    assert protos[1][2][:9] + protos[1][2][10:] == protos[2][2][:9] + protos[2][2][10:]
-    assert '#include "nerf_pl_b200.h"' in open(HEADER).read()
-    assert "nerf_pl_b200_masked_grid.h" in _lib.INCLUDES and "masked_grid_kernels.cuh" in _lib.HEADERS
-    assert lib.nerfb200_abi_version() == 3
+    assert sigma[:9] + sigma[10:] == rgb[:9] + rgb[10:]
 
 
 def test_workspace_sizes(lib):

@@ -1,9 +1,6 @@
-"""CPU checks of skip="samples": the float64 per-point rule (tests/sample_skip_ref.py) on hand cases, the companion
-header include/nerf_pl_b200_samples.h against _lib.SAMPLES_SIGNATURES, and the argument errors raised before any
-launch."""
+"""CPU checks of skip="samples": the float64 per-point rule (tests/sample_skip_ref.py) on hand cases, the workspace
+query, and the argument errors raised before any launch."""
 import ctypes
-import os
-import re
 
 import numpy as np
 import pytest
@@ -12,9 +9,6 @@ import torch
 import nerf_pl_b200 as nb
 from nerf_pl_b200 import _lib
 from tests import sample_skip_ref as sk
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "nerf_pl_b200_samples.h")
 
 
 def _words(cells, M):
@@ -98,50 +92,6 @@ def test_mask_bits_round_trip():
 def lib():
     _lib.build()
     return _lib.load()
-
-
-def _prototypes():
-    hdr = re.sub(r"/\*.*?\*/", " ", open(HEADER).read(), flags=re.S)
-    hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
-    protos = []
-    for decl in hdr.split(";"):
-        m = re.search(r"(\w[\w\s\*]*?)\b(nerfb200_\w+)\s*\((.*)\)\s*$", decl.strip(), re.S)
-        if m:
-            ret = " ".join(m.group(1).split())
-            protos.append((m.group(2), ret, [" ".join(a.split()) for a in m.group(3).split(",")]))
-    return protos
-
-
-def test_signature_table_matches_the_companion_header(lib):
-    protos = _prototypes()
-    names = [n for n, _, _ in protos]
-    assert names == list(_lib.SAMPLES_SIGNATURES)
-    assert not set(names) & (set(_lib.SIGNATURES) | set(_lib.METRICS_SIGNATURES) | set(_lib.VIEWS_SIGNATURES))
-    scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "size_t": ctypes.c_size_t, "int": ctypes.c_int32}
-    for name, ret, args in protos:
-        restype, argtypes = _lib.SAMPLES_SIGNATURES[name]
-        assert restype is scalars[ret], (name, ret)
-        assert len(argtypes) == len(args), (name, args)
-        for decl, t in zip(args, argtypes):
-            if "nerfb200_samples_args" in decl:
-                assert t is ctypes.POINTER(_lib.SamplesArgs)
-            elif "int64_t*" in decl.replace(" ", ""):
-                assert t is ctypes.POINTER(ctypes.c_int64)
-            elif "*" in decl:
-                assert t is ctypes.c_void_p, (name, decl, t)
-            else:
-                assert t is scalars[decl.replace("const ", "").rsplit(" ", 1)[0]], (name, decl, t)
-        fn = getattr(lib, name)
-        assert fn.restype is restype and list(fn.argtypes) == argtypes, name
-    assert '#include "nerf_pl_b200.h"' in open(HEADER).read()
-    assert "nerf_pl_b200_samples.h" in _lib.INCLUDES
-
-
-def test_args_struct_mirrors_the_header():
-    body = re.search(r"typedef struct nerfb200_samples_args \{(.*?)\}", open(HEADER).read(), re.S).group(1)
-    fields = [re.sub(r"\[.*\]", "", ln.strip().rstrip(";")).split()[-1].lstrip("*")
-              for ln in body.splitlines() if ln.strip()]
-    assert fields == [f for f, _ in _lib.SamplesArgs._fields_]
 
 
 def test_workspace_bytes_and_shape_checks(lib):

@@ -1,4 +1,4 @@
-"""The capturable entries of include/nerf_pl_b200_train_samples.h (nerfb200_train_samples_forward_dev / _backward_dev):
+"""The capturable entries of include/nerf_pl_b200.h (nerfb200_train_samples_forward_dev / _backward_dev):
 their declarations, and the argument errors they return before any launch, as tests/test_train_skip_cabi.py checks
 the eager entries."""
 import ctypes
@@ -9,7 +9,8 @@ import torch
 
 from nerf_pl_b200 import _lib
 
-from .test_train_skip_cabi import BAD, HEADER, _args
+from .test_cabi import HEADER
+from .test_train_skip_cabi import BAD, _args
 
 DEV_ENTRIES = ("nerfb200_train_samples_forward_dev", "nerfb200_train_samples_backward_dev")
 
@@ -20,18 +21,18 @@ def lib():
     return _lib.load()
 
 
-def test_capturable_entries_are_declared():
+def test_capturable_entries_are_declared_in_the_one_header():
     hdr = open(HEADER).read()
     for name in DEV_ENTRIES:
         assert re.search(rf"\bint {name}\(", hdr), name
-        assert name in _lib.TRAIN_SAMPLES_SIGNATURES
-    fwd = _lib.TRAIN_SAMPLES_SIGNATURES["nerfb200_train_samples_forward_dev"][1]
+        assert name in _lib.SIGNATURES
+    fwd = _lib.SIGNATURES["nerfb200_train_samples_forward_dev"][1]
     assert fwd[3] is ctypes.POINTER(ctypes.c_int64)           # live_samples_dev: a device int64[2]
-    bwd = _lib.TRAIN_SAMPLES_SIGNATURES["nerfb200_train_samples_backward_dev"][1]
+    bwd = _lib.SIGNATURES["nerfb200_train_samples_backward_dev"][1]
     assert len(bwd) == 9 and ctypes.POINTER(ctypes.c_int64) not in bwd     # no host counts
     # the eager entries keep their signatures
-    assert _lib.TRAIN_SAMPLES_SIGNATURES["nerfb200_train_samples_forward"][1][3] is ctypes.POINTER(ctypes.c_int64)
-    assert len(_lib.TRAIN_SAMPLES_SIGNATURES["nerfb200_train_samples_backward"][1]) == 10
+    assert _lib.SIGNATURES["nerfb200_train_samples_forward"][1][3] is ctypes.POINTER(ctypes.c_int64)
+    assert len(_lib.SIGNATURES["nerfb200_train_samples_backward"][1]) == 10
 
 
 def test_capturable_entries_argument_checks(lib):

@@ -1,9 +1,7 @@
-"""CPU-side checks of the view-batch entry: include/nerf_pl_b200_views.h against _lib.VIEWS_SIGNATURES, the library's
-export, the argument checks that need no GPU, and DeviceViewBatches' argument errors and its shared epoch logic."""
+"""CPU-side checks of the view-batch entry: the argument checks that need no GPU, and DeviceViewBatches' argument
+errors and its shared epoch logic."""
 import ctypes
 import inspect
-import os
-import re
 
 import pytest
 import torch
@@ -12,47 +10,11 @@ import nerf_pl_b200 as nb
 from nerf_pl_b200 import _lib
 from nerf_pl_b200 import data
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "nerf_pl_b200_views.h")
-
 
 @pytest.fixture(scope="module")
 def lib():
     _lib.build()
     return _lib.load()
-
-
-def _prototypes():
-    hdr = re.sub(r"/\*.*?\*/", " ", open(HEADER).read(), flags=re.S)
-    hdr = "\n".join(ln for ln in hdr.splitlines() if not ln.lstrip().startswith("#"))
-    protos = []
-    for decl in hdr.split(";"):
-        m = re.search(r"(.*?)\b(nerfb200_\w+)\s*\((.*)\)\s*$", decl.strip(), re.S)
-        if m:
-            ret = " ".join(re.split(r"[{}]", m.group(1))[-1].split())
-            protos.append((m.group(2), ret, [" ".join(a.split()) for a in m.group(3).split(",")]))
-    return protos
-
-
-def test_signature_table_matches_the_companion_header(lib):
-    protos = _prototypes()
-    names = [n for n, _, _ in protos]
-    assert names == list(_lib.VIEWS_SIGNATURES) == ["nerfb200_view_batch"]
-    assert not set(names) & (set(_lib.SIGNATURES) | set(_lib.METRICS_SIGNATURES))
-    scalars = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "float": ctypes.c_float}
-    for name, ret, args in protos:
-        restype, argtypes = _lib.VIEWS_SIGNATURES[name]
-        assert ret == "int" and restype is ctypes.c_int32
-        assert len(argtypes) == len(args), (name, args)
-        for decl, t in zip(args, argtypes):
-            if "*" in decl:
-                assert t is ctypes.c_void_p, (name, decl, t)
-            else:
-                assert t is scalars[decl.replace("const ", "").rsplit(" ", 1)[0]], (name, decl, t)
-        fn = getattr(lib, name)
-        assert fn.restype is restype and list(fn.argtypes) == argtypes, name
-    assert '#include "nerf_pl_b200.h"' in open(HEADER).read()
-    assert "nerf_pl_b200_views.h" in _lib.INCLUDES
 
 
 def test_view_batch_argument_checks(lib):
