@@ -20,6 +20,9 @@
 extern "C" {
 #endif
 
+/* Version 3 has grown in place: nerfb200_samples_args and nerfb200_train_samples_args gained fields at their ends.
+ * Zero in every new field keeps the earlier behaviour, but a caller compiled against the shorter structs is not
+ * supported: build against this header. */
 #define NERFB200_ABI_VERSION 3
 
 #define NERFB200_EINVAL (-1)      /* bad argument value / null pointer            */
@@ -497,11 +500,12 @@ int nerfb200_view_batch(const uint8_t* images, int64_t V, int32_t H, int32_t W, 
 /* ==== rendering with empty samples skipped (inference) ============================================
  * Definition and guarantees: DESIGN.md "Skipping empty samples". */
 
-/* One render of n_rays rays with perturb = noise_std = 0 in which a sample is evaluated only when its point
+/* One render of n_rays rays in which a sample is evaluated only when its point
  * o + d z (rounded as the render kernel rounds it) lies in the closed box of an occupied cell of the occupancy grid
  * (bits, N, ranges_host: as nerfb200_cull_count).  A skipped sample has sigma = 0.  A ray with a non-finite value or
  * far <= near, and a pass whose interval lengths delta |d| are not all finite, is evaluated at every sample.
- * Compositing, the inverse-CDF resampling (u = linspace(0, 1, N_importance)) and the merge are the render kernel's.
+ * Compositing, the inverse-CDF resampling (u = linspace(0, 1, N_importance), or the sorted random u with
+ * perturb > 0) and the merge are the render kernel's; the random inputs (fields at the end) are optional.
  *   rays: (n_rays, 8) fp32, 16-byte aligned.  live_flag: nullable (n_rays) uint8; a ray whose flag is 0 has every
  *   sample skipped.  Results: as nerfb200_render_args (rgb / depth_coarse only with test_time = 0, the fine ones
  *   with n_importance > 0); z_fine (n, S_f), weights_coarse (n, S_c), weights_fine (n, S_f) optional.
@@ -509,6 +513,11 @@ int nerfb200_view_batch(const uint8_t* images, int64_t V, int32_t H, int32_t W, 
  *   0 where skipped (rgb 0 in the coarse pass with test_time).  mask_coarse / mask_fine, optional (n, 6) uint32:
  *   bit b of word w set iff sample 32 w + b is evaluated.  live_samples_host[2] receives the evaluated coarse and
  *   fine sample counts.
+ *   Appended under version 3 (perturb .. rng_ray_offset; zero-filled, the render is as before): the random inputs of
+ * nerfb200_train_samples_args, checked by the same rules, so that a render perturbs the depths and adds noise as the
+ * training step does.  perturb_rand / noise_coarse / u_rand / noise_fine are rows of this call's rays.  With
+ * rng_in_kernel, ray r of the call draws as ray rng_ray_offset + r, so a render in chunks draws what one call over
+ * all rays draws; 0 <= rng_ray_offset and rng_ray_offset + n_rays <= 2^32.
  * n_samples in {32, 64, 128}, n_importance a multiple of 32, their sum <= 192, 0 <= n_rays <= 2^22.  Synchronises
  * the stream twice (each sample count sizes the launches after it); no MLP launch for a pass without an evaluated
  * sample. */
@@ -539,6 +548,15 @@ typedef struct nerfb200_samples_args {
   float* samples_fine;
   uint32_t* mask_coarse;
   uint32_t* mask_fine;
+  float perturb;
+  float noise_std;
+  const float* perturb_rand;
+  const float* noise_coarse;
+  const float* u_rand;
+  const float* noise_fine;
+  uint64_t rng_seed;
+  int32_t rng_in_kernel;
+  int64_t rng_ray_offset;
 } nerfb200_samples_args;
 
 /* Workspace bytes of nerfb200_render_samples for n_rays rays (0 for an unsupported shape). */
@@ -565,7 +583,13 @@ int nerfb200_render_samples(const nerfb200_samples_args* args, void* ws, size_t 
  * network rgb and sigma, 0 where skipped; 16-byte aligned), mask_coarse / mask_fine (n, 6) uint32 (bit b of word w:
  * sample 32 w + b evaluated).  The backward fills, when given: dsigma_coarse / dsigma_fine (rows) and dprergb_coarse /
  * dprergb_fine (rows, 3), the per-row d loss / d sigma and d loss / d (rgb before the sigmoid) of the evaluated
- * samples, rows in ray-major, depth-index order (live_samples_host rows per pass). */
+ * samples, rows in ray-major, depth-index order (live_samples_host rows per pass).
+ *   target and loss_out are both given (the fused loss) or both null: the forward then has no loss epilogue and the
+ * backward no MSE seed (loss_grad is ignored).
+ *   Appended under version 3 (g_rgb_coarse .. g_opacity_fine; zero-filled, the step is as before): the upstream
+ * gradients of the six results, each nullable, read by both backward entries.  Per pass the seed is
+ * composite_bwd_kernel's: g = g_rgb + [target] 2 (rgb - target) / (3 n_rays) * loss_grad, g_depth, and
+ * g_opacity - [white_back] sum g.  A pass with none of them (and no target) gets exact zero gradients. */
 typedef struct nerfb200_train_samples_args {
   const float* rays;
   int64_t n_rays;
@@ -606,6 +630,12 @@ typedef struct nerfb200_train_samples_args {
   float* dsigma_fine;
   float* dprergb_coarse;
   float* dprergb_fine;
+  const float* g_rgb_coarse;
+  const float* g_depth_coarse;
+  const float* g_opacity_coarse;
+  const float* g_rgb_fine;
+  const float* g_depth_fine;
+  const float* g_opacity_fine;
 } nerfb200_train_samples_args;
 
 /* Workspace bytes for n_rays rays: sized for every sample evaluated, so one workspace serves every step of a batch

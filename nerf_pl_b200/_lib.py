@@ -125,6 +125,15 @@ class SamplesArgs(ctypes.Structure):
         ("samples_fine", c_void_p),
         ("mask_coarse", c_void_p),
         ("mask_fine", c_void_p),
+        ("perturb", c_float),
+        ("noise_std", c_float),
+        ("perturb_rand", c_void_p),
+        ("noise_coarse", c_void_p),
+        ("u_rand", c_void_p),
+        ("noise_fine", c_void_p),
+        ("rng_seed", ctypes.c_uint64),
+        ("rng_in_kernel", c_int32),
+        ("rng_ray_offset", c_int64),
     ]
 
 
@@ -171,6 +180,12 @@ class TrainSamplesArgs(ctypes.Structure):
         ("dsigma_fine", c_void_p),
         ("dprergb_coarse", c_void_p),
         ("dprergb_fine", c_void_p),
+        ("g_rgb_coarse", c_void_p),
+        ("g_depth_coarse", c_void_p),
+        ("g_opacity_coarse", c_void_p),
+        ("g_rgb_fine", c_void_p),
+        ("g_depth_fine", c_void_p),
+        ("g_opacity_fine", c_void_p),
     ]
 
 

@@ -980,6 +980,7 @@ size_t samples_carve(long long n, int Sc, int K, void* base, SkipParams* p) {
   p->row_ray = c.take<int>(rows);
   p->row_z = c.take<float>(rows);
   p->mlp_out = c.take<float>(rows * 4);
+  p->zc = c.take<float>(n * Sc);    // the perturbed coarse depths (nerfb200_render_samples uses it with perturb > 0)
   return c.off;
 }
 
@@ -1002,6 +1003,25 @@ int samples_scan(const SkipParams& sp, cudaStream_t s, long long* total) {
   TRY(launch("render_samples scan launch", cull_scan_kernel, 1, 1024, 0, s, sp.cnt, sp.ofs, static_cast<long long>(sp.n)));
   CUDA_TRY(cudaMemcpyAsync(total, sp.ofs + sp.n, sizeof(*total), cudaMemcpyDeviceToHost, s), "render_samples readback");
   CUDA_TRY(cudaStreamSynchronize(s), "render_samples readback");
+  return 0;
+}
+
+// The random inputs of both per-sample skipping entries (the fields nerfb200_samples_args and
+// nerfb200_train_samples_args share), checked and copied into p.
+template <class A>
+int skip_randoms(const A* a, const char* who, SkipParams* p) {
+  const bool fine = a->n_importance > 0;
+  if (a->rng_in_kernel < 0 || a->rng_in_kernel > 2) return fail(NERFB200_EINVAL, "%s: rng_in_kernel must be 0, 1 or 2", who);
+  if (a->rng_in_kernel == 2 && !a->rng_seed) return fail(NERFB200_EINVAL, "%s: rng_in_kernel = 2 needs rng_seed", who);
+  if (!(a->perturb >= 0.f) || !(a->noise_std >= 0.f)) return fail(NERFB200_EINVAL, "%s: perturb / noise_std < 0", who);
+  if (a->perturb > 0.f && !a->rng_in_kernel && (!a->perturb_rand || (fine && !a->u_rand)))
+    return fail(NERFB200_EINVAL, "%s: perturb>0 needs perturb_rand and u_rand", who);
+  if (a->noise_std > 0.f && (!a->noise_coarse || (fine && !a->noise_fine)))
+    return fail(NERFB200_EINVAL, "%s: noise_std>0 needs noise_coarse and noise_fine", who);
+  p->perturb = a->perturb; p->noise_std = a->noise_std;
+  p->perturb_rand = a->perturb_rand; p->u_rand = a->u_rand;
+  p->noise[0] = a->noise_coarse; p->noise[1] = a->noise_fine;
+  p->rng_seed = a->rng_seed; p->rng_in_kernel = a->rng_in_kernel;
   return 0;
 }
 
@@ -1194,18 +1214,13 @@ int train_skip_setup(const nerfb200_train_samples_args* a, void* ws, size_t byte
   SkipParams& p = w->p;
   TRY(skip_grid(a->bits, a->N, a->ranges, &p.grid, who));
   const bool fine = a->n_importance > 0;
-  if (!a->rays || !a->packed_coarse || !a->bits || !a->target || !a->loss_out || !a->rgb_coarse || !a->depth_coarse ||
+  // target and loss_out: both (the fused loss) or neither (the upstream gradients alone)
+  if (!a->rays || !a->packed_coarse || !a->bits || !a->target != !a->loss_out || !a->rgb_coarse || !a->depth_coarse ||
       !a->opacity_coarse || !ws)
     return fail(NERFB200_EINVAL, "%s: NULL argument", who);
   if (fine && (!a->packed_fine || !a->rgb_fine || !a->depth_fine || !a->opacity_fine))
     return fail(NERFB200_EINVAL, "%s: packed_fine / fine outputs are NULL with N_importance>0", who);
-  if (a->rng_in_kernel < 0 || a->rng_in_kernel > 2) return fail(NERFB200_EINVAL, "%s: rng_in_kernel must be 0, 1 or 2", who);
-  if (a->rng_in_kernel == 2 && !a->rng_seed) return fail(NERFB200_EINVAL, "%s: rng_in_kernel = 2 needs rng_seed", who);
-  if (!(a->perturb >= 0.f) || !(a->noise_std >= 0.f)) return fail(NERFB200_EINVAL, "%s: perturb / noise_std < 0", who);
-  if (a->perturb > 0.f && !a->rng_in_kernel && (!a->perturb_rand || (fine && !a->u_rand)))
-    return fail(NERFB200_EINVAL, "%s: perturb>0 needs perturb_rand and u_rand", who);
-  if (a->noise_std > 0.f && (!a->noise_coarse || (fine && !a->noise_fine)))
-    return fail(NERFB200_EINVAL, "%s: noise_std>0 needs noise_coarse and noise_fine", who);
+  TRY(skip_randoms(a, who, &p));
   if ((reinterpret_cast<uintptr_t>(a->rays) | reinterpret_cast<uintptr_t>(a->packed_coarse) |
        reinterpret_cast<uintptr_t>(a->packed_fine) | reinterpret_cast<uintptr_t>(a->samples_coarse) |
        reinterpret_cast<uintptr_t>(a->samples_fine)) & 15)
@@ -1221,10 +1236,6 @@ int train_skip_setup(const nerfb200_train_samples_args* a, void* ws, size_t byte
   p.rgb_fine = a->rgb_fine; p.depth_fine = a->depth_fine; p.opacity_fine = a->opacity_fine;
   p.z_fine = a->z_fine; p.weights_coarse = a->weights_coarse; p.weights_fine = a->weights_fine;
   p.samples[0] = a->samples_coarse; p.samples[1] = a->samples_fine;
-  p.perturb = a->perturb; p.noise_std = a->noise_std;
-  p.perturb_rand = a->perturb_rand; p.u_rand = a->u_rand;
-  p.noise[0] = a->noise_coarse; p.noise[1] = a->noise_fine;
-  p.rng_seed = a->rng_seed; p.rng_in_kernel = a->rng_in_kernel;
   p.z_coarse = a->z_coarse;
   return 0;
 }
@@ -1293,8 +1304,9 @@ int train_skip_forward(const nerfb200_train_samples_args* a, const TrainSkipWs& 
     TRY(launch(what, skip_fine_stage_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
   }
   // losses.py / metrics.py on the results, one block in a fixed order
-  TRY(launch(what, mse_psnr_kernel, 1, 1024, 0, s, p.rgb_coarse, fine ? p.rgb_fine : nullptr, a->target, n * 3,
-             a->loss_out));
+  if (a->target)
+    TRY(launch(what, mse_psnr_kernel, 1, 1024, 0, s, p.rgb_coarse, fine ? p.rgb_fine : nullptr, a->target, n * 3,
+               a->loss_out));
   uint32_t* const mask_out[2] = {a->mask_coarse, a->mask_fine};
   for (int ps = 0; ps < (fine ? 2 : 1); ++ps)
     if (mask_out[ps])
@@ -1342,6 +1354,9 @@ int train_skip_backward(const nerfb200_train_samples_args* a, const TrainSkipWs&
     bp.sigma = pb.sigma; bp.rgb = pb.rgb;
     bp.noise = p.noise_std > 0.f ? p.noise[ps] : nullptr;
     bp.noise_std = p.noise_std; bp.white_back = p.white_back;
+    bp.g_rgb = ps ? a->g_rgb_fine : a->g_rgb_coarse;
+    bp.g_depth = ps ? a->g_depth_fine : a->g_depth_coarse;
+    bp.g_opac = ps ? a->g_opacity_fine : a->g_opacity_coarse;
     bp.rgb_out = ps ? p.rgb_fine : p.rgb_coarse;
     bp.target = a->target; bp.loss_grad = loss_grad;
     bp.dsigma = pb.dsigma; bp.dprergb = pb.dprergb;
@@ -2392,12 +2407,17 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
     return fail(NERFB200_EINVAL, "render_samples: rgb_coarse / depth_coarse is NULL with test_time=0");
   if (fine && (!a->packed_fine || !a->rgb_fine || !a->depth_fine || !a->opacity_fine))
     return fail(NERFB200_EINVAL, "render_samples: packed_fine / fine outputs are NULL with N_importance>0");
+  TRY(skip_randoms(a, "render_samples", &p));
+  if (a->rng_ray_offset < 0 || a->rng_ray_offset > (1LL << 32) - a->n_rays)
+    return fail(NERFB200_EINVAL, "render_samples: rng_ray_offset must be >= 0 with rng_ray_offset + n_rays <= 2^32");
   if ((reinterpret_cast<uintptr_t>(a->rays) | reinterpret_cast<uintptr_t>(a->packed_coarse) |
        reinterpret_cast<uintptr_t>(a->packed_fine) | reinterpret_cast<uintptr_t>(a->samples_coarse) |
        reinterpret_cast<uintptr_t>(a->samples_fine)) & 15)
     return fail(NERFB200_EINVAL, "render_samples: rays, packed images and samples must be 16-byte aligned");
   if (bytes < samples_carve(a->n_rays, a->n_samples, a->n_importance, ws, &p))
     return fail(NERFB200_EINVAL, "render_samples: workspace smaller than nerfb200_samples_workspace_bytes");
+  if (!(a->perturb > 0.f)) p.zc = nullptr;     // unperturbed: every kernel takes z_base's depths
+  p.ray0 = static_cast<uint32_t>(a->rng_ray_offset);
   DeviceInfo* d = nullptr;
   TRY(device_info(&d));
   p.rays = a->rays; p.n = static_cast<int>(a->n_rays); p.live_flag = a->live_flag;

@@ -5,10 +5,11 @@
 // pdf_to_cdf_ray, inverse_cdf, merge_rank, dir_embed_term, dir_bias), so an evaluated sample has the fused kernel's
 // sigma / rgb bit for bit and a ray with nothing to skip renders as render_rays renders it.
 //
-// One set of per-ray kernels serves both callers; the render path is the training path with perturb = 0,
-// noise_std = 0 and no depth or direction-row store.  Training (train_skip_kernels.cuh) jitters the coarse depths
-// and keeps them in the workspace (zc), adds noise to the evaluated sigma, resamples with the render kernel's sorted
-// random u and writes the fp16 direction rows its MLP saves for the backward; rendering has test_time and live_flag.
+// One set of per-ray kernels serves both callers; the render path is the training path without the direction-row
+// store.  With perturb > 0 a pass jitters the coarse depths and keeps them in the workspace (zc), with noise_std > 0
+// it adds noise to the evaluated sigma, and the resampling uses the render kernel's sorted random u; training
+// (train_skip_kernels.cuh) also writes the fp16 direction rows its MLP saves for the backward, rendering has
+// test_time and live_flag.  A render in chunks keys a ray's in-kernel random numbers by its index in the whole call.
 //
 // Per chunk of rays:  classify (coarse) -> scan -> [emit -> direction bias -> coarse MLP] -> coarse stage
 // (composite, resample, merge, classify fine) -> scan -> [emit -> fine MLP] -> fine stage (composite).
@@ -57,6 +58,7 @@ struct SkipParams {
   float* rgb_fine; float* depth_fine; float* opacity_fine;
   float* z_coarse; float* z_fine; float* weights_coarse; float* weights_fine;
   float* samples[2];            // optional (n, S, 4): rgb + sigma of every sample of the pass, 0 where skipped
+  uint32_t ray0;                // in-kernel random numbers: ray r of the launch draws as ray ray0 + r (a chunk's start)
 };
 
 __device__ __forceinline__ unsigned long long skip_key(const SkipParams& p) {
@@ -74,8 +76,9 @@ __device__ __forceinline__ float skip_z(const SkipParams& p, int r, int i, float
     const float zu = (i < Sc - 1) ? z_base(nr, fr, i + 1, Sc, ud) : z;
     const float lower = (i > 0) ? __fmul_rn(0.5f, __fadd_rn(zl, z)) : z;
     const float upper = (i < Sc - 1) ? __fmul_rn(0.5f, __fadd_rn(z, zu)) : z;
-    const float pu = p.rng_in_kernel ? philox_uniform(skip_key(p), static_cast<uint32_t>(r), static_cast<uint32_t>(i), 0u)
-                                     : __ldg(p.perturb_rand + static_cast<long long>(r) * Sc + i);
+    const float pu = p.rng_in_kernel
+                         ? philox_uniform(skip_key(p), static_cast<uint32_t>(r) + p.ray0, static_cast<uint32_t>(i), 0u)
+                         : __ldg(p.perturb_rand + static_cast<long long>(r) * Sc + i);
     const float pr = __fmul_rn(p.perturb, pu);
     z = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), pr));
   }
@@ -325,7 +328,7 @@ __global__ void __launch_bounds__(kSkipWarps * 32, 9) skip_coarse_stage_kernel(S
     if (p.perturb > 0.f) {
       const unsigned long long key = p.rng_in_kernel ? skip_key(p) : 0ull;
       for (int j = lane; j < K; j += 32)
-        w.zf[j] = p.rng_in_kernel ? philox_uniform(key, static_cast<uint32_t>(r), static_cast<uint32_t>(j), 1u)
+        w.zf[j] = p.rng_in_kernel ? philox_uniform(key, static_cast<uint32_t>(r) + p.ray0, static_cast<uint32_t>(j), 1u)
                                   : __ldg(p.u_rand + r * K + j);
     }
     __syncwarp();

@@ -14,7 +14,8 @@
 
 namespace nerfb200 {
 
-// composite_bwd_kernel's arithmetic (the fused MSE seed, white_back, noise, the ReLU mask) on one ray per warp, with
+// composite_bwd_kernel's arithmetic (its seed: upstream g_rgb / g_depth / g_opac and the fused MSE term, white_back,
+// noise, the ReLU mask, in its evaluation order) on one ray per warp, with
 // sigma / rgb of an evaluated sample read from its compacted row and sigma = 0, rgb = 0 (no noise) for a skipped one.
 // d sigma / d rgb_pre go to the evaluated rows only; rows n_rows .. n_pad - 1 (padding of the last MLP tile) get 0.
 // n_rows is read on the device (the pass's total in ofs), n_pad is its multiple of 128.
@@ -31,8 +32,11 @@ struct TrainSkipBwdParams {
   const float* noise;           // (n_rays, S) or null
   float noise_std;
   int white_back;
-  const float* rgb_out;         // (n_rays, 3) rendered colour of the pass
-  const float* target;          // (n_rays, 3)
+  const float* g_rgb;           // (n_rays, 3) upstream gradient of the pass's colour or null
+  const float* g_depth;         // (n_rays) or null
+  const float* g_opac;          // (n_rays) or null
+  const float* rgb_out;         // (n_rays, 3) rendered colour of the pass, used with `target`
+  const float* target;          // (n_rays, 3) or null: adds the MSE seed 2 (rgb_out - target) / (3 n_rays) * loss_grad
   const float* loss_grad;       // device scalar dL/dloss or null (= 1)
   float* dsigma;                // (n_pad)
   float* dprergb;               // (n_pad, 3)
@@ -45,17 +49,21 @@ __global__ void __launch_bounds__(kSkipWarps * 32) train_skip_bwd_kernel(const T
   const int S = p.S, P = S >> 5;
   float amax = 0.f, amax_rgb = 0.f;
   bool nonfinite = false;
-  const float lg = (p.loss_grad != nullptr) ? *p.loss_grad : 1.f;
-  const float kseed = 2.f * lg / (3.f * static_cast<float>(p.n_rays));
   for (long long ray = static_cast<long long>(blockIdx.x) * kSkipWarps + (threadIdx.x >> 5); ray < p.n_rays;
        ray += static_cast<long long>(gridDim.x) * kSkipWarps) {
     const float* rr = p.rays + ray * 8;
     const float dx = rr[3], dy = rr[4], dz = rr[5];
     const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
-    float g[3];
+    float g[3] = {0.f, 0.f, 0.f};
+    if (p.g_rgb != nullptr) { g[0] = p.g_rgb[ray * 3]; g[1] = p.g_rgb[ray * 3 + 1]; g[2] = p.g_rgb[ray * 3 + 2]; }
+    if (p.target != nullptr) {
+      const float lg = (p.loss_grad != nullptr) ? *p.loss_grad : 1.f;
+      const float k = 2.f * lg / (3.f * static_cast<float>(p.n_rays));
 #pragma unroll
-    for (int c = 0; c < 3; ++c) g[c] = 0.f + kseed * (p.rgb_out[ray * 3 + c] - p.target[ray * 3 + c]);
-    float go = 0.f;
+      for (int c = 0; c < 3; ++c) g[c] += k * (p.rgb_out[ray * 3 + c] - p.target[ray * 3 + c]);
+    }
+    const float gd = (p.g_depth != nullptr) ? p.g_depth[ray] : 0.f;
+    float go = (p.g_opac != nullptr) ? p.g_opac[ray] : 0.f;
     if (p.white_back) go -= g[0] + g[1] + g[2];
     const float* z = p.z + ray * S;
     const uint32_t* m = p.mask + ray * kSkipMaskWords;
@@ -90,7 +98,7 @@ __global__ void __launch_bounds__(kSkipWarps * 32) train_skip_bwd_kernel(const T
       pos[q] = s > 0.f;
       tloc[q] = prod;
       prod = __fmul_rn(prod, om[q]);
-      dw[q] = g[0] * col[q][0] + g[1] * col[q][1] + g[2] * col[q][2] + 0.f * z[i] + go;
+      dw[q] = g[0] * col[q][0] + g[1] * col[q][1] + g[2] * col[q][2] + gd * z[i] + go;
     }
     float incl = prod;
 #pragma unroll

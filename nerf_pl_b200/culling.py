@@ -29,7 +29,7 @@ import torch
 
 from . import _lib
 from .nerf import packed_weights
-from .rendering import render_rays
+from .rendering import _seed_fields, render_rays
 
 RESULT_KEYS = ("rgb_coarse", "depth_coarse", "opacity_coarse", "rgb_fine", "depth_fine", "opacity_fine")
 
@@ -220,13 +220,19 @@ def check_skip(skip: str, occupancy) -> None:
 def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupancy: OccupancyGrid, N_samples: int,
                    use_disp: bool, N_importance: int, white_back: bool, test_time: bool,
                    live_flag: Optional[torch.Tensor] = None, extras: bool = False,
-                   per_sample: bool = False) -> Dict[str, torch.Tensor]:
+                   per_sample: bool = False, perturb: float = 0.0, noise_std: float = 0.0,
+                   randoms=(None, None, None, None), rng_seed=None) -> Dict[str, torch.Tensor]:
     """Render every ray of ``rays`` (n, 8) with empty samples skipped (module docstring), in chunks of
     ``_SAMPLE_CHUNK`` rays.  Returns ``render_rays``' keys for ``test_time`` / ``N_importance``, ``extras`` as
     ``render_rays`` gives them, and ``'live_samples'``: (evaluated coarse samples, evaluated fine samples).
     ``live_flag`` (n) uint8: a ray whose flag is 0 has every sample skipped.  ``per_sample`` adds
     ``'samples_coarse'`` / ``'samples_fine'`` (n, S, 4: rgb and sigma, 0 where skipped) and ``'mask_coarse'`` /
-    ``'mask_fine'`` (n, 6) int32 (bit b of word w: sample 32 w + b evaluated).  Synchronises twice per chunk."""
+    ``'mask_fine'`` (n, 6) int32 (bit b of word w: sample 32 w + b evaluated).  Synchronises twice per chunk.
+
+    ``perturb`` / ``noise_std`` > 0 render as the training step does (``render_rays(..., occupancy=)``'s graph path,
+    the same values bit for bit): ``randoms`` = (perturb_rand, noise_coarse, u_rand, noise_fine), rows of ``rays``
+    (None where not used), and ``rng_seed`` an in-kernel seed as ``rendering._resolve_randoms`` returns it, under
+    which a ray draws by its index in ``rays`` whatever the chunk."""
     S_c, K = int(N_samples), int(N_importance)
     S_f = S_c + K
     if K > 0 and len(models) < 2:
@@ -254,6 +260,12 @@ def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupa
             opt["samples_fine"] = torch.empty(n, S_f, 4, **f32)
             opt["mask_fine"] = torch.empty(n, 6, dtype=torch.int32, device=dev)
     flag = None if live_flag is None else live_flag.to(torch.uint8).contiguous()
+    pr, nc, ur, nf = [None if t is None else t.detach().to(torch.float32).contiguous() for t in randoms]
+    for name, t, cols in (("perturb_rand", pr, S_c), ("noise_coarse", nc, S_c), ("u_rand", ur, K),
+                          ("noise_fine", nf, S_f)):
+        if t is not None and (tuple(t.shape) != (n, cols) or t.device != dev):
+            raise ValueError(f"{name} must be ({n}, {cols}) on {dev}, got {tuple(t.shape)} on {t.device}")
+    rng = _seed_fields(rng_seed)
     packed = (packed_weights(models[0]), packed_weights(models[1]) if K > 0 else None)
     ws = _lib.workspace(nbytes, dev)
     counts = [0, 0]
@@ -267,7 +279,9 @@ def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupa
             use_disp=int(bool(use_disp)), white_back=int(bool(white_back)), test_time=int(bool(test_time)),
             bits=occupancy.bits.data_ptr(), N=occupancy.N, ranges=_lib.ranges_host(*[occupancy.ranges[2 * a:2 * a + 2]
                                                                                        for a in range(3)]),
-            **{k: ptr(out.get(k)) for k in RESULT_KEYS}, **{k: ptr(t) for k, t in opt.items()})
+            **{k: ptr(out.get(k)) for k in RESULT_KEYS}, **{k: ptr(t) for k, t in opt.items()},
+            perturb=float(perturb), noise_std=float(noise_std), perturb_rand=ptr(pr), noise_coarse=ptr(nc),
+            u_rand=ptr(ur), noise_fine=ptr(nf), rng_ray_offset=lo, **rng)
         _lib.call("nerfb200_render_samples", dev, ctypes.byref(args), ws.data_ptr(), ws.numel(), got)
         counts[0] += got[0]
         counts[1] += got[1]

@@ -264,7 +264,8 @@ def render_rays(models: List[torch.nn.Module],
                 randoms: Optional[Dict[str, torch.Tensor]] = None,
                 match_reference_rng: bool = True,
                 extras: bool = False,
-                autograd_impl: str = "fused") -> Dict[str, torch.Tensor]:
+                autograd_impl: str = "fused",
+                occupancy=None) -> Dict[str, torch.Tensor]:
     """Render rays with the coarse (and fine) NeRF.  Drop-in for reference
     ``models.rendering.render_rays`` (models/rendering.py:58-244): same positional arguments,
     defaults and result keys/shapes/dtypes:
@@ -281,13 +282,28 @@ def render_rays(models: List[torch.nn.Module],
     result comes from ``nerf_pl_b200.training.FusedRenderFunction`` (fused forward with activation
     capture + hand-written backward); ``autograd_impl="torch"`` selects the plain torch-op
     evaluation instead (the gradient reference used by the tests).
+
+    ``occupancy`` (a ``nerf_pl_b200.OccupancyGrid``; for a ``DensityGrid`` pass its ``.grid``) skips empty samples
+    with ``skip="samples"``'s rule (DESIGN.md "Training with empty samples skipped"): a sample in no occupied cell
+    gets sigma = 0 and no noise, is not evaluated, has weight exactly 0 and receives no gradient.  Every ray is
+    rendered.  With a gradient graph (``train_skip.render_rays_train_skip``) every returned key is differentiable,
+    the values are ``render_rays_loss(..., occupancy=)``'s for the same randoms, and neither the forward nor the
+    backward synchronises; it needs ``test_time=False``, ``extras=False``, ``autograd_impl="fused"`` and the shapes
+    of ``train_skip.check_shape`` (ValueError otherwise).  Without one (validation, evaluation) the rays go through
+    ``culling.render_samples`` with the same randoms, giving the same values bit for bit.
     """
     del chunk
     if autograd_impl not in ("fused", "torch"):
         raise ValueError("autograd_impl must be 'fused' or 'torch'")
-    _check_render_inputs("render_rays", models, embeddings, N_importance, rays)
     needs_graph = torch.is_grad_enabled() and any(
         p.requires_grad for m in models[:2] for p in m.parameters())
+    if occupancy is not None:
+        _check_grid_call(occupancy, rays, int(N_samples), int(N_importance), needs_graph, test_time, extras,
+                         autograd_impl)
+    _check_render_inputs("render_rays", models, embeddings, N_importance, rays)
+    if occupancy is not None and rays.shape[0] > 0:
+        from .train_skip import check_grid
+        check_grid(occupancy, rays)
 
     dev = rays.device
     n = rays.shape[0]
@@ -300,6 +316,9 @@ def render_rays(models: List[torch.nn.Module],
     pr, nc, ur, nf, seed = _resolve_randoms(randoms, n, S_c, K, perturb, noise_std, dev, match_reference_rng)
     if seed is not None and needs_graph and (autograd_impl == "torch" or test_time):
         raise ValueError("in-kernel random numbers are not available on the torch-autograd path")
+    if occupancy is not None and n > 0:
+        return _render_rays_grid(models, rays_c, S_c, K, use_disp, perturb, noise_std, white_back, test_time, extras,
+                                 needs_graph, occupancy, (pr, nc, ur, nf), seed)
 
     if needs_graph and extras:
         raise ValueError("extras=True is an inference-only option (no gradient graph is built for the extra tensors)")
@@ -340,6 +359,40 @@ def render_rays(models: List[torch.nn.Module],
             result["weights_fine"] = w_f
         result["weights_coarse"] = w_c
     return result
+
+
+def _check_grid_call(occupancy, rays, S_c: int, K: int, needs_graph: bool, test_time, extras, autograd_impl) -> None:
+    """The checks of render_rays(..., occupancy=) that need no device: the grid's type and, with a gradient graph,
+    the options and shapes that path supports (ValueError)."""
+    from .culling import OccupancyGrid
+    from .train_skip import check_shape
+    if not isinstance(occupancy, OccupancyGrid):
+        raise ValueError("occupancy must be a nerf_pl_b200.OccupancyGrid (for a DensityGrid pass its .grid)")
+    if not needs_graph:
+        return
+    if test_time or extras or autograd_impl != "fused":
+        raise ValueError("render_rays(..., occupancy=) with a gradient graph needs test_time=False, extras=False and "
+                         "autograd_impl='fused' (render under torch.no_grad() for the others)")
+    n = rays.shape[0]
+    if n != 0:
+        check_shape(n, S_c, K)
+
+
+def _render_rays_grid(models, rays, S_c: int, K: int, use_disp, perturb: float, noise_std: float, white_back,
+                      test_time, extras, needs_graph: bool, occupancy, randoms, seed) -> Dict[str, torch.Tensor]:
+    """render_rays(..., occupancy=) of n >= 1 rays: the differentiable skipped step without a loss, or the skipped
+    render of every ray.  Returns render_rays' keys."""
+    if needs_graph:
+        from .train_skip import render_rays_train_skip
+        live = torch.empty(2, dtype=torch.int64, device=rays.device)      # the capturable entries: no read-back
+        res = render_rays_train_skip(models, rays, S_c, use_disp, perturb, noise_std, K, white_back, *randoms, None,
+                                     occupancy, rng_seed=seed, live_samples=live)
+    else:
+        from .culling import render_samples
+        res = render_samples(models, rays, occupancy, S_c, use_disp, K, white_back, test_time, extras=extras,
+                             perturb=perturb, noise_std=noise_std, randoms=randoms, rng_seed=seed)
+    del res["live_samples"]
+    return res
 
 
 @torch.no_grad()
@@ -419,7 +472,7 @@ def render_rays_loss(models: List[torch.nn.Module],
 
     ``occupancy`` (a ``nerf_pl_b200.OccupancyGrid``) skips the empty samples of every ray (``train_skip.py``,
     DESIGN.md "Training with empty samples skipped"): the result gains ``'live_samples'`` (evaluated coarse, fine
-    samples) and only ``loss`` carries a gradient.  It needs the render kernel's shapes and at most 2^22 rays
+    samples), and every result is differentiable, as without it.  It needs the render kernel's shapes and at most 2^22 rays
     (ValueError), and a grid on the rays' device (RuntimeError); each step synchronises once, to read back
     ``live_samples`` (``CapturedTrainStep(..., occupancy=grid)`` replays the step without synchronising)."""
     del chunk

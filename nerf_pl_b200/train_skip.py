@@ -1,5 +1,5 @@
-"""The training step with empty samples skipped: ``render_rays_loss(..., occupancy=grid)`` (DESIGN.md "Training with
-empty samples skipped").
+"""The training step with empty samples skipped: ``render_rays_loss(..., occupancy=grid)`` and, without the fused loss,
+``render_rays(..., occupancy=grid)`` under a gradient graph (DESIGN.md "Training with empty samples skipped", §10g).
 
 Every ray of the batch is rendered and enters the loss; inside a ray, a sample whose point lies in no occupied cell of
 ``grid`` gets sigma = 0 (no noise is added to it) and is not evaluated, so its weight is exactly 0 and it receives no
@@ -12,7 +12,8 @@ forward : ``nerfb200_train_samples_forward`` (include/nerf_pl_b200.h): perturbed
           random resampling and the merge, the loss.  Every launch is sized for the worst case and reads the
           step's sample counts on the device; the eager call reads the two counts back once at the end.
 backward: ``nerfb200_train_samples_backward``: per network, a plan kernel turns the device count into the launch
-          parameters, then the compositing backward over the sparse sample lists and the backward of a direct
+          parameters, then the compositing backward over the sparse sample lists (seeded by the upstream gradients
+          of the pass's rgb, depth and opacity, plus the fused MSE term with a target) and the backward of a direct
           ``NeRF.forward`` call (chain, wgrad, reduction, unfold).
 capturable mode (``live_samples=`` a device tensor): the ``_dev`` entries, which neither synchronise nor read host
           memory, so ``CapturedTrainStep(occupancy=grid)`` replays the step as one CUDA graph.
@@ -90,8 +91,9 @@ def _aligned16(t: torch.Tensor) -> torch.Tensor:
 
 
 class SkipRenderFunction(torch.autograd.Function):
-    """rays + randoms + target + 48 parameter tensors -> the six result tensors + loss4.  Only the loss carries a
-    gradient: the backward is seeded by d(loss4[2])."""
+    """rays + randoms [+ target] + 48 parameter tensors -> the six result tensors [+ loss4].  Every output carries a
+    gradient: the backward's seed per pass is the upstream gradient of its rgb, depth and opacity plus, with a target,
+    the fused MSE term scaled by d(loss4[2]) (composite_bwd_kernel's seed, include/nerf_pl_b200.h)."""
 
     @staticmethod
     def forward(ctx, cfg: Dict, rays, pr, nc, ur, nf, target, *params):
@@ -102,7 +104,7 @@ class SkipRenderFunction(torch.autograd.Function):
         out = [torch.empty(n, 3, **f32), torch.empty(n, **f32), torch.empty(n, **f32)]
         if K > 0:
             out += [torch.empty(n, 3, **f32), torch.empty(n, **f32), torch.empty(n, **f32)]
-        loss_out = torch.empty(4, **f32)
+        loss_out = torch.empty(4, **f32) if target is not None else None
         if K > 0:
             blob_c, blob_f = packed_weights_pair(models[0], models[1])
         else:
@@ -124,7 +126,7 @@ class SkipRenderFunction(torch.autograd.Function):
             n_samples=S_c, n_importance=K, use_disp=int(cfg["use_disp"]), white_back=int(cfg["white_back"]),
             perturb=cfg["perturb"], noise_std=cfg["noise_std"], perturb_rand=_ptr(pr), noise_coarse=_ptr(nc),
             u_rand=_ptr(ur), noise_fine=_ptr(nf), bits=grid.bits.data_ptr(), N=grid.N,
-            ranges=(ctypes.c_double * 6)(*grid.ranges), target=target.data_ptr(), loss_out=loss_out.data_ptr(),
+            ranges=(ctypes.c_double * 6)(*grid.ranges), target=_ptr(target), loss_out=_ptr(loss_out),
             **dict(zip(_OUTPUTS, [o.data_ptr() for o in out])), **{k: _ptr(t) for k, t in extras.items()}, **rng)
         if live_dev is None:
             live = (ctypes.c_int64 * 2)()
@@ -136,13 +138,13 @@ class SkipRenderFunction(torch.autograd.Function):
             _lib.call("nerfb200_train_samples_forward_dev", dev, ctypes.byref(args), lease.ws.buf.data_ptr(),
                       lease.ws.bytes, ctypes.cast(live_dev.data_ptr(), ctypes.POINTER(ctypes.c_int64)))
             cfg["live_samples"] = live_dev
-        ctx.args, ctx.live, ctx.lease, ctx.K = args, live, lease, K
+        ctx.args, ctx.live, ctx.lease, ctx.K, ctx.has_loss = args, live, lease, K, target is not None
         # what the args point to (detached aliases of the outputs: see FusedRenderFunction)
         ctx.keep = (rays, pr, nc, ur, nf, target, [o.detach() for o in out], blob_c, blob_f, grid.bits, seed)
         ctx.n_params = len(params)
         ctx.save_for_backward(*params)
         ctx.set_materialize_grads(False)
-        return tuple(out) + (loss_out,)
+        return tuple(out) + ((loss_out,) if target is not None else ())
 
     @staticmethod
     def backward(ctx, *gouts):
@@ -150,29 +152,36 @@ class SkipRenderFunction(torch.autograd.Function):
         if lease.ws is None:
             raise RuntimeError("the backward of this render has already run (retain_graph=True is not supported)")
         n_out = 6 if ctx.K > 0 else 3
-        if any(g is not None for g in gouts[:n_out]):
-            raise RuntimeError("with occupancy=, only the returned loss carries a gradient (use the 'loss' key)")
         params = list(ctx.saved_tensors)
-        g4 = gouts[n_out]
-        if g4 is None:
+        g6 = [None if t is None else t.detach().to(torch.float32).contiguous() for t in gouts[:n_out]]
+        g4 = gouts[n_out] if ctx.has_loss else None
+        if g4 is None and all(t is None for t in g6):
             lease.release()
             return (None,) * (7 + ctx.n_params)
-        g4 = g4.detach().to(torch.float32).contiguous()
+        args = ctx.args
+        for name, t in zip(_OUTPUTS, g6):
+            setattr(args, "g_" + name, _ptr(t))
+        if g4 is None:              # no MSE term in the seed
+            args.target = args.loss_out = None
+            loss_grad = None
+        else:
+            g4 = g4.detach().to(torch.float32).contiguous()
+            loss_grad = g4.data_ptr() + 8
         dev = params[0].device
         grads, tables = _grad_buffers(params, dev)
         nets = 2 if ctx.K > 0 else 1
         (pc, gc) = tables[0]
         pf, gf = tables[1] if nets > 1 else (None, None)
         if ctx.live is None:                     # capturable: the device path writes every network's gradients
-            _lib.call("nerfb200_train_samples_backward_dev", dev, ctypes.byref(ctx.args), lease.ws.buf.data_ptr(),
-                      lease.ws.bytes, g4.data_ptr() + 8, pc, pf, gc, gf)
+            _lib.call("nerfb200_train_samples_backward_dev", dev, ctypes.byref(args), lease.ws.buf.data_ptr(),
+                      lease.ws.bytes, loss_grad, pc, pf, gc, gf)
         else:
             for ps in range(nets):
                 if ctx.live[ps] == 0:            # no evaluated sample: nothing launched for this network
                     for t in grads[24 * ps:24 * ps + 24]:
                         t.zero_()
-            _lib.call("nerfb200_train_samples_backward", dev, ctypes.byref(ctx.args), lease.ws.buf.data_ptr(),
-                      lease.ws.bytes, ctx.live, g4.data_ptr() + 8, pc, pf, gc, gf)
+            _lib.call("nerfb200_train_samples_backward", dev, ctypes.byref(args), lease.ws.buf.data_ptr(),
+                      lease.ws.bytes, ctx.live, loss_grad, pc, pf, gc, gf)
         lease.release()
         ctx.keep = ctx.args = None
         if nets == 1:
@@ -181,11 +190,12 @@ class SkipRenderFunction(torch.autograd.Function):
 
 
 def render_rays_train_skip(models, rays, N_samples, use_disp, perturb, noise_std, N_importance, white_back, pr, nc, ur,
-                           nf, target, occupancy, rng_seed=None, extras: bool = False,
+                           nf, target: Optional[torch.Tensor], occupancy, rng_seed=None, extras: bool = False,
                            workspace: Optional[SkipTrainWorkspace] = None,
                            live_samples: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
     """``render_rays_train`` with empty samples skipped: the result keys of ``render_rays_loss`` plus
-    ``'live_samples'`` (evaluated coarse, fine samples).  ``extras`` adds, for tests: ``z_vals_coarse``,
+    ``'live_samples'`` (evaluated coarse, fine samples); with ``target=None``, ``render_rays``' keys plus
+    ``'live_samples'``, without the loss.  Every result tensor is differentiable.  ``extras`` adds, for tests: ``z_vals_coarse``,
     ``z_vals_fine``, ``weights_coarse``, ``weights_fine``, ``samples_coarse`` / ``samples_fine`` (n, S, 4: network
     rgb and sigma, 0 where skipped) and ``mask_coarse`` / ``mask_fine`` ((n, 6) int32, bit b of word w: sample
     32 w + b evaluated), and ``dsigma_coarse`` / ``dsigma_fine`` (n S) and ``dprergb_coarse`` / ``dprergb_fine``
@@ -217,17 +227,19 @@ def render_rays_train_skip(models, rays, N_samples, use_disp, perturb, noise_std
                perturb=float(perturb), noise_std=float(noise_std), white_back=bool(white_back), rng_seed=rng_seed,
                extras=ex, workspace=workspace, live_out=live_samples)
     params = _params_of(models, K)
-    target = target.detach().to(torch.float32).contiguous()
-    if target.shape != (n, 3):
-        raise ValueError("target must be (N_rays, 3)")
+    if target is not None:
+        target = target.detach().to(torch.float32).contiguous()
+        if target.shape != (n, 3):
+            raise ValueError("target must be (N_rays, 3)")
     outs = SkipRenderFunction.apply(cfg, _aligned16(rays), pr, nc, ur, nf, target, *params)
     res = {"rgb_coarse": outs[0], "depth_coarse": outs[1], "opacity_coarse": outs[2]}
     k = 3
     if K > 0:
         res.update(rgb_fine=outs[3], depth_fine=outs[4], opacity_fine=outs[5])
         k = 6
-    l4 = outs[k]
-    res.update(loss=l4[2], psnr=l4[3].detach(), mse_coarse=l4[0].detach(), mse_fine=l4[1].detach())
+    if target is not None:
+        l4 = outs[k]
+        res.update(loss=l4[2], psnr=l4[3].detach(), mse_coarse=l4[0].detach(), mse_fine=l4[1].detach())
     res["live_samples"] = cfg["live_samples"]
     names = dict(z_coarse="z_vals_coarse", z_fine="z_vals_fine")
     res.update({names.get(key, key): t for key, t in ex.items()})
