@@ -51,6 +51,38 @@ def point_evaluated(x, words, N, ranges):
     return out.reshape(x.shape[:-1])
 
 
+def touched_cells(x, N, ranges):
+    """(P, 8) int64 cell indices ``(cz * M + cy) * M + cx`` of the closed cell boxes holding each float32 point of x
+    (..., 3), flattened: point_evaluated's rule with every point at once (a cell is repeated when the point touches
+    fewer than 8); -1 for a point outside the box or NaN."""
+    M = N - 1
+    flat = np.asarray(x, F32).reshape(-1, 3).astype(np.float64)
+    lo = np.array(ranges[0::2], np.float64)
+    hi = np.array(ranges[1::2], np.float64)
+    scale = float(M) / (hi - lo)
+    g = (flat - lo) * scale
+    with np.errstate(invalid="ignore"):
+        inside = ((g >= 0.0) & (g <= M)).all(1)
+    g = np.where(inside[:, None], g, 0.0)
+    f = np.floor(g)
+    fl = f.astype(np.int64)
+    c1 = np.minimum(fl, M - 1)
+    c0 = np.where((f == g) & (fl > 0), fl - 1, c1)
+    cells = np.stack([(cz[:, 2] * M + cy[:, 1]) * M + cx[:, 0]
+                      for cz in (c0, c1) for cy in (c0, c1) for cx in (c0, c1)], 1)
+    cells[~inside] = -1
+    return cells
+
+
+def point_evaluated_vec(x, words, N, ranges):
+    """point_evaluated without the loop over points."""
+    cells = touched_cells(x, N, ranges)
+    w = np.asarray(words).view(np.uint32)
+    c = np.maximum(cells, 0)
+    on = ((w[c >> 5] >> (c & 31).astype(np.uint32)) & 1) == 1
+    return (on & (cells >= 0)).any(1).reshape(np.shape(x)[:-1])
+
+
 def plain_rays(rays):
     """(R,) bool: the rays evaluated at every sample of both passes (a non-finite value or far <= near)."""
     r = np.asarray(rays, F32)
@@ -72,7 +104,7 @@ def plain_pass(rays, z):
 
 def evaluated(rays, z, words, N, ranges):
     """(R, S) bool: the evaluated samples of one pass."""
-    ev = point_evaluated(sample_points(rays, z), words, N, ranges)
+    ev = point_evaluated_vec(sample_points(rays, z), words, N, ranges)
     ev[plain_pass(rays, z)] = True
     return ev
 
@@ -84,8 +116,8 @@ def mask_bits(mask_words, S):
     return ((w[:, i >> 5] >> (i & 31).astype(np.uint32)) & 1) == 1
 
 
-def z_base(rays, S):
-    """The coarse depths of render_rays at perturb = 0 without use_disp, in the kernel's float32 steps."""
+def z_base(rays, S, use_disp=False):
+    """The coarse depths of render_rays at perturb = 0, in the kernel's float32 steps (render_kernel.cuh z_base)."""
     r = np.asarray(rays, F32)
     if S <= 1:
         t = np.zeros(S, F32)
@@ -95,4 +127,9 @@ def z_base(rays, S):
         t = np.where(i < S // 2, (step * i.astype(F32)).astype(F32),
                      (F32(1) - (step * (S - 1 - i).astype(F32)).astype(F32)).astype(F32)).astype(F32)
     omt = (F32(1) - t).astype(F32)
+    if use_disp:
+        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+            a = ((F32(1) / r[:, 6:7]).astype(F32) * omt).astype(F32)
+            b = ((F32(1) / r[:, 7:8]).astype(F32) * t).astype(F32)
+            return (F32(1) / (a + b).astype(F32)).astype(F32)
     return ((r[:, 6:7] * omt).astype(F32) + (r[:, 7:8] * t).astype(F32)).astype(F32)

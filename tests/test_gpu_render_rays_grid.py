@@ -24,7 +24,7 @@ def _nb():
 
 
 def _grads(models, K):
-    return {f"{i}.{k}": p.grad.detach().cpu().numpy().astype(np.float64)
+    return {f"{i}.{k}": (p.grad if p.grad is not None else torch.zeros_like(p)).detach().cpu().numpy().astype(np.float64)
             for i, m in enumerate(models[:2 if K else 1]) for k, p in m.named_parameters()}
 
 
@@ -80,19 +80,21 @@ def test_full_grid_is_plain_render_rays(S, K, kind, use_disp, noise, white_back,
     assert _nb()._lib.load().nerfb200_check_status() == 0
 
 
-def _autograd_reference(models, rays, got, S, K, noise_std, white_back, randoms, w):
-    """The 48 gradients of sum_k <w_k, out_k> as an autograd composition: the evaluated rows through NeRF.forward,
-    float64 torch compositing with skipped samples at sigma = 0."""
+def _autograd_reference(models, rays, got, S, K, noise_std, white_back, randoms, w, copies=(0, 0)):
+    """The 24 or 48 gradients of sum_k <w_k, out_k> as an autograd composition: the evaluated rows through
+    NeRF.forward, float64 torch compositing with skipped samples at sigma = 0 (exact zeros for a network with no
+    evaluated row).  `copies` plants ts._last_row_counted in the coarse / fine pass."""
     nb = _nb()
     n = rays.shape[0]
     loss = 0.0
-    for ps, (model, Sp) in enumerate(((models[0], S), (models[1], S + K))):
+    for ps, (model, Sp) in enumerate(((models[0], S), (models[1], S + K))[:2 if K else 1]):
         name = "coarse" if ps == 0 else "fine"
         z = got["z_vals_" + name]
         ev = torch.from_numpy(sk.mask_bits(got["mask_" + name].cpu().numpy(), Sp)).cuda()
         xyz = (rays[:, None, 0:3] + rays[:, None, 3:6] * z[:, :, None])[ev]
         d = rays[:, None, 3:6].expand(n, Sp, 3)[ev]
-        out = model(torch.cat([nb.Embedding(3, 10)(xyz), nb.Embedding(3, 4)(d)], -1))
+        x = torch.cat([nb.Embedding(3, 10)(xyz), nb.Embedding(3, 4)(d)], -1)
+        out = ts._last_row_counted(model(x), copies[ps]) if x.shape[0] else x.new_zeros(0, 4)
         s_ev = out[:, 3].double()
         if noise_std > 0:
             s_ev = s_ev + randoms["noise_" + name][ev].double() * noise_std
@@ -102,7 +104,8 @@ def _autograd_reference(models, rays, got, S, K, noise_std, white_back, randoms,
         loss = loss + (c * w["rgb_" + name]).sum() + (dep * w["depth_" + name]).sum() + (op * w["opacity_" + name]).sum()
     for m in models:
         m.zero_grad(set_to_none=True)
-    loss.backward()
+    if loss.requires_grad:
+        loss.backward()
     return _grads(models, K)
 
 

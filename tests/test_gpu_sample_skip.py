@@ -72,7 +72,7 @@ def _samples(models, rays, grid, S, K, use_disp, white_back, test_time, **kw):
     return culling.render_samples(models, rays, grid, S, use_disp, K, white_back, test_time, extras=True, **kw)
 
 
-SHAPES = [(32, 0), (32, 64), (64, 0), (64, 64), (64, 128), (128, 0), (128, 64)]
+SHAPES = [(S, K) for S in (32, 64, 128) for K in range(0, 193 - S, 32)]     # every pair samples_shape_ok accepts
 
 
 @pytest.mark.parametrize("S,K", SHAPES)
