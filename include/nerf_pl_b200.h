@@ -518,6 +518,15 @@ int nerfb200_view_batch(const uint8_t* images, int64_t V, int32_t H, int32_t W, 
  * training step does.  perturb_rand / noise_coarse / u_rand / noise_fine are rows of this call's rays.  With
  * rng_in_kernel, ray r of the call draws as ray rng_ray_offset + r, so a render in chunks draws what one call over
  * all rays draws; 0 <= rng_ray_offset and rng_ray_offset + n_rays <= 2^32.
+ *   Appended under version 3 (early_stop, cut_coarse; zero-filled, the render is as before): early ray termination
+ * of a coarse-only render (DESIGN.md §10f).  With early_stop = eps > 0 the coarse samples are evaluated in rounds of
+ * one mask word; a ray is cut after the first word k whose float64 transmittance T_k falls below eps, and the
+ * samples of its later words are treated as empty (cleared in mask_coarse, not counted in live_samples_host).
+ * Every weight up to the end of the cut word, and every output of a ray never cut, is bit for bit the render's
+ * without termination.  cut_coarse, optional (n_rays) int32: the word each ray was cut after, or -1.  Needs
+ * n_importance = 0 (NERFB200_EUNSUPPORTED) and perturb = noise_std = 0; eps in [0, 1].  With n_samples = 32 there
+ * is one word, nothing can be dropped, and the render takes the path without termination (cut_coarse is then -1).
+ * The workspace is nerfb200_samples_workspace_bytes(n_rays, n_samples, 0); the stream is synchronised once per word.
  * n_samples in {32, 64, 128}, n_importance a multiple of 32, their sum <= 192, 0 <= n_rays <= 2^22.  Synchronises
  * the stream twice (each sample count sizes the launches after it); no MLP launch for a pass without an evaluated
  * sample. */
@@ -557,6 +566,8 @@ typedef struct nerfb200_samples_args {
   uint64_t rng_seed;
   int32_t rng_in_kernel;
   int64_t rng_ray_offset;
+  float early_stop;
+  int32_t* cut_coarse;
 } nerfb200_samples_args;
 
 /* Workspace bytes of nerfb200_render_samples for n_rays rays (0 for an unsupported shape). */

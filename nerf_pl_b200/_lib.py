@@ -23,7 +23,7 @@ if os.environ.get("NERFB200_LIB"):          # a library built elsewhere (e.g. wi
 SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
            "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h", "sample_skip_kernels.cuh",
-           "train_skip_kernels.cuh", "density_kernels.cuh", "masked_grid_kernels.cuh"]
+           "train_skip_kernels.cuh", "density_kernels.cuh", "masked_grid_kernels.cuh", "early_stop_kernels.cuh"]
 INCLUDES = ["nerf_pl_b200.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -134,6 +134,8 @@ class SamplesArgs(ctypes.Structure):
         ("rng_seed", ctypes.c_uint64),
         ("rng_in_kernel", c_int32),
         ("rng_ray_offset", c_int64),
+        ("early_stop", c_float),
+        ("cut_coarse", c_void_p),
     ]
 
 

@@ -20,6 +20,7 @@
 #include "train_skip_kernels.cuh"
 #include "density_kernels.cuh"
 #include "masked_grid_kernels.cuh"
+#include "early_stop_kernels.cuh"
 
 #include <thrust/iterator/transform_iterator.h>
 
@@ -1003,6 +1004,49 @@ int samples_scan(const SkipParams& sp, cudaStream_t s, long long* total) {
   TRY(launch("render_samples scan launch", cull_scan_kernel, 1, 1024, 0, s, sp.cnt, sp.ofs, static_cast<long long>(sp.n)));
   CUDA_TRY(cudaMemcpyAsync(total, sp.ofs + sp.n, sizeof(*total), cudaMemcpyDeviceToHost, s), "render_samples readback");
   CUDA_TRY(cudaStreamSynchronize(s), "render_samples readback");
+  return 0;
+}
+
+// The coarse pass of a coarse-only render with early ray termination (early_stop_kernels.cuh), after the
+// classification: one round per mask word, then the final stage.  The per-ray state lives in the fine depths' part
+// of the workspace, which a coarse-only render does not use: T and the state (12 bytes per ray) and the row bases
+// (8 bytes per ray and word), S_c / 4 + 12 bytes per ray against zf's 4 S_c.  The rounds' rows together are the
+// evaluated samples, at most the n S_c rows carved.
+int samples_early_stop(const SkipParams& p, float eps, int32_t* cut_out, int ray_blocks, cudaStream_t s,
+                       long long* live) {
+  EarlyStop e{};
+  e.eps = eps;
+  e.words = p.Sc / 32;
+  e.base = reinterpret_cast<long long*>(p.zf);
+  e.T = reinterpret_cast<double*>(e.base + static_cast<long long>(e.words) * p.n);
+  e.state = reinterpret_cast<int*>(e.T + p.n);
+  e.cut_out = cut_out;
+  const bool coarse_rgb = p.test_time == 0;
+  TRY(launch("render_samples early_stop start launch", early_stop_start_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, e));
+  long long rows = 0;
+  bool have_bias = false;
+  for (int k = 0; k < e.words; ++k) {
+    long long n_k = 0;
+    TRY(samples_scan(p, s, &n_k));
+    if (n_k > 0) {
+      TRY(launch("render_samples early_stop emit launch", early_stop_emit_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, e,
+                 k, rows));
+      if (coarse_rgb && !have_bias) {
+        TRY(launch("render_samples dir_bias launch", skip_dir_bias_kernel, grid_blocks(p.n, 1), kDirW, 0, s, p, 0, 1));
+        have_bias = true;
+      }
+      SkipParams q = p;          // the MLP writes this round's rows only
+      q.row_ray += rows;
+      q.row_z += rows;
+      q.mlp_out += rows * (coarse_rgb ? 4 : 1);
+      TRY(samples_mlp(q, 0, n_k, !coarse_rgb, s));
+    }
+    TRY(launch("render_samples early_stop round launch", early_stop_round_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, e,
+               k, coarse_rgb ? 0 : 1));
+    rows += n_k;
+  }
+  TRY(launch("render_samples early_stop final launch", early_stop_final_kernel, ray_blocks, kSkipWarps * 32, 0, s, p, e));
+  *live = rows;
   return 0;
 }
 
@@ -2396,6 +2440,15 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
   if (!samples_shape_ok(a->n_rays, a->n_samples, a->n_importance))
     return fail(NERFB200_EUNSUPPORTED, "render_samples: needs N_samples in {32, 64, 128}, N_importance a multiple of "
                 "32, N_samples + N_importance <= 192 and 0 <= n_rays <= 2^22");
+  if (!(a->early_stop >= 0.f && a->early_stop <= 1.f))
+    return fail(NERFB200_EINVAL, "render_samples: early_stop must be in [0, 1]");
+  const bool early_stop = a->early_stop > 0.f;
+  if (early_stop && a->n_importance > 0)
+    return fail(NERFB200_EUNSUPPORTED, "render_samples: early_stop needs N_importance = 0: with importance samples "
+                "at most about 5 %% of the evaluated fine samples lie behind the cut (DESIGN.md §10f), and cutting the "
+                "coarse pass would change z_vals_fine");
+  if (early_stop && (a->perturb > 0.f || a->noise_std > 0.f))
+    return fail(NERFB200_EINVAL, "render_samples: early_stop needs perturb = 0 and noise_std = 0");
   SkipParams p{};
   TRY(skip_grid(a->bits, a->N, a->ranges, &p.grid, "render_samples"));
   live_samples_host[0] = live_samples_host[1] = 0;
@@ -2436,6 +2489,13 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
   // coarse pass
   TRY(launch("render_samples classify launch", skip_classify_kernel, ray_blocks, kSkipWarps * 32, 0, s, p));
   long long n_c = 0, n_f = 0;
+  if (early_stop && p.Sc > 32) {
+    TRY(samples_early_stop(p, a->early_stop, a->cut_coarse, ray_blocks, s, &n_c));
+    live_samples_host[0] = n_c;
+    return 0;
+  }
+  if (early_stop && a->cut_coarse)     // one word: nothing can be dropped, no ray is cut
+    CUDA_TRY(cudaMemsetAsync(a->cut_coarse, 0xff, sizeof(int32_t) * p.n, s), "render_samples cut_coarse");
   TRY(samples_scan(p, s, &n_c));
   bool have_bias = false;
   if (n_c > 0) {

@@ -216,12 +216,32 @@ def check_skip(skip: str, occupancy) -> None:
         raise ValueError("skip='samples' needs an occupancy grid")
 
 
+def check_early_stop(early_stop: float, samples: bool, N_importance: int, perturb: float = 0.0,
+                     noise_std: float = 0.0) -> float:
+    """``early_stop`` (DESIGN.md §10f) as a float; ``samples`` is whether empty samples are skipped.  A ValueError for
+    anything the coarse-only termination does not support."""
+    eps = float(early_stop)
+    if not 0.0 <= eps <= 1.0:
+        raise ValueError(f"early_stop must be in [0, 1], got {early_stop!r}")
+    if eps > 0.0:
+        if not samples:
+            raise ValueError("early_stop > 0 needs skip='samples' (occupancy= for fuse_vertex_colors)")
+        if int(N_importance) > 0:
+            raise ValueError("early_stop > 0 needs N_importance = 0: with importance samples at most about 5 % of the "
+                             "evaluated fine samples lie behind the cut (DESIGN.md §10f), and cutting the coarse pass "
+                             "would change z_vals_fine")
+        if float(perturb) != 0.0 or float(noise_std) != 0.0:
+            raise ValueError("early_stop > 0 needs perturb = 0 and noise_std = 0")
+    return eps
+
+
 @torch.no_grad()
 def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupancy: OccupancyGrid, N_samples: int,
                    use_disp: bool, N_importance: int, white_back: bool, test_time: bool,
                    live_flag: Optional[torch.Tensor] = None, extras: bool = False,
                    per_sample: bool = False, perturb: float = 0.0, noise_std: float = 0.0,
-                   randoms=(None, None, None, None), rng_seed=None) -> Dict[str, torch.Tensor]:
+                   randoms=(None, None, None, None), rng_seed=None, *,
+                   early_stop: float = 0.0) -> Dict[str, torch.Tensor]:
     """Render every ray of ``rays`` (n, 8) with empty samples skipped (module docstring), in chunks of
     ``_SAMPLE_CHUNK`` rays.  Returns ``render_rays``' keys for ``test_time`` / ``N_importance``, ``extras`` as
     ``render_rays`` gives them, and ``'live_samples'``: (evaluated coarse samples, evaluated fine samples).
@@ -232,9 +252,20 @@ def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupa
     ``perturb`` / ``noise_std`` > 0 render as the training step does (``render_rays(..., occupancy=)``'s graph path,
     the same values bit for bit): ``randoms`` = (perturb_rand, noise_coarse, u_rand, noise_fine), rows of ``rays``
     (None where not used), and ``rng_seed`` an in-kernel seed as ``rendering._resolve_randoms`` returns it, under
-    which a ray draws by its index in ``rays`` whatever the chunk."""
+    which a ray draws by its index in ``rays`` whatever the chunk.
+
+    ``early_stop`` = eps > 0 (``N_importance = 0``, ``perturb = noise_std = 0``) stops each ray once it is opaque
+    (DESIGN.md §10f): the coarse samples are evaluated in rounds of one 32-sample mask word, and a ray whose float64
+    transmittance falls below eps after a word has its later words treated as empty.  Weights up to the end of the
+    cut word are bit-identical to ``early_stop = 0``, later ones are 0, a ray never cut is bit-identical in every
+    output, and |d opacity|, |d rgb| are at most ``T_cut (1 + S 1e-10) + 4e-6`` (|d depth| that times the ray's
+    largest depth).  ``'live_samples'`` counts what was evaluated; ``per_sample`` also returns ``'cut_coarse'`` (n)
+    int32, the word each ray was cut after or -1, and the masks without the dropped words.  With ``N_samples = 32``
+    there is one word and nothing to drop: the render takes the path without termination.  It synchronises once per
+    word of each chunk."""
     S_c, K = int(N_samples), int(N_importance)
     S_f = S_c + K
+    eps = check_early_stop(early_stop, True, K, perturb, noise_std)
     if K > 0 and len(models) < 2:
         raise ValueError("N_importance > 0 needs a fine model (models[1])")
     lib = _lib.load()
@@ -259,6 +290,8 @@ def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupa
         if K > 0:
             opt["samples_fine"] = torch.empty(n, S_f, 4, **f32)
             opt["mask_fine"] = torch.empty(n, 6, dtype=torch.int32, device=dev)
+        if eps > 0.0:
+            opt["cut_coarse"] = torch.empty(n, dtype=torch.int32, device=dev)
     flag = None if live_flag is None else live_flag.to(torch.uint8).contiguous()
     pr, nc, ur, nf = [None if t is None else t.detach().to(torch.float32).contiguous() for t in randoms]
     for name, t, cols in (("perturb_rand", pr, S_c), ("noise_coarse", nc, S_c), ("u_rand", ur, K),
@@ -281,7 +314,7 @@ def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupa
                                                                                        for a in range(3)]),
             **{k: ptr(out.get(k)) for k in RESULT_KEYS}, **{k: ptr(t) for k, t in opt.items()},
             perturb=float(perturb), noise_std=float(noise_std), perturb_rand=ptr(pr), noise_coarse=ptr(nc),
-            u_rand=ptr(ur), noise_fine=ptr(nf), rng_ray_offset=lo, **rng)
+            u_rand=ptr(ur), noise_fine=ptr(nf), rng_ray_offset=lo, early_stop=eps, **rng)
         _lib.call("nerfb200_render_samples", dev, ctypes.byref(args), ws.data_ptr(), ws.numel(), got)
         counts[0] += got[0]
         counts[1] += got[1]
@@ -291,25 +324,28 @@ def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupa
             out["z_vals_fine"] = opt["z_fine"]
             out["weights_fine"] = opt["weights_fine"]
     if per_sample:
-        out.update({k: v for k, v in opt.items() if k.startswith(("samples", "mask"))})
+        out.update({k: v for k, v in opt.items() if k.startswith(("samples", "mask", "cut"))})
     out["live_samples"] = tuple(counts)
     return out
 
 
 def render_culled_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupancy: OccupancyGrid,
                           N_samples: int, use_disp: bool, N_importance: int, white_back: bool, test_time: bool,
-                          extras: bool = False, sharded: bool = False) -> Dict[str, torch.Tensor]:
+                          extras: bool = False, sharded: bool = False, *,
+                          early_stop: float = 0.0) -> Dict[str, torch.Tensor]:
     """cull -> ``render_samples(live rays)`` -> scatter, with ``'live'``, ``'live_idx'`` and ``'live_samples'``.
     With ``extras`` every ray goes through ``render_samples``, the culled ones with every sample skipped, so that the
     extra tensors are full size; their results are then the vacuum value as well.  ``sharded`` splits the live rays
-    over the ranks (``render_rays_sharded``); ``'live_samples'`` then counts this rank's samples."""
+    over the ranks (``render_rays_sharded``); ``'live_samples'`` then counts this rank's samples.  ``early_stop``:
+    as for ``render_samples``."""
+    eps = check_early_stop(early_stop, True, N_importance)
     r = _check_rays(rays, occupancy)
     keys = result_keys(int(N_importance), bool(test_time))
     counts = [0, 0]
 
     def fn(live, flag=None):
         res = render_samples(models, live, occupancy, N_samples, use_disp, N_importance, white_back, test_time,
-                             live_flag=flag, extras=extras)
+                             live_flag=flag, extras=extras, early_stop=eps)
         ls = res.pop("live_samples")
         counts[0] += ls[0]
         counts[1] += ls[1]
@@ -334,7 +370,8 @@ def render_culled_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor,
 def render_rays_culled(models: List[torch.nn.Module], embeddings: List[torch.nn.Module], rays: torch.Tensor,
                        occupancy: OccupancyGrid, N_samples: int = 64, use_disp: bool = False, N_importance: int = 0,
                        white_back: bool = False, test_time: bool = True, *, perturb: float = 0,
-                       noise_std: float = 0, skip: str = "rays", extras: bool = False) -> Dict[str, torch.Tensor]:
+                       noise_std: float = 0, skip: str = "rays", extras: bool = False,
+                       early_stop: float = 0.0) -> Dict[str, torch.Tensor]:
     """``render_rays`` at inference with empty space skipped: the same keys, shapes and dtypes, plus ``'live'``
     (the number of rays rendered) and ``'live_idx'`` (their indices, int64).  Live rays are bit-identical to
     ``render_rays(..., perturb=0, noise_std=0)``; a culled ray gets the vacuum value, an approximation whose error
@@ -345,11 +382,16 @@ def render_rays_culled(models: List[torch.nn.Module], embeddings: List[torch.nn.
     ``skip="samples"`` also skips the empty samples of the live rays (module docstring; DESIGN.md "Skipping empty
     samples"): faster, no longer bit-identical, and the result holds ``'live_samples'`` (evaluated coarse, fine
     samples).  ``extras=True`` (with ``"samples"``) adds ``weights_coarse``, ``weights_fine`` and ``z_vals_fine`` as
-    ``render_rays`` does.  It synchronises twice per chunk of ``_SAMPLE_CHUNK`` live rays."""
+    ``render_rays`` does.  It synchronises twice per chunk of ``_SAMPLE_CHUNK`` live rays.
+
+    ``early_stop`` = eps > 0 (``skip="samples"``, ``N_importance = 0``) also stops each live ray once its
+    transmittance falls below eps after a 32-sample word, within the bound ``render_samples`` states (DESIGN.md §10f);
+    0 renders exactly as without it.  With ``N_samples = 32`` there is one word and nothing to stop."""
     if float(perturb) != 0.0 or float(noise_std) != 0.0:
         raise ValueError("render_rays_culled is inference only (perturb = 0, noise_std = 0): training must see the "
                          "background rays to learn that they are empty")
     check_skip(skip, occupancy)
+    eps = check_early_stop(early_stop, skip == "samples", N_importance)
     if extras and skip != "samples":
         raise ValueError("extras=True needs skip='samples' (render_rays(..., extras=True) renders every ray)")
     r = _check_rays(rays, occupancy)
@@ -357,7 +399,7 @@ def render_rays_culled(models: List[torch.nn.Module], embeddings: List[torch.nn.
         from .rendering import _check_render_inputs
         _check_render_inputs("render_rays_culled", models, embeddings, int(N_importance), r)
         return render_culled_samples(list(models), r, occupancy, int(N_samples), use_disp, int(N_importance),
-                                     white_back, test_time, extras=extras)
+                                     white_back, test_time, extras=extras, early_stop=eps)
 
     def fn(live):
         return render_rays(list(models), list(embeddings), live, int(N_samples), use_disp, 0, 0, int(N_importance),

@@ -12,7 +12,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
-from .culling import OccupancyGrid, check_skip, render_culled, render_culled_samples, result_keys
+from .culling import OccupancyGrid, check_early_stop, check_skip, render_culled, render_culled_samples, result_keys
 from .nerf import packed_weights
 from .rendering import render_rays
 from .sharded import render_rays_sharded
@@ -49,8 +49,8 @@ def to_uint8(img: torch.Tensor) -> torch.Tensor:
 @torch.no_grad()
 def batched_inference(models: Sequence[torch.nn.Module], embeddings: Sequence[torch.nn.Module],
                       rays: torch.Tensor, N_samples: int, N_importance: int, use_disp: bool,
-                      chunk: int = 1024 * 32, white_back: bool = False, sharded: bool = False, skip: str = "rays",
-                      occupancy: Optional[OccupancyGrid] = None) -> Dict[str, torch.Tensor]:
+                      chunk: int = 1024 * 32, white_back: bool = False, sharded: bool = False, skip: str = "rays", *,
+                      early_stop: float = 0.0, occupancy: Optional[OccupancyGrid] = None) -> Dict[str, torch.Tensor]:
     """Drop-in for eval.py:58-86 batched_inference(models, embeddings, rays, N_samples,
     N_importance, use_disp, chunk, white_back): perturb=0, noise_std=0, test_time=True.  The
     reference loops over 32768-ray chunks and concatenates; here the whole image is one launch
@@ -59,15 +59,19 @@ def batched_inference(models: Sequence[torch.nn.Module], embeddings: Sequence[to
     every ray is rendered) skips empty space: only the rays that cross an occupied cell are rendered, the others
     get the vacuum value, and the result also holds ``'live'`` and ``'live_idx'`` (nerf_pl_b200.culling, which also
     says what that does and does not guarantee).  With ``sharded`` the live rays are what is split, so the ranks
-    get equal work.  ``skip="samples"`` (needs ``occupancy``; pass both by keyword) also skips the empty samples of the live rays and adds
-    ``'live_samples'`` (nerf_pl_b200.culling)."""
+    get equal work.  ``skip="samples"`` (needs ``occupancy``; pass both by keyword) also skips the empty samples of
+    the live rays and adds ``'live_samples'`` (nerf_pl_b200.culling).  ``early_stop`` and ``occupancy`` are
+    keyword-only.  ``early_stop`` = eps > 0 (``skip="samples"``, ``N_importance = 0``)
+    stops each ray once it is opaque, within a stated bound (``render_rays_culled``; DESIGN.md §10f); with
+    ``N_samples = 32`` there is nothing to stop."""
     del chunk
     check_skip(skip, occupancy)
+    eps = check_early_stop(early_stop, skip == "samples", N_importance)
     if skip == "samples":
         from .rendering import _check_render_inputs
         _check_render_inputs("batched_inference", models, embeddings, int(N_importance), rays)
         return render_culled_samples(list(models), rays, occupancy, int(N_samples), use_disp, int(N_importance),
-                                     white_back, True, sharded=sharded)
+                                     white_back, True, sharded=sharded, early_stop=eps)
 
     def fn(r):
         # eval never consumes the reference's noise draws: do not materialise them for a whole image
@@ -84,14 +88,15 @@ def batched_inference(models: Sequence[torch.nn.Module], embeddings: Sequence[to
 def render_image(models, embeddings, H: int, W: int, focal: float, c2w, near: float, far: float,
                  N_samples: int = 64, N_importance: int = 64, use_disp: bool = False, white_back: bool = False,
                  ndc: bool = False, sharded: bool = False, device=None, skip: str = "rays",
-                 occupancy: Optional[OccupancyGrid] = None) -> Dict[str, torch.Tensor]:
+                 *, early_stop: float = 0.0, occupancy: Optional[OccupancyGrid] = None) -> Dict[str, torch.Tensor]:
     """Pose -> rays -> fused render -> (H, W, 3) uint8 image + float maps, all on the device
-    (test.ipynb cell 2 / eval.py:117-128).  ``occupancy`` and ``skip``: as for ``batched_inference``; the result then
-    also holds ``'live'`` (and ``'live_samples'`` with ``skip="samples"``)."""
+    (test.ipynb cell 2 / eval.py:117-128).  ``occupancy``, ``skip`` and ``early_stop``: as for ``batched_inference``;
+    the result then also holds ``'live'`` (and ``'live_samples'`` with ``skip="samples"``)."""
     check_skip(skip, occupancy)
+    eps = check_early_stop(early_stop, skip == "samples", N_importance)
     rays = generate_rays(H, W, focal, c2w, near, far, ndc=ndc, device=device)
     res = batched_inference(models, embeddings, rays, N_samples, N_importance, use_disp, 1024 * 32, white_back,
-                            sharded=sharded, occupancy=occupancy, skip=skip)
+                            sharded=sharded, occupancy=occupancy, skip=skip, early_stop=eps)
     typ = "fine" if N_importance > 0 else "coarse"
     out = {"rays": rays, "opacity": res[f"opacity_{typ}"].view(H, W)}
     if f"rgb_{typ}" in res:

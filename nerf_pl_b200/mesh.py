@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .culling import OccupancyGrid, render_rays_culled
+from .culling import OccupancyGrid, check_early_stop, render_rays_culled
 from .inference import to_uint8
 from .nerf import Embedding, packed_weights
 from .rendering import render_rays
@@ -213,7 +213,7 @@ def project_view(vertices: torch.Tensor, image: torch.Tensor, pose, focal: float
 def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: torch.Tensor, poses: Sequence,
                        focal: float, near: float, N_samples: int = 64, occ_threshold: float = 0.2,
                        white_back: bool = False, return_opacities: bool = False, *,
-                       occupancy: Optional[OccupancyGrid] = None):
+                       occupancy: Optional[OccupancyGrid] = None, early_stop: float = 0.0):
     """extract_color_mesh.py:206-284 (the default colour-averaging method) on the device.
 
     vertices (V, 3) fp32 world; images (n_views, H, W, 3) uint8 CUDA; poses: n_views (3, 4) camera-to-world;
@@ -223,7 +223,14 @@ def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: t
     (and the per-view opacities (n_views, V) when ``return_opacities``).
 
     ``occupancy``: each view's occlusion rays are rendered by ``render_rays_culled(..., skip="samples")`` on that grid
-    instead, so density in cells it calls empty does not occlude a vertex."""
+    instead, so density in cells it calls empty does not occlude a vertex.
+
+    ``early_stop`` = eps > 0 (needs ``occupancy``) stops each occlusion ray once it is opaque (DESIGN.md §10f).  A cut
+    ray has T_cut < eps, so its terminated and its full opacity both exceed ``1 - eps - 4e-6``: for
+    ``eps <= 1 - occ_threshold - 1e-5`` no ``opacity < occ_threshold`` decision changes and the colours are
+    bit-identical to ``early_stop = 0``; the opacities move by at most ``T_cut (1 + N_samples 1e-10) + 4e-6``.
+    With ``N_samples = 32`` there is nothing to stop."""
+    eps = check_early_stop(early_stop, occupancy is not None, 0)
     v = _cuda(vertices, "vertices").detach().to(torch.float32).contiguous()
     if occupancy is not None:
         _check_occupancy(occupancy, _device_of(model))
@@ -243,7 +250,7 @@ def fuse_vertex_colors(model: torch.nn.Module, vertices: torch.Tensor, images: t
                               match_reference_rng=False)
         else:
             res = render_rays_culled([model], emb, rays, occupancy, N_samples, False, 0, white_back, True,
-                                     skip="samples")
+                                     skip="samples", early_stop=eps)
         opacity = res["opacity_coarse"].contiguous()
         if return_opacities:
             opac.append(opacity)
