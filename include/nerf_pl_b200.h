@@ -527,6 +527,8 @@ int nerfb200_view_batch(const uint8_t* images, int64_t V, int32_t H, int32_t W, 
  * n_importance = 0 (NERFB200_EUNSUPPORTED) and perturb = noise_std = 0; eps in [0, 1].  With n_samples = 32 there
  * is one word, nothing can be dropped, and the render takes the path without termination (cut_coarse is then -1).
  * The workspace is nerfb200_samples_workspace_bytes(n_rays, n_samples, 0); the stream is synchronised once per word.
+ *   Appended under version 3 (levels; zero-filled, one level as before): the occupancy grid's number of cascade
+ * levels, 1..8 (see "cascaded occupancy grids" below); bits then holds levels bit fields.
  * n_samples in {32, 64, 128}, n_importance a multiple of 32, their sum <= 192, 0 <= n_rays <= 2^22.  Synchronises
  * the stream twice (each sample count sizes the launches after it); no MLP launch for a pass without an evaluated
  * sample. */
@@ -568,6 +570,7 @@ typedef struct nerfb200_samples_args {
   int64_t rng_ray_offset;
   float early_stop;
   int32_t* cut_coarse;
+  int32_t levels;
 } nerfb200_samples_args;
 
 /* Workspace bytes of nerfb200_render_samples for n_rays rays (0 for an unsupported shape). */
@@ -600,7 +603,8 @@ int nerfb200_render_samples(const nerfb200_samples_args* args, void* ws, size_t 
  *   Appended under version 3 (g_rgb_coarse .. g_opacity_fine; zero-filled, the step is as before): the upstream
  * gradients of the six results, each nullable, read by both backward entries.  Per pass the seed is
  * composite_bwd_kernel's: g = g_rgb + [target] 2 (rgb - target) / (3 n_rays) * loss_grad, g_depth, and
- * g_opacity - [white_back] sum g.  A pass with none of them (and no target) gets exact zero gradients. */
+ * g_opacity - [white_back] sum g.  A pass with none of them (and no target) gets exact zero gradients.
+ *   Appended under version 3 (levels; zero-filled, one level as before): as nerfb200_samples_args. */
 typedef struct nerfb200_train_samples_args {
   const float* rays;
   int64_t n_rays;
@@ -647,6 +651,7 @@ typedef struct nerfb200_train_samples_args {
   const float* g_rgb_fine;
   const float* g_depth_fine;
   const float* g_opacity_fine;
+  int32_t levels;
 } nerfb200_train_samples_args;
 
 /* Workspace bytes for n_rays rays: sized for every sample evaluated, so one workspace serves every step of a batch
@@ -743,6 +748,33 @@ int nerfb200_sigma_grid_masked(const void* packed, int64_t N, const double range
 int nerfb200_rgb_sigma_grid_masked(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
                                    int64_t occ_N, const double occ_ranges_host[6], int64_t chunk, void* ws,
                                    size_t bytes, float* rgbsigma_out, int64_t* evaluated_host, void* stream);
+
+/* ==== cascaded occupancy grids ======================================================================
+ * Definition and guarantees: DESIGN.md §10h.
+ *
+ * An occupancy grid of `levels` = L levels (1 <= L <= 8) over ranges_host.  Level 0's box is ranges_host as given;
+ * for k >= 1, with c_a = 0.5 (lo_a + hi_a) and h_a = 0.5 (hi_a - lo_a) in double, level k's range on axis a is
+ * c_a -+ 2^k h_a.  Every level has N points and M = N - 1 cells per axis with the one-level cell order, and level
+ * k's ceil(M^3 / 32) words follow level k - 1's in bits (density: M^3 floats per level, the same way).  A point
+ * belongs to the smallest level whose closed box holds it, compared in that level's grid coordinates
+ * (x - lo) * M / (hi - lo); inside it the one-level rule applies; outside the last level's box, or NaN, it is empty.
+ * A cell of level k >= 1 with every index a in [ceil(M / 4), floor(3 M / 4)) lies inside level k - 1's box: it is
+ * *inner*, never reached by that rule, never evaluated, and always density 0 and bit 0.
+ *
+ * The entries above that take an occupancy or density grid's size as an int64_t (N of nerfb200_occupancy_workspace_bytes,
+ * _pack, _popcount, nerfb200_cull_count and the density grid entries, occ_N of the masked grids) read a cascade from
+ * it: NERFB200_GRID_N(N, L) keeps N in the low 32 bits and L - 1 above them, so every one-level value means what it
+ * meant.  The argument structs take `levels` instead (their N is the point count).  Then:
+ *   - nerfb200_occupancy_pack reads sigma (L, N, N, N), level k's sigma grid over level k's box; each level is marked
+ *     with its inner cells empty, dilated within the level and packed with its inner cells cleared;
+ *   - nerfb200_occupancy_popcount counts the occupied cells of every level;
+ *   - nerfb200_cull_count walks each level's box in turn, so a culled ray has no point the rule finds occupied;
+ *   - the density grid update runs steps 1-5 level by level on the level's non-inner cells in cell order (inner cells
+ *     keep density 0 and bit 0), drawing cell c of level k with element 3 k + a (level 0: the one-level points),
+ *     dilates within each level and advances the key once; nerfb200_density_points numbers the cells it evaluates
+ *     level 0's first, then each further level's non-inner cells, in cell order;
+ *   - the workspaces are those of one level (reused level by level). */
+#define NERFB200_GRID_N(N, levels) ((int64_t)(N) + ((int64_t)(levels) - 1) * ((int64_t)1 << 32))
 
 #ifdef __cplusplus
 }

@@ -4,7 +4,8 @@ signatures, executed by hand-written wgmma (sm_90a) CUDA kernels through a C-ABI
 (``include/nerf_pl_b200.h``).  See DESIGN.md and INTEGRATION.md."""
 from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_forward_torch, nerf_parameters,
                    packed_weights)
-from .culling import OccupancyGrid, cull_rays, occupancy_grid, pack_occupancy, render_rays_culled, scatter_results
+from .culling import (OccupancyGrid, cull_rays, level_ranges, occupancy_cascade, occupancy_grid, pack_occupancy,
+                      render_rays_culled, scatter_results)
 from .data import DeviceRayBatches, DeviceViewBatches
 from .density_grid import DensityGrid
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
@@ -24,6 +25,7 @@ __all__ = [
     "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
     "vertex_normals", "normal_rays", "normal_vertex_colors",
     "OccupancyGrid", "occupancy_grid", "pack_occupancy", "cull_rays", "scatter_results", "render_rays_culled",
+    "level_ranges", "occupancy_cascade",
     "DensityGrid",
     "ssim", "visualize_depth",
     "DeviceViewBatches", "Views", "read_blender_views", "read_llff_views",

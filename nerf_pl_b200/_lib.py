@@ -136,6 +136,7 @@ class SamplesArgs(ctypes.Structure):
         ("rng_ray_offset", c_int64),
         ("early_stop", c_float),
         ("cut_coarse", c_void_p),
+        ("levels", c_int32),                    # cascade levels of the occupancy grid; 0 means 1
     ]
 
 
@@ -188,6 +189,7 @@ class TrainSamplesArgs(ctypes.Structure):
         ("g_rgb_fine", c_void_p),
         ("g_depth_fine", c_void_p),
         ("g_opacity_fine", c_void_p),
+        ("levels", c_int32),
     ]
 
 
@@ -378,6 +380,12 @@ def workspace(nbytes: int, device) -> torch.Tensor:
     """Scratch of ``nbytes`` bytes (a *_workspace_bytes entry's answer) on ``device``; at least one byte, so that the
     entries always see a non-NULL pointer."""
     return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
+def grid_n(N: int, levels: int = 1) -> int:
+    """The grid size argument of the occupancy, culling, density and masked-grid entries (NERFB200_GRID_N): N points
+    per axis in the low 32 bits and ``levels - 1`` above them; ``N`` itself for one level."""
+    return int(N) + (int(levels) - 1) * (1 << 32)
 
 
 def ranges_host(x_range, y_range, z_range):

@@ -897,12 +897,30 @@ bool normals_size_ok(long long V, long long T) {
 // ------------------------------------------------------------------ empty-space skipping
 // (kernels: occupancy_kernels.cuh)
 
-// The occupancy workspace of C cells: two byte-per-cell buffers the dilation passes alternate between.
+// The occupancy workspace of C cells: two byte-per-cell buffers the dilation passes alternate between.  A cascade
+// reuses them level by level.
 size_t occupancy_carve(long long C, void* base, uint8_t* buf[2]) {
   Carver c{static_cast<uint8_t*>(base), 0, 256};
   buf[0] = c.take(C);
   buf[1] = c.take(C);
   return c.off;
+}
+
+// Dilate one level's occupancy bytes a by `dilate` cells (Chebyshev, within the level; b is the other buffer) and
+// pack them into that level's words, the inner cells [ia, ib)^3 cleared.
+int occupancy_finish(uint8_t* a, uint8_t* b, long long M, long long ia, long long ib, int32_t dilate, uint32_t* bits,
+                     cudaStream_t s, const char* dilate_what, const char* pack_what) {
+  const long long C = M * M * M;
+  // a radius of M - 1 cells already reaches across the grid
+  const int radius = static_cast<int>(dilate < M - 1 ? dilate : M - 1);
+  if (radius > 0) {
+    const long long stride[3] = {1, M, M * M};
+    for (int ax = 0; ax < 3; ++ax) {
+      TRY(launch(dilate_what, occ_dilate_axis_kernel, grid_blocks(C, 256), 256, 0, s, a, b, M, stride[ax], radius));
+      std::swap(a, b);
+    }
+  }
+  return launch(pack_what, occ_pack_kernel, grid_blocks(C, 256), 256, 0, s, a, M, ia, ib, bits);
 }
 
 // The cull workspace of n rays (kCullTile rays per tile): live rays per tile and their exclusive scan.
@@ -921,7 +939,7 @@ int cull_prepare(const float* rays, int64_t n, void* ws, size_t bytes, CullParam
   if (reinterpret_cast<uintptr_t>(rays) & 15) return fail(NERFB200_EINVAL, "%s: rays must be 16-byte aligned", who);
   if (bytes < cull_carve(n, ws, p)) return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_cull_workspace_bytes", who);
   p->rays = rays; p->n = n;
-  p->bits = nullptr; p->flag = nullptr; p->live_idx = nullptr; p->live_rays = nullptr;
+  p->grid.bits = nullptr; p->flag = nullptr; p->live_idx = nullptr; p->live_rays = nullptr;
   return 0;
 }
 
@@ -948,14 +966,62 @@ int grid_box_ok(int64_t N, const double* ranges, const char* who) {
   return 0;
 }
 
-int density_box(int64_t N, const double* ranges, DensityBox* b, const char* who) {
-  TRY(grid_box_ok(N, ranges, who));
-  for (int a = 0; a < 3; ++a) {
-    b->lo[a] = ranges[2 * a];
-    b->hi[a] = ranges[2 * a + 1];
+// Axis a of cascade level k's box (DESIGN.md §10h): the range as given at level 0; for k >= 1, with
+// c = 0.5 (lo + hi) and h = 0.5 (hi - lo) in double, c -+ 2^k h (2^k h is exact, so each end is rounded once).
+void level_range(const double* ranges, int k, int a, double* lo, double* hi) {
+  if (k == 0) {
+    *lo = ranges[2 * a];
+    *hi = ranges[2 * a + 1];
+    return;
   }
-  b->M = N - 1;
+  const double c = 0.5 * (ranges[2 * a] + ranges[2 * a + 1]), h = 0.5 * (ranges[2 * a + 1] - ranges[2 * a]);
+  const double e = std::ldexp(h, k);
+  *lo = c - e;
+  *hi = c + e;
+}
+
+// The grid size argument of the occupancy, culling, density and masked-grid entries (NERFB200_GRID_N): N points per
+// axis in its low 32 bits and levels - 1 above them, so every value the one-level entries accepted means what it
+// meant.  A negative value stays an N, which the N check rejects.
+void grid_n(int64_t v, int64_t* N, int32_t* levels) {
+  if (v < 0) {
+    *N = v;
+    *levels = 1;
+    return;
+  }
+  const int64_t hi = v >> 32;
+  *N = v & 0xffffffffLL;
+  *levels = hi < kMaxLevels ? static_cast<int32_t>(hi + 1) : kMaxLevels + 1;
+}
+
+// grid_box_ok, and 1 <= levels <= kMaxLevels with every level's box finite with min != max.
+int levels_ok(int64_t N, int32_t levels, const double* ranges, const char* who) {
+  TRY(grid_box_ok(N, ranges, who));
+  if (levels < 1 || levels > kMaxLevels) return fail(NERFB200_EINVAL, "%s: levels must be in [1, 8]", who);
+  for (int k = 1; k < levels; ++k)
+    for (int a = 0; a < 3; ++a) {
+      double lo, hi;
+      level_range(ranges, k, a, &lo, &hi);
+      if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
+        return fail(NERFB200_EINVAL, "%s: level %d's box is not finite with min != max", who, k);
+    }
   return 0;
+}
+
+int density_box(int64_t N, int32_t levels, const double* ranges, int level, DensityBox* b, const char* who) {
+  TRY(levels_ok(N, levels, ranges, who));
+  for (int a = 0; a < 3; ++a) level_range(ranges, level, a, &b->lo[a], &b->hi[a]);
+  b->M = N - 1;
+  b->level = level;
+  b->ia = level ? inner_lo(b->M) : 0;
+  b->ib = level ? std::max(inner_hi(b->M), b->ia) : 0;
+  return 0;
+}
+
+// The cells of level k an update evaluates: all of level 0, the non-inner ones of a level k >= 1.
+long long level_cells(const DensityBox& b) {
+  const long long n = b.ib - b.ia;
+  return b.M * b.M * b.M - n * n * n;
 }
 
 
@@ -1069,15 +1135,20 @@ int skip_randoms(const A* a, const char* who, SkipParams* p) {
   return 0;
 }
 
-// The occupancy grid of the per-sample skipping entries and the masked grids.
-int skip_grid(const uint32_t* bits, int64_t N, const double* ranges, SkipGrid* g, const char* who) {
-  TRY(grid_box_ok(N, ranges, who));
-  for (int ax = 0; ax < 3; ++ax) {
-    g->lo[ax] = ranges[2 * ax];
-    g->scale[ax] = static_cast<double>(N - 1) / (ranges[2 * ax + 1] - ranges[2 * ax]);
-  }
+// The occupancy grid of the cell walk, the per-sample skipping entries and the masked grids: every level's box.
+int skip_grid(const uint32_t* bits, int64_t N, int32_t levels, const double* ranges, SkipGrid* g, const char* who) {
+  TRY(levels_ok(N, levels, ranges, who));
+  for (int k = 0; k < levels; ++k)
+    for (int ax = 0; ax < 3; ++ax) {
+      double lo, hi;
+      level_range(ranges, k, ax, &lo, &hi);
+      g->lo[k][ax] = lo;
+      g->scale[k][ax] = static_cast<double>(N - 1) / (hi - lo);
+    }
   g->bits = bits;
   g->M = N - 1;
+  g->words = ceil_div(g->M * g->M * g->M, 32);
+  g->levels = levels;
   return 0;
 }
 
@@ -1104,14 +1175,17 @@ size_t masked_grid_carve(long long chunk, void* base, MaskedGridParams* p, CubSc
 
 // Both masked grids (channels 1 or 4), after the entry's own checks of N and the output.  Per chunk: classify, scan,
 // one read-back of the evaluated count; with points to evaluate, emit, the point query and the scatter.
-int masked_grid(const void* packed, int64_t N, const double* ranges, const uint32_t* bits, int64_t occ_N,
+int masked_grid(const void* packed, int64_t N, const double* ranges, const uint32_t* bits, int64_t occ_grid_N,
                 const double* occ_ranges, int64_t chunk, void* ws, size_t bytes, float* out, int64_t* evaluated_host,
                 int channels, void* stream, const char* who) {
   if (chunk < 1) return fail(NERFB200_EINVAL, "%s: chunk < 1", who);
   if (!packed || !ranges || !bits || !occ_ranges || !ws || !out || !evaluated_host)
     return fail(NERFB200_EINVAL, "%s: NULL argument", who);
   MaskedGridParams p{};
-  TRY(skip_grid(bits, occ_N, occ_ranges, &p.occ, who));
+  int64_t occ_N;
+  int32_t occ_levels;
+  grid_n(occ_grid_N, &occ_N, &occ_levels);
+  TRY(skip_grid(bits, occ_N, occ_levels, occ_ranges, &p.occ, who));
   CubScratch sc;
   if (bytes < masked_grid_carve(chunk, ws, &p, &sc))
     return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_masked_grid_workspace_bytes(chunk)", who);
@@ -1256,7 +1330,7 @@ int train_skip_setup(const nerfb200_train_samples_args* a, void* ws, size_t byte
                 "N_samples + N_importance <= 192 and 1 <= n_rays <= 2^22", who);
   std::memset(w, 0, sizeof(*w));
   SkipParams& p = w->p;
-  TRY(skip_grid(a->bits, a->N, a->ranges, &p.grid, who));
+  TRY(skip_grid(a->bits, a->N, a->levels ? a->levels : 1, a->ranges, &p.grid, who));
   const bool fine = a->n_importance > 0;
   // target and loss_out: both (the fused loss) or neither (the upstream gradients alone)
   if (!a->rays || !a->packed_coarse || !a->bits || !a->target != !a->loss_out || !a->rgb_coarse || !a->depth_coarse ||
@@ -2316,43 +2390,49 @@ int nerfb200_normal_rays(const float* vertices, const double* normals, int64_t n
 }
 
 // ---- empty-space skipping (kernels: occupancy_kernels.cuh)
-size_t nerfb200_occupancy_workspace_bytes(int64_t N) {
-  if (N < 2 || N > kVolMaxN) return 0;
+size_t nerfb200_occupancy_workspace_bytes(int64_t grid_N) {
+  int64_t N;
+  int32_t levels;
+  grid_n(grid_N, &N, &levels);
+  if (N < 2 || N > kVolMaxN || levels > kMaxLevels) return 0;
   uint8_t* buf[2];
   return occupancy_carve((N - 1) * (N - 1) * (N - 1), nullptr, buf);
 }
 
-int nerfb200_occupancy_pack(const float* sigma, int64_t N, double sigma_threshold, int32_t dilate, void* ws,
+int nerfb200_occupancy_pack(const float* sigma, int64_t grid_N, double sigma_threshold, int32_t dilate, void* ws,
                             size_t bytes, uint32_t* bits, void* stream) {
+  int64_t N;
+  int32_t levels;
+  grid_n(grid_N, &N, &levels);
   if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "occupancy_pack: N must be in [2, 1625]");
+  if (levels < 1 || levels > kMaxLevels) return fail(NERFB200_EINVAL, "occupancy_pack: levels must be in [1, 8]");
   if (dilate < 0) return fail(NERFB200_EINVAL, "occupancy_pack: dilate < 0");
   if (sigma_threshold != sigma_threshold) return fail(NERFB200_EINVAL, "occupancy_pack: sigma_threshold is NaN");
   if (!sigma || !ws || !bits) return fail(NERFB200_EINVAL, "occupancy_pack: NULL argument");
   if (bytes < nerfb200_occupancy_workspace_bytes(N))
     return fail(NERFB200_EINVAL, "occupancy_pack: workspace smaller than nerfb200_occupancy_workspace_bytes");
-  const long long M = N - 1, C = M * M * M;
+  const long long M = N - 1, C = M * M * M, words = ceil_div(C, 32);
   uint8_t* buf[2];
   occupancy_carve(C, ws, buf);
-  uint8_t *a = buf[0], *b = buf[1];
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  TRY(launch("occupancy cells launch", occ_cells_kernel, grid_blocks(C, 256), 256, 0, s, sigma, N, sigma_threshold, a));
-  // a radius of M - 1 cells already reaches across the grid
-  const int radius = static_cast<int>(dilate < M - 1 ? dilate : M - 1);
-  if (radius > 0) {
-    const long long stride[3] = {1, M, M * M};
-    for (int ax = 0; ax < 3; ++ax) {
-      TRY(launch("occupancy dilate launch", occ_dilate_axis_kernel, grid_blocks(C, 256), 256, 0, s, a, b, M, stride[ax],
-                 radius));
-      std::swap(a, b);
-    }
+  for (int k = 0; k < levels; ++k) {
+    const long long ia = k ? inner_lo(M) : 0, ib = k ? std::max(inner_hi(M), ia) : 0;
+    TRY(launch("occupancy cells launch", occ_cells_kernel, grid_blocks(C, 256), 256, 0, s, sigma + k * N * N * N, N,
+               sigma_threshold, ia, ib, buf[0]));
+    TRY(occupancy_finish(buf[0], buf[1], M, ia, ib, dilate, bits + k * words, s, "occupancy dilate launch",
+                         "occupancy pack launch"));
   }
-  return launch("occupancy pack launch", occ_pack_kernel, grid_blocks(C, 256), 256, 0, s, a, C, bits);
+  return 0;
 }
 
-int nerfb200_occupancy_popcount(const uint32_t* bits, int64_t N, int64_t* count, void* stream) {
+int nerfb200_occupancy_popcount(const uint32_t* bits, int64_t grid_N, int64_t* count, void* stream) {
+  int64_t N;
+  int32_t levels;
+  grid_n(grid_N, &N, &levels);
   if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "occupancy_popcount: N must be in [2, 1625]");
+  if (levels < 1 || levels > kMaxLevels) return fail(NERFB200_EINVAL, "occupancy_popcount: levels must be in [1, 8]");
   if (!bits || !count) return fail(NERFB200_EINVAL, "occupancy_popcount: NULL argument");
-  const long long C = (N - 1) * (N - 1) * (N - 1), words = (C + 31) / 32;
+  const long long C = (N - 1) * (N - 1) * (N - 1), words = (C + 31) / 32 * levels;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaMemsetAsync(count, 0, sizeof(*count), s), "occupancy_popcount memset");
   return launch("occupancy_popcount launch", occ_popcount_kernel, grid_blocks(words, 256), 256, 0, s, bits, words,
@@ -2364,24 +2444,21 @@ size_t nerfb200_cull_workspace_bytes(int64_t n_rays) {
   return n_rays < 0 ? 0 : cull_carve(n_rays, nullptr, &p);
 }
 
-int nerfb200_cull_count(const float* rays, int64_t n_rays, const uint32_t* bits, int64_t N,
+int nerfb200_cull_count(const float* rays, int64_t n_rays, const uint32_t* bits, int64_t grid_N,
                         const double ranges_host[6], void* ws, size_t bytes, uint8_t* flag, int64_t* n_live_host,
                         void* stream) {
+  int64_t N;
+  int32_t levels;
+  grid_n(grid_N, &N, &levels);
   CullParams p;
   TRY(cull_prepare(rays, n_rays, ws, bytes, &p, "cull_count"));
   if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "cull_count: N must be in [2, 1625]");
   if (!n_live_host || !ranges_host) return fail(NERFB200_EINVAL, "cull_count: NULL argument");
-  for (int a = 0; a < 3; ++a) {
-    const double lo = ranges_host[2 * a], hi = ranges_host[2 * a + 1];
-    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi)
-      return fail(NERFB200_EINVAL, "cull_count: every range must be finite with min != max");
-    p.lo[a] = lo;
-    p.scale[a] = static_cast<double>(N - 1) / (hi - lo);
-  }
+  TRY(skip_grid(bits, N, levels, ranges_host, &p.grid, "cull_count"));
   *n_live_host = 0;
   if (n_rays == 0) return 0;
   if (!bits || !flag) return fail(NERFB200_EINVAL, "cull_count: NULL argument");
-  p.bits = bits; p.M = N - 1; p.flag = flag;
+  p.flag = flag;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   const long long tiles = ceil_div(n_rays, kCullTile);
   TRY(launch("cull classify launch", cull_classify_kernel, grid_blocks(tiles, 1), kCullTile, 0, s, p));
@@ -2450,7 +2527,7 @@ int nerfb200_render_samples(const nerfb200_samples_args* a, void* ws, size_t byt
   if (early_stop && (a->perturb > 0.f || a->noise_std > 0.f))
     return fail(NERFB200_EINVAL, "render_samples: early_stop needs perturb = 0 and noise_std = 0");
   SkipParams p{};
-  TRY(skip_grid(a->bits, a->N, a->ranges, &p.grid, "render_samples"));
+  TRY(skip_grid(a->bits, a->N, a->levels ? a->levels : 1, a->ranges, &p.grid, "render_samples"));
   live_samples_host[0] = live_samples_host[1] = 0;
   if (a->n_rays == 0) return 0;
   const bool fine = a->n_importance > 0, coarse_rgb = a->test_time == 0;
@@ -2661,33 +2738,55 @@ int nerfb200_visualize_depth(const float* depth, int64_t h, int64_t w, int64_t s
 }
 
 // ---- the density grid (kernels: density_kernels.cuh)
-size_t nerfb200_density_workspace_bytes(int64_t N, int64_t chunk) {
-  if (N < 2 || N > kVolMaxN || chunk < 1) return 0;
+size_t nerfb200_density_workspace_bytes(int64_t grid_N, int64_t chunk) {
+  int64_t N;
+  int32_t levels;
+  grid_n(grid_N, &N, &levels);
+  if (N < 2 || N > kVolMaxN || levels > kMaxLevels || chunk < 1) return 0;
   const long long C = (N - 1) * (N - 1) * (N - 1);
   float *xyz, *sigma;
   uint8_t* buf[2];
   return density_carve(C, chunk < C ? chunk : C, nullptr, &xyz, &sigma, buf);
 }
 
-int nerfb200_density_points(int64_t N, const double ranges_host[6], const int64_t* key_dev, int64_t start,
+int nerfb200_density_points(int64_t grid_N, const double ranges_host[6], const int64_t* key_dev, int64_t start,
                             int64_t count, float* xyz, void* stream) {
-  DensityBox b;
-  TRY(density_box(N, ranges_host, &b, "density_points"));
-  const long long C = b.M * b.M * b.M;
-  if (start < 0 || count < 0 || start > C || count > C - start)
+  int64_t N;
+  int32_t levels;
+  grid_n(grid_N, &N, &levels);
+  TRY(levels_ok(N, levels, ranges_host, "density_points"));
+  long long total = 0;
+  for (int k = 0; k < levels; ++k) {
+    DensityBox b;
+    TRY(density_box(N, levels, ranges_host, k, &b, "density_points"));
+    total += level_cells(b);
+  }
+  if (start < 0 || count < 0 || start > total || count > total - start)
     return fail(NERFB200_EINVAL, "density_points: cells [start, start + count) outside the grid");
   if (count == 0) return 0;
   if (!key_dev || !xyz) return fail(NERFB200_EINVAL, "density_points: NULL argument");
-  return launch("density_points launch", density_points_kernel, grid_blocks(count, 256), 256, 0, stream, b,
-                reinterpret_cast<const long long*>(key_dev), static_cast<long long>(start), static_cast<long long>(count),
-                xyz);
+  // the points of each level the range meets, level 0's cells first, then each further level's non-inner cells
+  long long base = 0;
+  for (int k = 0; k < levels; ++k) {
+    DensityBox b;
+    TRY(density_box(N, levels, ranges_host, k, &b, "density_points"));
+    const long long Ck = level_cells(b), lo = std::max<long long>(start, base),
+                    hi = std::min<long long>(start + count, base + Ck);
+    if (lo < hi)
+      TRY(launch("density_points launch", density_points_kernel, grid_blocks(hi - lo, 256), 256, 0, stream, b,
+                 reinterpret_cast<const long long*>(key_dev), lo - base, hi - lo, xyz + (lo - start) * 3));
+    base += Ck;
+  }
+  return 0;
 }
 
-int nerfb200_density_update(const void* packed, int64_t N, const double ranges_host[6], double sigma_threshold,
+int nerfb200_density_update(const void* packed, int64_t grid_N, const double ranges_host[6], double sigma_threshold,
                             float decay, int32_t dilate, int64_t chunk, int64_t* key_dev, float* density,
                             uint32_t* bits, void* ws, size_t bytes, void* stream) {
-  DensityBox b;
-  TRY(density_box(N, ranges_host, &b, "density_update"));
+  int64_t N;
+  int32_t levels;
+  grid_n(grid_N, &N, &levels);
+  TRY(levels_ok(N, levels, ranges_host, "density_update"));
   if (sigma_threshold != sigma_threshold) return fail(NERFB200_EINVAL, "density_update: sigma_threshold is NaN");
   if (!(decay >= 0.f && decay <= 1.f)) return fail(NERFB200_EINVAL, "density_update: decay must be in [0, 1]");
   if (dilate < 0) return fail(NERFB200_EINVAL, "density_update: dilate < 0");
@@ -2695,31 +2794,31 @@ int nerfb200_density_update(const void* packed, int64_t N, const double ranges_h
   if (!packed || !key_dev || !density || !bits || !ws) return fail(NERFB200_EINVAL, "density_update: NULL argument");
   if (bytes < nerfb200_density_workspace_bytes(N, chunk))
     return fail(NERFB200_EINVAL, "density_update: workspace smaller than nerfb200_density_workspace_bytes");
-  const long long M = b.M, C = M * M * M, ch = chunk < C ? chunk : C;
+  const long long M = N - 1, C = M * M * M, ch = chunk < C ? chunk : C, words = ceil_div(C, 32);
   float *xyz, *sigma;
   uint8_t* buf[2];
   density_carve(C, ch, ws, &xyz, &sigma, buf);
-  uint8_t *a = buf[0], *o = buf[1];
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   long long* key = reinterpret_cast<long long*>(key_dev);
-  for (long long c0 = 0; c0 < C; c0 += ch) {
-    const long long n = C - c0 < ch ? C - c0 : ch;
-    TRY(nerfb200_density_points(N, ranges_host, key_dev, c0, n, xyz, stream));
-    TRY(nerfb200_query_sigma(xyz, n, 3, packed, sigma, stream));
-    TRY(launch("density decay launch", density_decay_kernel, grid_blocks(n, 256), 256, 0, s, sigma, c0, n, decay,
-               sigma_threshold, density, a, c0 + n == C ? key : nullptr));
-  }
-  // the dilation and packing of nerfb200_occupancy_pack
-  const int radius = static_cast<int>(dilate < M - 1 ? dilate : M - 1);
-  if (radius > 0) {
-    const long long stride[3] = {1, M, M * M};
-    for (int ax = 0; ax < 3; ++ax) {
-      TRY(launch("density dilate launch", occ_dilate_axis_kernel, grid_blocks(C, 256), 256, 0, s, a, o, M, stride[ax],
-                 radius));
-      std::swap(a, o);
+  for (int k = 0; k < levels; ++k) {
+    DensityBox b;
+    TRY(density_box(N, levels, ranges_host, k, &b, "density_update"));
+    const long long Ck = level_cells(b);
+    // no launch below writes the inner cells' bytes: 0 for the dilation
+    if (b.ib > b.ia) CUDA_TRY(cudaMemsetAsync(buf[0], 0, C, s), "density_update memset");
+    for (long long c0 = 0; c0 < Ck; c0 += ch) {
+      const long long n = Ck - c0 < ch ? Ck - c0 : ch;
+      TRY(launch("density_points launch", density_points_kernel, grid_blocks(n, 256), 256, 0, s, b,
+                 reinterpret_cast<const long long*>(key_dev), c0, n, xyz));
+      TRY(nerfb200_query_sigma(xyz, n, 3, packed, sigma, stream));
+      TRY(launch("density decay launch", density_decay_kernel, grid_blocks(n, 256), 256, 0, s, sigma, b, c0, n, decay,
+                 sigma_threshold, density + k * C, buf[0], k + 1 == levels && c0 + n == Ck ? key : nullptr));
     }
+    // the dilation and packing of nerfb200_occupancy_pack
+    TRY(occupancy_finish(buf[0], buf[1], M, b.ia, b.ib, dilate, bits + k * words, s, "density dilate launch",
+                         "density pack launch"));
   }
-  return launch("density pack launch", occ_pack_kernel, grid_blocks(C, 256), 256, 0, s, a, C, bits);
+  return 0;
 }
 
 // ---- grids through an occupancy grid (kernels: masked_grid_kernels.cuh)
@@ -2734,8 +2833,8 @@ int nerfb200_sigma_grid_masked(const void* packed, int64_t N, const double range
                                int64_t occ_N, const double occ_ranges_host[6], int64_t chunk, void* ws, size_t bytes,
                                float* sigma_out, int64_t* evaluated_host, void* stream) {
   if (N < 2) return fail(NERFB200_EINVAL, "sigma_grid_masked: N < 2");
-  return masked_grid(packed, N, ranges_host, bits, occ_N, occ_ranges_host, chunk, ws, bytes, sigma_out, evaluated_host,
-                     1, stream, "sigma_grid_masked");
+  return masked_grid(packed, N, ranges_host, bits, occ_N, occ_ranges_host, chunk, ws, bytes, sigma_out,
+                     evaluated_host, 1, stream, "sigma_grid_masked");
 }
 
 int nerfb200_rgb_sigma_grid_masked(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
@@ -2747,6 +2846,5 @@ int nerfb200_rgb_sigma_grid_masked(const void* packed, int64_t N, const double r
   return masked_grid(packed, N, ranges_host, bits, occ_N, occ_ranges_host, chunk, ws, bytes, rgbsigma_out,
                      evaluated_host, 4, stream, "rgb_sigma_grid_masked");
 }
-
 
 }  // extern "C"

@@ -8,16 +8,42 @@
 // (cx, cy, cz) spans [x_cx, x_cx+1] x [y_cy, y_cy+1] x [z_cz, z_cz+1] with x_j = linspace(x_range, N)[j] etc.,
 // its corners are sigma[cy + dy, cx + dx, cz + dz], its flat index is c = (cz * M + cy) * M + cx with M = N - 1
 // (x fastest), and it is bit c % 32 of word c / 32.  The bits past the last cell are 0.
+//
+// CASCADE (DESIGN.md §10h).  A grid of L levels holds L such bit fields, level k's ceil(M^3 / 32) words after level
+// k - 1's.  Level 0 is the given box; level k >= 1 has the same centre and 2^k times its half-extent.  A point
+// belongs to the smallest level whose closed box contains it; a cell of level k >= 1 whose closed box lies inside
+// level k - 1's (an *inner* cell, inner_cell) is never reached by that rule and is always 0.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
 
 namespace nerfb200 {
 
+constexpr int kMaxLevels = 8;
+
+// The occupancy grid as its readers take it: point_occupied (sample_skip_kernels.cuh) and the cell walk below.
+struct SkipGrid {
+  const uint32_t* bits;   // level k's bit field at bits + k * words
+  long long M, words;     // cells per axis; words per level
+  int levels;
+  double lo[kMaxLevels][3], scale[kMaxLevels][3];   // level k's grid coordinate g = (x - lo) * scale; box [0, M]^3
+};
+
+// Level k - 1's box is [M/4, 3M/4] on each axis of level k's grid coordinates, so cell index a of level k >= 1 is
+// inside it on that axis iff 4 a >= M and 4 (a + 1) <= 3 M: a in [inner_lo(M), inner_hi(M)).  A cell is inner iff
+// all three of its indices are.  Level 0 passes an empty range (0, 0).
+__host__ __device__ __forceinline__ long long inner_lo(long long M) { return (M + 3) / 4; }
+__host__ __device__ __forceinline__ long long inner_hi(long long M) { return 3 * M / 4; }
+__device__ __forceinline__ bool inner_cell(long long cx, long long cy, long long cz, long long ia, long long ib) {
+  return cx >= ia && cx < ib && cy >= ia && cy < ib && cz >= ia && cz < ib;
+}
+
 // ---- 1. sigma grid -> cells -> dilation -> bits ---------------------------------------------------------
 // A cell is occupied iff a corner has sigma > thr, which is "the largest of its 8 corners > thr" with a NaN
-// corner counting as not above.  The comparison is made in double, as marching cubes makes it.
-__global__ void occ_cells_kernel(const float* __restrict__ sigma, long long N, double thr, uint8_t* __restrict__ occ) {
+// corner counting as not above.  The comparison is made in double, as marching cubes makes it.  The inner cells
+// [ia, ib)^3 of a cascade level are empty, so they dilate nothing.
+__global__ void occ_cells_kernel(const float* __restrict__ sigma, long long N, double thr, long long ia, long long ib,
+                                 uint8_t* __restrict__ occ) {
   const long long M = N - 1, C = M * M * M;
   for (long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
     const long long cx = c % M, cy = (c / M) % M, cz = c / (M * M);
@@ -27,7 +53,7 @@ __global__ void occ_cells_kernel(const float* __restrict__ sigma, long long N, d
       const long long j = cx + (q & 1), i = cy + ((q >> 1) & 1), k = cz + ((q >> 2) & 1);
       any |= static_cast<double>(sigma[(i * N + j) * N + k]) > thr;
     }
-    occ[c] = any;
+    occ[c] = any && !inner_cell(cx, cy, cz, ia, ib);
   }
 }
 
@@ -46,11 +72,14 @@ __global__ void occ_dilate_axis_kernel(const uint8_t* __restrict__ in, uint8_t* 
 }
 
 // 32 cells per word by warp ballot.  The launch has a multiple of 32 threads and every lane of a warp runs the
-// same number of rounds (the bound is rounded up to a whole word).
-__global__ void occ_pack_kernel(const uint8_t* __restrict__ occ, long long C, uint32_t* __restrict__ bits) {
-  const long long C_pad = (C + 31) / 32 * 32;
+// same number of rounds (the bound is rounded up to a whole word).  The inner cells [ia, ib)^3 are cleared, which
+// the dilation may have set.
+__global__ void occ_pack_kernel(const uint8_t* __restrict__ occ, long long M, long long ia, long long ib,
+                                uint32_t* __restrict__ bits) {
+  const long long C = M * M * M, C_pad = (C + 31) / 32 * 32;
   for (long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x; c < C_pad; c += (long long)gridDim.x * blockDim.x) {
-    const unsigned w = __ballot_sync(0xffffffffu, c < C && occ[c] != 0);
+    const bool on = c < C && occ[c] != 0 && !(ia < ib && inner_cell(c % M, (c / M) % M, c / (M * M), ia, ib));
+    const unsigned w = __ballot_sync(0xffffffffu, on);
     if ((threadIdx.x & 31) == 0) bits[c >> 5] = w;
   }
 }
@@ -67,9 +96,7 @@ __global__ void occ_popcount_kernel(const uint32_t* __restrict__ bits, long long
 struct CullParams {
   const float* rays;      // (n, 8) [o, d, near, far]
   long long n;
-  const uint32_t* bits;
-  long long M;            // cells per axis
-  double lo[3], scale[3]; // grid coordinate g = (p - lo) * scale, scale = M / (hi - lo): the box is [0, M]^3
+  SkipGrid grid;
   uint8_t* flag;          // (n)
   int* tcnt;              // live rays of each tile
   long long* tofs;        // exclusive scan of tcnt, n_tiles + 1
@@ -79,25 +106,18 @@ struct CullParams {
 
 constexpr int kCullTile = 256;   // rays per tile = threads per block
 
-// Live iff the segment o + t d, t in [near, far], crosses an occupied cell.  Amanatides-Woo in grid coordinates,
-// in double; each boundary time is recomputed from the cell index, so no error accumulates along the walk.
-// Space outside the box is empty.  A ray the walk cannot judge (a non-finite value, far <= near) is live: the
-// renderer then sees it unchanged.
-__device__ __forceinline__ bool cull_ray_live(const CullParams& p, const float* r) {
-  float v[8];
-#pragma unroll
-  for (int a = 0; a < 8; ++a) v[a] = r[a];
-  bool finite = true;
-#pragma unroll
-  for (int a = 0; a < 8; ++a) finite &= isfinite(v[a]);
-  if (!finite || !(v[7] > v[6])) return true;
-  const double M = static_cast<double>(p.M);
+// Whether the segment o + t d, t in [near, far] (v: a finite ray with far > near) crosses an occupied cell of level
+// k.  Amanatides-Woo in grid coordinates, in double; each boundary time is recomputed from the cell index, so no
+// error accumulates along the walk.  Space outside the level's box is empty.
+__device__ __forceinline__ bool cull_level_live(const SkipGrid& g, int k, const float v[8]) {
+  const double M = static_cast<double>(g.M);
+  const uint32_t* bits = g.bits + k * g.words;
   double o[3], d[3], inv[3];
   double t0 = v[6], t1 = v[7];
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
-    o[a] = (static_cast<double>(v[a]) - p.lo[a]) * p.scale[a];
-    d[a] = static_cast<double>(v[3 + a]) * p.scale[a];
+    o[a] = (static_cast<double>(v[a]) - g.lo[k][a]) * g.scale[k][a];
+    d[a] = static_cast<double>(v[3 + a]) * g.scale[k][a];
     if (d[a] == 0.0) {
       inv[a] = 0.0;
       if (o[a] < 0.0 || o[a] > M) return false;
@@ -117,10 +137,10 @@ __device__ __forceinline__ bool cull_ray_live(const CullParams& p, const float* 
     cell[a] = static_cast<long long>(fmin(fmax(g, 0.0), M - 1.0));
   }
   const double inf = __longlong_as_double(0x7ff0000000000000LL);
-  const long long steps = 3 * p.M + 3;
+  const long long steps = 3 * g.M + 3;
   for (long long s = 0; s < steps; ++s) {
-    const long long c = (cell[2] * p.M + cell[1]) * p.M + cell[0];
-    if ((p.bits[c >> 5] >> (c & 31)) & 1u) return true;
+    const long long c = (cell[2] * g.M + cell[1]) * g.M + cell[0];
+    if ((bits[c >> 5] >> (c & 31)) & 1u) return true;
 #pragma unroll
     for (int a = 0; a < 3; ++a)
       tnext[a] = d[a] == 0.0 ? inf : (static_cast<double>(cell[a] + (d[a] > 0.0 ? 1 : 0)) - o[a]) * inv[a];
@@ -131,9 +151,25 @@ __device__ __forceinline__ bool cull_ray_live(const CullParams& p, const float* 
       if (a != ax) continue;
       if (!(tnext[a] <= t1)) return false;
       cell[a] += d[a] > 0.0 ? 1 : -1;
-      if (cell[a] < 0 || cell[a] >= p.M) return false;
+      if (cell[a] < 0 || cell[a] >= g.M) return false;
     }
   }
+  return false;
+}
+
+// Live iff the segment crosses an occupied cell of some level: the walk of each level's box in turn.  Inner cells
+// are 0, so this finds every cell point_occupied can find.  A ray the walk cannot judge (a non-finite value,
+// far <= near) is live: the renderer then sees it unchanged.
+__device__ __forceinline__ bool cull_ray_live(const CullParams& p, const float* r) {
+  float v[8];
+#pragma unroll
+  for (int a = 0; a < 8; ++a) v[a] = r[a];
+  bool finite = true;
+#pragma unroll
+  for (int a = 0; a < 8; ++a) finite &= isfinite(v[a]);
+  if (!finite || !(v[7] > v[6])) return true;
+  for (int k = 0; k < p.grid.levels; ++k)
+    if (cull_level_live(p.grid, k, v)) return true;
   return false;
 }
 

@@ -16,17 +16,12 @@
 // The per-ray kernels run one warp per ray in grid-stride order, so no result depends on the launch shape.
 #pragma once
 #include "aux_kernels.cuh"
+#include "occupancy_kernels.cuh"
 
 namespace nerfb200 {
 
 constexpr int kSkipMaskWords = kMaxSf / 32;   // evaluated-sample bits of one ray and pass: bit i of word w = sample 32 w + i
 constexpr int kSkipWarps = 4;                 // rays (warps) per block of the per-ray kernels
-
-struct SkipGrid {
-  const uint32_t* bits;   // occupancy bit field (occupancy_kernels.cuh: cell (cz * M + cy) * M + cx)
-  long long M;            // cells per axis
-  double lo[3], scale[3]; // grid coordinate g = (x - lo) * scale; the box is [0, M]^3
-};
 
 struct SkipParams {
   const float* rays;            // (n, 8) [o, d, near, far], 16-byte aligned
@@ -87,25 +82,39 @@ __device__ __forceinline__ float skip_z(const SkipParams& p, int r, int i, float
 
 __device__ __forceinline__ bool mask_bit(const uint32_t* m, int i) { return (m[i >> 5] >> (i & 31)) & 1u; }
 
-// Whether the point x lies in the closed box of an occupied cell.  In grid coordinates, compared in double; a
-// coordinate on a cell boundary belongs to both cells, so a point on a shared face, edge or corner checks every
-// cell that touches it.  Outside the box [0, M]^3 (and for a NaN) nothing is occupied.
+// Whether the point x lies in the closed box of an occupied cell of its level: the smallest level whose closed box
+// [0, M]^3 holds its grid coordinates.  In grid coordinates, compared in double; a coordinate on a cell boundary
+// belongs to both cells, so a point on a shared face, edge or corner checks every cell that touches it.  Outside
+// the last level's box (and for a NaN) nothing is occupied.
 __device__ __forceinline__ bool point_occupied(const SkipGrid& g, const float x[3]) {
+  const double Md = static_cast<double>(g.M);
+  double v[3];
+  int k = 0;
+#pragma unroll 1
+  for (;; ++k) {
+    if (k == g.levels) return false;
+    bool in = true;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      v[a] = (static_cast<double>(x[a]) - g.lo[k][a]) * g.scale[k][a];
+      in &= v[a] >= 0.0 && v[a] <= Md;
+    }
+    if (in) break;
+  }
+  const uint32_t* bits = g.bits + k * g.words;
   long long c0[3], c1[3];
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
-    const double v = (static_cast<double>(x[a]) - g.lo[a]) * g.scale[a];
-    if (!(v >= 0.0 && v <= static_cast<double>(g.M))) return false;
-    const double f = floor(v);
+    const double f = floor(v[a]);
     const long long fl = static_cast<long long>(f);
     c1[a] = fl < g.M - 1 ? fl : g.M - 1;
-    c0[a] = (f == v && fl > 0) ? fl - 1 : c1[a];
+    c0[a] = (f == v[a] && fl > 0) ? fl - 1 : c1[a];
   }
   for (long long cz = c0[2]; cz <= c1[2]; ++cz)
     for (long long cy = c0[1]; cy <= c1[1]; ++cy)
       for (long long cx = c0[0]; cx <= c1[0]; ++cx) {
         const long long c = (cz * g.M + cy) * g.M + cx;
-        if ((__ldg(g.bits + (c >> 5)) >> (c & 31)) & 1u) return true;
+        if ((__ldg(bits + (c >> 5)) >> (c & 31)) & 1u) return true;
       }
   return false;
 }

@@ -19,10 +19,16 @@ adds a margin, but sigma is only sampled at the grid points and the trained sigm
 zero: the error of a culled pixel is an empirical bound governed by ``N``, ``sigma_threshold`` and ``dilate``, not
 a proof.  Space outside the grid's box counts as empty.  Culling is for inference only: training must see the
 background rays to learn that they are empty.
+
+``levels = L > 1`` makes the grid a cascade (DESIGN.md §10h): level 0 is the given box and level k has the same
+centre and ``2^k`` times its half-extent, each with the same ``N``.  A point belongs to the smallest level whose box
+holds it, so a 360° scene keeps fine cells on the object and coarse ones over the background it would otherwise
+lose; only space outside the last level counts as empty.  Every consumer takes the grid as it is.
 """
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Callable, Dict, List, Optional, Sequence
 
 import torch
@@ -32,52 +38,102 @@ from .nerf import packed_weights
 from .rendering import _seed_fields, render_rays
 
 RESULT_KEYS = ("rgb_coarse", "depth_coarse", "opacity_coarse", "rgb_fine", "depth_fine", "opacity_fine")
+MAX_LEVELS = 8
+
+
+def level_ranges(x_range, y_range, z_range, level: int):
+    """The (x_range, y_range, z_range) of cascade level ``level``: the ranges as given at level 0; for k >= 1, with
+    ``c = 0.5 (lo + hi)`` and ``h = 0.5 (hi - lo)`` in float64, ``(c - 2^k h, c + 2^k h)`` per axis."""
+    r = tuple(_lib.ranges_host(x_range, y_range, z_range))
+    if level == 0:
+        return r[0:2], r[2:4], r[4:6]
+    out = []
+    for a in range(3):
+        lo, hi = r[2 * a], r[2 * a + 1]
+        c, h = 0.5 * (lo + hi), 0.5 * (hi - lo)
+        e = math.ldexp(h, int(level))
+        out.append((c - e, c + e))
+    return tuple(out)
+
+
+def inner_cells(N: int, level: int):
+    """The inner cell indices ``[a, b)`` of one axis of a level: a cell of level k >= 1 whose indices all lie in
+    it is inside level k - 1's box, never looked up and always empty.  ``(0, 0)`` at level 0."""
+    M = int(N) - 1
+    if level == 0:
+        return 0, 0
+    a = (M + 3) // 4
+    return a, max(3 * M // 4, a)
+
+
+def _check_levels(levels, who: str) -> int:
+    if int(levels) != levels or not 1 <= int(levels) <= MAX_LEVELS:
+        raise ValueError(f"{who}: levels = {levels!r} must be an int in [1, {MAX_LEVELS}]")
+    return int(levels)
 
 
 class OccupancyGrid:
     """The occupied cells of a ``N``-point grid over ``x_range x y_range x z_range``: ``bits`` is a CUDA tensor of
     ``ceil((N-1)^3 / 32)`` uint32 words (stored as int32), one bit per cell, x fastest.  Cell ``(cx, cy, cz)`` spans
     ``[x_cx, x_cx+1] x [y_cy, y_cy+1] x [z_cz, z_cz+1]`` of ``np.linspace(*range, N)``; note that ``nb.sigma_grid``
-    indexes ``[y, x, z]``, and this object does not."""
+    indexes ``[y, x, z]``, and this object does not.
 
-    def __init__(self, bits: torch.Tensor, N: int, x_range, y_range, z_range, dilate: int = 0):
+    ``levels = L > 1``: a cascade (module docstring) of L such bit fields, level k's words after level k - 1's, each
+    over ``level_ranges(..., k)``; the inner cells of levels k >= 1 (``inner_cells``) are 0."""
+
+    def __init__(self, bits: torch.Tensor, N: int, x_range, y_range, z_range, dilate: int = 0, levels: int = 1):
         N = int(N)
         if not 2 <= N <= 1625:
             raise ValueError(f"OccupancyGrid: N = {N} outside [2, 1625]")
+        levels = _check_levels(levels, "OccupancyGrid")
         words = ((N - 1) ** 3 + 31) // 32
         if not isinstance(bits, torch.Tensor) or not bits.is_cuda:
             raise RuntimeError("OccupancyGrid: bits must be a CUDA tensor (nerf_pl_b200 has no CPU fallback)")
-        if bits.dtype not in (torch.int32, torch.uint32) or bits.numel() != words:
-            raise ValueError(f"OccupancyGrid: bits must hold {words} 32-bit words")
+        if bits.dtype not in (torch.int32, torch.uint32) or bits.numel() != words * levels:
+            raise ValueError(f"OccupancyGrid: bits must hold {words * levels} 32-bit words")
         self.bits = bits.contiguous().view(torch.int32).reshape(-1)
         self.N = N
         self.ranges = tuple(_lib.ranges_host(x_range, y_range, z_range))
         if any(self.ranges[2 * a] == self.ranges[2 * a + 1] for a in range(3)):
             raise ValueError("OccupancyGrid: every range needs min != max")
         self.dilate = int(dilate)
+        self.levels = levels
 
     @property
     def device(self) -> torch.device:
         return self.bits.device
 
+    def grid_n(self) -> int:
+        """The grid size argument of the C entries (``_lib.grid_n``): N, with the level count above it."""
+        return _lib.grid_n(self.N, self.levels)
+
     def n_cells(self) -> int:
-        return (self.N - 1) ** 3
+        """The cells a point can be looked up in: every cell of level 0, the non-inner ones of the other levels."""
+        a, b = inner_cells(self.N, 1)
+        return self.levels * (self.N - 1) ** 3 - (self.levels - 1) * (b - a) ** 3
 
     def occupied_fraction(self) -> float:
-        """Occupied cells over all cells (a popcount reduction on the device)."""
+        """Occupied cells over ``n_cells()`` (a popcount reduction on the device)."""
         count = torch.empty(1, dtype=torch.int64, device=self.device)
-        _lib.call("nerfb200_occupancy_popcount", self.device, self.bits.data_ptr(), self.N, count.data_ptr())
+        _lib.call("nerfb200_occupancy_popcount", self.device, self.bits.data_ptr(), self.grid_n(), count.data_ptr())
         return int(count.item()) / self.n_cells()
 
     def to_dense(self) -> torch.Tensor:
-        """(N-1, N-1, N-1) bool, indexed ``[cx, cy, cz]`` (for tests and inspection)."""
+        """(N-1, N-1, N-1) bool, indexed ``[cx, cy, cz]`` (for tests and inspection); a cascade has a leading level
+        axis, (L, N-1, N-1, N-1)."""
         M = self.N - 1
         shifts = torch.arange(32, dtype=torch.int32, device=self.device)
-        flat = ((self.bits[:, None] >> shifts) & 1).reshape(-1)[:M ** 3].bool()
-        return flat.view(M, M, M).permute(2, 1, 0).contiguous()
+        words = self.bits.view(self.levels, -1)
+        flat = ((words[:, :, None] >> shifts) & 1).reshape(self.levels, -1)[:, :M ** 3].bool()
+        dense = flat.view(self.levels, M, M, M).permute(0, 3, 2, 1).contiguous()
+        return dense[0] if self.levels == 1 else dense
 
     def state_dict(self) -> Dict[str, object]:
-        return {"bits": self.bits.detach().cpu(), "N": self.N, "ranges": tuple(self.ranges), "dilate": self.dilate}
+        """The grid's state; ``levels`` only for a cascade, so a one-level grid saves what it always saved."""
+        st = {"bits": self.bits.detach().cpu(), "N": self.N, "ranges": tuple(self.ranges), "dilate": self.dilate}
+        if self.levels > 1:
+            st["levels"] = self.levels
+        return st
 
     def load_state_dict(self, state: Dict[str, object]) -> "OccupancyGrid":
         self.__dict__.update(OccupancyGrid.from_state_dict(state, self.device).__dict__)
@@ -87,29 +143,36 @@ class OccupancyGrid:
     def from_state_dict(cls, state: Dict[str, object], device="cuda") -> "OccupancyGrid":
         """The grid of a ``state_dict()`` saved beside a checkpoint, on ``device``."""
         r = tuple(state["ranges"])
-        return cls(torch.as_tensor(state["bits"]).to(device), state["N"], r[0:2], r[2:4], r[4:6], state["dilate"])
+        return cls(torch.as_tensor(state["bits"]).to(device), state["N"], r[0:2], r[2:4], r[4:6], state["dilate"],
+                   state.get("levels", 1))
 
 
 @torch.no_grad()
 def pack_occupancy(sigma: torch.Tensor, x_range, y_range, z_range, sigma_threshold: float,
-                   dilate: int = 1) -> OccupancyGrid:
+                   dilate: int = 1, levels: int = 1) -> OccupancyGrid:
     """The occupancy grid of a CUDA (N, N, N) sigma grid in ``nb.sigma_grid``'s order (``sigma[i, j, k] =
     sigma(x_j, y_i, z_k)``): a cell is occupied iff the largest sigma of its 8 corners is ``> sigma_threshold``; the
-    set is dilated by ``dilate`` cells in Chebyshev distance and packed."""
+    set is dilated by ``dilate`` cells in Chebyshev distance and packed.
+
+    ``levels = L > 1``: sigma is (L, N, N, N), level k's grid over ``level_ranges(..., k)``; each level is marked
+    with its inner cells empty, dilated within the level and packed with its inner cells cleared."""
+    levels = _check_levels(levels, "pack_occupancy")
     if not isinstance(sigma, torch.Tensor) or not sigma.is_cuda:
         raise RuntimeError("pack_occupancy: sigma must be a CUDA tensor (nerf_pl_b200 has no CPU fallback)")
-    if sigma.dim() != 3 or not (sigma.shape[0] == sigma.shape[1] == sigma.shape[2]):
-        raise ValueError("sigma must be (N, N, N)")
+    cube = sigma.shape[-3:]
+    if sigma.dim() != (3 if levels == 1 else 4) or not (cube[0] == cube[1] == cube[2]) or \
+            (levels > 1 and sigma.shape[0] != levels):
+        raise ValueError("sigma must be (N, N, N)" if levels == 1 else f"sigma must be ({levels}, N, N, N)")
     s = sigma.detach().to(torch.float32).contiguous()
-    N = s.shape[0]
+    N = s.shape[-1]
     nbytes = _lib.load().nerfb200_occupancy_workspace_bytes(N)
     if nbytes == 0:
         raise ValueError(f"pack_occupancy: N = {N} outside [2, 1625]")
     ws = _lib.workspace(nbytes, s.device)
-    bits = torch.empty(((N - 1) ** 3 + 31) // 32, dtype=torch.int32, device=s.device)
-    _lib.call("nerfb200_occupancy_pack", s.device, s.data_ptr(), N, float(sigma_threshold), int(dilate), ws.data_ptr(),
-              ws.numel(), bits.data_ptr())
-    return OccupancyGrid(bits, N, x_range, y_range, z_range, dilate)
+    bits = torch.empty(levels * (((N - 1) ** 3 + 31) // 32), dtype=torch.int32, device=s.device)
+    _lib.call("nerfb200_occupancy_pack", s.device, s.data_ptr(), _lib.grid_n(N, levels), float(sigma_threshold),
+              int(dilate), ws.data_ptr(), ws.numel(), bits.data_ptr())
+    return OccupancyGrid(bits, N, x_range, y_range, z_range, dilate, levels)
 
 
 @torch.no_grad()
@@ -119,10 +182,24 @@ def occupancy_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, si
     points, with ``N`` and the ranges as for mesh extraction, then ``pack_occupancy``.  The float sigma grid is
     transient.  A ray that only crosses unoccupied cells will be given the vacuum value, so choose
     ``sigma_threshold`` well below the density of anything visible (see the module docstring for what is and is
-    not guaranteed)."""
+    not guaranteed).  ``occupancy_cascade`` builds a cascade."""
+    return occupancy_cascade(model, N, x_range, y_range, z_range, sigma_threshold, 1, dilate, chunk)
+
+
+@torch.no_grad()
+def occupancy_cascade(model: torch.nn.Module, N: int, x_range, y_range, z_range, sigma_threshold: float, levels: int,
+                      dilate: int = 1, chunk: int = 1 << 21) -> OccupancyGrid:
+    """``occupancy_grid`` with ``levels`` cascade levels (module docstring) around the box of ``x_range x y_range x
+    z_range``: ``nb.sigma_grid`` on each level's box (``level_ranges``), L N^3 points, then
+    ``pack_occupancy(..., levels=levels)``.  ``levels = 1`` is ``occupancy_grid``."""
     from .mesh import sigma_grid     # mesh imports inference, which imports this module
-    sigma = sigma_grid(model, int(N), x_range, y_range, z_range, chunk)
-    grid = pack_occupancy(sigma, x_range, y_range, z_range, sigma_threshold, dilate)
+    levels = _check_levels(levels, "occupancy_cascade")
+    if levels == 1:
+        sigma = sigma_grid(model, int(N), x_range, y_range, z_range, chunk)
+    else:
+        sigma = torch.stack([sigma_grid(model, int(N), *level_ranges(x_range, y_range, z_range, k), chunk)
+                             for k in range(levels)])
+    grid = pack_occupancy(sigma, x_range, y_range, z_range, sigma_threshold, dilate, levels)
     del sigma
     return grid
 
@@ -150,7 +227,7 @@ def cull_rays(rays: torch.Tensor, occupancy: OccupancyGrid, return_flag: bool = 
     ws = _lib.workspace(_lib.load().nerfb200_cull_workspace_bytes(n), dev)
     flag = torch.empty(n, dtype=torch.uint8, device=dev)
     n_live = ctypes.c_int64()
-    _lib.call("nerfb200_cull_count", dev, r.data_ptr(), n, occupancy.bits.data_ptr(), occupancy.N,
+    _lib.call("nerfb200_cull_count", dev, r.data_ptr(), n, occupancy.bits.data_ptr(), occupancy.grid_n(),
               (ctypes.c_double * 6)(*occupancy.ranges), ws.data_ptr(), ws.numel(), flag.data_ptr(), ctypes.byref(n_live))
     live_idx = torch.empty(n_live.value, dtype=torch.int64, device=dev)
     live_rays = torch.empty(n_live.value, 8, dtype=torch.float32, device=dev)
@@ -312,6 +389,7 @@ def render_samples(models: Sequence[torch.nn.Module], rays: torch.Tensor, occupa
             use_disp=int(bool(use_disp)), white_back=int(bool(white_back)), test_time=int(bool(test_time)),
             bits=occupancy.bits.data_ptr(), N=occupancy.N, ranges=_lib.ranges_host(*[occupancy.ranges[2 * a:2 * a + 2]
                                                                                        for a in range(3)]),
+            levels=occupancy.levels,
             **{k: ptr(out.get(k)) for k in RESULT_KEYS}, **{k: ptr(t) for k, t in opt.items()},
             perturb=float(perturb), noise_std=float(noise_std), perturb_rand=ptr(pr), noise_coarse=ptr(nc),
             u_rand=ptr(ur), noise_fine=ptr(nf), rng_ray_offset=lo, early_stop=eps, **rng)

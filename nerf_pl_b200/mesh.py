@@ -72,8 +72,9 @@ def _masked_grid(entry: str, model: torch.nn.Module, N: int, ranges, occupancy, 
         raise ValueError(f"chunk = {chunk} must be >= 1")
     ws = _lib.workspace(nbytes, dev)
     evaluated = ctypes.c_int64()
-    _lib.call(entry, dev, blob.data_ptr(), N, ranges, occ.bits.data_ptr(), occ.N, (ctypes.c_double * 6)(*occ.ranges),
-              chunk, ws.data_ptr(), ws.numel(), out.data_ptr(), ctypes.byref(evaluated))
+    _lib.call(entry, dev, blob.data_ptr(), N, ranges, occ.bits.data_ptr(), occ.grid_n(),
+              (ctypes.c_double * 6)(*occ.ranges), chunk, ws.data_ptr(), ws.numel(), out.data_ptr(),
+              ctypes.byref(evaluated))
     return out, int(evaluated.value)
 
 

@@ -126,7 +126,8 @@ class SkipRenderFunction(torch.autograd.Function):
             n_samples=S_c, n_importance=K, use_disp=int(cfg["use_disp"]), white_back=int(cfg["white_back"]),
             perturb=cfg["perturb"], noise_std=cfg["noise_std"], perturb_rand=_ptr(pr), noise_coarse=_ptr(nc),
             u_rand=_ptr(ur), noise_fine=_ptr(nf), bits=grid.bits.data_ptr(), N=grid.N,
-            ranges=(ctypes.c_double * 6)(*grid.ranges), target=_ptr(target), loss_out=_ptr(loss_out),
+            ranges=(ctypes.c_double * 6)(*grid.ranges), levels=grid.levels, target=_ptr(target),
+            loss_out=_ptr(loss_out),
             **dict(zip(_OUTPUTS, [o.data_ptr() for o in out])), **{k: _ptr(t) for k, t in extras.items()}, **rng)
         if live_dev is None:
             live = (ctypes.c_int64 * 2)()

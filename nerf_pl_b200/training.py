@@ -466,7 +466,8 @@ class CapturedTrainStep:
             self._check_grid(occupancy, dev)
             r = occupancy.ranges
             self._grid = occupancy if self.density_grid is not None else \
-                OccupancyGrid(occupancy.bits.clone(), occupancy.N, r[0:2], r[2:4], r[4:6], occupancy.dilate)
+                OccupancyGrid(occupancy.bits.clone(), occupancy.N, r[0:2], r[2:4], r[4:6], occupancy.dilate,
+                              occupancy.levels)
             self.workspace = SkipTrainWorkspace(dev, B, S_c, K)
             self._live = torch.zeros(2, dtype=torch.int64, device=dev)
         self._perm = batches.next_permutation().clone()
@@ -591,6 +592,8 @@ class CapturedTrainStep:
             raise ValueError("set_occupancy needs a grid of the captured N, ranges and dilate "
                              f"({g.N}, {tuple(g.ranges)}, {g.dilate}); got ({grid.N}, {tuple(grid.ranges)}, "
                              f"{grid.dilate})")
+        if grid.levels != g.levels:
+            raise ValueError(f"set_occupancy needs a grid of the captured levels ({g.levels}); got {grid.levels}")
         g.bits.copy_(grid.bits)
 
     def step(self):
