@@ -1,6 +1,7 @@
 // Empty-space skipping at render time: an occupancy bit field built from a dense sigma grid, rays classified
-// against it by an exact cell walk, the live rays compacted in order, and the rendered results scattered back
-// over a vacuum background.  The render kernel is not involved: these kernels run in front of and behind it.
+// against it by a cell walk over closed cells grown by a sample's float32 rounding, the live rays compacted in
+// order, and the rendered results scattered back over a vacuum background.  The render kernel is not involved:
+// these kernels run in front of and behind it.
 // Conventions and the conservativeness argument: DESIGN.md "Empty-space skipping".
 //
 // AXIS ORDER.  The sigma grid is the one of nerfb200_sigma_grid: sigma[i, j, k] = sigma(x_j, y_i, z_k), flat
@@ -106,53 +107,141 @@ struct CullParams {
 
 constexpr int kCullTile = 256;   // rays per tile = threads per block
 
-// Whether the segment o + t d, t in [near, far] (v: a finite ray with far > near) crosses an occupied cell of level
-// k.  Amanatides-Woo in grid coordinates, in double; each boundary time is recomputed from the cell index, so no
-// error accumulates along the walk.  Space outside the level's box is empty.
+// Whether the segment o + t d, t in [t0, t1] meets cell c's closed box grown by del[a] on each axis: a slab test in
+// grid coordinates.  A zero direction component has del = 0 and tests its coordinate against [c, c + 1] exactly.
+__device__ __forceinline__ bool cull_grown_cell_meets(int cx, int cy, int cz, const double o[3], const double d[3],
+                                                      const double inv[3], const double del[3], double t0, double t1) {
+  const int c[3] = {cx, cy, cz};
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double lo = static_cast<double>(c[a]), hi = static_cast<double>(c[a] + 1);
+    if (d[a] == 0.0) {
+      if (o[a] < lo || o[a] > hi) return false;
+    } else {
+      const double ta = (lo - del[a] - o[a]) * inv[a], tb = (hi + del[a] - o[a]) * inv[a];
+      t0 = fmax(t0, fmin(ta, tb));
+      t1 = fmin(t1, fmax(ta, tb));
+    }
+  }
+  return t0 <= t1;
+}
+
+// Whether level k calls the segment o + t d, t in [near, far] (v: a finite ray with far > near) live: whether it meets
+// the closed box of an occupied cell grown by del_a = 2^-22 |scale_a| (|o_a| + |d_a| max(|near|, |far|)) grid units
+// on each axis a (0 where d_a = 0), which covers the float32 rounding of every sample point the renderer places on
+// the segment (DESIGN.md §10 "Live").  A level with del_a >= 1/2 on some axis is live wherever its grown box meets
+// the segment.
+//
+// Amanatides-Woo in grid coordinates, in double, over the segment clipped to the grown box; each boundary time is
+// recomputed from the cell index, so no error accumulates along the walk.  The walk runs on the lattice extended by
+// a ring of empty cells -1 and M, which holds the part of the segment in the grown margin outside the box.  At each
+// visited cell it takes, on each axis whose face the segment comes within del_a of inside the cell (within
+// del_a / |d_a| of the time it crosses that face), the neighbour across that face: every cell cell + s with s_a in
+// {-1, 0, 1} so allowed is a candidate, and an occupied candidate is confirmed by a slab test against its grown box.
+// With del < 1 every cell whose grown box meets the segment is a candidate of some visited cell, so the result is
+// the grown-box rule.  A segment usually enters and leaves a cell across faces, whose single-axis neighbours are
+// the previous and next visited cells; those are not probed twice, so a step reads one bit unless the segment
+// passes near an edge.
 __device__ __forceinline__ bool cull_level_live(const SkipGrid& g, int k, const float v[8]) {
   const double M = static_cast<double>(g.M);
   const uint32_t* bits = g.bits + k * g.words;
-  double o[3], d[3], inv[3];
+  const double tmax = fmax(fabs(static_cast<double>(v[6])), fabs(static_cast<double>(v[7])));
+  double o[3], d[3], inv[3], del[3];
   double t0 = v[6], t1 = v[7];
+  bool coarse = false;
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
     o[a] = (static_cast<double>(v[a]) - g.lo[k][a]) * g.scale[k][a];
     d[a] = static_cast<double>(v[3 + a]) * g.scale[k][a];
     if (d[a] == 0.0) {
       inv[a] = 0.0;
+      del[a] = 0.0;
       if (o[a] < 0.0 || o[a] > M) return false;
     } else {
       inv[a] = 1.0 / d[a];
-      const double ta = (0.0 - o[a]) * inv[a], tb = (M - o[a]) * inv[a];
+      // rounded as written (no contraction), so that tests/occupancy_ref.py restates it bit for bit
+      const double ao = fabs(static_cast<double>(v[a])), ad = fabs(static_cast<double>(v[3 + a]));
+      del[a] = __dmul_rn(0x1p-22 * fabs(g.scale[k][a]), __dadd_rn(ao, __dmul_rn(ad, tmax)));
+      coarse |= del[a] >= 0.5;
+      const double ta = (0.0 - del[a] - o[a]) * inv[a], tb = (M + del[a] - o[a]) * inv[a];
       t0 = fmax(t0, fmin(ta, tb));
       t1 = fmin(t1, fmax(ta, tb));
     }
   }
   if (!(t0 <= t1)) return false;
-  long long cell[3];
-  double tnext[3];
+  if (coarse) return true;
+  // cell indices in [-1, M] (M <= 1624) fit an int; only the flat bit index needs 64 bits
+  const int Mi = static_cast<int>(g.M);
+  int cell[3];
+  double tnext[3], eps[3];
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
-    const double g = floor(o[a] + t0 * d[a]);
-    cell[a] = static_cast<long long>(fmin(fmax(g, 0.0), M - 1.0));
+    const double f = floor(__dadd_rn(o[a], __dmul_rn(t0, d[a])));
+    cell[a] = static_cast<int>(fmin(fmax(f, -1.0), M));
+    eps[a] = __dmul_rn(del[a], fabs(inv[a]));   // del_a grid units in time along the ray
   }
   const double inf = __longlong_as_double(0x7ff0000000000000LL);
-  const long long steps = 3 * g.M + 3;
-  for (long long s = 0; s < steps; ++s) {
-    const long long c = (cell[2] * g.M + cell[1]) * g.M + cell[0];
-    if ((bits[c >> 5] >> (c & 31)) & 1u) return true;
+  const int steps = 3 * (Mi + 2) + 3;
+  double te = t0;   // when the segment entered the current cell
+  int entry = -1;   // the axis it entered across (-1: the first cell)
+  for (int s = 0; s < steps; ++s) {
+    double tlow[3];   // when the segment crosses the cell's face behind it on each axis
 #pragma unroll
-    for (int a = 0; a < 3; ++a)
+    for (int a = 0; a < 3; ++a) {
       tnext[a] = d[a] == 0.0 ? inf : (static_cast<double>(cell[a] + (d[a] > 0.0 ? 1 : 0)) - o[a]) * inv[a];
+      tlow[a] = d[a] == 0.0 ? -inf : (static_cast<double>(cell[a] + (d[a] > 0.0 ? 0 : 1)) - o[a]) * inv[a];
+    }
     const int ax = tnext[0] <= tnext[1] ? (tnext[0] <= tnext[2] ? 0 : 2) : (tnext[1] <= tnext[2] ? 1 : 2);
+    const double tmin = fmin(fmin(tnext[0], tnext[1]), tnext[2]);   // tnext[ax], without indexing by a variable
+    const bool more = tmin <= t1;
+    const double tx = fmin(tmin, t1);
+    // The faces the segment comes within del_a of while inside the cell: the one behind it (back) if it entered
+    // within eps_a of crossing it, the one ahead (ahead) if it leaves within eps_a of crossing that.  A zero
+    // component sits at o_a: on the cell's low face iff o_a == cell_a.
+    bool back[3], ahead[3];
+    unsigned wide = 0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      back[a] = d[a] == 0.0 ? o[a] - static_cast<double>(cell[a]) <= 0.0 : te - tlow[a] <= eps[a];
+      ahead[a] = d[a] == 0.0 ? static_cast<double>(cell[a] + 1) - o[a] <= 0.0 : tnext[a] - tx <= eps[a];
+      wide |= (back[a] || ahead[a] ? 1u : 0u) << a;
+    }
+    // The cell the walk came from and the one it goes to next are visited cells, probed on their own visits: a
+    // single-axis offset onto one of them is dropped (offsets combined with another axis are kept).
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const bool alone = !(wide & ~(1u << a));
+      if (a == entry && alone) back[a] = false;
+      if (a == ax && more && alone) ahead[a] = false;
+    }
+    int s0[3], s1[3];   // offsets on the cell's own axes: -1 toward lower indices, +1 toward higher
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const bool lower = d[a] < 0.0 ? ahead[a] : back[a], upper = d[a] < 0.0 ? back[a] : ahead[a];
+      s0[a] = lower ? -1 : 0;
+      s1[a] = upper ? 1 : 0;
+    }
+    // scalar loop indices: an index array would live in local memory
+    const int x0 = max(cell[0] + s0[0], 0), x1 = min(cell[0] + s1[0], Mi - 1);
+    const int y0 = max(cell[1] + s0[1], 0), y1 = min(cell[1] + s1[1], Mi - 1);
+    const int z0 = max(cell[2] + s0[2], 0), z1 = min(cell[2] + s1[2], Mi - 1);
+    for (int cz = z0; cz <= z1; ++cz)
+      for (int cy = y0; cy <= y1; ++cy)
+        for (int cx = x0; cx <= x1; ++cx) {
+          const long long b = (static_cast<long long>(cz) * g.M + cy) * g.M + cx;
+          if (((bits[b >> 5] >> (b & 31)) & 1u) && cull_grown_cell_meets(cx, cy, cz, o, d, inv, del, t0, t1))
+            return true;
+        }
+    if (!more) return false;
     // unrolled over the axis so that the per-axis arrays stay in registers
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
       if (a != ax) continue;
-      if (!(tnext[a] <= t1)) return false;
       cell[a] += d[a] > 0.0 ? 1 : -1;
-      if (cell[a] < 0 || cell[a] >= g.M) return false;
+      if (cell[a] < -1 || cell[a] > Mi) return false;
     }
+    entry = ax;
+    te = tmin;
   }
   return false;
 }

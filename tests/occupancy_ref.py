@@ -7,9 +7,9 @@ The conventions it restates (DESIGN.md "Empty-space skipping"):
   corner points has ``sigma > threshold``; arrays of cells here are indexed ``occ[cx, cy, cz]``;
 * the occupied set is dilated by ``dilate`` cells in Chebyshev distance;
 * the bit field holds cell ``c = (cz * M + cy) * M + cx`` (``M = N - 1``, x fastest) as bit ``c % 32`` of word ``c // 32``;
-* a ray ``[o, d, near, far]`` is live iff the segment ``o + t d``, ``t in [near, far]``, clipped to the grid's box,
-  crosses an occupied cell (Amanatides-Woo); outside the box is empty; a ray with a non-finite value or
-  ``far <= near`` is live;
+* a ray ``[o, d, near, far]`` is live iff the segment ``o + t d``, ``t in [near, far]``, meets the closed box of an
+  occupied cell grown by the float32 rounding bound ``delta`` of ray_live; outside the box is empty; a ray with a
+  non-finite value or ``far <= near`` is live;
 * a culled ray gets what a ray through vacuum renders: opacity 0, depth 0, rgb 1 with ``white_back`` else 0.
 """
 import numpy as np
@@ -62,64 +62,143 @@ def occupancy(sigma, threshold, r):
     return dilate(cells_from_sigma(sigma, threshold), r)
 
 
+GROWTH = 2.0 ** -22     # delta_a = GROWTH |scale_a| (|o_a| + |d_a| max(|near|, |far|)): 4 float32 unit roundoffs
+
+
+def _geometry(r, ranges, M):
+    """Grid coordinates of float64 rays r (n, 8): o, d, zero (d == 0), inv (1 / d, 0 where zero) and the growth
+    delta (n, 3) of each axis, each computed as the device computes it."""
+    lo = np.array([a for a, _ in ranges], np.float64)
+    hi = np.array([b for _, b in ranges], np.float64)
+    scale = M / (hi - lo)
+    o = (r[:, :3] - lo) * scale
+    d = r[:, 3:6] * scale
+    zero = d == 0.0
+    inv = np.where(zero, 0.0, 1.0 / np.where(zero, 1.0, d))
+    tmax = np.maximum(np.abs(r[:, 6]), np.abs(r[:, 7]))
+    delta = np.where(zero, 0.0, GROWTH * np.abs(scale) * (np.abs(r[:, :3]) + np.abs(r[:, 3:6]) * tmax[:, None]))
+    return o, d, zero, inv, delta
+
+
+def _slab(o, d, zero, inv, lo, hi, t0, t1):
+    """(meets, margin): whether o + t d, t in [t0, t1], meets the box [lo, hi] (all (n, 3); t0, t1 (n,)), the
+    device's slab test; an axis with d == 0 tests o against [lo, hi] exactly.  ``margin`` is, in cells, how far a face
+    of the box would have to move to flip the answer: the gap between the latest entry and the earliest exit time over
+    the sum of 1 / |d| of the two axes that set them (t0 and t1 count 0)."""
+    ta, tb = (lo - o) * inv, (hi - o) * inv
+    tl = np.where(zero, -np.inf, np.minimum(ta, tb))
+    th = np.where(zero, np.inf, np.maximum(ta, tb))
+    w = np.where(zero, 0.0, np.abs(inv))
+    tl = np.concatenate([t0[:, None], tl], 1)
+    th = np.concatenate([t1[:, None], th], 1)
+    w = np.concatenate([np.zeros((len(o), 1)), w], 1)
+    i, j = np.argmax(tl, 1), np.argmin(th, 1)
+    rows = np.arange(len(o))
+    a, b = tl[rows, i], th[rows, j]
+    inside = ~(zero & ((o < lo) | (o > hi))).any(1)
+    ww = w[rows, i] + w[rows, j]
+    margin = np.where(ww > 0.0, np.abs(b - a) / np.where(ww > 0.0, ww, 1.0), np.inf)
+    return inside & (a <= b), np.where(inside, margin, np.inf)
+
+
+_OFFSETS = np.array([(x, y, z) for z in (-1, 0, 1) for y in (-1, 0, 1) for x in (-1, 0, 1)], np.int64)
+
+
 def ray_live(rays, occ, ranges):
     """(flag (n) bool, margin (n) float64).  ``ranges`` = ((xmin, xmax), (ymin, ymax), (zmin, zmax)); the rays are
-    taken in float32, as the device takes them.  ``margin`` is, in cells, how far the ray's walk stayed from every
-    decision that a rounding could flip: a cell edge or corner passed, the end of the segment against a cell face,
-    the start point against a cell face, the box against the segment.  It only covers the walk up to the cell that
-    decided the flag."""
+    taken in float32, as the device takes them.
+
+    A ray is live iff the segment meets the closed box of an occupied cell grown by delta_a grid units on each axis
+    (GROWTH; 0 on an axis with d_a = 0), or some delta_a >= 1/2 and the segment meets the box grown alike.  This is
+    the device's walk step by step: the segment clipped to the grown box, Amanatides-Woo over the lattice extended by a
+    ring of empty cells -1 and M, and at each visited cell the neighbours across the faces the segment comes within
+    delta of (within delta / |d| of crossing them), each occupied one confirmed by a slab test against its grown box.
+    The device also skips the neighbours that are the previous and next visited cells, which changes no flag.
+
+    ``margin`` is, in cells, how far the ray stayed from every grown-box decision a rounding could flip: the clip
+    against the grown box, and the slab test of every occupied cell next to (or at) a visited cell, admitted or
+    not.  It covers the walk up to the cell that decided the flag."""
     occ = np.asarray(occ, bool)
     M = occ.shape[0]
     r = np.asarray(rays, np.float32).astype(np.float64).reshape(-1, 8)
     n = len(r)
-    lo = np.array([a for a, _ in ranges], np.float64)
-    hi = np.array([b for _, b in ranges], np.float64)
-    scale = M / (hi - lo)
     flag = np.zeros(n, bool)
     margin = np.full(n, np.inf)
     guard = ~np.isfinite(r).all(1) | ~(r[:, 7] > r[:, 6])
     flag[guard] = True
     with np.errstate(all="ignore"):
-        o = (r[:, :3] - lo) * scale
-        d = r[:, 3:6] * scale
-        zero = d == 0.0
-        inv = np.where(zero, 0.0, 1.0 / d)
-        ta, tb = (0.0 - o) * inv, (M - o) * inv
-        tlo = np.where(zero, -np.inf, np.minimum(ta, tb))
-        thi = np.where(zero, np.inf, np.maximum(ta, tb))
-        t0 = np.maximum(r[:, 6], tlo.max(1))
-        t1 = np.minimum(r[:, 7], thi.min(1))
-        outside = (zero & ((o < 0.0) | (o > M))).any(1)
-        speed = np.abs(d)
-        margin = np.minimum(margin, np.where(zero, np.minimum(np.abs(o), np.abs(o - M)), np.inf).min(1))
-        margin = np.minimum(margin, np.abs(t1 - t0) * speed.max(1))
-        idx = np.nonzero(~guard & ~outside & (t0 <= t1))[0]
-        p0 = o[idx] + t0[idx, None] * d[idx]
-        cell = np.clip(np.floor(p0), 0, M - 1).astype(np.int64)
-        k = np.round(p0)
-        margin[idx] = np.minimum(margin[idx], np.where((k <= 0) | (k >= M), np.inf, np.abs(p0 - k)).min(1))
-        for _ in range(3 * M + 3):
+        o, d, zero, inv, delta = _geometry(r, ranges, M)
+        ok, m = _slab(o, d, zero, inv, -delta, M + delta, r[:, 6], r[:, 7])
+        margin = np.minimum(margin, m)
+        ta, tb = (-delta - o) * inv, (M + delta - o) * inv
+        t0 = np.maximum(r[:, 6], np.where(zero, -np.inf, np.minimum(ta, tb)).max(1))
+        t1 = np.minimum(r[:, 7], np.where(zero, np.inf, np.maximum(ta, tb)).min(1))
+        ok &= ~guard
+        coarse = ok & (delta >= 0.5).any(1)
+        flag[coarse] = True
+        margin = np.minimum(margin, np.where(zero, np.inf, np.abs(delta - 0.5)).min(1))
+        idx = np.nonzero(ok & ~coarse)[0]
+        cell = np.clip(np.floor(o[idx] + t0[idx, None] * d[idx]), -1, M).astype(np.int64)
+        te = t0[idx]
+        for _ in range(3 * (M + 2) + 3):
             if len(idx) == 0:
                 break
-            hit = occ[cell[:, 0], cell[:, 1], cell[:, 2]]
-            flag[idx[hit]] = True
-            idx, cell = idx[~hit], cell[~hit]
-            oo, dd, zz = o[idx], d[idx], zero[idx]
-            tn = np.where(zz, np.inf, ((cell + (dd > 0.0)) - oo) * inv[idx])
+            oo, dd, zz, ii, de = o[idx], d[idx], zero[idx], inv[idx], delta[idx]
+            tn = np.where(zz, np.inf, ((cell + (dd > 0.0)) - oo) * ii)
             ax = np.argmin(tn, 1)
             rows = np.arange(len(idx))
-            tmin = tn[rows, ax]
-            gap = np.where(zz, np.inf, (tn - tmin[:, None]) * speed[idx])
-            gap[rows, ax] = np.inf
-            cell[rows, ax] += np.where(dd[rows, ax] > 0.0, 1, -1)
-            inside = (cell[rows, ax] >= 0) & (cell[rows, ax] < M)
-            # leaving the box ends the walk whichever side of t1 the crossing falls on
-            end = np.where(inside & np.isfinite(tmin), np.abs(tmin - t1[idx]) * speed[idx][rows, ax], np.inf)
-            margin[idx] = np.minimum(margin[idx], np.minimum(gap.min(1), end))
-            go = (tmin <= t1[idx]) & inside
-            idx, cell = idx[go], cell[go]
+            tnext = tn[rows, ax]
+            tx = np.minimum(tnext, t1[idx])
+            # the faces behind and ahead that the segment comes within delta of inside the cell, by crossing time
+            tlow = np.where(zz, -np.inf, ((cell + (dd < 0.0)) - oo) * ii)
+            eps = de * np.abs(ii)
+            back = np.where(zz, oo - cell <= 0.0, te[:, None] - tlow <= eps)
+            ahead = np.where(zz, (cell + 1) - oo <= 0.0, tn - tx[:, None] <= eps)
+            c0 = cell - np.where(dd < 0.0, ahead, back)
+            c1 = cell + np.where(dd < 0.0, back, ahead)
+            hit = np.zeros(len(idx), bool)
+            for off in _OFFSETS:
+                c = cell + off
+                sel = np.nonzero(((c >= 0) & (c < M)).all(1))[0]
+                sel = sel[occ[c[sel, 0], c[sel, 1], c[sel, 2]]]
+                if len(sel) == 0:
+                    continue
+                cs = c[sel].astype(np.float64)
+                meets, m = _slab(oo[sel], dd[sel], zz[sel], ii[sel], cs - de[sel], (cs + 1.0) + de[sel],
+                                 t0[idx[sel]], t1[idx[sel]])
+                margin[idx[sel]] = np.minimum(margin[idx[sel]], m)
+                admitted = ((c[sel] >= c0[sel]) & (c[sel] <= c1[sel])).all(1)
+                hit[sel] |= meets & admitted
+            flag[idx[hit]] = True
+            step = cell[rows, ax] + np.where(dd[rows, ax] > 0.0, 1, -1)
+            go = ~hit & (tnext <= t1[idx]) & (step >= -1) & (step <= M)
+            cell[rows, ax] = step
+            idx, cell, te = idx[go], cell[go], tnext[go]
     margin[guard] = np.inf
     return flag, margin
+
+
+def brute_live(rays, occ, ranges):
+    """(n,) bool: the grown-box rule of ray_live by a slab test of every segment, t in [near, far], against every
+    occupied cell's grown box, in float64.  For small grids."""
+    occ = np.asarray(occ, bool)
+    M = occ.shape[0]
+    r = np.asarray(rays, np.float32).astype(np.float64).reshape(-1, 8)
+    n = len(r)
+    guard = ~np.isfinite(r).all(1) | ~(r[:, 7] > r[:, 6])
+    cells = np.argwhere(occ).astype(np.float64)                 # (C, 3) [cx, cy, cz]
+    live = guard.copy()
+    with np.errstate(all="ignore"):
+        o, d, zero, inv, delta = _geometry(r, ranges, M)
+        box, _ = _slab(o, d, zero, inv, -delta, M + delta, r[:, 6], r[:, 7])
+        live |= ~guard & box & (delta >= 0.5).any(1)
+        rest = np.nonzero(~live)[0]
+        t0, t1 = r[rest, 6], r[rest, 7]
+        for c in cells:                                         # every ray against one cell's grown box at a time
+            c = np.broadcast_to(c, (len(rest), 3))
+            meets, _ = _slab(o[rest], d[rest], zero[rest], inv[rest], c - delta[rest], (c + 1.0) + delta[rest], t0, t1)
+            live[rest] |= meets
+    return live
 
 
 def vacuum_results(n, keys, white_back):

@@ -665,6 +665,14 @@ def _render_sets(rays_np, words, N, ranges, S=32, K=64):
     return ev_c, ev_f, zf
 
 
+def _cull_keeps_evaluated(rays_np, words, N, ranges, ev_c, ev_f):
+    """nb.cull_rays keeps every ray with an evaluated sample (the cell walk is a superset of the lookup)."""
+    flag = _nb().cull_rays(torch.from_numpy(np.ascontiguousarray(rays_np, F32)).cuda(), _grid(words, N, ranges),
+                           return_flag=True)[2].cpu().numpy().astype(bool)
+    lost = (ev_c.any(1) | ev_f.any(1)) & ~flag
+    assert not lost.any(), np.nonzero(lost)[0]
+
+
 def _rule_sets(rays_np, words, N, ranges, zf, S=32):
     return (sk.evaluated(rays_np, sk.z_base(rays_np, S), words, N, ranges),
             sk.evaluated(rays_np, zf, words, N, ranges))
@@ -692,6 +700,8 @@ def test_lattice_faces_edges_and_corners(kind, dev):
         assert np.array_equal(rc, ev_c)
     mc, mf = _rule_sets(mirror, words, M + 1, rev, rzf)
     assert np.array_equal(rc, mc) and np.array_equal(rf, mf)
+    _cull_keeps_evaluated(rays, words, M + 1, box, ev_c, ev_f)
+    _cull_keeps_evaluated(mirror, words, M + 1, rev, rc, rf)
     print(f"\n[{kind}] evaluated coarse {ev_c.mean():.3f} fine {ev_f.mean():.3f}")
 
 
@@ -725,6 +735,7 @@ def test_box_boundary(dev):
     assert np.array_equal(ev_c, want_c) and np.array_equal(ev_f, want_f)
     want_all = np.array(want_all)
     assert ev_c[want_all].all() and not ev_c[~want_all].any()
+    _cull_keeps_evaluated(rays, words, N, box, ev_c, ev_f)
 
 
 @pytest.mark.parametrize("N", [2, 33, 34])

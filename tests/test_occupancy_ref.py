@@ -142,13 +142,15 @@ def test_ray_walk_guards():
 
 def test_margin_flags_the_rays_that_graze_an_edge():
     occ = np.zeros((4, 4, 4), bool)
+    occ[1, 2, 2] = True                                       # x [-1, 0] x y [0, 1] x z [0, 1]
     box = ((-2.0, 2.0),) * 3
-    rays = np.array([[-5, 0.5, 0.5, 1, 0, 0, 0, 10],          # mid-cell all the way
-                     [-5, 0.5 + 1e-6, 0.5, 1, 1e-7, 0, 0, 10],
-                     [-5, -1.0, -1.0, 1, 0.2, 0.2, 0, 10]],    # passes exactly through the edge y = z = 0 at x = 0
+    rays = np.array([[-5, -0.5, -0.5, 1, 0, 0, 0, 10],        # mid-cell all the way, half a cell from the cell
+                     [-5, -0.5 - 1e-6, -0.5, 1, 1e-7, 0, 0, 10],
+                     [-5, -1.0, -1.0, 1, 0.2, 0.2, 0, 10]],    # touches the cell only at its corner x = y = z = 0
                     np.float32)
-    _, margin = oc.ray_live(rays, occ, box)
-    assert margin[0] >= 0.49 and margin[1] >= 0.49 and margin[2] < 1e-6
+    flag, margin = oc.ray_live(rays, occ, box)
+    assert flag.tolist() == [False, False, True]
+    assert margin[0] >= 0.49 and margin[1] >= 0.49 and margin[2] < 1e-4
 
 
 def test_vacuum_values_and_scatter():
