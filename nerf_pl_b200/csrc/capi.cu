@@ -21,7 +21,10 @@
 #include "density_kernels.cuh"
 #include "masked_grid_kernels.cuh"
 #include "early_stop_kernels.cuh"
+#include "sparse_mc_kernels.cuh"
+#include "../../include/nerf_pl_b200_sparse_mc.h"
 
+#include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
 
 using namespace nerfb200;
@@ -1220,6 +1223,110 @@ int masked_grid(const void* packed, int64_t N, const double* ranges, const uint3
   }
   *evaluated_host = evaluated;
   return 0;
+}
+
+// ------------------------------------------------------------------ sparse marching cubes
+// (kernels: sparse_mc_kernels.cuh, entries: include/nerf_pl_b200_sparse_mc.h)
+constexpr long long kSmcMaxN = 2048;
+constexpr long long kSmcChunkBricks = 4096;   // active bricks per point query: at most 2^21 rows
+constexpr long long kSmcMaxCount = 0x7fffffffLL;
+
+long long smc_bricks(long long N) { return ceil_div(N, kBrick); }
+
+using SmcVertIt = thrust::transform_iterator<SmcVerts, const unsigned*, unsigned long long>;
+using SmcTriIt = thrust::transform_iterator<SmcTris, const unsigned*, unsigned long long>;
+using SmcIndexIt = thrust::counting_iterator<int>;
+
+// The plan workspace: per brick its map slot, flag, evaluated count and three lists; the selection counts.
+size_t smc_plan_carve(long long N, void* base, SparseMcParams* p, CubScratch* s) {
+  const long long nb = smc_bricks(N), B = nb * nb * nb;
+  size_t tb = 0;
+  cub::DeviceSelect::Flagged(nullptr, tb, SmcIndexIt(0), static_cast<const uint8_t*>(nullptr), static_cast<int*>(nullptr),
+                             static_cast<int*>(nullptr), static_cast<int>(B));
+  s->temp_bytes = tb;
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  p->nsel = c.take<int>(4);
+  p->map = c.take<int>(B);
+  p->flag = c.take(B);
+  p->cnt = c.take<int>(B);
+  p->cand = c.take<int>(B);
+  p->active = c.take<int>(B);
+  p->march = c.take<int>(B);
+  s->temp = c.take(s->temp_bytes);
+  return c.off;
+}
+
+// The count / emit workspace of A active and Mb march bricks: V and T, the row counts and offsets, the active
+// bricks' values, one query's rows, the march bricks' counts and offsets, and the scans' scratch.
+size_t smc_carve(long long A, long long Mb, void* base, SparseMcParams* p, unsigned long long** rcnt,
+                 unsigned long long** vt, CubScratch* s) {
+  const long long rows = std::min(A, kSmcChunkBricks) * kBrickPoints;
+  size_t t1 = 0, t2 = 0, t3 = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, t1, static_cast<const unsigned long long*>(nullptr),
+                                static_cast<unsigned long long*>(nullptr), static_cast<int>(A + 1));
+  cub::DeviceScan::ExclusiveSum(nullptr, t2, SmcVertIt(nullptr, SmcVerts()), static_cast<unsigned long long*>(nullptr),
+                                static_cast<int>(Mb + 1));
+  cub::DeviceScan::ExclusiveSum(nullptr, t3, SmcTriIt(nullptr, SmcTris()), static_cast<unsigned long long*>(nullptr),
+                                static_cast<int>(Mb + 1));
+  s->temp_bytes = std::max({t1, t2, t3});
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  *vt = c.take<unsigned long long>(2);
+  *rcnt = c.take<unsigned long long>(A + 1);
+  p->rofs = c.take<unsigned long long>(A + 1);
+  p->vals = c.take<float>(A * kBrickPoints);
+  p->xyz = c.take<float>(rows * 3);
+  p->dst = c.take<long long>(rows);
+  p->out = c.take<float>(rows);
+  p->bcnt = c.take<unsigned>(Mb + 1);
+  p->vofs = c.take<unsigned long long>(Mb + 1);
+  p->tofs = c.take<unsigned long long>(Mb + 1);
+  s->temp = c.take(s->temp_bytes);
+  return c.off;
+}
+
+// The emit workspace of V vertex and T triangle keys: both sort buffers of each and the sorts' scratch.
+size_t smc_emit_carve(long long V, long long T, void* base, unsigned long long* vk[2], unsigned long long* tk[2],
+                      CubScratch* s) {
+  size_t t1 = 0, t2 = 0;
+  cub::DoubleBuffer<unsigned long long> kb(nullptr, nullptr);
+  cub::DeviceRadixSort::SortKeys(nullptr, t1, kb, static_cast<int>(V), 0, 64);
+  cub::DeviceRadixSort::SortKeys(nullptr, t2, kb, static_cast<int>(T), 0, 64);
+  s->temp_bytes = std::max(t1, t2);
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  vk[0] = c.take<unsigned long long>(V);
+  vk[1] = c.take<unsigned long long>(V);
+  tk[0] = c.take<unsigned long long>(T);
+  tk[1] = c.take<unsigned long long>(T);
+  s->temp = c.take(s->temp_bytes);
+  return c.off;
+}
+
+bool smc_counts_ok(long long N, long long A, long long Mb) {
+  const long long nb = smc_bricks(N);
+  return N >= 2 && N <= kSmcMaxN && A >= 0 && Mb >= A && Mb <= nb * nb * nb && (A > 0 || Mb == 0);
+}
+
+// The mesh grid, N and (with bits) the occupancy grid into p.
+int smc_grids(int64_t N, const double* ranges, const uint32_t* bits, int64_t occ_grid_N, const double* occ_ranges,
+              SparseMcParams* p, const char* who) {
+  if (N < 2 || N > kSmcMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 2048]", who);
+  if (!ranges || !bits || !occ_ranges) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  int64_t occ_N;
+  int32_t occ_levels;
+  grid_n(occ_grid_N, &occ_N, &occ_levels);
+  TRY(skip_grid(bits, occ_N, occ_levels, occ_ranges, &p->m.occ, who));
+  for (int a = 0; a < 3; ++a) { p->m.lo[a] = ranges[2 * a]; p->m.hi[a] = ranges[2 * a + 1]; }
+  p->m.N = N;
+  p->m.start = 0;
+  p->nb = smc_bricks(N);
+  return 0;
+}
+
+int smc_select(const SparseMcParams& p, CubScratch& sc, int* out, int* count, cudaStream_t s, const char* what) {
+  size_t tb = sc.temp_bytes;
+  const long long B = p.nb * p.nb * p.nb;
+  return cub_launch(cub::DeviceSelect::Flagged(sc.temp, tb, SmcIndexIt(0), p.flag, out, count, static_cast<int>(B), s),
+                    what);
 }
 
 // ------------------------------------------------------------------ training with empty samples skipped
@@ -2845,6 +2952,177 @@ int nerfb200_rgb_sigma_grid_masked(const void* packed, int64_t N, const double r
     return fail(NERFB200_EINVAL, "rgb_sigma_grid_masked: out must be 16-byte aligned");
   return masked_grid(packed, N, ranges_host, bits, occ_N, occ_ranges_host, chunk, ws, bytes, rgbsigma_out,
                      evaluated_host, 4, stream, "rgb_sigma_grid_masked");
+}
+
+// ---- sparse marching cubes (include/nerf_pl_b200_sparse_mc.h, kernels: sparse_mc_kernels.cuh)
+size_t nerfb200_sparse_mc_plan_workspace_bytes(int64_t N) {
+  if (N < 2 || N > kSmcMaxN) return 0;
+  SparseMcParams p{};
+  CubScratch sc;
+  return smc_plan_carve(N, nullptr, &p, &sc);
+}
+
+int nerfb200_sparse_mc_plan(int64_t N, const double ranges_host[6], const uint32_t* bits, int64_t occ_N,
+                            const double occ_ranges_host[6], void* plan_ws, size_t plan_bytes, int64_t bricks_host[2],
+                            void* stream) {
+  const char* who = "sparse_mc_plan";
+  SparseMcParams p{};
+  TRY(smc_grids(N, ranges_host, bits, occ_N, occ_ranges_host, &p, who));
+  if (!plan_ws || !bricks_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  CubScratch sc;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long B = p.nb * p.nb * p.nb;
+  TRY(launch("sparse_mc candidate launch", smc_candidate_kernel, grid_blocks(B, 256), 256, 0, s, p));
+  TRY(smc_select(p, sc, p.cand, p.nsel + 0, s, "sparse_mc candidate select"));
+  TRY(launch("sparse_mc classify launch", smc_classify_kernel, grid_blocks(B, 1), kBrickPoints, 0, s, p));
+  TRY(smc_select(p, sc, p.active, p.nsel + 1, s, "sparse_mc active select"));
+  TRY(launch("sparse_mc map launch", smc_map_kernel, grid_blocks(B, 256), 256, 0, s, p));
+  TRY(launch("sparse_mc march flag launch", smc_march_flag_kernel, grid_blocks(B, 256), 256, 0, s, p));
+  TRY(smc_select(p, sc, p.march, p.nsel + 2, s, "sparse_mc march select"));
+  int h[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(h, p.nsel + 1, sizeof(h), cudaMemcpyDeviceToHost, s), "sparse_mc plan readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "sparse_mc plan readback");
+  bricks_host[0] = h[0];
+  bricks_host[1] = h[1];
+  return 0;
+}
+
+size_t nerfb200_sparse_mc_workspace_bytes(int64_t N, int64_t active, int64_t march) {
+  if (!smc_counts_ok(N, active, march)) return 0;
+  SparseMcParams p{};
+  unsigned long long *rcnt, *vt;
+  CubScratch sc;
+  return smc_carve(active, march, nullptr, &p, &rcnt, &vt, &sc);
+}
+
+int nerfb200_sparse_mc_count(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
+                             int64_t occ_N, const double occ_ranges_host[6], double threshold, void* plan_ws,
+                             size_t plan_bytes, const int64_t bricks_host[2], void* ws, size_t bytes,
+                             int64_t counts_host[2], void* stream) {
+  const char* who = "sparse_mc_count";
+  SparseMcParams p{};
+  TRY(smc_grids(N, ranges_host, bits, occ_N, occ_ranges_host, &p, who));
+  if (!packed || !plan_ws || !bricks_host || !ws || !counts_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  const long long A = bricks_host[0], Mb = bricks_host[1];
+  if (!smc_counts_ok(N, A, Mb)) return fail(NERFB200_EINVAL, "%s: bricks_host is not a plan's {active, march}", who);
+  CubScratch sc;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  unsigned long long *rcnt, *vt;
+  if (bytes < smc_carve(A, Mb, ws, &p, &rcnt, &vt, &sc))
+    return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_sparse_mc_workspace_bytes(N, active, march)", who);
+  p.thr = threshold;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int h[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(h, p.nsel + 1, sizeof(h), cudaMemcpyDeviceToHost, s), "sparse_mc count readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "sparse_mc count readback");
+  if (h[0] != A || h[1] != Mb) return fail(NERFB200_EINVAL, "%s: bricks_host differs from the plan's", who);
+  if (A == 0) {
+    CUDA_TRY(cudaMemsetAsync(vt, 0, 2 * sizeof(unsigned long long), s), "sparse_mc count memset");
+    counts_host[0] = counts_host[1] = 0;
+    return 0;
+  }
+  // sigma: rows of the active bricks in order, one point query per kSmcChunkBricks bricks
+  TRY(launch("sparse_mc row counts launch", smc_row_counts_kernel, grid_blocks(A + 1, 256), 256, 0, s, p, rcnt));
+  size_t tb = sc.temp_bytes;
+  TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, rcnt, p.rofs, static_cast<int>(A + 1), s), "sparse_mc row scan"));
+  CUDA_TRY(cudaMemsetAsync(p.vals, 0, static_cast<size_t>(A) * kBrickPoints * sizeof(float), s), "sparse_mc memset");
+  const long long chunks = ceil_div(A, kSmcChunkBricks);
+  std::vector<unsigned long long> bound(chunks + 1);
+  CUDA_TRY(cudaMemcpy2DAsync(bound.data(), sizeof(unsigned long long), p.rofs, kSmcChunkBricks * sizeof(unsigned long long),
+                             sizeof(unsigned long long), chunks, cudaMemcpyDeviceToHost, s), "sparse_mc row readback");
+  CUDA_TRY(cudaMemcpyAsync(bound.data() + chunks, p.rofs + A, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s),
+           "sparse_mc row readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "sparse_mc row readback");
+  for (long long c = 0; c < chunks; ++c) {
+    const long long rows = static_cast<long long>(bound[c + 1] - bound[c]);
+    if (rows == 0) continue;
+    p.slot0 = c * kSmcChunkBricks;
+    p.slots = std::min(kSmcChunkBricks, A - p.slot0);
+    TRY(launch("sparse_mc sigma emit launch", smc_sigma_emit_kernel, grid_blocks(p.slots, 1), kBrickPoints, 0, s, p));
+    TRY(nerfb200_query_sigma(p.xyz, rows, 3, packed, p.out, stream));
+    TRY(launch("sparse_mc sigma scatter launch", smc_sigma_scatter_kernel, grid_blocks(rows, 256), 256, 0, s, p, rows));
+  }
+  // march: vertices and triangles per march brick
+  CUDA_TRY(cudaMemsetAsync(p.bcnt + Mb, 0, sizeof(unsigned), s), "sparse_mc count memset");
+  TRY(launch("sparse_mc march count launch", smc_march_count_kernel, grid_blocks(Mb, 1), kBrickPoints, 0, s, p));
+  tb = sc.temp_bytes;
+  TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, SmcVertIt(p.bcnt, SmcVerts()), p.vofs,
+                                               static_cast<int>(Mb + 1), s), "sparse_mc vertex scan"));
+  tb = sc.temp_bytes;
+  TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, SmcTriIt(p.bcnt, SmcTris()), p.tofs,
+                                               static_cast<int>(Mb + 1), s), "sparse_mc triangle scan"));
+  CUDA_TRY(cudaMemcpyAsync(vt, p.vofs + Mb, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s), "sparse_mc count copy");
+  CUDA_TRY(cudaMemcpyAsync(vt + 1, p.tofs + Mb, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s), "sparse_mc count copy");
+  unsigned long long c2[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(c2, vt, sizeof(c2), cudaMemcpyDeviceToHost, s), "sparse_mc count readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "sparse_mc count readback");
+  if (c2[0] > static_cast<unsigned long long>(kSmcMaxCount) || c2[1] > static_cast<unsigned long long>(kSmcMaxCount))
+    return fail(NERFB200_EUNSUPPORTED, "%s: %llu vertices and %llu triangles: both must stay below 2^31", who, c2[0], c2[1]);
+  counts_host[0] = static_cast<int64_t>(c2[0]);
+  counts_host[1] = static_cast<int64_t>(c2[1]);
+  return 0;
+}
+
+size_t nerfb200_sparse_mc_emit_workspace_bytes(int64_t n_vertices, int64_t n_triangles) {
+  if (n_vertices < 0 || n_triangles < 0 || n_vertices > kSmcMaxCount || n_triangles > kSmcMaxCount) return 0;
+  unsigned long long *vk[2], *tk[2];
+  CubScratch sc;
+  return smc_emit_carve(n_vertices, n_triangles, nullptr, vk, tk, &sc);
+}
+
+int nerfb200_sparse_mc_emit(int64_t N, double threshold, void* plan_ws, size_t plan_bytes,
+                            const int64_t bricks_host[2], void* ws, size_t bytes, const int64_t counts_host[2],
+                            void* emit_ws, size_t emit_bytes, double* vertices, int32_t* triangles, void* stream) {
+  const char* who = "sparse_mc_emit";
+  if (N < 2 || N > kSmcMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 2048]", who);
+  if (!plan_ws || !bricks_host || !ws || !counts_host || !emit_ws) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  const long long A = bricks_host[0], Mb = bricks_host[1], V = counts_host[0], T = counts_host[1];
+  if (!smc_counts_ok(N, A, Mb)) return fail(NERFB200_EINVAL, "%s: bricks_host is not a plan's {active, march}", who);
+  if (V < 0 || T < 0 || V > kSmcMaxCount || T > kSmcMaxCount || (V == 0 && T > 0))
+    return fail(NERFB200_EINVAL, "%s: counts_host is not count's {V, T}", who);
+  if ((V > 0 && !vertices) || (T > 0 && !triangles)) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  SparseMcParams p{};
+  p.m.N = N;
+  p.nb = smc_bricks(N);
+  p.thr = threshold;
+  CubScratch sc, se;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  unsigned long long *rcnt, *vt;
+  if (bytes < smc_carve(A, Mb, ws, &p, &rcnt, &vt, &sc))
+    return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_sparse_mc_workspace_bytes(N, active, march)", who);
+  unsigned long long *vk[2], *tk[2];
+  if (emit_bytes < smc_emit_carve(V, T, emit_ws, vk, tk, &se))
+    return fail(NERFB200_EINVAL, "%s: emit workspace smaller than nerfb200_sparse_mc_emit_workspace_bytes(V, T)", who);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  unsigned long long c2[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(c2, vt, sizeof(c2), cudaMemcpyDeviceToHost, s), "sparse_mc emit readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "sparse_mc emit readback");
+  if (c2[0] != static_cast<unsigned long long>(V) || c2[1] != static_cast<unsigned long long>(T))
+    return fail(NERFB200_EINVAL, "%s: counts_host differs from count's", who);
+  if (V == 0) return 0;
+  p.vkeys = vk[0];
+  p.tkeys = tk[0];
+  TRY(launch("sparse_mc march emit launch", smc_march_emit_kernel, grid_blocks(Mb, 1), kBrickPoints, 0, s, p));
+  cub::DoubleBuffer<unsigned long long> vb(vk[0], vk[1]), tbuf(tk[0], tk[1]);
+  size_t tb = se.temp_bytes;
+  TRY(cub_launch(cub::DeviceRadixSort::SortKeys(se.temp, tb, vb, static_cast<int>(V), 0, bits_for(3 * N * N * N), s),
+                 "sparse_mc vertex sort"));
+  tb = se.temp_bytes;
+  TRY(cub_launch(cub::DeviceRadixSort::SortKeys(se.temp, tb, tbuf, static_cast<int>(T), 0,
+                                                bits_for(5 * (N - 1) * (N - 1) * (N - 1)), s), "sparse_mc triangle sort"));
+  p.vkeys = vb.Current();
+  p.tkeys = tbuf.Current();
+  p.n_verts = V;
+  p.n_tris = T;
+  p.vertices = vertices;
+  p.triangles = triangles;
+  TRY(launch("sparse_mc vertices launch", smc_vertices_kernel, grid_blocks(V, 256), 256, 0, s, p));
+  TRY(launch("sparse_mc triangles launch", smc_triangles_kernel, grid_blocks(T, 256), 256, 0, s, p));
+  return 0;
 }
 
 }  // extern "C"

@@ -61,26 +61,66 @@ struct McParams {
   int* triangles;         // (T, 3)
 };
 
-__device__ __forceinline__ bool mc_in(const McParams& p, long long i, long long j, long long k) {
-  return static_cast<double>(p.sigma[(i * p.n1 + j) * p.n2 + k]) > p.thr;
-}
+// The rules of marching cubes on any value source, shared by the dense kernels below and the sparse ones
+// (sparse_mc_kernels.cuh).  `in(i, j, k)` says whether point (i, j, k) is inside: double(value) > thr.
+__device__ __forceinline__ bool mc_inside(float v, double thr) { return static_cast<double>(v) > thr; }
 
-// bit a set: the edge from (i,j,k) along axis a exists and changes sign
-__device__ __forceinline__ unsigned mc_point_mask(const McParams& p, long long i, long long j, long long k) {
-  const bool c = mc_in(p, i, j, k);
+// bit a set: the edge from (i,j,k) along axis a exists in an (n0, n1, n2) grid and changes sign
+template <class In>
+__device__ __forceinline__ unsigned mc_edge_mask(const In& in, long long i, long long j, long long k, long long n0,
+                                                 long long n1, long long n2) {
+  const bool c = in(i, j, k);
   unsigned m = 0;
-  if (i + 1 < p.n0 && mc_in(p, i + 1, j, k) != c) m |= 1u;
-  if (j + 1 < p.n1 && mc_in(p, i, j + 1, k) != c) m |= 2u;
-  if (k + 1 < p.n2 && mc_in(p, i, j, k + 1) != c) m |= 4u;
+  if (i + 1 < n0 && in(i + 1, j, k) != c) m |= 1u;
+  if (j + 1 < n1 && in(i, j + 1, k) != c) m |= 2u;
+  if (k + 1 < n2 && in(i, j, k + 1) != c) m |= 4u;
   return m;
 }
 
-__device__ __forceinline__ unsigned mc_cube_index(const McParams& p, long long i, long long j, long long k) {
+// bit c set: corner (i + (c & 1), j + (c >> 1 & 1), k + (c >> 2 & 1)) of cell (i, j, k) is inside
+template <class In>
+__device__ __forceinline__ unsigned mc_cube(const In& in, long long i, long long j, long long k) {
   unsigned cube = 0;
 #pragma unroll
   for (int c = 0; c < 8; ++c)
-    if (mc_in(p, i + (c & 1), j + ((c >> 1) & 1), k + ((c >> 2) & 1))) cube |= 1u << c;
+    if (in(i + (c & 1), j + ((c >> 1) & 1), k + ((c >> 2) & 1))) cube |= 1u << c;
   return cube;
+}
+
+// Edge e of the case table (nb_mc_tri_edges): its axis and the offset d of its lower endpoint from the cell's corner.
+__device__ __forceinline__ int mc_edge_endpoint(int e, long long d[3]) {
+  const int axis = e >> 2, r = e & 3;
+  const int o1 = axis == 0 ? 1 : 0, o2 = axis == 2 ? 1 : 2;   // the two other axes, increasing
+  d[0] = d[1] = d[2] = 0;
+  d[o1] = r & 1;
+  d[o2] = r >> 1;
+  return axis;
+}
+
+// The vertex on the edge from (i, j, k) along `axis` with values f0 -> f1: a + (thr - f0)/(f1 - f0) on that axis,
+// in double.
+__device__ __forceinline__ void mc_vertex(long long i, long long j, long long k, int axis, double thr, float f0,
+                                          float f1, double* out) {
+  const double a = static_cast<double>(f0), b = static_cast<double>(f1);
+  const double t = __ddiv_rn(__dsub_rn(thr, a), __dsub_rn(b, a));
+  double pos[3] = {static_cast<double>(i), static_cast<double>(j), static_cast<double>(k)};
+  pos[axis] = __dadd_rn(pos[axis], t);
+  out[0] = pos[0];
+  out[1] = pos[1];
+  out[2] = pos[2];
+}
+
+__device__ __forceinline__ bool mc_in(const McParams& p, long long i, long long j, long long k) {
+  return mc_inside(p.sigma[(i * p.n1 + j) * p.n2 + k], p.thr);
+}
+
+__device__ __forceinline__ unsigned mc_point_mask(const McParams& p, long long i, long long j, long long k) {
+  return mc_edge_mask([&](long long a, long long b, long long c) { return mc_in(p, a, b, c); }, i, j, k, p.n0, p.n1,
+                      p.n2);
+}
+
+__device__ __forceinline__ unsigned mc_cube_index(const McParams& p, long long i, long long j, long long k) {
+  return mc_cube([&](long long a, long long b, long long c) { return mc_in(p, a, b, c); }, i, j, k);
 }
 
 __global__ void mc_classify_kernel(McParams p) {
@@ -102,19 +142,12 @@ __global__ void mc_emit_vertices_kernel(McParams p) {
     if (p.vcnt[q] == 0) continue;
     const long long i = q / (p.n1 * p.n2), j = (q / p.n2) % p.n1, k = q % p.n2;
     const unsigned m = mc_point_mask(p, i, j, k);
-    const double f0 = static_cast<double>(p.sigma[q]);
     long long v = p.vofs[q];
     const long long step[3] = {p.n1 * p.n2, p.n2, 1};
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
       if (!(m & (1u << a))) continue;
-      const double f1 = static_cast<double>(p.sigma[q + step[a]]);
-      const double t = __ddiv_rn(__dsub_rn(p.thr, f0), __dsub_rn(f1, f0));
-      double pos[3] = {static_cast<double>(i), static_cast<double>(j), static_cast<double>(k)};
-      pos[a] = __dadd_rn(pos[a], t);
-      p.vertices[v * 3 + 0] = pos[0];
-      p.vertices[v * 3 + 1] = pos[1];
-      p.vertices[v * 3 + 2] = pos[2];
+      mc_vertex(i, j, k, a, p.thr, p.sigma[q], p.sigma[q + step[a]], p.vertices + v * 3);
       ++v;
     }
   }
@@ -132,12 +165,8 @@ __global__ void mc_emit_triangles_kernel(McParams p) {
     long long out = p.cofs[c];
     for (int t = 0; t < nt; ++t) {
       for (int s = 0; s < 3; ++s) {
-        const int e = nb_mc_tri_edges[cube][t * 3 + s];
-        const int axis = e >> 2, r = e & 3;
-        const int o1 = axis == 0 ? 1 : 0, o2 = axis == 2 ? 1 : 2;   // the two other axes, increasing
-        long long d[3] = {0, 0, 0};
-        d[o1] = r & 1;
-        d[o2] = r >> 1;
+        long long d[3];
+        const int axis = mc_edge_endpoint(nb_mc_tri_edges[cube][t * 3 + s], d);
         const long long qi = i + d[0], qj = j + d[1], qk = k + d[2];
         const unsigned below = mc_point_mask(p, qi, qj, qk) & ((1u << axis) - 1u);
         p.triangles[out * 3 + s] = p.vofs[(qi * p.n1 + qj) * p.n2 + qk] + __popc(below);

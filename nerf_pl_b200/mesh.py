@@ -127,6 +127,42 @@ def marching_cubes(sigma: torch.Tensor, threshold: float) -> Tuple[torch.Tensor,
     return verts, tris
 
 
+SPARSE_MC_MAX_N = 2048
+
+
+@torch.no_grad()
+def sparse_marching_cubes(model: torch.nn.Module, N: int, x_range, y_range, z_range, threshold: float, *,
+                          occupancy: OccupancyGrid) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``marching_cubes(sigma_grid(model, N, x_range, y_range, z_range, occupancy=occupancy), threshold)`` without the
+    dense N^3 grid, for N in [2, 2048]: the same index-space vertices (V, 3) float64 and triangles (T, 3) int32, bit
+    for bit and in the same order (DESIGN.md §10i).  Only the 8^3-point bricks that hold a point the grid evaluates
+    (and their lower neighbours) are queried, stored and marched, so memory follows the occupied volume."""
+    dev = _device_of(model)
+    occ = _check_occupancy(occupancy, dev)
+    N = int(N)
+    if not 2 <= N <= SPARSE_MC_MAX_N:
+        raise ValueError(f"sparse_marching_cubes: N = {N} outside [2, {SPARSE_MC_MAX_N}]")
+    lib = _lib.load()
+    ranges = _lib.ranges_host(x_range, y_range, z_range)
+    occ_ranges = (ctypes.c_double * 6)(*occ.ranges)
+    plan = _lib.workspace(lib.nerfb200_sparse_mc_plan_workspace_bytes(N), dev)
+    bricks = (ctypes.c_int64 * 2)()
+    _lib.call("nerfb200_sparse_mc_plan", dev, N, ranges, occ.bits.data_ptr(), occ.grid_n(), occ_ranges,
+              plan.data_ptr(), plan.numel(), bricks)
+    ws = _lib.workspace(lib.nerfb200_sparse_mc_workspace_bytes(N, bricks[0], bricks[1]), dev)
+    counts = (ctypes.c_int64 * 2)()
+    _lib.call("nerfb200_sparse_mc_count", dev, packed_weights(model).data_ptr(), N, ranges, occ.bits.data_ptr(),
+              occ.grid_n(), occ_ranges, float(threshold), plan.data_ptr(), plan.numel(), bricks, ws.data_ptr(),
+              ws.numel(), counts)
+    verts = torch.empty(counts[0], 3, dtype=torch.float64, device=dev)
+    tris = torch.empty(counts[1], 3, dtype=torch.int32, device=dev)
+    emit = _lib.workspace(lib.nerfb200_sparse_mc_emit_workspace_bytes(counts[0], counts[1]), dev)
+    _lib.call("nerfb200_sparse_mc_emit", dev, N, float(threshold), plan.data_ptr(), plan.numel(), bricks,
+              ws.data_ptr(), ws.numel(), counts, emit.data_ptr(), emit.numel(),
+              verts.data_ptr() if counts[0] else None, tris.data_ptr() if counts[1] else None)
+    return verts, tris
+
+
 @torch.no_grad()
 def to_world(vertices: torch.Tensor, N: int, x_range, y_range, z_range) -> torch.Tensor:
     """extract_color_mesh.py:148-154 on the device, quirks included: divides by N (not N - 1) and swaps the
@@ -162,11 +198,16 @@ def extract_mesh(model: torch.nn.Module, N_grid: int, x_range, y_range, z_range,
                  keep_largest: bool = True, *,
                  occupancy: Optional[OccupancyGrid] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """extract_color_mesh.py:113-171: world vertices (V, 3) fp32 and triangles (T, 3) int32 on the device.
-    ``occupancy``: the sigma grid is ``sigma_grid(..., occupancy=occupancy)``, so density the grid calls empty
-    never reaches marching cubes."""
-    sigma = sigma_grid(model, N_grid, x_range, y_range, z_range, occupancy=occupancy)
-    vidx, tris = marching_cubes(sigma, sigma_threshold)
-    del sigma
+    ``occupancy``: the mesh is ``marching_cubes(sigma_grid(..., occupancy=occupancy), sigma_threshold)``, so density
+    the grid calls empty never reaches marching cubes; it is computed by ``sparse_marching_cubes``, which never builds
+    the dense grid, so N_grid may go up to 2048."""
+    if occupancy is not None:
+        vidx, tris = sparse_marching_cubes(model, N_grid, x_range, y_range, z_range, sigma_threshold,
+                                           occupancy=occupancy)
+    else:
+        sigma = sigma_grid(model, N_grid, x_range, y_range, z_range)
+        vidx, tris = marching_cubes(sigma, sigma_threshold)
+        del sigma
     verts = to_world(vidx, N_grid, x_range, y_range, z_range)
     if keep_largest:
         verts, tris = keep_largest_cluster(verts, tris)
