@@ -6,6 +6,7 @@ from .nerf import (Embedding, NeRF, invalidate_packed, nerf_forward_fused, nerf_
                    packed_weights)
 from .culling import (OccupancyGrid, cull_rays, level_ranges, occupancy_cascade, occupancy_grid, pack_occupancy,
                       render_rays_culled, scatter_results)
+from .baked import BakedVolume, bake_volume, render_baked
 from .data import DeviceRayBatches, DeviceViewBatches
 from .density_grid import DensityGrid
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
@@ -27,6 +28,7 @@ __all__ = [
     "vertex_normals", "normal_rays", "normal_vertex_colors",
     "OccupancyGrid", "occupancy_grid", "pack_occupancy", "cull_rays", "scatter_results", "render_rays_culled",
     "level_ranges", "occupancy_cascade",
+    "BakedVolume", "bake_volume", "render_baked",
     "DensityGrid",
     "ssim", "visualize_depth",
     "DeviceViewBatches", "Views", "read_blender_views", "read_llff_views",

@@ -24,10 +24,12 @@ SOURCES = ["capi.cu"]
 HEADERS = ["ptx.cuh", "layout.h", "mlp_engine.cuh", "render_kernel.cuh", "aux_kernels.cuh", "bwd_kernels.cuh",
            "mesh_kernels.cuh", "mc_table.h", "occupancy_kernels.cuh", "metrics_kernels.cuh", "jet_lut.h", "sample_skip_kernels.cuh",
            "train_skip_kernels.cuh", "density_kernels.cuh", "masked_grid_kernels.cuh", "early_stop_kernels.cuh",
-           "sparse_mc_kernels.cuh"]
+           "sparse_mc_kernels.cuh", "baked_kernels.cuh"]
 INCLUDES = ["nerf_pl_b200.h"]
 # the entries of the sparse marching cubes, declared in their own header (SPARSE_MC_SIGNATURES)
 SPARSE_MC_INCLUDE = "nerf_pl_b200_sparse_mc.h"
+# the entries of the baked volumes, declared in their own header (BAKED_SIGNATURES)
+BAKED_INCLUDE = "nerf_pl_b200_baked.h"
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -304,6 +306,19 @@ SPARSE_MC_SIGNATURES = {
                                        _vp, _vp]),
 }
 
+# Every entry include/nerf_pl_b200_baked.h declares, in header order, as SIGNATURES.
+BAKED_SIGNATURES = {
+    "nerfb200_baked_bytes": (_sz, [_i64, _i64]),
+    "nerfb200_baked_workspace_bytes": (_sz, [_i64, _i64, _i64]),
+    "nerfb200_baked_bake": (_i32, [_vp, _i64, POINTER(_f64), _vp, _i64, POINTER(_f64), _vp, _sz, POINTER(_i64), _vp, _sz,
+                                   _vp, _sz, _vp]),
+    "nerfb200_baked_from_grid_count": (_i32, [_vp, _i64, _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_baked_from_grid": (_i32, [_vp, _i64, _vp, _sz, _i64, _vp, _sz, _vp]),
+    "nerfb200_baked_to_dense": (_i32, [_vp, _sz, _i64, _i64, _vp, _vp]),
+    "nerfb200_baked_render": (_i32, [_vp, _sz, _i64, POINTER(_f64), _i64, _vp, _i64, _f64, _i32, _f64, _vp, _vp, _vp,
+                                     _vp]),
+}
+
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
@@ -317,7 +332,7 @@ def needs_build() -> bool:
         return True
     t = os.path.getmtime(LIB_PATH)
     deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS]
-    deps += [os.path.join(_HERE, "..", "include", f) for f in INCLUDES + [SPARSE_MC_INCLUDE]]
+    deps += [os.path.join(_HERE, "..", "include", f) for f in INCLUDES + [SPARSE_MC_INCLUDE, BAKED_INCLUDE]]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
@@ -351,7 +366,7 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (restype, argtypes) in {**SIGNATURES, **SPARSE_MC_SIGNATURES}.items():
+            for name, (restype, argtypes) in {**SIGNATURES, **SPARSE_MC_SIGNATURES, **BAKED_SIGNATURES}.items():
                 fn = getattr(lib, name)
                 fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:

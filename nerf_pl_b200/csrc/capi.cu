@@ -22,7 +22,9 @@
 #include "masked_grid_kernels.cuh"
 #include "early_stop_kernels.cuh"
 #include "sparse_mc_kernels.cuh"
+#include "baked_kernels.cuh"
 #include "../../include/nerf_pl_b200_sparse_mc.h"
+#include "../../include/nerf_pl_b200_baked.h"
 
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -1327,6 +1329,89 @@ int smc_select(const SparseMcParams& p, CubScratch& sc, int* out, int* count, cu
   const long long B = p.nb * p.nb * p.nb;
   return cub_launch(cub::DeviceSelect::Flagged(sc.temp, tb, SmcIndexIt(0), p.flag, out, count, static_cast<int>(B), s),
                     what);
+}
+
+// The evaluated points of the A > 0 active bricks through the point query on compacted rows: their row counts (rcnt)
+// and first rows (p.rofs), then per kSmcChunkBricks bricks the rows (smc_sigma_emit_kernel), the query into p.out
+// (sigma, or with `rgb` the four channels of nerfb200_query_rgb_sigma) and `scatter(rows)`, which enqueues the chunk's
+// scatter.  Reads the chunks' row bounds back, so it synchronises.
+template <class Scatter>
+int smc_query(SparseMcParams& p, const CubScratch& sc, unsigned long long* rcnt, long long A, const void* packed,
+              bool rgb, cudaStream_t s, Scatter&& scatter) {
+  TRY(launch("sparse_mc row counts launch", smc_row_counts_kernel, grid_blocks(A + 1, 256), 256, 0, s, p, rcnt));
+  size_t tb = sc.temp_bytes;
+  TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, rcnt, p.rofs, static_cast<int>(A + 1), s), "sparse_mc row scan"));
+  const long long chunks = ceil_div(A, kSmcChunkBricks);
+  std::vector<unsigned long long> bound(chunks + 1);
+  CUDA_TRY(cudaMemcpy2DAsync(bound.data(), sizeof(unsigned long long), p.rofs, kSmcChunkBricks * sizeof(unsigned long long),
+                             sizeof(unsigned long long), chunks, cudaMemcpyDeviceToHost, s), "sparse_mc row readback");
+  CUDA_TRY(cudaMemcpyAsync(bound.data() + chunks, p.rofs + A, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s),
+           "sparse_mc row readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "sparse_mc row readback");
+  for (long long c = 0; c < chunks; ++c) {
+    const long long rows = static_cast<long long>(bound[c + 1] - bound[c]);
+    if (rows == 0) continue;
+    p.slot0 = c * kSmcChunkBricks;
+    p.slots = std::min(kSmcChunkBricks, A - p.slot0);
+    TRY(launch("sparse_mc sigma emit launch", smc_sigma_emit_kernel, grid_blocks(p.slots, 1), kBrickPoints, 0, s, p));
+    TRY(rgb ? nerfb200_query_rgb_sigma(p.xyz, rows, 3, packed, p.out, s)
+            : nerfb200_query_sigma(p.xyz, rows, 3, packed, p.out, s));
+    TRY(scatter(rows));
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------ baked volumes
+// (kernels: baked_kernels.cuh, entries: include/nerf_pl_b200_baked.h).  The brick plan and its workspace are the
+// sparse marching cubes' (nerfb200_sparse_mc_plan); a volume stores the plan's march bricks.
+size_t baked_bytes(long long N, long long bricks) {
+  const long long nb = smc_bricks(N);
+  return static_cast<size_t>(bricks) * kBakedPoints * sizeof(float4) + static_cast<size_t>(nb * nb * nb) * sizeof(int);
+}
+
+bool baked_bricks_ok(long long N, long long bricks) {
+  const long long nb = smc_bricks(N);
+  return N >= 2 && N <= kSmcMaxN && bricks >= 0 && bricks <= nb * nb * nb;
+}
+
+// The bake's workspace for A active bricks: the row counts and offsets, one query's rows (positions, destinations and
+// four outputs each) and the scan's scratch.
+size_t baked_carve(long long A, void* base, SparseMcParams* p, unsigned long long** rcnt, CubScratch* s) {
+  const long long rows = std::min(A, kSmcChunkBricks) * kBrickPoints;
+  size_t tb = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tb, static_cast<const unsigned long long*>(nullptr),
+                                static_cast<unsigned long long*>(nullptr), static_cast<int>(A + 1));
+  s->temp_bytes = tb;
+  Carver c{static_cast<uint8_t*>(base), 0, 256};
+  *rcnt = c.take<unsigned long long>(A + 1);
+  p->rofs = c.take<unsigned long long>(A + 1);
+  p->xyz = c.take<float>(rows * 3);
+  p->dst = c.take<long long>(rows);
+  p->out = c.take<float>(rows * 4);
+  s->temp = c.take(s->temp_bytes);
+  return c.off;
+}
+
+// A volume buffer of `bricks` stored bricks at N: its data and map.
+int baked_volume(const void* volume, size_t volume_bytes, int64_t N, int64_t bricks, float4** data, int** map,
+                 const char* who) {
+  if (N < 2 || N > kSmcMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 2048]", who);
+  if (!baked_bricks_ok(N, bricks)) return fail(NERFB200_EINVAL, "%s: bricks must be in [0, ceil(N / 8)^3]", who);
+  if (!volume) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (volume_bytes != baked_bytes(N, bricks))
+    return fail(NERFB200_EINVAL, "%s: volume_bytes differs from nerfb200_baked_bytes(N, bricks)", who);
+  *data = static_cast<float4*>(const_cast<void*>(volume));
+  *map = reinterpret_cast<int*>(static_cast<uint8_t*>(const_cast<void*>(volume)) +
+                                static_cast<size_t>(bricks) * kBakedPoints * sizeof(float4));
+  return 0;
+}
+
+// The map of the `count` bricks of `list` (device values) and zeroed data.
+int baked_map(const int* list, const int* count, long long nb, long long bricks, float4* data, int* map, cudaStream_t s) {
+  CUDA_TRY(cudaMemsetAsync(map, 0xff, static_cast<size_t>(nb * nb * nb) * sizeof(int), s), "baked memset");
+  if (bricks == 0) return 0;
+  CUDA_TRY(cudaMemsetAsync(data, 0, static_cast<size_t>(bricks) * kBakedPoints * sizeof(float4), s), "baked memset");
+  return launch("baked map launch", baked_map_kernel, grid_blocks(bricks, 256), 256, 0, s, list, count, map);
 }
 
 // ------------------------------------------------------------------ training with empty samples skipped
@@ -3025,30 +3110,14 @@ int nerfb200_sparse_mc_count(const void* packed, int64_t N, const double ranges_
     return 0;
   }
   // sigma: rows of the active bricks in order, one point query per kSmcChunkBricks bricks
-  TRY(launch("sparse_mc row counts launch", smc_row_counts_kernel, grid_blocks(A + 1, 256), 256, 0, s, p, rcnt));
-  size_t tb = sc.temp_bytes;
-  TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, rcnt, p.rofs, static_cast<int>(A + 1), s), "sparse_mc row scan"));
   CUDA_TRY(cudaMemsetAsync(p.vals, 0, static_cast<size_t>(A) * kBrickPoints * sizeof(float), s), "sparse_mc memset");
-  const long long chunks = ceil_div(A, kSmcChunkBricks);
-  std::vector<unsigned long long> bound(chunks + 1);
-  CUDA_TRY(cudaMemcpy2DAsync(bound.data(), sizeof(unsigned long long), p.rofs, kSmcChunkBricks * sizeof(unsigned long long),
-                             sizeof(unsigned long long), chunks, cudaMemcpyDeviceToHost, s), "sparse_mc row readback");
-  CUDA_TRY(cudaMemcpyAsync(bound.data() + chunks, p.rofs + A, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s),
-           "sparse_mc row readback");
-  CUDA_TRY(cudaStreamSynchronize(s), "sparse_mc row readback");
-  for (long long c = 0; c < chunks; ++c) {
-    const long long rows = static_cast<long long>(bound[c + 1] - bound[c]);
-    if (rows == 0) continue;
-    p.slot0 = c * kSmcChunkBricks;
-    p.slots = std::min(kSmcChunkBricks, A - p.slot0);
-    TRY(launch("sparse_mc sigma emit launch", smc_sigma_emit_kernel, grid_blocks(p.slots, 1), kBrickPoints, 0, s, p));
-    TRY(nerfb200_query_sigma(p.xyz, rows, 3, packed, p.out, stream));
-    TRY(launch("sparse_mc sigma scatter launch", smc_sigma_scatter_kernel, grid_blocks(rows, 256), 256, 0, s, p, rows));
-  }
+  TRY(smc_query(p, sc, rcnt, A, packed, false, s, [&](long long rows) {
+    return launch("sparse_mc sigma scatter launch", smc_sigma_scatter_kernel, grid_blocks(rows, 256), 256, 0, s, p, rows);
+  }));
   // march: vertices and triangles per march brick
   CUDA_TRY(cudaMemsetAsync(p.bcnt + Mb, 0, sizeof(unsigned), s), "sparse_mc count memset");
   TRY(launch("sparse_mc march count launch", smc_march_count_kernel, grid_blocks(Mb, 1), kBrickPoints, 0, s, p));
-  tb = sc.temp_bytes;
+  size_t tb = sc.temp_bytes;
   TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, SmcVertIt(p.bcnt, SmcVerts()), p.vofs,
                                                static_cast<int>(Mb + 1), s), "sparse_mc vertex scan"));
   tb = sc.temp_bytes;
@@ -3123,6 +3192,150 @@ int nerfb200_sparse_mc_emit(int64_t N, double threshold, void* plan_ws, size_t p
   TRY(launch("sparse_mc vertices launch", smc_vertices_kernel, grid_blocks(V, 256), 256, 0, s, p));
   TRY(launch("sparse_mc triangles launch", smc_triangles_kernel, grid_blocks(T, 256), 256, 0, s, p));
   return 0;
+}
+
+// ---- baked volumes (include/nerf_pl_b200_baked.h, kernels: baked_kernels.cuh)
+size_t nerfb200_baked_bytes(int64_t N, int64_t bricks) {
+  return baked_bricks_ok(N, bricks) ? baked_bytes(N, bricks) : 0;
+}
+
+size_t nerfb200_baked_workspace_bytes(int64_t N, int64_t active, int64_t march) {
+  if (!smc_counts_ok(N, active, march)) return 0;
+  SparseMcParams p{};
+  unsigned long long* rcnt;
+  CubScratch sc;
+  return baked_carve(active, nullptr, &p, &rcnt, &sc);
+}
+
+int nerfb200_baked_bake(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits, int64_t occ_N,
+                        const double occ_ranges_host[6], void* plan_ws, size_t plan_bytes, const int64_t bricks_host[2],
+                        void* ws, size_t bytes, void* volume, size_t volume_bytes, void* stream) {
+  const char* who = "baked_bake";
+  SparseMcParams p{};
+  TRY(smc_grids(N, ranges_host, bits, occ_N, occ_ranges_host, &p, who));
+  if (!packed || !plan_ws || !bricks_host || !ws || !volume) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  const long long A = bricks_host[0], Mb = bricks_host[1];
+  if (!smc_counts_ok(N, A, Mb)) return fail(NERFB200_EINVAL, "%s: bricks_host is not a plan's {active, march}", who);
+  CubScratch sc, sq;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  unsigned long long* rcnt;
+  if (bytes < baked_carve(A, ws, &p, &rcnt, &sq))
+    return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_baked_workspace_bytes(N, active, march)", who);
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, Mb, &data, &map, who));
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int h[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(h, p.nsel + 1, sizeof(h), cudaMemcpyDeviceToHost, s), "baked bake readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "baked bake readback");
+  if (h[0] != A || h[1] != Mb) return fail(NERFB200_EINVAL, "%s: bricks_host differs from the plan's", who);
+  TRY(baked_map(p.march, p.nsel + 2, p.nb, Mb, data, map, s));
+  if (A == 0) return 0;
+  TRY(smc_query(p, sq, rcnt, A, packed, true, s, [&](long long rows) {
+    return launch("baked scatter launch", baked_scatter_kernel, grid_blocks(rows, 256), 256, 0, s, p, map, data, rows);
+  }));
+  return launch("baked apron launch", baked_apron_kernel, grid_blocks(Mb * kBakedPoints, 256), 256, 0, s, p.march,
+                p.nsel + 2, map, p.nb, data);
+}
+
+int nerfb200_baked_from_grid_count(const float* rgbsigma, int64_t N, void* plan_ws, size_t plan_bytes,
+                                   int64_t bricks_host[1], void* stream) {
+  const char* who = "baked_from_grid_count";
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
+  if (!rgbsigma || !plan_ws || !bricks_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  SparseMcParams p{};
+  p.nb = smc_bricks(N);
+  CubScratch sc;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long B = p.nb * p.nb * p.nb;
+  TRY(launch("baked grid flag launch", baked_grid_flag_kernel, grid_blocks(B, 1), 256, 0, s,
+             reinterpret_cast<const float4*>(rgbsigma), static_cast<long long>(N), p.nb, p.flag));
+  TRY(smc_select(p, sc, p.march, p.nsel + 2, s, "baked grid select"));
+  int h = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h, p.nsel + 2, sizeof(h), cudaMemcpyDeviceToHost, s), "baked from_grid readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "baked from_grid readback");
+  bricks_host[0] = h;
+  return 0;
+}
+
+int nerfb200_baked_from_grid(const float* rgbsigma, int64_t N, void* plan_ws, size_t plan_bytes, int64_t bricks,
+                             void* volume, size_t volume_bytes, void* stream) {
+  const char* who = "baked_from_grid";
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
+  if (!rgbsigma || !plan_ws) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who));
+  SparseMcParams p{};
+  p.nb = smc_bricks(N);
+  CubScratch sc;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int h = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h, p.nsel + 2, sizeof(h), cudaMemcpyDeviceToHost, s), "baked from_grid readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "baked from_grid readback");
+  if (h != bricks) return fail(NERFB200_EINVAL, "%s: bricks differs from nerfb200_baked_from_grid_count's", who);
+  TRY(baked_map(p.march, p.nsel + 2, p.nb, bricks, data, map, s));
+  if (bricks == 0) return 0;
+  return launch("baked grid copy launch", baked_grid_copy_kernel, grid_blocks(bricks * kBakedPoints, 256), 256, 0, s,
+                reinterpret_cast<const float4*>(rgbsigma), static_cast<long long>(N), p.march, p.nsel + 2, p.nb, data);
+}
+
+int nerfb200_baked_to_dense(const void* volume, size_t volume_bytes, int64_t N, int64_t bricks, float* rgbsigma,
+                            void* stream) {
+  const char* who = "baked_to_dense";
+  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who));
+  if (!rgbsigma) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  return launch("baked to_dense launch", baked_to_dense_kernel, grid_blocks(N * N * N, 256), 256, 0, stream, data, map,
+                static_cast<long long>(N), smc_bricks(N), reinterpret_cast<float4*>(rgbsigma));
+}
+
+int nerfb200_baked_render(const void* volume, size_t volume_bytes, int64_t N, const double ranges_host[6], int64_t bricks,
+                          const float* rays, int64_t n_rays, double step, int32_t white_back, double early_stop,
+                          float* rgb, float* depth, float* opacity, void* stream) {
+  const char* who = "baked_render";
+  BakedRenderParams r{};
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who));
+  if (!ranges_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  for (int a = 0; a < 3; ++a) {
+    const float lo = static_cast<float>(ranges_host[2 * a]), hi = static_cast<float>(ranges_host[2 * a + 1]);
+    const float scale = static_cast<float>(static_cast<double>(N - 1) / (ranges_host[2 * a + 1] - ranges_host[2 * a]));
+    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi || !std::isfinite(scale) || scale == 0.f)
+      return fail(NERFB200_EINVAL, "%s: every range must be finite with min != max in float32", who);
+    r.lo[a] = lo;
+    r.scale[a] = scale;
+  }
+  const float s32 = static_cast<float>(step);
+  if (!(step > 0.0) || !std::isfinite(s32) || !(s32 > 0.f))
+    return fail(NERFB200_EINVAL, "%s: step must be > 0 and finite in float32", who);
+  if (!(early_stop >= 0.0 && early_stop <= 1.0)) return fail(NERFB200_EINVAL, "%s: early_stop must be in [0, 1]", who);
+  if (white_back != 0 && white_back != 1) return fail(NERFB200_EINVAL, "%s: white_back must be 0 or 1", who);
+  if (n_rays < 0) return fail(NERFB200_EINVAL, "%s: n_rays < 0", who);
+  if (n_rays > 0 && (!rays || !rgb || !depth || !opacity)) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (n_rays == 0) return 0;
+  r.data = data;
+  r.map = map;
+  r.N = static_cast<int>(N);
+  r.nb = static_cast<int>(smc_bricks(N));
+  r.step = s32;
+  r.eps = static_cast<float>(early_stop);
+  r.white_back = static_cast<float>(white_back);
+  r.rays = rays;
+  r.n = n_rays;
+  r.rgb = rgb;
+  r.depth = depth;
+  r.opacity = opacity;
+  return launch("baked render launch", baked_render_kernel, grid_blocks(n_rays, kBakedThreads, 0x7fffffffLL),
+                kBakedThreads, 0, stream, r);
 }
 
 }  // extern "C"
