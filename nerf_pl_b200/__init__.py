@@ -12,7 +12,7 @@ from .density_grid import DensityGrid
 from .inference import batched_inference, generate_rays, mse_psnr, query_sigma, render_image, to_uint8
 from .mesh import (extract_mesh, fuse_vertex_colors, marching_cubes, normal_rays, normal_vertex_colors, pack_volume,
                    sparse_marching_cubes,
-                   query_rgb_sigma, rgb_sigma_grid, sigma_grid, vertex_normals, write_ply, write_vol)
+                   query_rgb_sh, query_rgb_sigma, rgb_sigma_grid, sigma_grid, vertex_normals, write_ply, write_vol)
 from .metrics import ssim, visualize_depth
 from .optim import FusedAdam
 from .rendering import render_rays, render_rays_host, render_rays_loss, sample_pdf, searchsorted, volume_render
@@ -24,7 +24,7 @@ __all__ = [
     "nerf_forward_fused", "nerf_forward_torch", "nerf_forward_train", "nerf_parameters", "packed_weights",
     "batched_inference", "generate_rays", "render_image", "to_uint8", "query_sigma", "mse_psnr",
     "sigma_grid", "marching_cubes", "sparse_marching_cubes", "extract_mesh", "fuse_vertex_colors", "write_ply",
-    "query_rgb_sigma", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
+    "query_rgb_sigma", "query_rgb_sh", "rgb_sigma_grid", "pack_volume", "write_vol", "DeviceRayBatches", "CapturedTrainStep",
     "vertex_normals", "normal_rays", "normal_vertex_colors",
     "OccupancyGrid", "occupancy_grid", "pack_occupancy", "cull_rays", "scatter_results", "render_rays_culled",
     "level_ranges", "occupancy_cascade",

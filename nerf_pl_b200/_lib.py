@@ -30,6 +30,8 @@ INCLUDES = ["nerf_pl_b200.h"]
 SPARSE_MC_INCLUDE = "nerf_pl_b200_sparse_mc.h"
 # the entries of the baked volumes, declared in their own header (BAKED_SIGNATURES)
 BAKED_INCLUDE = "nerf_pl_b200_baked.h"
+# the entries of the view-dependent baked volumes, declared in their own header (BAKED_SH_SIGNATURES)
+BAKED_SH_INCLUDE = "nerf_pl_b200_baked_sh.h"
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -319,6 +321,22 @@ BAKED_SIGNATURES = {
                                      _vp]),
 }
 
+# Every entry include/nerf_pl_b200_baked_sh.h declares, in header order, as SIGNATURES.
+BAKED_SH_SIGNATURES = {
+    "nerfb200_baked_sh_bytes": (_sz, [_i64, _i64]),
+    "nerfb200_baked_sh_workspace_bytes": (_sz, [_i64, _i64, _i64]),
+    "nerfb200_baked_sh_bake": (_i32, [_vp, _i64, POINTER(_f64), _vp, _i64, POINTER(_f64), _vp, _sz, POINTER(_i64), _vp,
+                                      _sz, _vp, _sz, _vp]),
+    "nerfb200_baked_sh_from_grid_count": (_i32, [_vp, _i64, _vp, _sz, POINTER(_i64), _vp]),
+    "nerfb200_baked_sh_from_grid": (_i32, [_vp, _i64, _vp, _sz, _i64, _vp, _sz, _vp]),
+    "nerfb200_baked_sh_to_dense": (_i32, [_vp, _sz, _i64, _i64, _vp, _vp]),
+    "nerfb200_baked_sh_render": (_i32, [_vp, _sz, _i64, POINTER(_f64), _i64, _vp, _i64, _f64, _i32, _f64, _vp, _vp,
+                                        _vp, _vp]),
+    "nerfb200_query_rgb_sh_workspace_bytes": (_sz, []),
+    "nerfb200_query_rgb_sh": (_i32, [_vp, _i64, _i64, _vp, _vp, _sz, _vp, _vp]),
+    "nerfb200_sh_fit_host": (_i32, [POINTER(_f32), POINTER(_f32)]),
+}
+
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", "nvcc"):
@@ -332,7 +350,7 @@ def needs_build() -> bool:
         return True
     t = os.path.getmtime(LIB_PATH)
     deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS]
-    deps += [os.path.join(_HERE, "..", "include", f) for f in INCLUDES + [SPARSE_MC_INCLUDE, BAKED_INCLUDE]]
+    deps += [os.path.join(_HERE, "..", "include", f) for f in INCLUDES + [SPARSE_MC_INCLUDE, BAKED_INCLUDE, BAKED_SH_INCLUDE]]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
@@ -366,7 +384,7 @@ def load() -> ctypes.CDLL:
                     f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                     "(nerf_pl_b200 has no CPU fallback)")
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (restype, argtypes) in {**SIGNATURES, **SPARSE_MC_SIGNATURES, **BAKED_SIGNATURES}.items():
+            for name, (restype, argtypes) in {**SIGNATURES, **SPARSE_MC_SIGNATURES, **BAKED_SIGNATURES, **BAKED_SH_SIGNATURES}.items():
                 fn = getattr(lib, name)
                 fn.restype, fn.argtypes = restype, argtypes
             if lib.nerfb200_abi_version() != ABI_VERSION:

@@ -154,6 +154,8 @@ struct MlpParams {
   const __half* dirrow;
   // and the row count: *n_dev rows (the launch is sized for p.n, the carved worst case); tr.n_pad is derived from it
   const long long* n_dev;
+  // SH mode (kSh; raw_xyz): the table of sh_table_kernel (kShTableFloats), out is (n, kShOut)
+  const float* sh;
 };
 constexpr int kSkipDirStride = 2 * kDirW;   // per ray: the coarse network's direction bias, then the fine one's
 
@@ -166,7 +168,9 @@ constexpr int kSkipDirStride = 2 * kDirW;   // per ray: the coarse network's dir
 // gW_dir[:, 256:283].  Padding rows of the last tile are stored as copies of row n - 1 (their gradient is 0), so every
 // row below n_pad is written by this launch whatever an earlier, longer launch left in the workspace.  Its row count is
 // read on the device (n_dev), so a CUDA graph can capture the launch; CTAs past the count's tiles write nothing.
-template <bool kSave, bool kRowsSave = false>
+// kSh (raw positions, not kSave): the SH mode of DESIGN.md §10k.  One trunk pass and the direction layer's MMAs per
+// row, then per direction of the table its rgb and the projection (epi_sh); out receives kShOut floats per row.
+template <bool kSave, bool kRowsSave = false, bool kSh = false>
 __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   Scratch* sc = reinterpret_cast<Scratch*>(smem + kSmemScratch);
@@ -176,6 +180,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
     return;
   }
   load_consts(smem, 0, p.net);
+  if constexpr (kSh) {
+    float4* dst = reinterpret_cast<float4*>(smem + kSmemSh);
+    for (int i = threadIdx.x; i < kShTableFloats / 4; i += blockDim.x) dst[i] = __ldg(reinterpret_cast<const float4*>(p.sh) + i);
+  }
   __syncthreads();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -187,7 +195,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
     regs_dec<kRegsAux>();
     if (warp == kProducerWarp && lane == 0) {
       RingState rs;
-      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) produce_tile(rs, smem, bars, p.net, so, !so && !rows);
+      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) produce_tile(rs, smem, bars, p.net, so, !so && !rows && !kSh);
     }
   } else {
     regs_inc<kRegsConsumer>();
@@ -260,6 +268,20 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
       const DirSrc ds = p.raw_xyz ? DirSrc{kZeroDirRow.v, 0, tile * 128, p.n, nullptr}
                                   : DirSrc{p.x, p.x_stride, tile * 128, p.n, kSave ? p.xdir : nullptr};
       float sig[2], rgb[2][3];
+      if constexpr (kSh) {
+        float coef[2][kShLane];
+        wg_tile<false, false, false, true>(c, kSmemEnc, dbias, nullptr, sig, rgb, coef);
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const long long gi = tile * 128 + c.row[s];
+          if (gi >= p.n) continue;
+          const float sg = c.cst[kF32BSigma] + sig[s];
+          float* o = p.out + gi * kShOut + kShLane * c.q;
+#pragma unroll
+          for (int i = 0; i < kShLane; ++i) o[i] = (kShLane * c.q + i == 3) ? sg : coef[s][i];
+        }
+        continue;
+      }
       if (rows) {
         const float* rbias[2];
 #pragma unroll
@@ -311,6 +333,27 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_forward_kernel(const MlpParam
       }
     }
   }
+}
+
+// ------------------------------------------------ the SH mode's table (DESIGN.md §10k)
+// The fit's fixed directions (float32 unit vectors) and P = pinv(Y) (row m, column j), made on the host.
+struct ShFit {
+  float dirs[kShDirs * 3];
+  float proj[kShBasis * kShDirs];
+};
+static_assert(sizeof(ShFit) <= 4000, "ShFit is passed as a kernel parameter");
+
+// One block of kDirW threads per direction j: its bias row, the render path's dir_bias for a ray of direction d_j
+// (skip_dir_bias_kernel), and its projection weight per output float (mlp_engine.cuh).
+__global__ void __launch_bounds__(kDirW) sh_table_kernel(const __grid_constant__ ShFit fit, const uint8_t* net,
+                                                          float* table) {
+  __shared__ float direnc[28];
+  const int j = blockIdx.x, t = threadIdx.x;
+  if (t < 15) dir_embed_term(t, fit.dirs + 3 * j, direnc);
+  __syncthreads();
+  const float* f32 = reinterpret_cast<const float*>(net + kHalfRegionBytes);
+  table[j * kDirW + t] = dir_bias(f32, __ldg(f32 + kF32Bias + 8 * 256 + t), t, direnc);
+  if (t < kShOut) table[kShDirs * kDirW + j * kShOut + t] = t == 3 ? 0.f : fit.proj[(t < 3 ? 0 : (t - 1) / 3) * kShDirs + j];
 }
 
 // ------------------------------------------------ Embedding.forward (models/nerf.py:21-38)

@@ -15,6 +15,10 @@
 //             cell lies in.  A sample outside the box or in a brick that is not stored has sigma = 0, so alpha = 0:
 //             such runs of samples are jumped over, and a jump is taken only after the last sample it skips is found
 //             in the same brick as the first (see baked_skip), so skipping never changes a value.
+//
+// The kernels are templated on kW, the float4 count per point: 1 for the volume above, 7 for the view-dependent one
+// of DESIGN.md §10k, whose point is (c_r0, c_g0, c_b0, sigma) and then c_{r,g,b; m} for m = 1..8 (degree-2 spherical
+// harmonics of PlenOctrees' eval_sh); its render evaluates the colour at each ray's direction.
 #pragma once
 #include <cstdint>
 #include <cub/cub.cuh>
@@ -37,7 +41,8 @@ __global__ void baked_map_kernel(const int* list, const int* count, int* vmap) {
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n; s += gridDim.x * blockDim.x) vmap[list[s]] = s;
 }
 
-// Row r of the rgb + sigma query (p.out holds 4 floats per row) to its point in its march brick's storage.
+// Row r of the point query (p.out holds kW float4 per row) to its point in its march brick's storage.
+template <int kW>
 __global__ void baked_scatter_kernel(SparseMcParams p, const int* vmap, float4* data, long long rows) {
   for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < rows; r += (long long)gridDim.x * blockDim.x) {
     const long long dst = p.dst[r];
@@ -45,12 +50,15 @@ __global__ void baked_scatter_kernel(SparseMcParams p, const int* vmap, float4* 
     int a, b, c;
     brick_point(static_cast<int>(dst % kBrickPoints), a, b, c);
     const long long m = vmap[p.active[s]];
-    data[m * kBakedPoints + baked_point(a, b, c)] = reinterpret_cast<const float4*>(p.out)[r];
+#pragma unroll
+    for (int w = 0; w < kW; ++w)
+      data[(m * kBakedPoints + baked_point(a, b, c)) * kW + w] = reinterpret_cast<const float4*>(p.out)[r * kW + w];
   }
 }
 
 // Every apron point (a, b or c = 8) of every stored brick from its neighbour's first points, or 0 where the neighbour
 // is not stored or lies past the lattice.  Reads interior points only, which the scatter wrote.
+template <int kW>
 __global__ void baked_apron_kernel(const int* list, const int* count, const int* vmap, long long nb, float4* data) {
   const long long n = static_cast<long long>(*count) * kBakedPoints;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
@@ -63,18 +71,22 @@ __global__ void baked_apron_kernel(const int* list, const int* count, const int*
     I += a >> 3;
     J += b >> 3;
     K += c >> 3;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (I < nb && J < nb && K < nb) {
-      const long long m = vmap[(I * nb + J) * nb + K];
-      if (m >= 0) v = data[m * kBakedPoints + baked_point(a & 7, b & 7, c & 7)];
+#pragma unroll
+    for (int w = 0; w < kW; ++w) {
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (I < nb && J < nb && K < nb) {
+        const long long m = vmap[(I * nb + J) * nb + K];
+        if (m >= 0) v = data[(m * kBakedPoints + baked_point(a & 7, b & 7, c & 7)) * kW + w];
+      }
+      data[(s * kBakedPoints + t) * kW + w] = v;
     }
-    data[s * kBakedPoints + t] = v;
   }
 }
 
 // ---- from a dense grid ----------------------------------------------------------------------------------------------
 // One CTA per brick: whether one of its 9^3 lattice points holds a sigma with max(sigma, 0) != 0 (NaN and +inf
-// included), i.e. !(sigma <= 0).
+// included), i.e. !(sigma <= 0).  Sigma is the w of a point's first float4.
+template <int kW>
 __global__ void __launch_bounds__(256) baked_grid_flag_kernel(const float4* grid, long long N, long long nb,
                                                               uint8_t* flag) {
   const long long B = nb * nb * nb;
@@ -85,7 +97,7 @@ __global__ void __launch_bounds__(256) baked_grid_flag_kernel(const float4* grid
     for (int t = threadIdx.x; t < kBakedPoints; t += blockDim.x) {
       const long long i = I * kBrick + t / (kBakedSide * kBakedSide), j = J * kBrick + (t / kBakedSide) % kBakedSide,
                       k = K * kBrick + t % kBakedSide;
-      if (i < N && j < N && k < N) any |= !(grid[(i * N + j) * N + k].w <= 0.f);
+      if (i < N && j < N && k < N) any |= !(grid[((i * N + j) * N + k) * kW].w <= 0.f);
     }
     any = __syncthreads_or(any);
     if (threadIdx.x == 0) flag[br] = any;
@@ -93,6 +105,7 @@ __global__ void __launch_bounds__(256) baked_grid_flag_kernel(const float4* grid
 }
 
 // The 9^3 points of every stored brick from the dense grid, 0 past the lattice.
+template <int kW>
 __global__ void baked_grid_copy_kernel(const float4* grid, long long N, const int* list, const int* count, long long nb,
                                        float4* data) {
   const long long n = static_cast<long long>(*count) * kBakedPoints;
@@ -103,20 +116,25 @@ __global__ void baked_grid_copy_kernel(const float4* grid, long long N, const in
     brick_coords(list[s], nb, I, J, K);
     const long long i = I * kBrick + t / (kBakedSide * kBakedSide), j = J * kBrick + (t / kBakedSide) % kBakedSide,
                     k = K * kBrick + t % kBakedSide;
-    data[e] = (i < N && j < N && k < N) ? grid[(i * N + j) * N + k] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const bool in = i < N && j < N && k < N;
+#pragma unroll
+    for (int w = 0; w < kW; ++w)
+      data[e * kW + w] = in ? grid[((i * N + j) * N + k) * kW + w] : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
 
 // ---- back to a dense grid -------------------------------------------------------------------------------------------
 // Point (i, j, k) from the brick that holds it at a, b, c < 8; (0, 0, 0, 0) where that brick is not stored.
+template <int kW>
 __global__ void baked_to_dense_kernel(const float4* data, const int* vmap, long long N, long long nb, float4* out) {
   const long long total = N * N * N;
   for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
     const long long i = q / (N * N), j = (q / N) % N, k = q % N;
     const long long m = vmap[((i >> 3) * nb + (j >> 3)) * nb + (k >> 3)];
-    out[q] = m < 0 ? make_float4(0.f, 0.f, 0.f, 0.f)
-                   : data[m * kBakedPoints + baked_point(static_cast<int>(i & 7), static_cast<int>(j & 7),
-                                                         static_cast<int>(k & 7))];
+    const long long src = (m * kBakedPoints + baked_point(static_cast<int>(i & 7), static_cast<int>(j & 7),
+                                                           static_cast<int>(k & 7))) * kW;
+#pragma unroll
+    for (int w = 0; w < kW; ++w) out[q * kW + w] = m < 0 ? make_float4(0.f, 0.f, 0.f, 0.f) : data[src + w];
   }
 }
 
@@ -211,6 +229,28 @@ __device__ __forceinline__ float baked_lerp(float a, float b, float f) {
   return __fadd_rn(__fmul_rn(__fsub_rn(1.f, f), a), __fmul_rn(f, b));
 }
 
+// PlenOctrees' eval_sh constants, degree 2.
+constexpr float kShC0 = 0.28209479177387814f;
+constexpr float kShC1 = 0.4886025119029199f;
+constexpr float kShC2_0 = 1.0925484305920792f, kShC2_1 = -1.0925484305920792f, kShC2_2 = 0.31539156525252005f,
+                kShC2_3 = -1.0925484305920792f, kShC2_4 = 0.5462742152960396f;
+
+// The 9 basis values at the unit direction (x, y, z), each operation rounded once in the order written.
+__device__ __forceinline__ void sh_basis(float x, float y, float z, float (&Y)[kShBasis]) {
+  Y[0] = kShC0;
+  Y[1] = -__fmul_rn(kShC1, y);
+  Y[2] = __fmul_rn(kShC1, z);
+  Y[3] = -__fmul_rn(kShC1, x);
+  Y[4] = __fmul_rn(__fmul_rn(kShC2_0, x), y);
+  Y[5] = __fmul_rn(__fmul_rn(kShC2_1, y), z);
+  Y[6] = __fmul_rn(kShC2_2, __fsub_rn(__fsub_rn(__fmul_rn(2.f, __fmul_rn(z, z)), __fmul_rn(x, x)), __fmul_rn(y, y)));
+  Y[7] = __fmul_rn(__fmul_rn(kShC2_3, x), z);
+  Y[8] = __fmul_rn(kShC2_4, __fsub_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
+}
+
+// kW = 7: a sample's colour is clamp(sum_m cbar_{ch,m} Y_m(d / |d|), 0, 1), cbar the trilinear coefficients; the other
+// six float4 of its corners are read only when alpha != 0.
+template <int kW>
 __global__ void __launch_bounds__(kBakedThreads) baked_render_kernel(BakedRenderParams r) {
   for (long long ray = blockIdx.x * (long long)blockDim.x + threadIdx.x; ray < r.n;
        ray += (long long)gridDim.x * blockDim.x) {
@@ -222,9 +262,11 @@ __global__ void __launch_bounds__(kBakedThreads) baked_render_kernel(BakedRender
     for (int c = 0; c < 8; ++c) finite &= isfinite(R[c]);
     long long K = 0;
     float dt = 0.f;
+    float Y[kShBasis];
     if (finite && far > near) {
       const float nd = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])),
                                             __fmul_rn(d[2], d[2])));
+      if constexpr (kW > 1) sh_basis(__fdiv_rn(d[0], nd), __fdiv_rn(d[1], nd), __fdiv_rn(d[2], nd), Y);
       dt = __fdiv_rn(r.step, nd);
       if (dt > 0.f && isfinite(dt)) {
         const float kf = floorf(__fdiv_rn(__fsub_rn(far, near), dt));
@@ -254,12 +296,12 @@ __global__ void __launch_bounds__(kBakedThreads) baked_render_kernel(BakedRender
         cell[a] = min(static_cast<int>(u[a]), r.N - 2);
         f[a] = __fsub_rn(u[a], static_cast<float>(cell[a]));
       }
-      const float4* p = r.data + static_cast<long long>(slot) * kBakedPoints +
-                        baked_point(cell[1] & 7, cell[0] & 7, cell[2] & 7);
+      const float4* p = r.data + (static_cast<long long>(slot) * kBakedPoints +
+                                  baked_point(cell[1] & 7, cell[0] & 7, cell[2] & 7)) * kW;
       float4 v[8];
 #pragma unroll
       for (int c = 0; c < 8; ++c)   // c: bit 2 along i (y), bit 1 along j (x), bit 0 along k (z)
-        v[c] = __ldg(p + baked_point(c >> 2, (c >> 1) & 1, c & 1));
+        v[c] = __ldg(p + baked_point(c >> 2, (c >> 1) & 1, c & 1) * kW);
       float val[4];
 #pragma unroll
       for (int ch = 0; ch < 4; ++ch) {
@@ -275,6 +317,29 @@ __global__ void __launch_bounds__(kBakedThreads) baked_render_kernel(BakedRender
       }
       const float alpha = __fsub_rn(1.f, expf(-__fmul_rn(val[3], r.step)));
       if (alpha != 0.f) {         // alpha = 0 leaves every sum and T as they are
+        if constexpr (kW > 1) {
+          float col[3];
+#pragma unroll
+          for (int ch = 0; ch < 3; ++ch) col[ch] = __fmul_rn(val[ch], Y[0]);
+#pragma unroll
+          for (int w4 = 1; w4 < kW; ++w4) {
+#pragma unroll
+            for (int c = 0; c < 8; ++c) v[c] = __ldg(p + baked_point(c >> 2, (c >> 1) & 1, c & 1) * kW + w4);
+#pragma unroll
+            for (int l = 0; l < 4; ++l) {
+              float x[8];
+#pragma unroll
+              for (int c = 0; c < 8; ++c) x[c] = l == 0 ? v[c].x : l == 1 ? v[c].y : l == 2 ? v[c].z : v[c].w;
+              const float z00 = baked_lerp(x[0], x[1], f[2]), z01 = baked_lerp(x[2], x[3], f[2]);
+              const float z10 = baked_lerp(x[4], x[5], f[2]), z11 = baked_lerp(x[6], x[7], f[2]);
+              const float cb = baked_lerp(baked_lerp(z00, z01, f[0]), baked_lerp(z10, z11, f[0]), f[1]);
+              const int e = 4 * (w4 - 1) + l;      // coefficient 1 + e / 3 of channel e % 3
+              col[e % 3] = __fmaf_rn(cb, Y[1 + e / 3], col[e % 3]);
+            }
+          }
+#pragma unroll
+          for (int ch = 0; ch < 3; ++ch) val[ch] = fminf(fmaxf(col[ch], 0.f), 1.f);
+        }
         const float w = __fmul_rn(alpha, T);
         cr = __fadd_rn(cr, __fmul_rn(w, val[0]));
         cg = __fadd_rn(cg, __fmul_rn(w, val[1]));

@@ -25,6 +25,7 @@
 #include "baked_kernels.cuh"
 #include "../../include/nerf_pl_b200_sparse_mc.h"
 #include "../../include/nerf_pl_b200_baked.h"
+#include "../../include/nerf_pl_b200_baked_sh.h"
 
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -149,6 +150,8 @@ int device_info(DeviceInfo** out) {
                                   static_cast<int>(kSmemTotal)), "smem attr mlp(save)");
     CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kSmemTotal)), "smem attr mlp(save rows)");
+    CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(kSmemTotal)), "smem attr mlp(sh)");
     CUDA_TRY(cudaFuncSetAttribute(chain_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(kChSmemTotal)), "smem attr chain");
     CUDA_TRY(cudaFuncSetAttribute(chain_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -662,7 +665,8 @@ int backward_tail(const TrainLayout& L, const float* const* const params[2], flo
 }
 
 // The four entries of mlp_forward_kernel, after their own checks: one CTA per 128-row tile, at most one per SM.  With
-// a NeRF.forward training workspace `ws` the save-mode instantiation also stores what nerfb200_nerf_backward reads.
+// a NeRF.forward training workspace `ws` the save-mode instantiation also stores what nerfb200_nerf_backward reads;
+// with p.sh the SH mode runs.
 int launch_mlp(MlpParams p, void* ws, void* stream, const char* what) {
   DeviceInfo* d = nullptr;
   TRY(device_info(&d));
@@ -676,7 +680,8 @@ int launch_mlp(MlpParams p, void* ws, void* stream, const char* what) {
     p.tr = L.pass[0];
     p.xdir = L.xdir;
   }
-  return launch(what, ws ? mlp_forward_kernel<true> : mlp_forward_kernel<false>, ctas, kThreads, kSmemTotal, stream, p);
+  return launch(what, p.sh ? mlp_forward_kernel<false, false, true> : ws ? mlp_forward_kernel<true> : mlp_forward_kernel<false>,
+                ctas, kThreads, kSmemTotal, stream, p);
 }
 
 // The tensor table of both Adam entries: each tensor checked (steps: the device step counts, or null) and given its
@@ -1333,11 +1338,11 @@ int smc_select(const SparseMcParams& p, CubScratch& sc, int* out, int* count, cu
 
 // The evaluated points of the A > 0 active bricks through the point query on compacted rows: their row counts (rcnt)
 // and first rows (p.rofs), then per kSmcChunkBricks bricks the rows (smc_sigma_emit_kernel), the query into p.out
-// (sigma, or with `rgb` the four channels of nerfb200_query_rgb_sigma) and `scatter(rows)`, which enqueues the chunk's
-// scatter.  Reads the chunks' row bounds back, so it synchronises.
+// (`channels`: 1 for sigma, 4 for nerfb200_query_rgb_sigma, 28 for nerfb200_query_rgb_sh with its workspace sh_ws)
+// and `scatter(rows)`, which enqueues the chunk's scatter.  Reads the chunks' row bounds back, so it synchronises.
 template <class Scatter>
 int smc_query(SparseMcParams& p, const CubScratch& sc, unsigned long long* rcnt, long long A, const void* packed,
-              bool rgb, cudaStream_t s, Scatter&& scatter) {
+              int channels, void* sh_ws, cudaStream_t s, Scatter&& scatter) {
   TRY(launch("sparse_mc row counts launch", smc_row_counts_kernel, grid_blocks(A + 1, 256), 256, 0, s, p, rcnt));
   size_t tb = sc.temp_bytes;
   TRY(cub_launch(cub::DeviceScan::ExclusiveSum(sc.temp, tb, rcnt, p.rofs, static_cast<int>(A + 1), s), "sparse_mc row scan"));
@@ -1354,29 +1359,38 @@ int smc_query(SparseMcParams& p, const CubScratch& sc, unsigned long long* rcnt,
     p.slot0 = c * kSmcChunkBricks;
     p.slots = std::min(kSmcChunkBricks, A - p.slot0);
     TRY(launch("sparse_mc sigma emit launch", smc_sigma_emit_kernel, grid_blocks(p.slots, 1), kBrickPoints, 0, s, p));
-    TRY(rgb ? nerfb200_query_rgb_sigma(p.xyz, rows, 3, packed, p.out, s)
-            : nerfb200_query_sigma(p.xyz, rows, 3, packed, p.out, s));
+    TRY(channels == 28 ? nerfb200_query_rgb_sh(p.xyz, rows, 3, packed, sh_ws, nerfb200_query_rgb_sh_workspace_bytes(),
+                                               p.out, s)
+        : channels == 4 ? nerfb200_query_rgb_sigma(p.xyz, rows, 3, packed, p.out, s)
+                        : nerfb200_query_sigma(p.xyz, rows, 3, packed, p.out, s));
     TRY(scatter(rows));
   }
   return 0;
 }
 
 // ------------------------------------------------------------------ baked volumes
-// (kernels: baked_kernels.cuh, entries: include/nerf_pl_b200_baked.h).  The brick plan and its workspace are the
-// sparse marching cubes' (nerfb200_sparse_mc_plan); a volume stores the plan's march bricks.
-size_t baked_bytes(long long N, long long bricks) {
+// (kernels: baked_kernels.cuh, entries: include/nerf_pl_b200_baked.h, and include/nerf_pl_b200_baked_sh.h for the
+// view-dependent kind of kW = 7 float4 per point).  The brick plan and its workspace are the sparse marching cubes'
+// (nerfb200_sparse_mc_plan); a volume stores the plan's march bricks.
+constexpr long long kBakedShMaxN = 1024;
+long long baked_max_n(int W) { return W == 1 ? kSmcMaxN : kBakedShMaxN; }          // bake, render
+long long baked_dense_max_n(int W) { return W == 1 ? kVolMaxN : kBakedShMaxN; }    // from_grid, to_dense
+const char* baked_api(int W) { return W == 1 ? "nerfb200_baked" : "nerfb200_baked_sh"; }
+
+size_t baked_bytes(long long N, long long bricks, int W = 1) {
   const long long nb = smc_bricks(N);
-  return static_cast<size_t>(bricks) * kBakedPoints * sizeof(float4) + static_cast<size_t>(nb * nb * nb) * sizeof(int);
+  return static_cast<size_t>(bricks) * kBakedPoints * W * sizeof(float4) + static_cast<size_t>(nb * nb * nb) * sizeof(int);
 }
 
-bool baked_bricks_ok(long long N, long long bricks) {
+bool baked_bricks_ok(long long N, long long bricks, int W = 1) {
   const long long nb = smc_bricks(N);
-  return N >= 2 && N <= kSmcMaxN && bricks >= 0 && bricks <= nb * nb * nb;
+  return N >= 2 && N <= baked_max_n(W) && bricks >= 0 && bricks <= nb * nb * nb;
 }
 
 // The bake's workspace for A active bricks: the row counts and offsets, one query's rows (positions, destinations and
-// four outputs each) and the scan's scratch.
-size_t baked_carve(long long A, void* base, SparseMcParams* p, unsigned long long** rcnt, CubScratch* s) {
+// 4 W outputs each), the scan's scratch and, for W > 1, the SH query's table (sh_ws).
+size_t baked_carve(long long A, void* base, SparseMcParams* p, unsigned long long** rcnt, CubScratch* s, int W = 1,
+                   void** sh_ws = nullptr) {
   const long long rows = std::min(A, kSmcChunkBricks) * kBrickPoints;
   size_t tb = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tb, static_cast<const unsigned long long*>(nullptr),
@@ -1387,31 +1401,222 @@ size_t baked_carve(long long A, void* base, SparseMcParams* p, unsigned long lon
   p->rofs = c.take<unsigned long long>(A + 1);
   p->xyz = c.take<float>(rows * 3);
   p->dst = c.take<long long>(rows);
-  p->out = c.take<float>(rows * 4);
+  p->out = c.take<float>(rows * 4 * W);
   s->temp = c.take(s->temp_bytes);
+  if (W > 1) *sh_ws = c.take<float>(kShTableFloats);
   return c.off;
 }
 
-// A volume buffer of `bricks` stored bricks at N: its data and map.
+// A volume buffer of `bricks` stored bricks at N, W float4 per point: its data and map.
 int baked_volume(const void* volume, size_t volume_bytes, int64_t N, int64_t bricks, float4** data, int** map,
-                 const char* who) {
-  if (N < 2 || N > kSmcMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 2048]", who);
-  if (!baked_bricks_ok(N, bricks)) return fail(NERFB200_EINVAL, "%s: bricks must be in [0, ceil(N / 8)^3]", who);
+                 const char* who, int W = 1) {
+  if (N < 2 || N > baked_max_n(W)) return fail(NERFB200_EINVAL, "%s: N must be in [2, %lld]", who, baked_max_n(W));
+  if (!baked_bricks_ok(N, bricks, W)) return fail(NERFB200_EINVAL, "%s: bricks must be in [0, ceil(N / 8)^3]", who);
   if (!volume) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  if (volume_bytes != baked_bytes(N, bricks))
-    return fail(NERFB200_EINVAL, "%s: volume_bytes differs from nerfb200_baked_bytes(N, bricks)", who);
+  if (volume_bytes != baked_bytes(N, bricks, W))
+    return fail(NERFB200_EINVAL, "%s: volume_bytes differs from %s_bytes(N, bricks)", who, baked_api(W));
   *data = static_cast<float4*>(const_cast<void*>(volume));
   *map = reinterpret_cast<int*>(static_cast<uint8_t*>(const_cast<void*>(volume)) +
-                                static_cast<size_t>(bricks) * kBakedPoints * sizeof(float4));
+                                static_cast<size_t>(bricks) * kBakedPoints * W * sizeof(float4));
   return 0;
 }
 
 // The map of the `count` bricks of `list` (device values) and zeroed data.
-int baked_map(const int* list, const int* count, long long nb, long long bricks, float4* data, int* map, cudaStream_t s) {
+int baked_map(const int* list, const int* count, long long nb, long long bricks, float4* data, int* map, cudaStream_t s,
+              int W = 1) {
   CUDA_TRY(cudaMemsetAsync(map, 0xff, static_cast<size_t>(nb * nb * nb) * sizeof(int), s), "baked memset");
   if (bricks == 0) return 0;
-  CUDA_TRY(cudaMemsetAsync(data, 0, static_cast<size_t>(bricks) * kBakedPoints * sizeof(float4), s), "baked memset");
+  CUDA_TRY(cudaMemsetAsync(data, 0, static_cast<size_t>(bricks) * kBakedPoints * W * sizeof(float4), s), "baked memset");
   return launch("baked map launch", baked_map_kernel, grid_blocks(bricks, 256), 256, 0, s, list, count, map);
+}
+
+// The entries of both kinds, kW float4 per point (`who`: the entry's name in messages).
+template <int kW>
+int baked_bake(const char* who, const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
+               int64_t occ_N, const double occ_ranges_host[6], void* plan_ws, size_t plan_bytes,
+               const int64_t bricks_host[2], void* ws, size_t bytes, void* volume, size_t volume_bytes, void* stream) {
+  if (N < 2 || N > baked_max_n(kW)) return fail(NERFB200_EINVAL, "%s: N must be in [2, %lld]", who, baked_max_n(kW));
+  SparseMcParams p{};
+  TRY(smc_grids(N, ranges_host, bits, occ_N, occ_ranges_host, &p, who));
+  if (!packed || !plan_ws || !bricks_host || !ws || !volume) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  const long long A = bricks_host[0], Mb = bricks_host[1];
+  if (!smc_counts_ok(N, A, Mb)) return fail(NERFB200_EINVAL, "%s: bricks_host is not a plan's {active, march}", who);
+  CubScratch sc, sq;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  unsigned long long* rcnt;
+  void* sh_ws = nullptr;
+  if (bytes < baked_carve(A, ws, &p, &rcnt, &sq, kW, &sh_ws))
+    return fail(NERFB200_EINVAL, "%s: workspace smaller than %s_workspace_bytes(N, active, march)", who, baked_api(kW));
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, Mb, &data, &map, who, kW));
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int h[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(h, p.nsel + 1, sizeof(h), cudaMemcpyDeviceToHost, s), "baked bake readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "baked bake readback");
+  if (h[0] != A || h[1] != Mb) return fail(NERFB200_EINVAL, "%s: bricks_host differs from the plan's", who);
+  TRY(baked_map(p.march, p.nsel + 2, p.nb, Mb, data, map, s, kW));
+  if (A == 0) return 0;
+  TRY(smc_query(p, sq, rcnt, A, packed, 4 * kW, sh_ws, s, [&](long long rows) {
+    return launch("baked scatter launch", baked_scatter_kernel<kW>, grid_blocks(rows, 256), 256, 0, s, p, map, data, rows);
+  }));
+  return launch("baked apron launch", baked_apron_kernel<kW>, grid_blocks(Mb * kBakedPoints, 256), 256, 0, s, p.march,
+                p.nsel + 2, map, p.nb, data);
+}
+
+template <int kW>
+int baked_from_grid_count(const char* who, const float* grid, int64_t N, void* plan_ws, size_t plan_bytes,
+                          int64_t bricks_host[1], void* stream) {
+  const long long top = baked_dense_max_n(kW);
+  if (N < 2 || N > top) return fail(NERFB200_EINVAL, "%s: N must be in [2, %lld]", who, top);
+  if (!grid || !plan_ws || !bricks_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  SparseMcParams p{};
+  p.nb = smc_bricks(N);
+  CubScratch sc;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long B = p.nb * p.nb * p.nb;
+  TRY(launch("baked grid flag launch", baked_grid_flag_kernel<kW>, grid_blocks(B, 1), 256, 0, s,
+             reinterpret_cast<const float4*>(grid), static_cast<long long>(N), p.nb, p.flag));
+  TRY(smc_select(p, sc, p.march, p.nsel + 2, s, "baked grid select"));
+  int h = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h, p.nsel + 2, sizeof(h), cudaMemcpyDeviceToHost, s), "baked from_grid readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "baked from_grid readback");
+  bricks_host[0] = h;
+  return 0;
+}
+
+template <int kW>
+int baked_from_grid(const char* who, const float* grid, int64_t N, void* plan_ws, size_t plan_bytes, int64_t bricks,
+                    void* volume, size_t volume_bytes, void* stream) {
+  const long long top = baked_dense_max_n(kW);
+  if (N < 2 || N > top) return fail(NERFB200_EINVAL, "%s: N must be in [2, %lld]", who, top);
+  if (!grid || !plan_ws) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who, kW));
+  SparseMcParams p{};
+  p.nb = smc_bricks(N);
+  CubScratch sc;
+  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
+    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int h = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h, p.nsel + 2, sizeof(h), cudaMemcpyDeviceToHost, s), "baked from_grid readback");
+  CUDA_TRY(cudaStreamSynchronize(s), "baked from_grid readback");
+  if (h != bricks) return fail(NERFB200_EINVAL, "%s: bricks differs from %s_from_grid_count's", who, baked_api(kW));
+  TRY(baked_map(p.march, p.nsel + 2, p.nb, bricks, data, map, s, kW));
+  if (bricks == 0) return 0;
+  return launch("baked grid copy launch", baked_grid_copy_kernel<kW>, grid_blocks(bricks * kBakedPoints, 256), 256, 0, s,
+                reinterpret_cast<const float4*>(grid), static_cast<long long>(N), p.march, p.nsel + 2, p.nb, data);
+}
+
+template <int kW>
+int baked_to_dense(const char* who, const void* volume, size_t volume_bytes, int64_t N, int64_t bricks, float* grid,
+                   void* stream) {
+  const long long top = baked_dense_max_n(kW);
+  if (N < 2 || N > top) return fail(NERFB200_EINVAL, "%s: N must be in [2, %lld]", who, top);
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who, kW));
+  if (!grid) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  return launch("baked to_dense launch", baked_to_dense_kernel<kW>, grid_blocks(N * N * N, 256), 256, 0, stream, data,
+                map, static_cast<long long>(N), smc_bricks(N), reinterpret_cast<float4*>(grid));
+}
+
+template <int kW>
+int baked_render(const char* who, const void* volume, size_t volume_bytes, int64_t N, const double ranges_host[6],
+                 int64_t bricks, const float* rays, int64_t n_rays, double step, int32_t white_back, double early_stop,
+                 float* rgb, float* depth, float* opacity, void* stream) {
+  BakedRenderParams r{};
+  float4* data;
+  int* map;
+  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who, kW));
+  if (!ranges_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  for (int a = 0; a < 3; ++a) {
+    const float lo = static_cast<float>(ranges_host[2 * a]), hi = static_cast<float>(ranges_host[2 * a + 1]);
+    const float scale = static_cast<float>(static_cast<double>(N - 1) / (ranges_host[2 * a + 1] - ranges_host[2 * a]));
+    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi || !std::isfinite(scale) || scale == 0.f)
+      return fail(NERFB200_EINVAL, "%s: every range must be finite with min != max in float32", who);
+    r.lo[a] = lo;
+    r.scale[a] = scale;
+  }
+  const float s32 = static_cast<float>(step);
+  if (!(step > 0.0) || !std::isfinite(s32) || !(s32 > 0.f))
+    return fail(NERFB200_EINVAL, "%s: step must be > 0 and finite in float32", who);
+  if (!(early_stop >= 0.0 && early_stop <= 1.0)) return fail(NERFB200_EINVAL, "%s: early_stop must be in [0, 1]", who);
+  if (white_back != 0 && white_back != 1) return fail(NERFB200_EINVAL, "%s: white_back must be 0 or 1", who);
+  if (n_rays < 0) return fail(NERFB200_EINVAL, "%s: n_rays < 0", who);
+  if (n_rays > 0 && (!rays || !rgb || !depth || !opacity)) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (n_rays == 0) return 0;
+  r.data = data;
+  r.map = map;
+  r.N = static_cast<int>(N);
+  r.nb = static_cast<int>(smc_bricks(N));
+  r.step = s32;
+  r.eps = static_cast<float>(early_stop);
+  r.white_back = static_cast<float>(white_back);
+  r.rays = rays;
+  r.n = n_rays;
+  r.rgb = rgb;
+  r.depth = depth;
+  r.opacity = opacity;
+  return launch("baked render launch", baked_render_kernel<kW>, grid_blocks(n_rays, kBakedThreads, 0x7fffffffLL),
+                kBakedThreads, 0, stream, r);
+}
+
+// The SH fit of DESIGN.md §10k, made once in float64 and rounded to float32: the Fibonacci-sphere directions and
+// P = pinv(Y) = (Y^T Y)^-1 Y^T, Y the 64 x 9 basis matrix at the float32 directions (cond(Y) = 1.014, so the normal
+// equations lose nothing that float32 keeps).
+struct ShFitHost {
+  ShFit f;
+  ShFitHost() {
+    const double C0 = 0.28209479177387814, C1 = 0.4886025119029199;
+    const double C2[5] = {1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792,
+                          0.5462742152960396};
+    double Y[kShDirs][kShBasis];
+    for (int j = 0; j < kShDirs; ++j) {
+      const double z = 1.0 - (2.0 * j + 1.0) / kShDirs, phi = j * M_PI * (3.0 - std::sqrt(5.0));
+      const double rr = std::sqrt(1.0 - z * z);
+      const double d[3] = {rr * std::cos(phi), rr * std::sin(phi), z};
+      for (int a = 0; a < 3; ++a) f.dirs[3 * j + a] = static_cast<float>(d[a]);
+      const double x = f.dirs[3 * j], y = f.dirs[3 * j + 1], zz = f.dirs[3 * j + 2];
+      const double b[kShBasis] = {C0, -C1 * y, C1 * zz, -C1 * x, C2[0] * x * y, C2[1] * y * zz,
+                                  C2[2] * (2.0 * zz * zz - x * x - y * y), C2[3] * x * zz, C2[4] * (x * x - y * y)};
+      for (int m = 0; m < kShBasis; ++m) Y[j][m] = b[m];
+    }
+    // [Y^T Y | Y^T], reduced by Gauss-Jordan with partial pivoting to [I | P]
+    double M[kShBasis][kShBasis + kShDirs];
+    for (int a = 0; a < kShBasis; ++a) {
+      for (int b = 0; b < kShBasis; ++b) {
+        double acc = 0.0;
+        for (int j = 0; j < kShDirs; ++j) acc += Y[j][a] * Y[j][b];
+        M[a][b] = acc;
+      }
+      for (int j = 0; j < kShDirs; ++j) M[a][kShBasis + j] = Y[j][a];
+    }
+    for (int c = 0; c < kShBasis; ++c) {
+      int piv = c;
+      for (int r = c + 1; r < kShBasis; ++r)
+        if (std::fabs(M[r][c]) > std::fabs(M[piv][c])) piv = r;
+      for (int k = 0; k < kShBasis + kShDirs; ++k) std::swap(M[c][k], M[piv][k]);
+      const double inv = 1.0 / M[c][c];
+      for (int k = 0; k < kShBasis + kShDirs; ++k) M[c][k] *= inv;
+      for (int r = 0; r < kShBasis; ++r) {
+        if (r == c) continue;
+        const double g = M[r][c];
+        for (int k = 0; k < kShBasis + kShDirs; ++k) M[r][k] -= g * M[c][k];
+      }
+    }
+    for (int m = 0; m < kShBasis; ++m)
+      for (int j = 0; j < kShDirs; ++j) f.proj[m * kShDirs + j] = static_cast<float>(M[m][kShBasis + j]);
+  }
+};
+const ShFit& sh_fit() {
+  static const ShFitHost h;
+  return h.f;
 }
 
 // ------------------------------------------------------------------ training with empty samples skipped
@@ -3111,7 +3316,7 @@ int nerfb200_sparse_mc_count(const void* packed, int64_t N, const double ranges_
   }
   // sigma: rows of the active bricks in order, one point query per kSmcChunkBricks bricks
   CUDA_TRY(cudaMemsetAsync(p.vals, 0, static_cast<size_t>(A) * kBrickPoints * sizeof(float), s), "sparse_mc memset");
-  TRY(smc_query(p, sc, rcnt, A, packed, false, s, [&](long long rows) {
+  TRY(smc_query(p, sc, rcnt, A, packed, 1, nullptr, s, [&](long long rows) {
     return launch("sparse_mc sigma scatter launch", smc_sigma_scatter_kernel, grid_blocks(rows, 256), 256, 0, s, p, rows);
   }));
   // march: vertices and triangles per march brick
@@ -3210,132 +3415,108 @@ size_t nerfb200_baked_workspace_bytes(int64_t N, int64_t active, int64_t march) 
 int nerfb200_baked_bake(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits, int64_t occ_N,
                         const double occ_ranges_host[6], void* plan_ws, size_t plan_bytes, const int64_t bricks_host[2],
                         void* ws, size_t bytes, void* volume, size_t volume_bytes, void* stream) {
-  const char* who = "baked_bake";
-  SparseMcParams p{};
-  TRY(smc_grids(N, ranges_host, bits, occ_N, occ_ranges_host, &p, who));
-  if (!packed || !plan_ws || !bricks_host || !ws || !volume) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  const long long A = bricks_host[0], Mb = bricks_host[1];
-  if (!smc_counts_ok(N, A, Mb)) return fail(NERFB200_EINVAL, "%s: bricks_host is not a plan's {active, march}", who);
-  CubScratch sc, sq;
-  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
-    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
-  unsigned long long* rcnt;
-  if (bytes < baked_carve(A, ws, &p, &rcnt, &sq))
-    return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_baked_workspace_bytes(N, active, march)", who);
-  float4* data;
-  int* map;
-  TRY(baked_volume(volume, volume_bytes, N, Mb, &data, &map, who));
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int h[2] = {0, 0};
-  CUDA_TRY(cudaMemcpyAsync(h, p.nsel + 1, sizeof(h), cudaMemcpyDeviceToHost, s), "baked bake readback");
-  CUDA_TRY(cudaStreamSynchronize(s), "baked bake readback");
-  if (h[0] != A || h[1] != Mb) return fail(NERFB200_EINVAL, "%s: bricks_host differs from the plan's", who);
-  TRY(baked_map(p.march, p.nsel + 2, p.nb, Mb, data, map, s));
-  if (A == 0) return 0;
-  TRY(smc_query(p, sq, rcnt, A, packed, true, s, [&](long long rows) {
-    return launch("baked scatter launch", baked_scatter_kernel, grid_blocks(rows, 256), 256, 0, s, p, map, data, rows);
-  }));
-  return launch("baked apron launch", baked_apron_kernel, grid_blocks(Mb * kBakedPoints, 256), 256, 0, s, p.march,
-                p.nsel + 2, map, p.nb, data);
+  return baked_bake<1>("baked_bake", packed, N, ranges_host, bits, occ_N, occ_ranges_host, plan_ws, plan_bytes,
+                       bricks_host, ws, bytes, volume, volume_bytes, stream);
 }
 
 int nerfb200_baked_from_grid_count(const float* rgbsigma, int64_t N, void* plan_ws, size_t plan_bytes,
                                    int64_t bricks_host[1], void* stream) {
-  const char* who = "baked_from_grid_count";
-  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
-  if (!rgbsigma || !plan_ws || !bricks_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  SparseMcParams p{};
-  p.nb = smc_bricks(N);
-  CubScratch sc;
-  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
-    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const long long B = p.nb * p.nb * p.nb;
-  TRY(launch("baked grid flag launch", baked_grid_flag_kernel, grid_blocks(B, 1), 256, 0, s,
-             reinterpret_cast<const float4*>(rgbsigma), static_cast<long long>(N), p.nb, p.flag));
-  TRY(smc_select(p, sc, p.march, p.nsel + 2, s, "baked grid select"));
-  int h = 0;
-  CUDA_TRY(cudaMemcpyAsync(&h, p.nsel + 2, sizeof(h), cudaMemcpyDeviceToHost, s), "baked from_grid readback");
-  CUDA_TRY(cudaStreamSynchronize(s), "baked from_grid readback");
-  bricks_host[0] = h;
-  return 0;
+  return baked_from_grid_count<1>("baked_from_grid_count", rgbsigma, N, plan_ws, plan_bytes, bricks_host, stream);
 }
 
 int nerfb200_baked_from_grid(const float* rgbsigma, int64_t N, void* plan_ws, size_t plan_bytes, int64_t bricks,
                              void* volume, size_t volume_bytes, void* stream) {
-  const char* who = "baked_from_grid";
-  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
-  if (!rgbsigma || !plan_ws) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  float4* data;
-  int* map;
-  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who));
-  SparseMcParams p{};
-  p.nb = smc_bricks(N);
-  CubScratch sc;
-  if (plan_bytes < smc_plan_carve(N, plan_ws, &p, &sc))
-    return fail(NERFB200_EINVAL, "%s: plan workspace smaller than nerfb200_sparse_mc_plan_workspace_bytes(N)", who);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int h = 0;
-  CUDA_TRY(cudaMemcpyAsync(&h, p.nsel + 2, sizeof(h), cudaMemcpyDeviceToHost, s), "baked from_grid readback");
-  CUDA_TRY(cudaStreamSynchronize(s), "baked from_grid readback");
-  if (h != bricks) return fail(NERFB200_EINVAL, "%s: bricks differs from nerfb200_baked_from_grid_count's", who);
-  TRY(baked_map(p.march, p.nsel + 2, p.nb, bricks, data, map, s));
-  if (bricks == 0) return 0;
-  return launch("baked grid copy launch", baked_grid_copy_kernel, grid_blocks(bricks * kBakedPoints, 256), 256, 0, s,
-                reinterpret_cast<const float4*>(rgbsigma), static_cast<long long>(N), p.march, p.nsel + 2, p.nb, data);
+  return baked_from_grid<1>("baked_from_grid", rgbsigma, N, plan_ws, plan_bytes, bricks, volume, volume_bytes, stream);
 }
 
 int nerfb200_baked_to_dense(const void* volume, size_t volume_bytes, int64_t N, int64_t bricks, float* rgbsigma,
                             void* stream) {
-  const char* who = "baked_to_dense";
-  if (N < 2 || N > kVolMaxN) return fail(NERFB200_EINVAL, "%s: N must be in [2, 1625]", who);
-  float4* data;
-  int* map;
-  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who));
-  if (!rgbsigma) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  return launch("baked to_dense launch", baked_to_dense_kernel, grid_blocks(N * N * N, 256), 256, 0, stream, data, map,
-                static_cast<long long>(N), smc_bricks(N), reinterpret_cast<float4*>(rgbsigma));
+  return baked_to_dense<1>("baked_to_dense", volume, volume_bytes, N, bricks, rgbsigma, stream);
 }
 
 int nerfb200_baked_render(const void* volume, size_t volume_bytes, int64_t N, const double ranges_host[6], int64_t bricks,
                           const float* rays, int64_t n_rays, double step, int32_t white_back, double early_stop,
                           float* rgb, float* depth, float* opacity, void* stream) {
-  const char* who = "baked_render";
-  BakedRenderParams r{};
-  float4* data;
-  int* map;
-  TRY(baked_volume(volume, volume_bytes, N, bricks, &data, &map, who));
-  if (!ranges_host) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  for (int a = 0; a < 3; ++a) {
-    const float lo = static_cast<float>(ranges_host[2 * a]), hi = static_cast<float>(ranges_host[2 * a + 1]);
-    const float scale = static_cast<float>(static_cast<double>(N - 1) / (ranges_host[2 * a + 1] - ranges_host[2 * a]));
-    if (!std::isfinite(lo) || !std::isfinite(hi) || lo == hi || !std::isfinite(scale) || scale == 0.f)
-      return fail(NERFB200_EINVAL, "%s: every range must be finite with min != max in float32", who);
-    r.lo[a] = lo;
-    r.scale[a] = scale;
-  }
-  const float s32 = static_cast<float>(step);
-  if (!(step > 0.0) || !std::isfinite(s32) || !(s32 > 0.f))
-    return fail(NERFB200_EINVAL, "%s: step must be > 0 and finite in float32", who);
-  if (!(early_stop >= 0.0 && early_stop <= 1.0)) return fail(NERFB200_EINVAL, "%s: early_stop must be in [0, 1]", who);
-  if (white_back != 0 && white_back != 1) return fail(NERFB200_EINVAL, "%s: white_back must be 0 or 1", who);
-  if (n_rays < 0) return fail(NERFB200_EINVAL, "%s: n_rays < 0", who);
-  if (n_rays > 0 && (!rays || !rgb || !depth || !opacity)) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
-  if (n_rays == 0) return 0;
-  r.data = data;
-  r.map = map;
-  r.N = static_cast<int>(N);
-  r.nb = static_cast<int>(smc_bricks(N));
-  r.step = s32;
-  r.eps = static_cast<float>(early_stop);
-  r.white_back = static_cast<float>(white_back);
-  r.rays = rays;
-  r.n = n_rays;
-  r.rgb = rgb;
-  r.depth = depth;
-  r.opacity = opacity;
-  return launch("baked render launch", baked_render_kernel, grid_blocks(n_rays, kBakedThreads, 0x7fffffffLL),
-                kBakedThreads, 0, stream, r);
+  return baked_render<1>("baked_render", volume, volume_bytes, N, ranges_host, bricks, rays, n_rays, step, white_back,
+                         early_stop, rgb, depth, opacity, stream);
+}
+
+// ---- view-dependent baked volumes (include/nerf_pl_b200_baked_sh.h)
+size_t nerfb200_baked_sh_bytes(int64_t N, int64_t bricks) {
+  return baked_bricks_ok(N, bricks, 7) ? baked_bytes(N, bricks, 7) : 0;
+}
+
+size_t nerfb200_baked_sh_workspace_bytes(int64_t N, int64_t active, int64_t march) {
+  if (N > kBakedShMaxN || !smc_counts_ok(N, active, march)) return 0;
+  SparseMcParams p{};
+  unsigned long long* rcnt;
+  CubScratch sc;
+  void* sh_ws;
+  return baked_carve(active, nullptr, &p, &rcnt, &sc, 7, &sh_ws);
+}
+
+int nerfb200_baked_sh_bake(const void* packed, int64_t N, const double ranges_host[6], const uint32_t* bits,
+                           int64_t occ_N, const double occ_ranges_host[6], void* plan_ws, size_t plan_bytes,
+                           const int64_t bricks_host[2], void* ws, size_t bytes, void* volume, size_t volume_bytes,
+                           void* stream) {
+  return baked_bake<7>("baked_sh_bake", packed, N, ranges_host, bits, occ_N, occ_ranges_host, plan_ws, plan_bytes,
+                       bricks_host, ws, bytes, volume, volume_bytes, stream);
+}
+
+int nerfb200_baked_sh_from_grid_count(const float* grid, int64_t N, void* plan_ws, size_t plan_bytes,
+                                      int64_t bricks_host[1], void* stream) {
+  return baked_from_grid_count<7>("baked_sh_from_grid_count", grid, N, plan_ws, plan_bytes, bricks_host, stream);
+}
+
+int nerfb200_baked_sh_from_grid(const float* grid, int64_t N, void* plan_ws, size_t plan_bytes, int64_t bricks,
+                                void* volume, size_t volume_bytes, void* stream) {
+  return baked_from_grid<7>("baked_sh_from_grid", grid, N, plan_ws, plan_bytes, bricks, volume, volume_bytes, stream);
+}
+
+int nerfb200_baked_sh_to_dense(const void* volume, size_t volume_bytes, int64_t N, int64_t bricks, float* grid,
+                               void* stream) {
+  return baked_to_dense<7>("baked_sh_to_dense", volume, volume_bytes, N, bricks, grid, stream);
+}
+
+int nerfb200_baked_sh_render(const void* volume, size_t volume_bytes, int64_t N, const double ranges_host[6],
+                             int64_t bricks, const float* rays, int64_t n_rays, double step, int32_t white_back,
+                             double early_stop, float* rgb, float* depth, float* opacity, void* stream) {
+  return baked_render<7>("baked_sh_render", volume, volume_bytes, N, ranges_host, bricks, rays, n_rays, step,
+                         white_back, early_stop, rgb, depth, opacity, stream);
+}
+
+size_t nerfb200_query_rgb_sh_workspace_bytes(void) { return static_cast<size_t>(kShTableFloats) * sizeof(float); }
+
+int nerfb200_query_rgb_sh(const float* xyz, int64_t n, int64_t xyz_stride, const void* packed, void* ws, size_t bytes,
+                          float* out, void* stream) {
+  const char* who = "query_rgb_sh";
+  if (n < 0) return fail(NERFB200_EINVAL, "%s: n < 0", who);
+  if (n == 0) return 0;
+  if (!xyz || !packed || !ws || !out) return fail(NERFB200_EINVAL, "%s: NULL argument", who);
+  if (xyz_stride < 3) return fail(NERFB200_EINVAL, "%s: xyz_stride < 3", who);
+  if (reinterpret_cast<uintptr_t>(out) & 15) return fail(NERFB200_EINVAL, "%s: out must be 16-byte aligned", who);
+  if (reinterpret_cast<uintptr_t>(ws) & 15) return fail(NERFB200_EINVAL, "%s: ws must be 16-byte aligned", who);
+  if (bytes < nerfb200_query_rgb_sh_workspace_bytes())
+    return fail(NERFB200_EINVAL, "%s: workspace smaller than nerfb200_query_rgb_sh_workspace_bytes()", who);
+  DeviceInfo* d = nullptr;
+  TRY(device_info(&d));
+  float* table = static_cast<float*>(ws);
+  TRY(launch("query_rgb_sh table launch", sh_table_kernel, kShDirs, kDirW, 0, stream, sh_fit(),
+             static_cast<const uint8_t*>(packed), table));
+  MlpParams p{};
+  p.raw_xyz = 1;
+  p.x = xyz; p.x_stride = xyz_stride; p.n = n;
+  p.net = static_cast<const uint8_t*>(packed);
+  p.out = out;
+  p.sh = table;
+  return launch_mlp(p, nullptr, stream, "query_rgb_sh launch");
+}
+
+int nerfb200_sh_fit_host(float dirs[192], float proj[576]) {
+  if (!dirs || !proj) return fail(NERFB200_EINVAL, "sh_fit_host: NULL argument");
+  std::memcpy(dirs, sh_fit().dirs, sizeof(sh_fit().dirs));
+  std::memcpy(proj, sh_fit().proj, sizeof(sh_fit().proj));
+  return 0;
 }
 
 }  // extern "C"

@@ -329,14 +329,63 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v;
 }
 
+__device__ __forceinline__ float sigmoid_ref(float x) { return 1.f / (1.f + expf(-x)); }
+
+// ---- view-dependent colour (DESIGN.md §10k): degree-2 spherical harmonics fitted over kShDirs fixed directions
+constexpr int kShDirs = 64;
+constexpr int kShBasis = 9;
+constexpr int kShOut = 28;               // floats per point: (c_r0, c_g0, c_b0, sigma), then c_{r,g,b; m}, m = 1..8
+constexpr int kShLane = kShOut / 4;      // output floats 7 q .. 7 q + 6 belong to lane q of a quad
+// The table of the SH mode, in its workspace and resident in shared memory: [kShDirs][kDirW] direction biases
+// (dir_bias of each direction), then [kShDirs][kShOut] the projection weight of each direction per output float
+// (P[m, j] for the float holding channel ch of coefficient m; 0 for sigma).
+constexpr int kShTableFloats = kShDirs * kDirW + kShDirs * kShOut;
+constexpr uint32_t kSmemSh = kSmemScratch + 1024;       // after the Barriers, which is all mlp_forward_kernel keeps there
+static_assert(sizeof(Barriers) <= 1024 && 1024 + kShTableFloats * 4 <= kScratchBytes, "SH table must fit the scratch");
+
+// The SH epilogue: acc holds the direction layer's W' h8 without its bias (mma_layer<3>).  For each direction j in
+// order its rgb is epi_dir's with the direction's bias row, quad-summed and passed through the sigmoid as in the
+// rgb + sigma query (every lane holds it), and each lane accumulates its 7 output floats of both rows.
+__device__ __forceinline__ void epi_sh(WgCtx& c, const float (&acc)[128], const float* table,
+                                       float (*coef)[kShLane]) {
+  const float* wrgb = c.cst + kF32WRgb;
+  const float* proj = table + kShDirs * kDirW + kShLane * c.q;
+  int ch[kShLane];
+#pragma unroll
+  for (int i = 0; i < kShLane; ++i) {
+    const int o = kShLane * c.q + i;
+    ch[i] = o < 3 ? o : (o - 1) % 3;          // o = 3 (sigma) has weight 0
+    coef[0][i] = coef[1][i] = 0.f;
+  }
+#pragma unroll 1
+  for (int j = 0; j < kShDirs; ++j) {
+    const float* b = table + j * kDirW;
+    const float* const db[2] = {b, b};
+    float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    epi_dir<false>(c, acc, db, wrgb, rgb);
+#pragma unroll
+    for (int s = 0; s < 2; ++s)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) rgb[s][k] = sigmoid_ref(c.cst[kF32BRgb + k] + quad_sum(rgb[s][k]));
+#pragma unroll
+    for (int i = 0; i < kShLane; ++i) {
+      const float w = proj[j * kShOut + i];
+#pragma unroll
+      for (int s = 0; s < 2; ++s)
+        coef[s][i] = fmaf(w, ch[i] == 0 ? rgb[s][0] : ch[i] == 1 ? rgb[s][1] : rgb[s][2], coef[s][i]);
+    }
+  }
+}
+
 // The MLP of one tile for this warpgroup.  Pre-condition: the ENC tile (enc_off) holds the encoded input
 // of the warpgroup's rows and is visible to the async proxy.  Returns per row (s = 0, 1) the complete
 // sigma-head and rgb-head pre-activation sums without their biases (every lane of the quad holds them).
 //   dbias[s]: direction bias vector of row s (smem, 128 floats); kDirSlice: b' from the image, the
 //   direction part goes through the tensor core (NeRF.forward mode, ds says where the directions are).
-template <bool kSigmaOnly, bool kDirSlice, bool kSave>
+//   kSh: the SH mode; instead of rgb, coef receives this lane's output floats of both rows (epi_sh).
+template <bool kSigmaOnly, bool kDirSlice, bool kSave, bool kSh = false>
 __device__ __forceinline__ void wg_tile(WgCtx& c, uint32_t enc_off, const float* const (&dbias)[2], const DirSrc* ds,
-                                        float (&sig)[2], float (&rgb)[2][3]) {
+                                        float (&sig)[2], float (&rgb)[2][3], float (*coef)[kShLane] = nullptr) {
   float acc[128];
   uint32_t h[64];
   const float* bias = c.cst + kF32Bias;
@@ -357,7 +406,10 @@ __device__ __forceinline__ void wg_tile(WgCtx& c, uint32_t enc_off, const float*
   }
   mma_layer<1>(c, acc, h, enc_desc, ring_desc);
   epi_hidden<true, kSave>(c, 7, acc, h, bias + 7 * 256, wsig, sig);
-  if (!kSigmaOnly) {
+  if constexpr (kSh) {
+    mma_layer<3>(c, acc, h, enc_desc, ring_desc);
+    epi_sh(c, acc, reinterpret_cast<const float*>(c.smem + kSmemSh), coef);
+  } else if (!kSigmaOnly) {
     if (kDirSlice) {
       write_dir_rows(c, enc_off, *ds);
       mma_layer<4>(c, acc, h, enc_desc, ring_desc);
@@ -369,7 +421,7 @@ __device__ __forceinline__ void wg_tile(WgCtx& c, uint32_t enc_off, const float*
 #pragma unroll
   for (int s = 0; s < 2; ++s) {
     sig[s] = quad_sum(sig[s]);
-    if (!kSigmaOnly) {
+    if (!kSigmaOnly && !kSh) {
       rgb[s][0] = quad_sum(rgb[s][0]);
       rgb[s][1] = quad_sum(rgb[s][1]);
       rgb[s][2] = quad_sum(rgb[s][2]);
@@ -392,7 +444,5 @@ __device__ __forceinline__ void wg_init(WgCtx& c, uint8_t* smem, Barriers* bars)
   c.save_act = nullptr; c.save_mask = nullptr; c.save_d = nullptr; c.save_n = 0;
   c.grow[0] = c.grow[1] = -1;
 }
-
-__device__ __forceinline__ float sigmoid_ref(float x) { return 1.f / (1.f + expf(-x)); }
 
 }  // namespace nerfb200

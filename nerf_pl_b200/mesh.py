@@ -399,6 +399,23 @@ def query_rgb_sigma(model: torch.nn.Module, xyz: torch.Tensor) -> torch.Tensor:
 
 
 @torch.no_grad()
+def query_rgb_sh(model: torch.nn.Module, xyz: torch.Tensor) -> torch.Tensor:
+    """(n, 28) fp32 of ``model`` at positions xyz (n, 3), one fused launch after a small table launch (DESIGN.md
+    §10k): (c_r0, c_g0, c_b0, sigma), then c_{r,g,b; m} for m = 1..8, the degree-2 spherical-harmonic coefficients
+    (PlenOctrees' eval_sh basis) fitted by P = pinv(Y) to the sigmoid rgb at 64 fixed directions; sigma is
+    ``query_rgb_sigma``'s bit for bit."""
+    x = _cuda(xyz, "xyz").detach().to(torch.float32).contiguous()
+    if x.dim() != 2 or x.shape[1] != 3:
+        raise ValueError("xyz must be (n, 3)")
+    out = torch.empty(x.shape[0], 28, dtype=torch.float32, device=x.device)
+    blob = packed_weights(model)
+    ws = _lib.workspace(_lib.load().nerfb200_query_rgb_sh_workspace_bytes(), x.device)
+    _lib.call("nerfb200_query_rgb_sh", x.device, x.data_ptr(), x.shape[0], 3, blob.data_ptr(), ws.data_ptr(),
+              ws.numel(), out.data_ptr())
+    return out
+
+
+@torch.no_grad()
 def rgb_sigma_grid(model: torch.nn.Module, N: int, x_range, y_range, z_range, chunk: int = 1 << 21, *,
                    occupancy: Optional[OccupancyGrid] = None, return_evaluated: bool = False):
     """(N, N, N, 4) fp32 [sigmoid rgb, raw sigma] of ``model`` on the grid of ``sigma_grid`` with the direction
@@ -431,6 +448,9 @@ def pack_volume(rgbsigma: torch.Tensor, x_range) -> torch.Tensor:
     correctly rounded), a8 = trunc(255 a) and r = trunc(255 rgb).  Only ``x_range`` enters alpha, as in the
     notebook.  N <= 1625 (the indices are uint32)."""
     g = _cuda(rgbsigma, "rgbsigma").detach().to(torch.float32).contiguous()
+    if g.dim() == 4 and g.shape[3] == 28:
+        raise ValueError("pack_volume: a view-dependent (N, N, N, 28) grid has no .vol form; the Unity file holds the "
+                         "direction-0 colour of an (N, N, N, 4) grid")
     if g.dim() != 4 or g.shape[3] != 4 or not (g.shape[0] == g.shape[1] == g.shape[2]):
         raise ValueError("rgbsigma must be (N, N, N, 4)")
     N = g.shape[0]
